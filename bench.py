@@ -1,10 +1,13 @@
 #!/usr/bin/env python
 """bench.py -- projections/sec on the headline scene (100k Gaussians, 512x512 cone-beam, 50 views).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
-A "step" is one forward X-ray projection of the synthetic scene (views cycle through the 50 angles).
+A "step" is one forward X-ray projection of the synthetic scene (views cycle through the 50 angles).  The scene is
+generated from fixed seeds, so the same arguments give the same inputs on every run.  --dump-outputs DIR writes what
+the last timed step returned (the detector image, image.npy, and with one GPU the per-Gaussian radii, radii.npy) as
+float32 arrays, so that two builds can be compared output for output.
 
 ours arm
   value     projections/s with every input resident in HBM: K steps through the asynchronous C ABI
@@ -22,7 +25,7 @@ ours arm
   roofline  the dominant kernel (raster_render_kernel) re-run alone on the forward's state
             (r2x_raster_render_only), CUDA events, L2 flushed; achieved = (32 R + 4 N) bytes / duration
             against the measured HBM copy peak (MEASURED_PEAKS.json).  The kernel is FP32/MUFU-bound, not
-            HBM-bound (DESIGN.md section 5), so the fraction is small by construction; the FP32-issue fraction is
+            HBM-bound (DESIGN.md section 5), so the fraction is small by construction; the MUFU.EX2 fraction is
             reported beside it.
   cpu_baseline  the CPU oracle port (oracle/r2_oracle.c, OpenMP) on the host cores, 2 projections of the
             same scene; cpu_baseline_torch = the pure-PyTorch CPU additive projector of SURVEY 8(d)
@@ -30,7 +33,7 @@ ours arm
 
 reference arm (--impl reference)
   The reference has no CPU implementation of this path: its "own implementation" IS a CUDA rasterizer.  The
-  arm therefore times the UNMODIFIED reference CUDA sources compiled for sm_100a into oracle/_ref/libr2ref.so
+  arm therefore times the UNMODIFIED reference CUDA sources compiled for sm_90a into oracle/_ref/libr2ref.so
   (oracle/build_ref.sh) on the GPU with the identical per-step event / L2-flush protocol; if that library is
   absent it falls back to the CPU oracle port.  Rank 0 only.
 """
@@ -80,7 +83,12 @@ def parse_args():
     ap.add_argument("--cpu-baseline-child", default=None, choices=["port", "torch"], help=argparse.SUPPRESS)
     ap.add_argument("--reduce", default="p2p", choices=["p2p", "nccl"],
                     help="N > 1: how the per-rank partial images are summed (NVLink peer-memory kernel | NCCL)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
 
 
 # ------------------------------------------------------------------------------------------------
@@ -146,7 +154,7 @@ def load_peaks() -> tuple[float, str]:
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not measured)"
 
 
 def load_traffic() -> float | None:
@@ -313,6 +321,13 @@ def parity_vs_reference(render_view, cloud, views, dev, W, H, which=(0, 17, 34))
     return res
 
 
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: each array as out_dir/<name>.npy in float32."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
+
+
 # ------------------------------------------------------------------------------------------------
 def run_ours(args, rank, world, local_rank):
     import torch
@@ -375,21 +390,28 @@ def run_ours(args, rank, world, local_rank):
         if int(flag.item()) == 0:
             reducer, args.reduce = None, "nccl"
     final = torch.empty((1, H, W), dtype=torch.float32, device=dev)
+    last = {}       # what the latest step returned to its caller (a reference to the output buffer, no copy)
 
     def step(i):
         if reducer is not None:
             fwd(i, out=reducer.partial().view(1, H, W))
-            reducer.reduce(final)
+            last["image"] = reducer.reduce(final)
             return
         out = fwd(i)
         if world > 1:
             dist.all_reduce(out, op=dist.ReduceOp.SUM)
+        last["image"] = out
 
     sampler = ClockSampler(local_rank)
     sync()
     with sampler:
         ms = timed_steps(step, args.steps, args.warmup, flush, sync)
     total_ms = float(sum(ms))
+    if args.dump_outputs and rank == 0:
+        dump = {"image": last["image"]}
+        if world == 1:
+            dump["radii"] = eng.radii
+        dump_outputs(args.dump_outputs, dump)
     # back-to-back (warm L2, launches pipelined) for information; with N > 1 the all-reduce of step i runs on a
     # side stream and overlaps the render of step i+1 (ring of output buffers)
     sync()
@@ -450,19 +472,16 @@ def run_ours(args, rank, world, local_rank):
                 "timed": "r2x_raster_render_only = two small memsets (queue head, arrival counters) + the render kernel, CUDA events, L2 flushed",
                 "note": "kernel is FP32-issue-bound (multiplicative forward differences: ~5 issue slots and 0.5 "
                         "MUFU.EX2 per pixel-Gaussian pair), not HBM-bound; see DESIGN.md section 5"}
-    try:   # the bounds that do apply (both measured on this part, scripts/micro/): MUFU.EX2 rate and the FP32 issue rate
+    try:   # the bound that does apply: the MUFU.EX2 rate at the SM clock sampled during the timed steps
         props = torch.cuda.get_device_properties(dev)
-        mhz = float(sampler.summary().get("sm_mhz") or 0.0) or 1965.0
+        clk = sampler.summary()
+        mhz = float(clk.get("sm_mhz") or clk.get("sm_max_mhz") or 0.0)
         sms = props.multi_processor_count
-        ex2_peak = 15.85 * sms * mhz * 1e6
-        roofline["mufu"] = {"achieved": 0.5 * pairs / t_render, "peak": ex2_peak, "unit": "ex2/s",
-                            "frac": 0.5 * pairs / t_render / ex2_peak, "ex2_per_pair": 0.5,
-                            "peak_source": f"15.85 ex2/clk/SM (measured, mufu_rate.cu) x {sms} SMs x {mhz:.0f} MHz"}
-        loop_peak = 19.9 * sms * mhz * 1e6
-        roofline["issue"] = {"achieved": pairs / t_render, "peak": loop_peak, "unit": "pairs/s", "frac": pairs / t_render / loop_peak,
-                             "peak_source": f"19.9 pairs/clk/SM: the kernel's inner loop (f32x2 multiplicative differences) alone, "
-                                            f"all operands in registers (measured, render_loop4.cu; profiles/r02_micro_render_loop4.txt) "
-                                            f"x {sms} SMs x {mhz:.0f} MHz"}
+        ex2_peak = 16.0 * sms * mhz * 1e6
+        roofline["mufu"] = {"achieved": 0.5 * pairs / t_render, "peak": ex2_peak or None, "unit": "ex2/s",
+                            "frac": 0.5 * pairs / t_render / ex2_peak if ex2_peak else None, "ex2_per_pair": 0.5,
+                            "peak_source": f"16 ex2/clk/SM (CUDA programming guide, compute capability 9.0) x {sms} SMs "
+                                           f"x {mhz:.0f} MHz (nvidia-smi, median over the timed steps)"}
     except Exception as e:   # informational only
         roofline["mufu"] = {"error": str(e)}
 
@@ -616,6 +635,8 @@ def run_reference(args):
     except Exception:
         have_gpu = False
     if not have_gpu:
+        if args.dump_outputs:
+            raise SystemExit("bench.py: --dump-outputs with --impl reference needs a GPU and oracle/_ref/libr2ref.so")
         cb = cpu_baseline(cloud, views, 2)
         base.update(value=cb["value"], ms_per_step=1e3 / cb["value"], cpu_baseline=cb,
                     e2e={"value": cb["value"], "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
@@ -652,6 +673,8 @@ def run_reference(args):
     with sampler:
         ms = timed_steps(step, args.steps, args.warmup, flush, sync)
     total_ms = float(sum(ms))
+    if args.dump_outputs:       # the binding's output buffers hold the last timed step
+        dump_outputs(args.dump_outputs, {"image": out, "radii": radii})
     value = args.steps / (total_ms * 1e-3)
     # back-to-back, warm L2
     sync()
@@ -690,7 +713,7 @@ def run_reference(args):
     e2e_value = args.steps / (time.perf_counter() - t0)
     base.update(value=value, ms_per_step=total_ms / args.steps, value_warm_l2_back_to_back=warm,
                 clocks=sampler.summary(), gpu_launches=0,
-                reference_kind="the reference's own CUDA rasterizer (RAS/*.cu, unmodified) compiled for sm_100a into "
+                reference_kind="the reference's own CUDA rasterizer (RAS/*.cu, unmodified) compiled for sm_90a into "
                                "oracle/_ref/libr2ref.so with a GLM stand-in; called through its C++ API "
                                "CudaRasterizer::Rasterizer::forward with persistent scratch buffers (cheaper than its "
                                "torch binding, which re-allocates them every call)",
@@ -723,7 +746,7 @@ def main():
     import torch
 
     if not torch.cuda.is_available():
-        print(json.dumps({"metric": METRIC, "error": "no CUDA device: the B200 path has no CPU fallback"}), flush=True)
+        print(json.dumps({"metric": METRIC, "error": "no CUDA device: the GPU path has no CPU fallback"}), flush=True)
         return 1
     if world > 1:
         import torch.distributed as dist

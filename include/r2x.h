@@ -1,5 +1,5 @@
 /*
- * r2x.h -- C ABI of libr2xray.so, the B200-native X-ray Gaussian rasterizer + voxelizer.
+ * r2x.h -- C ABI of libr2xray.so, the H100-native X-ray Gaussian rasterizer + voxelizer.
  *
  * Drop-in boundary for the reference's native entry points (plain pointers and sizes, no torch types):
  *

@@ -1,7 +1,8 @@
 #!/usr/bin/env bash
 # Builds the UNMODIFIED reference CUDA rasterizer/voxelizer (6 .cu files, compiled from where they
-# lie under /root/reference) + oracle/ref_shim.cu into oracle/_ref/libr2ref.so for sm_100a.
-# Test/baseline infrastructure only; oracle/_ref/ is git-ignored but travels to the GPU box.
+# lie in the reference checkout, R2_REFERENCE_ROOT or /root/reference) + oracle/ref_shim.cu into oracle/_ref/libr2ref.so
+# for sm_90a.  Baseline infrastructure only (golden-vector generation, the bench's reference arm);
+# oracle/_ref/ is git-ignored.
 # Needs: oracle/glm_standin (the reference's GLM submodule is un-vendored) and -include cstdint
 # (RAS/rasterizer_impl.h:24 uses std::uintptr_t without the header).
 set -euo pipefail
@@ -10,12 +11,12 @@ REF="${R2_REFERENCE_ROOT:-/root/reference}"
 SUB="$REF/r2_gaussian/submodules/xray-gaussian-rasterization-voxelization"
 OUT="$HERE/_ref"
 if [ ! -d "$SUB/cuda_rasterizer" ]; then
-  echo "build_ref: $SUB not present (GPU box?) - keeping prebuilt $OUT" >&2
+  echo "build_ref: $SUB not present - keeping prebuilt $OUT" >&2
   exit 0
 fi
 mkdir -p "$OUT/obj"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-FLAGS=(-std=c++17 -O3 -gencode arch=compute_100a,code=sm_100a -lineinfo -Xcompiler -fPIC
+FLAGS=(-std=c++17 -O3 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC
        -I"$HERE/glm_standin" -I"$SUB" -include cstdint -w)
 srcs=(cuda_rasterizer/forward.cu cuda_rasterizer/backward.cu cuda_rasterizer/rasterizer_impl.cu
       cuda_voxelizer/forward.cu cuda_voxelizer/backward.cu cuda_voxelizer/voxelizer_impl.cu)

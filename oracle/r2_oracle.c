@@ -8,10 +8,10 @@
  *
  * Parity pinning: the reference ships NO golden vectors or tests for this
  * path (SURVEY.md section 4).  This restatement is pinned instead against the
- * reference's own CUDA sources compiled for sm_100a into oracle/_ref/
+ * reference's own CUDA sources compiled for sm_90a into oracle/_ref/
  * (oracle/build_ref.sh, with oracle/glm_standin standing in for the
- * un-vendored GLM submodule) and run on a B200: tests/test_ref_gpu.py compares
- * oracle vs oracle/_ref bit-exactly on radii / tiles_touched / sort keys and
+ * un-vendored GLM submodule) and run on the GPU, whose outputs are stored under
+ * tests/golden/ref/: tests/test_ref_gpu.py compares them with the oracle bit-exactly on radii / tiles_touched / sort keys and
  * to 1e-5 on intensities, and tests/golden/ holds vectors produced by that
  * reference build (tests/golden/make_golden.py).
  *

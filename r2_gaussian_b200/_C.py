@@ -49,7 +49,7 @@ def _ptr(t) -> int | None:
 def _require_cuda(t: torch.Tensor, name: str):
     if not isinstance(t, torch.Tensor) or t.device.type != "cuda":
         raise RuntimeError(
-            f"{name} must be a CUDA tensor: the B200 rasterizer/voxelizer has no CPU fallback "
+            f"{name} must be a CUDA tensor: the GPU rasterizer/voxelizer has no CPU fallback "
             f"(got {getattr(t, 'device', type(t))})"
         )
 

@@ -1,7 +1,7 @@
-"""r2_gaussian_b200 -- Blackwell-native X-ray Gaussian rasterizer + voxelizer (the R2-Gaussian hot path).
+"""r2_gaussian_b200 -- H100-native X-ray Gaussian rasterizer + voxelizer (the R2-Gaussian hot path).
 
 Layout
-  csrc/             hand-written sm_100a CUDA kernels + the C ABI (include/r2x.h) -> libr2xray.so
+  csrc/             hand-written sm_90a CUDA kernels + the C ABI (include/r2x.h) -> libr2xray.so
   _lib, _C          ctypes binding; the reference extension's five entry points over the C ABI
   rasterization, voxelization
                     the reference's Python surface (settings NamedTuples, nn.Modules, autograd bridges)

@@ -1,9 +1,9 @@
-"""Build libr2xray.so (the sm_100a CUDA kernels + C ABI) in-tree with nvcc.
+"""Build libr2xray.so (the sm_90a CUDA kernels + C ABI) in-tree with nvcc.
 
     python -m r2_gaussian_b200.build [--force] [--verbose]
 
-The shared library is written next to this file (git-ignored, but it travels to the GPU box with the
-gpurun snapshot).  No torch headers are involved: the C ABI takes raw device pointers.
+The shared library is written next to this file (git-ignored build product).  No torch headers are involved: the
+C ABI takes raw device pointers.
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ HEADERS = ["r2x_common.cuh", "r2x_matcalc.cuh", "r2x_binning.cuh", "r2x_raster.c
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
 

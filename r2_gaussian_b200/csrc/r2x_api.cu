@@ -1,6 +1,7 @@
 // r2x_api.cu -- the C ABI declared in include/r2x.h: buffer carving, stage orchestration, error
 // reporting.  Stage order (both pipelines): preprocess -> scan(tiles_touched) -> [sync variant: read R,
 // obtain the binning buffer] -> emit instances -> stable tile-id sort + ranges -> render.
+#include <atomic>
 #include <cstdio>
 #include <cstring>
 #include <string>
@@ -29,6 +30,22 @@ int fail(cudaError_t e, const char* what, const char* file, int line) {
 int fail_msg(int code, const char* msg) {
     g_err = msg;
     return code;
+}
+cudaError_t sm_count(int* n) {
+    // Per-device cache; concurrent first calls store the same value, so relaxed atomics suffice.
+    static std::atomic<int> cache[64];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    int v = (dev >= 0 && dev < 64) ? cache[dev].load(std::memory_order_relaxed) : 0;
+    if (v <= 0) {
+        e = cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+        if (e != cudaSuccess) return e;
+        if (v <= 0) return cudaErrorInvalidDevice;
+        if (dev >= 0 && dev < 64) cache[dev].store(v, std::memory_order_relaxed);
+    }
+    *n = v;
+    return cudaSuccess;
 }
 
 namespace {

@@ -323,7 +323,7 @@ __global__ void __launch_bounds__(SORT_THREADS) sort_hist_kernel(const uint32_t*
 
 // exclusive scan of n = 256*nb uint32 in place, one CTA of 1024 threads.  A thread owns SS_RUN consecutive
 // entries per sweep: it sums them (independent uint4 loads, one exposed latency), the CTA scans the 1024 sums
-// once, and the thread walks its run again (L1/L2 hits) writing the prefixes -- two sweeps for nb = 296.
+// once, and the thread walks its run again (L1/L2 hits) writing the prefixes -- two sweeps for nb = SORT_MAX_BLOCKS.
 constexpr int SS_RUN = 64;
 
 __global__ void __launch_bounds__(1024) sort_scan_kernel(uint32_t* __restrict__ hist, int n) {
@@ -846,7 +846,9 @@ int launch_sort_and_ranges(cudaStream_t st, long long R_launch, int num_tiles, c
     }
     if (sorted_keys_out) *sorted_keys_out = bv.keys[cur];
     long long nbr = (R_launch + 255) / 256;
-    const int gr = (int)(nbr < 148 * 8 ? nbr : 148 * 8);
+    int sms;
+    R2X_CUDA_OK(sm_count(&sms));
+    const int gr = (int)(nbr < sms * 8 ? nbr : sms * 8);
     tile_ranges_kernel<<<gr, 256, 0, st>>>(bv.keys[cur], d_total, bv.capacity, ranges);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;

@@ -35,7 +35,7 @@ struct BinningView {
 constexpr int SORT_THREADS = 256;
 constexpr int SORT_ITEMS = 16;                         // keys per thread per sub-chunk
 constexpr int SORT_CHUNK = SORT_THREADS * SORT_ITEMS;  // 4096
-constexpr int SORT_MAX_BLOCKS = 296;                   // 2 CTAs per SM on 148 SMs
+constexpr int SORT_MAX_BLOCKS = 264;                   // 2 CTAs per SM on the 132 SMs of an H100 SXM
 
 // ---- work plan for the per-tile kernels -------------------------------------------------------
 // Per-tile lists are cut into chunks of at most C instances (C = the launch's chunk size, 64..PLAN_CHUNK, decided ON
@@ -64,12 +64,12 @@ constexpr int VOX_CHUNK_CAP = 4096;
 __host__ __device__ __forceinline__ uint32_t plan_chunk_for(uint32_t R, int chunk_override, int chunk_cap) {
     const uint32_t cap = (uint32_t)(chunk_cap > PLAN_CHUNK ? chunk_cap : PLAN_CHUNK);
     if (chunk_override > 0) return (uint32_t)(chunk_override < PLAN_MIN_CHUNK ? PLAN_MIN_CHUNK : ((uint32_t)chunk_override > cap ? cap : (uint32_t)chunk_override));
-    // Rasterizer (cap = PLAN_CHUNK).  Measured (B200, warp-specialised render kernel): the largest chunk wins at every
-    // instance count -- 256 vs 192 / 128 / 64 on the 1.06 M-instance headline scene: 78 / 84 / 97 / 132 us -- because a
-    // work item costs the producer warp a fixed latency chain.
+    // Rasterizer (cap = PLAN_CHUNK): the largest chunk, because a work item costs the producer warp of the
+    // warp-specialised render kernel a fixed latency chain.  Measured (H100 SXM, 400 W, headline scene of 1.06 M
+    // instances, render kernel alone): chunks of 256 / 192 / 128 / 64 take 86 / 95 / 104 / 161 us.
     if (cap <= (uint32_t)PLAN_CHUNK) return (uint32_t)PLAN_CHUNK;
     // Voxelizer (cap = VOX_CHUNK_CAP): a tile list is only cut when that is needed to keep a few thousand work items
-    // in the queue (64 tiles of a TV crop over 592 CTAs: chunks of 256; 32768 tiles of a 256^3 query: one item per tile,
+    // in the queue (64 tiles of a TV crop over the persistent grid: chunks of 256; 32768 tiles of a 256^3 query: one item per tile,
     // so no partial sums leave the CTA and no arrival counters are touched).
     const uint32_t want = (R / 4096u + (uint32_t)PLAN_CHUNK - 1u) / (uint32_t)PLAN_CHUNK * (uint32_t)PLAN_CHUNK;
     return want < (uint32_t)PLAN_CHUNK ? (uint32_t)PLAN_CHUNK : (want > cap ? cap : want);

@@ -309,7 +309,9 @@ int launch_two_level(cudaStream_t st, int P, const uint16_t* cube, const uint32_
     R2X_PASS(launch_direct_fill(st, P, tl.cube1, tl.tiles1, tl.offsets1, tl.db1, tl.ranges1, tl.plan1, b1, tl.gx1, tl.gy1,
                            tl.status1));
     // ---- level 2: supertile lists -> tile lists
-    const int grid = 148 * 4;
+    int sms;
+    R2X_CUDA_OK(sm_count(&sms));
+    const int grid = sms * 4;
     fine_count_kernel<<<grid, L2_CHUNK, 0, st>>>(tl.plan1, tl.ranges1, tl.list1, cube, tl.gx1, tl.gy1, tl.table2a,
                                                  tl.table2b, status);
     fine_scan_kernel<<<tl.T1, SUP_TILES, 0, st>>>(tl.plan1, tl.table2a, tl.table2b, tl.gx1, tl.gy1, gx, gy, gz,

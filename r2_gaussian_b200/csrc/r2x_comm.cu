@@ -91,7 +91,9 @@ int launch_peer_allreduce(cudaStream_t st, int world, int rank, const float* con
     if (((size_t)out & 15) != 0) return fail_msg(R2X_ERR_INVALID, "r2x_peer_allreduce_sum: out must be 16-byte aligned");
     long long nb = ((n >> 2) + 255) / 256;
     if (nb < 1) nb = 1;
-    if (nb > 148) nb = 148;     // all CTAs spin on the flags: keep the grid within one wave
+    int sms;
+    R2X_CUDA_OK(sm_count(&sms));
+    if (nb > sms) nb = sms;     // all CTAs spin on the flags: keep the grid within one wave
     if (timeout_cycles <= 0) timeout_cycles = 1ll << 32;   // ~2 s
     peer_allreduce_kernel<<<(unsigned)nb, 256, 0, st>>>(pk, world, rank, epoch, out, n, status, timeout_cycles);
     R2X_CUDA_OK(cudaGetLastError());

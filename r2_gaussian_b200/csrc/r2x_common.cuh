@@ -1,4 +1,4 @@
-// r2x_common.cuh -- shared device helpers for the sm_100a X-ray Gaussian kernels.
+// r2x_common.cuh -- shared device helpers for the sm_90a X-ray Gaussian kernels.
 #pragma once
 #include <cstdint>
 #include <cstdlib>
@@ -18,6 +18,9 @@ namespace r2x {
 
 int fail(cudaError_t e, const char* what, const char* file, int line);
 int fail_msg(int code, const char* msg);
+// Streaming multiprocessors of the current device (132 on an H100 SXM), queried once per device: persistent and
+// grid-stride launches size their grids from it.  A failed query is returned as an error, never guessed.
+cudaError_t sm_count(int* n);
 
 // ---------------------------------------------------------------------------------------------
 // Folded parameter activations (SURVEY 8(f) rank 2; the reference applies them as separate torch kernels,
@@ -217,7 +220,9 @@ __device__ __forceinline__ uint32_t atom_add_release_gpu(uint32_t* addr, uint32_
     return old;
 }
 
-// packed FP32 pairs (sm_100: FMUL2 / FFMA2 -- one issue slot for two lanes of math)
+// FP32 pairs carried in one 64-bit register pair.  Hopper has no packed FP32 arithmetic, so each operation is two
+// scalar FMUL / FADD / FFMA with the same round-to-nearest, no-flush semantics per lane; pack2 / unpack2 are register
+// renames that the compiler removes.
 __device__ __forceinline__ uint64_t pack2(float a, float b) {
     uint64_t r;
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
@@ -227,19 +232,19 @@ __device__ __forceinline__ void unpack2(uint64_t v, float& a, float& b) {
     asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
 }
 __device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    unpack2(a, a0, a1); unpack2(b, b0, b1);
+    return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    unpack2(a, a0, a1); unpack2(b, b0, b1);
+    return pack2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    float a0, a1, b0, b1, c0, c1;
+    unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
+    return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
 __device__ __forceinline__ float ex2_approx(float x) {

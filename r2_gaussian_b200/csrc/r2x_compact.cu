@@ -88,7 +88,9 @@ int launch_gather_rows(cudaStream_t st, int ntensors, const r2x_gather_desc* des
         if (descs[i].width > widest) widest = descs[i].width;
     }
     long long nb = (nsel * widest + 255) / 256;
-    if (nb > 148 * 8) nb = 148 * 8;
+    int sms;
+    R2X_CUDA_OK(sm_count(&sms));
+    if (nb > sms * 8) nb = sms * 8;
     gather_rows_kernel<<<dim3((unsigned)nb, (unsigned)ntensors), 256, 0, st>>>(pk, select, nsel);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;

@@ -231,7 +231,9 @@ int launch_knn3(cudaStream_t st, int P, const float* points, float* out, void* s
     const KnnScratch s = knn_view(scratch, P);
     const size_t C = (size_t)s.G * s.G * s.G;
     knn_init_kernel<<<1, 32, 0, st>>>(s.bbox);
-    knn_bbox_kernel<<<148 * 4, 256, 0, st>>>(P, points, s.bbox);
+    int sms;
+    R2X_CUDA_OK(sm_count(&sms));
+    knn_bbox_kernel<<<sms * 4, 256, 0, st>>>(P, points, s.bbox);
     R2X_CUDA_OK(cudaMemsetAsync(s.count, 0, C * sizeof(uint32_t), st));
     const int nb = (P + 255) / 256;
     knn_count_kernel<<<nb, 256, 0, st>>>(P, points, s.bbox, s.G, s.count);

@@ -333,7 +333,9 @@ int launch_adam(cudaStream_t st, int ngroups, const r2x_adam_group* groups, doub
     if (maxn == 0) return 0;
     const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
     long long nb = (maxn + 255) / 256;
-    if (nb > 148 * 16) nb = 148 * 16;
+    int sms;
+    R2X_CUDA_OK(sm_count(&sms));
+    if (nb > sms * 16) nb = sms * 16;
     // 1 - beta in double, then float: what torch passes to lerp_/addcmul_ (betas are doubles in the ABI: 1.f - 0.999f would be off by 1.3e-5 relative)
     adam_kernel<<<dim3((unsigned)nb, (unsigned)ngroups), 256, 0, st>>>(
         pk, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps, (float)(1.0 / bc1),

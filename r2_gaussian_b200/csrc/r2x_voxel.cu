@@ -1,4 +1,4 @@
-// r2x_voxel.cu -- density-volume (3-D voxelizer) kernels for sm_100a.
+// r2x_voxel.cu -- density-volume (3-D voxelizer) kernels for sm_90a.
 //
 // Replaces the reference's VOX/forward.cu (preprocessCUDA :58-178, renderCUDA :183-315) and
 // VOX/backward.cu (renderCUDA :216-374, computeCov3DCUDA :86-177, preprocessCUDA :180-213).
@@ -220,7 +220,7 @@ __device__ __forceinline__ void vadd_if_alpha(float& acc, float e) {
 // 8 voxels of one z column.  q(k) = q0 + lin*dz + F2*dz^2 - log2 rho with dz = dz0 - k has constant second
 // differences along z, so alpha(k) = 2^-q(k) advances by multiplicative forward differences exactly as in
 // r2x_raster.cu::render_fast_8: alpha(k+1) = alpha(k) D(k), D(k+1) = D(k) K, K = 2^(-2 F2) = r2.z; runs of 4 voxels,
-// the column's two runs packed in f32x2 registers; the reference's alpha < 1e-6 skip is tested on alpha itself.
+// the column's two runs packed in register pairs (pack2 / mul2); the reference's alpha < 1e-6 skip is tested on alpha itself.
 __device__ __forceinline__ void voxel_fast_8(float (&acc)[8], const float4 r0, const float4 r1, const float4 r2,
                                              float fx, float fy, float fz0) {
     const float dx = r0.x - fx, dy = r0.y - fy, dz0 = r0.z - fz0;
@@ -677,15 +677,17 @@ int launch_voxel_preprocess(cudaStream_t st, int P, const float* means, const fl
     return 0;
 }
 
-static int vpersistent_grid(long long max_items) {
-    const long long cap = 148ll * 4;   // 4 CTAs of 256 threads per SM (54 registers/thread)
+static int vpersistent_grid(long long max_items, int sms) {
+    const long long cap = sms * 4ll;   // 4 CTAs of 256 threads per SM (54 registers/thread)
     return (int)(max_items < cap ? (max_items > 0 ? max_items : 1) : cap);
 }
 
 int launch_voxel_render(cudaStream_t st, const VoxelGrid& vg, const VoxelGeom& geom, const uint2* ranges,
                         const uint32_t* point_list, const TilePlan& plan, long long R_launch, float* out_volume) {
     const long long items = (long long)plan.num_tiles + R_launch / PLAN_CHUNK + 1;
-    voxel_render_kernel<<<vpersistent_grid(items), VR_THREADS, 0, st>>>(vg, ranges, point_list, geom.rec, plan,
+    int sms;
+    R2X_CUDA_OK(sm_count(&sms));
+    voxel_render_kernel<<<vpersistent_grid(items, sms), VR_THREADS, 0, st>>>(vg, ranges, point_list, geom.rec, plan,
                                                                         out_volume);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
@@ -695,8 +697,10 @@ int launch_voxel_render_bwd(cudaStream_t st, const VoxelGrid& vg, const VoxelGeo
                             const uint32_t* point_list, const uint32_t* inst_pos, const TilePlan& plan,
                             long long R_launch, const float* dL_dvol, float4* inst_grad) {
     const long long items = (long long)plan.num_tiles + R_launch / PLAN_CHUNK + 1;
+    int sms;
+    R2X_CUDA_OK(sm_count(&sms));
     R2X_CUDA_OK(cudaMemsetAsync(plan.counter + 1, 0, sizeof(uint32_t), st));
-    voxel_render_bwd_kernel<<<vpersistent_grid(items), 256, 0, st>>>(vg, ranges, point_list, inst_pos, geom, geom.rec, plan,
+    voxel_render_bwd_kernel<<<vpersistent_grid(items, sms), 256, 0, st>>>(vg, ranges, point_list, inst_pos, geom, geom.rec, plan,
                                                                      dL_dvol, inst_grad);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;

@@ -4,7 +4,7 @@ Mirrors PYX/rasterization.py of the reference (PYX = r2_gaussian/submodules/
 xray-gaussian-rasterization-voxelization/xray_gaussian_rasterization_voxelization):
 `GaussianRasterizationSettings` (:200-211), `GaussianRasterizer` (:214-264) and the autograd bridge
 `_RasterizeGaussians` (:46-196) -- same names, argument order, return values, gradient order and error
-behaviour -- over the B200-native library (r2_gaussian_b200._C).
+behaviour -- over the H100-native library (r2_gaussian_b200._C).
 """
 from __future__ import annotations
 

@@ -397,7 +397,7 @@ def _add_dataclass_args(parser, cls, skip=()):
 
 
 def main(argv=None):
-    ap = argparse.ArgumentParser(description="Train R2-Gaussian on one scene (B200-native pipeline)")
+    ap = argparse.ArgumentParser(description="Train R2-Gaussian on one scene (H100-native pipeline)")
     ap.add_argument("-s", "--source_path", required=True)
     ap.add_argument("-m", "--model_path", default="")
     _add_dataclass_args(ap, ModelParams, skip=("source_path", "model_path"))

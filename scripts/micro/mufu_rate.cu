@@ -1,5 +1,5 @@
 // Micro-benchmark: sustained MUFU.EX2 throughput per SM (and with an FFMA/ISETP mix like the render loop).
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o mufu_rate mufu_rate.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o mufu_rate mufu_rate.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ float ex2(float x) { float y; asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }

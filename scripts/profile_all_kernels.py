@@ -113,7 +113,7 @@ def _hbm_peak():
         return float(json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
                                                  "MEASURED_PEAKS.json")))["hbm_gbs"])
     except (OSError, KeyError, ValueError):
-        return 6486.1  # the pool's measured copy bandwidth when the driver's file is absent
+        return 3350.0  # H100 SXM data-sheet HBM3 bandwidth when no measured peak is present
 
 
 HBM_PEAK_GBPS = _hbm_peak()

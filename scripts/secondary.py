@@ -24,7 +24,7 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 
-def measure(dev=None, peak_gbs: float = 6486.1, quick: bool = False, trace=lambda msg: None) -> dict:
+def measure(dev=None, peak_gbs: float = 3350.0, quick: bool = False, trace=lambda msg: None) -> dict:
     import torch
 
     import bench

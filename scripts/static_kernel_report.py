@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Static evidence for every kernel of libr2xray.so (no GPU needed): registers / shared memory / spills from
 `cuobjdump -res-usage`, and the count of the SASS mnemonics that show what the kernel is built from -- UBLKCP (TMA bulk
-copy), LDGSTS (cp.async), SYNCS (mbarrier), MUFU.EX2, FMUL2 / FFMA2 / FADD2 (packed FP32), ATOM / RED (atomics),
+copy), LDGSTS (cp.async), SYNCS (mbarrier), MUFU.EX2, FSET / FMNMX, ATOM / RED (atomics),
 BAR (barriers) -- from `cuobjdump -sass`.
 
     python scripts/static_kernel_report.py > profiles/r02_static_kernel_report.txt"""
@@ -13,7 +13,7 @@ from collections import Counter
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "r2_gaussian_b200", "libr2xray.so")
-WATCH = ["UBLKCP", "LDGSTS", "SYNCS", "MUFU.EX2", "FMUL2", "FFMA2", "FADD2", "FSET", "FMNMX3", "VOTE", "ATOMS", "ATOMG", "RED",
+WATCH = ["UBLKCP", "LDGSTS", "SYNCS", "MUFU.EX2", "FSET", "FMNMX", "VOTE", "ATOMS", "ATOMG", "RED",
          "BAR", "ACQBULK", "LDS", "STS", "LDG", "STG"]
 
 
@@ -51,7 +51,7 @@ def main():
                 if op == w or op.startswith(w + ".") or (w == "MUFU.EX2" and op.startswith("MUFU.EX2")):
                     counts[cur][w] += 1
     names = demangle(sorted(usage))
-    print(f"# {os.path.relpath(SO, ROOT)}: {len(usage)} kernels, sm_100a; columns: registers, stack bytes, static shared bytes, SASS instructions, watched mnemonics")
+    print(f"# {os.path.relpath(SO, ROOT)}: {len(usage)} kernels, sm_90a; columns: registers, stack bytes, static shared bytes, SASS instructions, watched mnemonics")
     for mangled in sorted(usage, key=lambda k: names[k]):
         u = usage[mangled]
         short = re.sub(r"\(.*", "", names[mangled].replace("(anonymous namespace)::", "")).replace("void ", "")

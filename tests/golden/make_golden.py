@@ -1,9 +1,9 @@
 """Generate the golden vectors under tests/golden/ from the UNMODIFIED reference CUDA sources.
 
-Run on a B200 box (the reference library only exists as oracle/_ref/libr2ref.so, built by
-oracle/build_ref.sh from /root/reference in the build container):
+Run on a GPU machine where oracle/_ref/libr2ref.so has been built (oracle/build_ref.sh, with R2_REFERENCE_ROOT
+naming the reference checkout):
 
-    gpurun -- 'python tests/golden/make_golden.py gpurun_out/golden'
+    python tests/golden/make_golden.py /tmp/golden
 
 and copy the resulting .npz files into tests/golden/.  Each file holds the inputs of one small scene and
 what the reference produced for it: radii, tiles_touched, the sorted 64-bit keys and point list, the

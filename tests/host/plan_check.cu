@@ -1,6 +1,6 @@
 // Host-side check of the work-plan arithmetic in r2_gaussian_b200/csrc/r2x_binning.cuh (plan_chunk_for, plan_slice are
 // __host__ __device__): the chunk policy per consumer and the equal-slice cut of a tile list.  Built (cross-compiled for
-// sm_100a, host code run) by tests/test_plan_cpu.py; no GPU needed.
+// sm_90a, host code run) by tests/test_plan_cpu.py; no GPU needed.
 #include <cstdio>
 #include <cstdlib>
 #include "../../r2_gaussian_b200/csrc/r2x_binning.cuh"

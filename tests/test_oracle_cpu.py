@@ -1,5 +1,5 @@
 """CPU tests of the oracle itself (no GPU): against an independent float64 textbook statement of the
-math, against the committed golden vectors produced by the compiled reference on a B200
+math, against the committed golden vectors produced by the compiled reference on the GPU
 (tests/golden/), and through the structural properties the pipeline must satisfy."""
 import os
 
@@ -133,7 +133,7 @@ def test_backward_finite_difference_density():
 
 
 def test_golden_vectors():
-    """Outputs of the compiled reference (oracle/_ref on a B200, tests/golden/make_golden.py) vs the oracle."""
+    """Outputs of the compiled reference (oracle/_ref run on the GPU, tests/golden/make_golden.py) vs the oracle."""
     files = sorted(f for f in os.listdir(GOLD) if f.endswith(".npz") and f.split("_")[0] in ("raster", "voxel")) \
         if os.path.isdir(GOLD) else []
     if not files:

@@ -1,4 +1,4 @@
-"""GPU parity: our sm_100a rasterizer (through the C ABI) against the CPU oracle.
+"""GPU parity: our sm_90a rasterizer (through the C ABI) against the CPU oracle.
 
 Bars (BASELINE.json north_star): bit-exact radii / tiles_touched / tile rectangles / depth bits / the
 multiset of 64-bit sort keys; pixel intensities within 1e-5 relative (of the image scale -- a pair that

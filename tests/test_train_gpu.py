@@ -8,6 +8,8 @@ import types
 import numpy as np
 import pytest
 
+import util
+
 torch = pytest.importorskip("torch")
 import torch.nn.functional as F
 
@@ -405,30 +407,45 @@ def test_fused_losses_against_reference_golden_vectors(tag):
 def _reference_gaussian_model():
     """The reference's own GaussianModel class (r2_gaussian/gaussian/gaussian_model.py), imported unchanged from the
     copy scripts/run_reference_drivers.py --prepare puts under baseline/_ref (with the import placeholders of
-    scripts/ref_shims for plyfile & co. and this repository's simple_knn)."""
+    scripts/ref_shims for plyfile & co. and this repository's simple_knn).  Needed only to record the golden digests."""
     import importlib
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     ref = os.path.join(root, "baseline", "_ref")
-    if not os.path.isdir(os.path.join(ref, "r2_gaussian")):
-        pytest.fail("baseline/_ref is empty: run `python scripts/run_reference_drivers.py --prepare` in the build container")
+    assert os.path.isdir(os.path.join(ref, "r2_gaussian")), \
+        "recording needs baseline/_ref: run `python scripts/run_reference_drivers.py --prepare`"
     for p in (os.path.join(root, "scripts", "ref_shims"), ref):
         if p not in sys.path:
             sys.path.insert(0, p)
     return importlib.import_module("r2_gaussian.gaussian.gaussian_model").GaussianModel
 
 
+_GROUPS = (("xyz", "_xyz"), ("density", "_density"), ("scaling", "_scaling"), ("rotation", "_rotation"))
+
+
+def _model_outputs(m, g, rng):
+    """What densify_and_prune leaves behind: its return value, the CUDA RNG state, parameters, both Adam moments,
+    max_radii2D and the densification statistics."""
+    out = {"returned": g, "rng": rng, "max_radii2D": m.max_radii2D, "xyz_gradient_accum": m.xyz_gradient_accum,
+           "denom": m.denom}
+    for name, attr in _GROUPS:
+        p = getattr(m, attr)
+        out[name] = p
+        out[name + "_exp_avg"] = m.optimizer.state[p]["exp_avg"]
+        out[name + "_exp_avg_sq"] = m.optimizer.state[p]["exp_avg_sq"]
+    return out
+
+
 @pytest.mark.parametrize("max_num", [None, 10])
 def test_densify_and_prune_bit_equal_to_the_reference_class(max_num):
-    """Device-side compaction (r2x_mask_select + r2x_gather_rows) against the reference's cat / boolean-mask sequence,
-    run live from the reference's own class: parameters, both Adam moments, max_radii2D, statistics, row order and the
-    CUDA RNG stream are bit-identical (max_num=10: the densification branch is skipped, prune only)."""
-    RefModel = _reference_gaussian_model()
-    groups = (("xyz", "_xyz"), ("density", "_density"), ("scaling", "_scaling"), ("rotation", "_rotation"))
+    """Device-side compaction (r2x_mask_select + r2x_gather_rows) against the reference's cat / boolean-mask sequence
+    of the reference's own class, stored as digests (tests/golden/ref/): parameters, both Adam moments, max_radii2D,
+    statistics, row order and the CUDA RNG stream are bit-identical (max_num=10: the densification branch is skipped,
+    prune only)."""
     gm, xyz, dens = _make_model(n=6000, seed=5)
     torch.manual_seed(1)
     for _ in range(3):      # a few optimizer steps so that the Adam moments are non-trivial
-        for _, attr in groups:
+        for _, attr in _GROUPS:
             p = getattr(gm, attr)
             p.grad = torch.randn_like(p) * 1e-2
         gm.optimizer.step()
@@ -439,40 +456,39 @@ def test_densify_and_prune_bit_equal_to_the_reference_class(max_num):
     with torch.no_grad():
         gm._scaling[: n // 2] += 2.0
         gm._density[::17] = -9.0
-    # the reference model in exactly the same state
-    ref = RefModel(np.array(gm.scale_bound))
-    ref.create_from_pcd(xyz, dens, 1.0)
-    ref.training_setup(_opt_args())
-    with torch.no_grad():
-        for name, attr in groups:
-            getattr(ref, attr).copy_(getattr(gm, attr))
-    for g_ref, (name, attr) in zip(ref.optimizer.param_groups, groups):
-        assert g_ref["name"] == name
-        src = gm.optimizer.state[getattr(gm, attr)]
-        ref.optimizer.state[g_ref["params"][0]] = {"step": src["step"].clone(), "exp_avg": src["exp_avg"].clone(),
-                                                   "exp_avg_sq": src["exp_avg_sq"].clone()}
-    ref.max_radii2D = gm.max_radii2D.clone()
-    ref.xyz_gradient_accum = gm.xyz_gradient_accum.clone()
-    ref.denom = gm.denom.clone()
     bbox = torch.tensor([[-0.75, -0.75, -0.75], [0.75, 0.75, 0.75]], device="cuda")
     args = (5e-4, 1e-3, 35.0, 0.3, max_num, 0.01, bbox)
-    torch.manual_seed(123)
-    with torch.no_grad():
-        g_ref = ref.densify_and_prune(*args)
-    rng_ref = torch.cuda.get_rng_state()
+
+    def reference():
+        # the reference model in exactly the same state
+        ref = _reference_gaussian_model()(np.array(gm.scale_bound))
+        ref.create_from_pcd(xyz, dens, 1.0)
+        ref.training_setup(_opt_args())
+        with torch.no_grad():
+            for name, attr in _GROUPS:
+                getattr(ref, attr).copy_(getattr(gm, attr))
+        for g_ref, (name, attr) in zip(ref.optimizer.param_groups, _GROUPS):
+            assert g_ref["name"] == name
+            src = gm.optimizer.state[getattr(gm, attr)]
+            ref.optimizer.state[g_ref["params"][0]] = {"step": src["step"].clone(), "exp_avg": src["exp_avg"].clone(),
+                                                       "exp_avg_sq": src["exp_avg_sq"].clone()}
+        ref.max_radii2D = gm.max_radii2D.clone()
+        ref.xyz_gradient_accum = gm.xyz_gradient_accum.clone()
+        ref.denom = gm.denom.clone()
+        torch.manual_seed(123)
+        with torch.no_grad():
+            g_ref = ref.densify_and_prune(*args)
+        return _model_outputs(ref, g_ref, torch.cuda.get_rng_state())
+
+    want = util.ref_digests(f"densify_and_prune_{max_num}", reference)
     torch.manual_seed(123)
     with torch.no_grad():
         g_our = gm.densify_and_prune(*args)
-    assert torch.equal(torch.cuda.get_rng_state(), rng_ref)      # the same stream of random numbers has been consumed
-    assert torch.equal(g_our, g_ref)
-    assert gm.get_xyz.shape[0] == ref.get_xyz.shape[0] and gm.get_xyz.shape[0] != n
-    for name, attr in groups:
-        a, b = getattr(gm, attr), getattr(ref, attr)
-        assert torch.equal(a.detach(), b.detach()), name
-        sa, sb = gm.optimizer.state[a], ref.optimizer.state[b]
-        assert torch.equal(sa["exp_avg"], sb["exp_avg"]) and torch.equal(sa["exp_avg_sq"], sb["exp_avg_sq"]), name
-    assert torch.equal(gm.max_radii2D, ref.max_radii2D)
-    assert torch.equal(gm.xyz_gradient_accum, ref.xyz_gradient_accum) and torch.equal(gm.denom, ref.denom)
+    assert gm.get_xyz.shape[0] != n
+    got = _model_outputs(gm, g_our, torch.cuda.get_rng_state())
+    assert set(got) == set(want)
+    for k, v in got.items():
+        assert util.tensor_digest(v) == want[k], k    # "rng": the same stream of random numbers has been consumed
 
 
 def test_select_and_gather_rows_against_torch_indexing():

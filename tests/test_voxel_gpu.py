@@ -1,4 +1,4 @@
-"""GPU parity: our sm_100a voxelizer (through the C ABI) against the CPU oracle."""
+"""GPU parity: our sm_90a voxelizer (through the C ABI) against the CPU oracle."""
 import numpy as np
 import pytest
 

@@ -1,8 +1,10 @@
-"""Shared helpers for the parity tests: scene cases, running our C ABI, the oracle and (GPU box only)
-the compiled reference in oracle/_ref."""
+"""Shared helpers for the parity tests: scene cases, running our C ABI, the oracle, and the reference project's own
+kernels as stored golden records (tests/golden/ref/, see ref_raster)."""
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
+import json
 import os
 
 import numpy as np
@@ -11,6 +13,11 @@ from r2_gaussian_b200 import scene
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF_LIB = os.path.join(ROOT, "oracle", "_ref", "libr2ref.so")
+REF_GOLDEN = os.path.join(ROOT, "tests", "golden", "ref")
+# Set to a directory to (re)generate the golden records: the reference's kernels (oracle/_ref/libr2ref.so, built by
+# oracle/build_ref.sh) are run on the GPU and what the tests compare against is written there, e.g.
+#     R2X_RECORD_REF_GOLDEN=/tmp/ref python -m pytest -m gpu tests/test_ref_gpu.py tests/test_parity_baseline_gpu.py
+RECORD_DIR = os.environ.get("R2X_RECORD_REF_GOLDEN") or None
 
 
 def case(name: str):
@@ -229,7 +236,221 @@ def assert_grads_close(got: dict, want: dict, keys, rtol=2e-4, atol_rel=2e-5, la
         assert m <= 1.0, f"{label}{k}: mismatch {m:.3g} x tolerance"
 
 
-# ---- the compiled reference (GPU box) ---------------------------------------------------------
+# ---- the reference's outputs, stored -------------------------------------------------------------
+# A record keeps, for every array a test compares bit for bit, the SHA-256 of its bytes, and for every array compared
+# within a tolerance, max|x| over the whole array, the values at a fixed sample of positions (the largest entries and a
+# seeded random set) and sums over blocks that tile the whole array (square / cubic blocks of an image or volume, runs
+# of rows of a gradient column): the records stay small however large the scene, and a fault anywhere in an array
+# still moves the sum of its block.
+N_SAMPLE = 96         # flat positions of an image / volume
+N_SAMPLE_ROWS = 20    # rows (Gaussians) of a gradient array
+N_BLOCKS = 512        # at most this many blocks of an image / volume
+N_ROW_BLOCKS = 16     # runs of rows per gradient column
+
+
+def _block_sums(a, absolute=False):
+    """float64 sums of an image / volume over square (cubic) blocks, the edge a power-of-two multiple of the tile edge
+    (16 pixels, 8 voxels) chosen so that there are at most N_BLOCKS; and the element count of each block."""
+    a = np.asarray(a, dtype=np.float64)
+    a = np.abs(a) if absolute else a
+    edge = 16 if a.ndim == 2 else 8
+    while np.prod([-(-n // edge) for n in a.shape]) > N_BLOCKS:
+        edge *= 2
+    nb = [-(-n // edge) for n in a.shape]
+    pad = np.zeros([k * edge for k in nb]); pad[tuple(slice(0, n) for n in a.shape)] = a
+    cnt = np.zeros_like(pad); cnt[tuple(slice(0, n) for n in a.shape)] = 1.0
+    shape = [x for k in nb for x in (k, edge)]
+    axes = tuple(range(1, 2 * a.ndim, 2))
+    return pad.reshape(shape).sum(axis=axes).reshape(-1), cnt.reshape(shape).sum(axis=axes).reshape(-1)
+
+
+def _row_block_sums(a, absolute=False):
+    """float64 sums of each column of a [rows, k] array over N_ROW_BLOCKS runs of consecutive rows: [blocks, k]."""
+    a = np.asarray(a, dtype=np.float64).reshape(len(a), -1)
+    a = np.abs(a) if absolute else a
+    cuts = np.linspace(0, len(a), N_ROW_BLOCKS + 1).astype(np.int64)
+    return np.stack([a[lo:hi].sum(axis=0) for lo, hi in zip(cuts[:-1], cuts[1:])]), np.diff(cuts)
+
+
+def _digest(a) -> np.ndarray:
+    return np.frombuffer(hashlib.sha256(np.ascontiguousarray(a).tobytes()).digest(), dtype=np.uint8)
+
+
+def _sample(a, n):
+    a = np.asarray(a).reshape(len(a), -1) if n == N_SAMPLE_ROWS else np.asarray(a).reshape(-1)
+    if len(a) <= n:
+        return np.arange(len(a), dtype=np.int64)
+    mag = np.abs(a.reshape(len(a), -1)).max(axis=1)
+    top = np.argsort(-mag, kind="stable")[: n // 4]
+    rest = np.setdiff1d(np.arange(len(a)), top)
+    pick = np.random.RandomState(0).choice(rest, n - len(top), replace=False)
+    return np.sort(np.concatenate([top, pick])).astype(np.int64)
+
+
+class RefRecord:
+    """The reference's outputs for one call, as stored in tests/golden/ref/<name>.npz."""
+
+    def __init__(self, data: dict):
+        self.d = data
+        self.R = int(data["R"])
+
+    @classmethod
+    def from_outputs(cls, res: dict, exact: dict, tolerant: dict, grads: dict | None):
+        d = {"R": np.int64(res["R"])}
+        for k, a in exact.items():
+            d[f"sha_{k}"] = _digest(a)
+        for k, a in tolerant.items():
+            idx = _sample(a, N_SAMPLE)
+            d[f"max_{k}"] = np.float64(np.abs(a).max()) if a.size else np.float64(0.0)
+            d[f"idx_{k}"] = idx.astype(np.int32)
+            d[f"val_{k}"] = np.asarray(a).reshape(-1)[idx]
+            d[f"bsum_{k}"] = _block_sums(a)[0].astype(np.float32)
+        for k, a in (grads or {}).items():
+            a = np.asarray(a).reshape(len(a), -1)
+            idx = _sample(a, N_SAMPLE_ROWS)
+            d[f"gmax_{k}"] = np.float64(np.abs(a).max()) if a.size else np.float64(0.0)
+            d[f"gidx_{k}"] = idx.astype(np.int32)
+            d[f"gval_{k}"] = a[idx]
+            d[f"gbsum_{k}"] = _row_block_sums(a)[0].astype(np.float32)
+        return cls(d)
+
+    def assert_equal(self, key, a):
+        assert np.array_equal(_digest(a), self.d[f"sha_{key}"]), f"{key}: differs from the reference"
+
+    def assert_close(self, key, a, rel=1e-5, abs_=1e-7):
+        """|a - ref| <= rel * max|ref| + abs_ at the stored positions, max|a| within the same bar of max|ref|, and every
+        block sum within (elements of the block) x that bar of the reference's (the bound the per-element bar implies;
+        1e-6 relative allows for the float32 storage of the reference's sums)."""
+        scale = float(self.d[f"max_{key}"])
+        bar = rel * scale + abs_
+        sums, cnt = _block_sums(a)
+        flat = np.asarray(a, dtype=np.float64).reshape(-1)
+        want = self.d[f"val_{key}"].astype(np.float64)
+        err = float(np.abs(flat[self.d[f"idx_{key}"]] - want).max()) if want.size else 0.0
+        err = max(err, abs(float(np.abs(flat).max()) - scale) if flat.size else 0.0)
+        assert err <= bar, f"{key}: max |ours - ref| = {err:.3g} vs scale {scale:.3g}"
+        ref_sums = self.d[f"bsum_{key}"].astype(np.float64)
+        over = np.abs(sums - ref_sums) / (cnt * bar + 1e-6 * np.abs(ref_sums) + 1e-30)
+        assert over.max(initial=0.0) <= 1.0, f"{key}: block {int(over.argmax())} sum off by {over.max():.3g} x its bar"
+        return err / max(scale, 1e-30)
+
+    @property
+    def grad_keys(self):
+        return [k[5:] for k in self.d if k.startswith("gmax_")]
+
+    def assert_grads_close(self, got: dict, keys, rtol=2e-4, atol_rel=2e-5, label=""):
+        """util.assert_grads_close at the stored rows, with the scales of the whole arrays."""
+        for k in keys:
+            scale = float(self.d[f"gmax_{k}"])
+            if k == "dL_drot":
+                scale = max(scale, float(self.d["gmax_dL_dscale"]))
+            idx = self.d[f"gidx_{k}"]
+            a = np.asarray(got[k]).reshape(len(got[k]), -1)
+            m = grad_mismatch(a[idx], self.d[f"gval_{k}"], rtol, atol_rel, scale)
+            assert m <= 1.0, f"{label}{k}: mismatch {m:.3g} x tolerance"
+            # runs of rows: the sum of the per-element tolerances over the run, with sum |ref| taken as sum |ours|
+            # (the two differ by far less than the run's tolerance); 1e-6 relative for the float32 storage
+            sums, n = _row_block_sums(a)
+            babs = _row_block_sums(a, absolute=True)[0]
+            ref_sums = self.d[f"gbsum_{k}"].astype(np.float64)
+            tol = (rtol + 1e-6) * babs + atol_rel * scale * n[:, None] + 1e-30
+            over = np.abs(sums - ref_sums) / tol
+            assert over.max(initial=0.0) <= 1.0, f"{label}{k}: a run of rows sums off by {over.max():.3g} x tolerance"
+
+
+def _save(path, d: dict):
+    """One record = a JSON index of (name, dtype, shape) + one byte blob: two zip entries instead of one per array."""
+    keys = sorted(d)
+    arrs = [np.asarray(d[k]) for k in keys]
+    meta = json.dumps([[k, a.dtype.str, list(a.shape)] for k, a in zip(keys, arrs)]).encode()
+    blob = np.frombuffer(b"".join(np.ascontiguousarray(a).tobytes() for a in arrs), dtype=np.uint8)
+    os.makedirs(os.path.dirname(path), exist_ok=True)
+    np.savez_compressed(path, meta=np.frombuffer(meta, dtype=np.uint8), blob=blob)
+
+
+def _load(path) -> dict:
+    assert os.path.exists(path), f"golden record {path} is missing"
+    with np.load(path) as z:
+        meta, blob = json.loads(z["meta"].tobytes()), z["blob"].tobytes()
+    d, off = {}, 0
+    for k, dt, shape in meta:
+        n = int(np.prod(shape, dtype=np.int64)) * np.dtype(dt).itemsize
+        d[k] = np.frombuffer(blob[off:off + n], dtype=dt).reshape(tuple(shape))
+        off += n
+    return d
+
+
+def _ref_record(name: str, run, backward: bool):
+    if RECORD_DIR and (backward or not os.path.exists(os.path.join(RECORD_DIR, name + ".npz"))):
+        rec = run()
+        _save(os.path.join(RECORD_DIR, name + ".npz"), rec.d)
+        return rec
+    # a forward-only call may reuse a full record
+    return RefRecord(_load(os.path.join(RECORD_DIR or REF_GOLDEN, name + ".npz")))
+
+
+def ref_raster(name, cloud, view, dL=None, cov3D_precomp=None) -> RefRecord:
+    """The reference rasterizer's outputs for this scene (forward, and backward when dL is given)."""
+    def run():
+        ref = run_ref_raster(cloud, view, dL, cov3D_precomp=cov3D_precomp)
+        vis = ref["radii"] > 0
+        exact = {"radii": ref["radii"].astype(np.int32), "tiles_touched": ref["tiles_touched"],
+                 "keys": ref["keys"], "keys_sorted": np.sort(ref["keys"]), "point_list": ref["point_list"],
+                 "ranges": ref["ranges"]}
+        for k in ("depth", "xy", "cov3D", "conic_opacity", "mu"):
+            exact[k + "_vis"] = ref[k][vis].view(np.uint32)
+        return RefRecord.from_outputs(ref, exact, {"image": ref["image"]}, ref.get("grads"))
+    return _ref_record(name, run, dL is not None)
+
+
+def ref_voxel(name, cloud, nV, sV, ctr, dL=None, cov3D_precomp=None) -> RefRecord:
+    """The reference voxelizer's outputs for this grid (forward, and backward when dL is given)."""
+    def run():
+        ref = run_ref_voxel(cloud, nV, sV, ctr, dL, cov3D_precomp=cov3D_precomp)
+        vis = ref["tiles_touched"] > 0
+        exact = {k: ref[k].astype(np.int32) for k in ("radii_x", "radii_y", "radii_z")}
+        exact.update(tiles_touched=ref["tiles_touched"], keys=ref["keys"], keys_sorted=np.sort(ref["keys"]),
+                     point_list=ref["point_list"], ranges=ref["ranges"])
+        for k in ("xyz_vol", "depth", "conic_opacity"):
+            exact[k + "_vis"] = ref[k][vis].view(np.uint32)
+        return RefRecord.from_outputs(ref, exact, {"vol": ref["vol"]}, ref.get("grads"))
+    return _ref_record(name, run, dL is not None)
+
+
+def ref_mark_visible(name, means, view_t, proj_t) -> np.ndarray:
+    """The reference's markVisible flags for these (device) points, stored whole (one byte per point)."""
+    path = os.path.join(REF_GOLDEN, name + ".npz")
+    if RECORD_DIR:
+        import torch
+        lib = need_ref()
+        present = torch.zeros(means.shape[0], dtype=torch.bool, device=means.device)
+        p = lambda x: C.c_void_p(x.data_ptr())
+        lib.ref_mark_visible(means.shape[0], p(means), p(view_t), p(proj_t), p(present))
+        torch.cuda.synchronize()
+        out = present.cpu().numpy()
+        _save(os.path.join(RECORD_DIR, name + ".npz"), {"present": np.packbits(out), "n": np.int64(out.size)})
+        return out
+    z = _load(path)
+    return np.unpackbits(z["present"])[: int(z["n"])].astype(bool)
+
+
+def ref_digests(name, run) -> dict:
+    """SHA-256 of each array `run()` returns (a dict of tensors / arrays), computed now when recording, else stored."""
+    path = os.path.join(REF_GOLDEN, name + ".npz")
+    if RECORD_DIR:
+        out = {k: np.array(tensor_digest(v)) for k, v in run().items()}
+        _save(os.path.join(RECORD_DIR, name + ".npz"), out)
+        return {k: str(v) for k, v in out.items()}
+    return {k: str(v) for k, v in _load(path).items()}
+
+
+def tensor_digest(x) -> str:
+    if hasattr(x, "detach"):
+        x = x.detach().cpu().contiguous().numpy()
+    return _digest(np.asarray(x)).tobytes().hex() + f":{np.asarray(x).dtype}:{tuple(np.asarray(x).shape)}"
+
+
+# ---- the compiled reference (recording only) --------------------------------------------------
 _ref = None
 
 
@@ -245,15 +466,8 @@ def ref_lib():
 
 
 def need_ref():
-    """The compiled reference (oracle/_ref/libr2ref.so).  It is built in the build container (where
-    /root/reference exists) and travels to the GPU box; a GPU box without it is a broken snapshot, so
-    the parity tests FAIL there instead of skipping."""
-    import pytest
-
     lib = ref_lib()
-    if lib is None:
-        pytest.fail("oracle/_ref/libr2ref.so is missing: run `bash oracle/build_ref.sh` in the build container "
-                    "(needs /root/reference) before sending the tree to the GPU box")
+    assert lib is not None, "recording golden records needs oracle/_ref/libr2ref.so (oracle/build_ref.sh)"
     return lib
 
 
