@@ -255,6 +255,31 @@ int r2x_mask_select(void* stream, int n, const unsigned char* mask, int* idx_out
                     size_t scratch_bytes);
 int r2x_gather_rows(void* stream, int ntensors, const r2x_gather_desc* descs, const int* select, long long nsel);
 
+/* ---- FDK reconstruction (initial volume for the point cloud) ------------------------------------ */
+/* Replaces TIGRE's `algs.fdk` (r2_gaussian/utils/ct_utils.py::recon_volume, called by initialize_pcd.py).  Lengths in
+ * the scene-scaled units of the dataset readers.  projs[N,H,W] (rows = v, columns = u); viewmatrices / projmatrices
+ * [N,16] are the rasterizer's per-view matrices, tan_fovx / tan_fovy the values render() passes (parallel beam: 1).
+ *   1. cone beam: cosine weight P * DSD / sqrt(DSD^2 + u^2 + v^2) at the pixel centres;
+ *   2. band-limited Ram-Lak filter along each row, linear convolution, at the isocentre pitch D (cone:
+ *      dDetector_u * DSO / DSD = 2 tan_fovx DSO / W; parallel: 2 / W, the rasterizer's detector spans ndc [-1,1]);
+ *   3. voxel-driven backprojection: voxel centres center - s/2 + (i + 1/2) s/n, projected through projmatrix and the
+ *      rasterizer's ndc -> pixel mapping, bilinear sample (0 outside the detector), weight U^2 with U = DSO / z_view
+ *      (cone; 0 for z_view <= 0) or 1 (parallel); out_volume[nx,ny,nz] = (pi / N) * sum over views in index order.
+ * No Parker weights: a cone-beam short scan is reconstructed as if it were a full one (as TIGRE's default fdk).
+ * Deterministic (no atomics).  `scratch` holds r2x_fdk_scratch_bytes(N, H, W) (the filtered views).  Asynchronous on
+ * `stream`.  Limits: W <= 16384, N * H < 2^31, nx <= 262140, nz <= 524280. */
+size_t r2x_fdk_scratch_bytes(int n_views, int H, int W);
+int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+            const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float dso, int nx, int ny, int nz,
+            float sx, float sy, float sz, float cx, float cy, float cz, float* out_volume, void* scratch,
+            size_t scratch_bytes);
+/* The two stages of r2x_fdk on their own (measurement): filtered[N,H,W] = steps 1-2; out_volume = step 3 of it. */
+int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, float tan_fovx, float tan_fovy,
+                   int mode, float dso, float* filtered);
+int r2x_fdk_backproject(void* stream, int n_views, int H, int W, const float* filtered, const float* viewmatrices,
+                        const float* projmatrices, int mode, float dso, int nx, int ny, int nz, float sx, float sy,
+                        float sz, float cx, float cy, float cz, float* out_volume);
+
 /* ---- multi-GPU exchange step: one-shot sum over NVLink peer memory ------------------------------ */
 /* The Gaussian-sharded projector (one process per GPU, every rank renders its index shard) needs ONE exchange per
  * projection: the sum of the per-rank partial detector images (BASELINE north_star; the reference itself is

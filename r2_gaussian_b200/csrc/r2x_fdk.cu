@@ -1,0 +1,250 @@
+// r2x_fdk.cu -- FDK (Feldkamp-Davis-Kress) reconstruction of a density volume from cone- or parallel-beam projections.
+//
+// The reference initialises its Gaussians from TIGRE's `algs.fdk` (r2_gaussian/utils/ct_utils.py::recon_volume called
+// by initialize_pcd.py).  FDK is a weighted ramp filter along the detector rows followed by one voxel-driven
+// backprojection; both are small data-parallel kernels, and the geometry they need is the rasterizer's own:
+//
+//   fdk_filter_kernel       one CTA per detector row: cosine weight (cone beam), stage the row in shared memory between
+//                           two rows of zeros, then the band-limited Ram-Lak filter as a linear convolution over the
+//                           whole row, using the symmetric odd-only taps:
+//                             Q_j = (r_j / 4 - sum_{k odd} (r_{j-k} + r_{j+k}) / (pi^2 k^2)) / D
+//                           (D = isocentre pitch), summed for k = 1, 3, 5, ... in that order.
+//   fdk_backproject_kernel  a thread owns one (x, y) voxel column and a run of FDK_ZR voxels along z.  Every view's
+//                           homogeneous coordinates are affine in z, so the per-view setup (4 matrix rows, staged per
+//                           chunk of views in shared memory) is paid once per run.  Each voxel centre goes through the
+//                           same projmatrix, homogeneous divide and ndc -> pixel mapping as the rasterizer, the
+//                           filtered view is sampled bilinearly through L1/L2 (__ldg; 0 outside the detector) and
+//                           weighted by U^2, U = DSO / z_view (cone; 1 for parallel beam).  The views are summed in
+//                           index order in registers and each voxel is stored once: no atomics, so the volume is
+//                           bitwise reproducible.
+//
+// The float64 NumPy statement of the same definition is oracle/fdk_oracle.py.
+#include <cmath>
+#include <cstdint>
+
+#include "../../include/r2x.h"
+#include "r2x_common.cuh"
+
+namespace r2x {
+
+constexpr int FDK_MAX_W = 16384;     // filter row staging: (3 W + W / 2) floats of shared memory (<= 227 KB)
+constexpr int FDK_BX = 32, FDK_BY = 4; // backprojection CTA: 32 y-columns x 4 x-columns
+constexpr int FDK_ZR = 8;            // voxels per thread along z
+constexpr int FDK_VCHUNK = 32;       // views staged in shared memory at a time
+
+static size_t fdk_al256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+size_t fdk_scratch_bytes(int N, int H, int W) {
+    if (N < 1 || H < 1 || W < 1) return 256;
+    return fdk_al256((size_t)N * H * W * sizeof(float)) + 256;
+}
+
+static size_t fdk_filter_smem(int W) { return (size_t)(3 * W + (W + 1) / 2) * sizeof(float); }
+
+__global__ void __launch_bounds__(256) fdk_filter_kernel(int H, int W, const float* __restrict__ projs, float tanx,
+                                                         float tany, int cone, float inv_delta, float* __restrict__ q) {
+    extern __shared__ float sm[];
+    float* row = sm;              // [3W]: zeros | weighted row | zeros
+    float* g = sm + 3 * W;        // [(W+1)/2]: g[m] = 1 / (pi^2 (2m+1)^2)
+    const size_t r = blockIdx.x;  // view * H + detector row
+    const float* src = projs + r * W;
+    const float step = 2.0f / (float)W, first = 1.0f / (float)W - 1.0f;
+    const float b = cone ? fmaf((float)(r % H), 2.0f / (float)H, 1.0f / (float)H - 1.0f) * tany : 0.0f;
+    for (int j = threadIdx.x; j < W; j += blockDim.x) {
+        float p = src[j];
+        if (cone) {
+            const float a = fmaf((float)j, step, first) * tanx;
+            p *= rsqrtf(fmaf(a, a, fmaf(b, b, 1.0f)));
+        }
+        row[j] = 0.0f;
+        row[W + j] = p;
+        row[2 * W + j] = 0.0f;
+    }
+    for (int m = threadIdx.x; m < (W + 1) / 2; m += blockDim.x) {
+        const float k = (float)(2 * m + 1);
+        g[m] = 1.0f / (9.869604401089358f * k * k);
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < W; j += blockDim.x) {
+        const float* c = row + W + j;
+        float acc = 0.0f;
+        for (int m = 0, k = 1; k < W; ++m, k += 2) acc = fmaf(g[m], c[-k] + c[k], acc);
+        q[r * W + j] = fmaf(0.25f, c[0], -acc) * inv_delta;
+    }
+}
+
+template <bool CONE>
+__global__ void __launch_bounds__(FDK_BX * FDK_BY) fdk_backproject_kernel(
+    int N, int H, int W, const float* __restrict__ q, const float* __restrict__ viewm, const float* __restrict__ projm,
+    float dso, int nx, int ny, int nz, float ox, float oy, float oz, float dx, float dy, float dz, float scale,
+    float* __restrict__ vol) {
+    // per view: projmatrix rows 0, 1, 3 and viewmatrix row 2 as (m[r], m[4+r], m[8+r], m[12+r])
+    __shared__ float4 mat[FDK_VCHUNK][4];
+    const int y = blockIdx.x * FDK_BX + threadIdx.x;
+    const int x = blockIdx.y * FDK_BY + threadIdx.y;
+    const int z0 = blockIdx.z * FDK_ZR;
+    const int tid = threadIdx.y * FDK_BX + threadIdx.x;
+    const bool live = x < nx && y < ny;
+    const float X = fmaf((float)x, dx, ox), Y = fmaf((float)y, dy, oy), Z0 = fmaf((float)z0, dz, oz);
+    const float half_w = 0.5f * (float)W, half_h = 0.5f * (float)H;
+    const float cen_w = 0.5f * (float)(W - 1), cen_h = 0.5f * (float)(H - 1);
+    const size_t view_stride = (size_t)H * W;
+    float acc[FDK_ZR];
+#pragma unroll
+    for (int k = 0; k < FDK_ZR; ++k) acc[k] = 0.0f;
+
+    for (int c0 = 0; c0 < N; c0 += FDK_VCHUNK) {
+        const int nc = min(FDK_VCHUNK, N - c0);
+        __syncthreads();
+        for (int e = tid; e < nc * 4; e += FDK_BX * FDK_BY) {
+            const int v = e >> 2, slot = e & 3;
+            const float* m = (slot == 3 ? viewm : projm) + (size_t)(c0 + v) * 16;
+            const int rr = slot == 3 ? 2 : (slot == 2 ? 3 : slot);
+            mat[v][slot] = make_float4(m[rr], m[4 + rr], m[8 + rr], m[12 + rr]);
+        }
+        __syncthreads();
+        if (!live) continue;
+        for (int v = 0; v < nc; ++v) {
+            const float4 P0 = mat[v][0], P1 = mat[v][1], P3 = mat[v][2], V2 = mat[v][3];
+            const float ax = fmaf(P0.z, Z0, fmaf(P0.y, Y, fmaf(P0.x, X, P0.w)));
+            const float ay = fmaf(P1.z, Z0, fmaf(P1.y, Y, fmaf(P1.x, X, P1.w)));
+            const float aw = fmaf(P3.z, Z0, fmaf(P3.y, Y, fmaf(P3.x, X, P3.w))) + 1e-7f;  // the rasterizer's divide
+            const float sx = P0.z * dz, sy = P1.z * dz, sw = P3.z * dz;
+            float av = 0.0f, sv = 0.0f;
+            if (CONE) {
+                av = fmaf(V2.z, Z0, fmaf(V2.y, Y, fmaf(V2.x, X, V2.w)));
+                sv = V2.z * dz;
+            }
+            const float* qv = q + (size_t)(c0 + v) * view_stride;
+#pragma unroll
+            for (int k = 0; k < FDK_ZR; ++k) {
+                const float fk = (float)k;
+                float w = 1.0f;
+                if (CONE) {
+                    const float zv = fmaf(fk, sv, av);
+                    if (!(zv > 0.0f)) continue;
+                    const float u = dso * __frcp_rn(zv);
+                    w = u * u;
+                }
+                const float pw = __frcp_rn(fmaf(fk, sw, aw));
+                const float px = fmaf(fmaf(fk, sx, ax) * pw, half_w, cen_w);
+                const float py = fmaf(fmaf(fk, sy, ay) * pw, half_h, cen_h);
+                if (!(px > -1.0f && px < (float)W && py > -1.0f && py < (float)H)) continue;
+                const float fx0 = floorf(px), fy0 = floorf(py);
+                const int ix = (int)fx0, iy = (int)fy0;
+                const float fx = px - fx0, fy = py - fy0;
+                const long long base = (long long)iy * W + ix;
+                float s00 = 0.0f, s01 = 0.0f, s10 = 0.0f, s11 = 0.0f;
+                if (iy >= 0) {
+                    if (ix >= 0) s00 = __ldg(qv + base);
+                    if (ix + 1 < W) s01 = __ldg(qv + base + 1);
+                }
+                if (iy + 1 < H) {
+                    if (ix >= 0) s10 = __ldg(qv + base + W);
+                    if (ix + 1 < W) s11 = __ldg(qv + base + W + 1);
+                }
+                const float top = fmaf(fx, s01 - s00, s00), bot = fmaf(fx, s11 - s10, s10);
+                acc[k] = fmaf(w, fmaf(fy, bot - top, top), acc[k]);
+            }
+        }
+    }
+    if (!live) return;
+    float* out = vol + ((size_t)x * ny + y) * nz;
+#pragma unroll
+    for (int k = 0; k < FDK_ZR; ++k)
+        if (z0 + k < nz) out[z0 + k] = acc[k] * scale;
+}
+
+static int fdk_filter(cudaStream_t st, int N, int H, int W, const float* projs, float tanx, float tany, int mode,
+                      float dso, float* q) {
+    const size_t smem = fdk_filter_smem(W);
+    if (smem > 48 * 1024)
+        R2X_CUDA_OK(cudaFuncSetAttribute(fdk_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // isocentre pitch: cone dDetector_u * DSO / DSD = 2 tan_fovx DSO / W; parallel 2 / W (ndc [-1,1] = scene [-1,1])
+    const double delta = mode == 1 ? 2.0 * (double)tanx * (double)dso / W : 2.0 / W;
+    fdk_filter_kernel<<<(unsigned)((long long)N * H), 256, smem, st>>>(H, W, projs, tanx, tany, mode, (float)(1.0 / delta),
+                                                                       q);
+    R2X_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+static int fdk_backproject(cudaStream_t st, int N, int H, int W, const float* q, const float* viewm, const float* projm,
+                           int mode, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
+                           float cz, float* vol) {
+    const float dx = sx / nx, dy = sy / ny, dz = sz / nz;
+    const float ox = cx - 0.5f * sx + 0.5f * dx, oy = cy - 0.5f * sy + 0.5f * dy, oz = cz - 0.5f * sz + 0.5f * dz;
+    const dim3 grid((ny + FDK_BX - 1) / FDK_BX, (nx + FDK_BY - 1) / FDK_BY, (nz + FDK_ZR - 1) / FDK_ZR);
+    const dim3 block(FDK_BX, FDK_BY);
+    const float scale = (float)(3.141592653589793 / N);
+    if (mode == 1)
+        fdk_backproject_kernel<true><<<grid, block, 0, st>>>(N, H, W, q, viewm, projm, dso, nx, ny, nz, ox, oy, oz, dx, dy,
+                                                            dz, scale, vol);
+    else
+        fdk_backproject_kernel<false><<<grid, block, 0, st>>>(N, H, W, q, viewm, projm, dso, nx, ny, nz, ox, oy, oz, dx,
+                                                             dy, dz, scale, vol);
+    R2X_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+static int fdk_validate(int N, int H, int W, const float* projs, const float* viewm, const float* projm,
+                        float tanx, float tany, int mode, float dso, int nx, int ny, int nz, float sx, float sy,
+                        float sz, const void* out, const void* scratch, size_t scratch_bytes) {
+    if (N < 1 || H < 1 || W < 1) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad N/H/W (each must be >= 1)");
+    if (W > FDK_MAX_W) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad W (detector rows wider than 16384 pixels)");
+    if ((long long)N * H > 0x7fffffffLL) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad N*H (too many detector rows)");
+    if (nx < 1 || ny < 1 || nz < 1) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad grid (each size must be >= 1)");
+    if ((nx + FDK_BY - 1) / FDK_BY > 65535 || (nz + FDK_ZR - 1) / FDK_ZR > 65535)
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad grid (too large)");
+    if (mode != 0 && mode != 1) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad mode (0 = parallel, 1 = cone)");
+    if (mode == 1 && !(dso > 0.0f && std::isfinite(dso)))
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad DSO (cone beam needs DSO > 0)");
+    if (mode == 1 && !(tanx > 0.0f && tany > 0.0f && std::isfinite(tanx) && std::isfinite(tany)))
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad tan_fov (cone beam needs tan_fovx, tan_fovy > 0)");
+    if (!(sx > 0.0f && sy > 0.0f && sz > 0.0f)) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad sVoxel (must be > 0)");
+    if (!projs || !viewm || !projm || !out || !scratch) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad pointer (NULL)");
+    if (scratch_bytes < fdk_scratch_bytes(N, H, W)) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad scratch (too small)");
+    return 0;
+}
+
+}  // namespace r2x
+
+extern "C" {
+
+size_t r2x_fdk_scratch_bytes(int n_views, int H, int W) { return r2x::fdk_scratch_bytes(n_views, H, W); }
+
+int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+            const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float dso, int nx, int ny, int nz,
+            float sx, float sy, float sz, float cx, float cy, float cz, float* out_volume, void* scratch,
+            size_t scratch_bytes) {
+    if (int rc = r2x::fdk_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode,
+                                   dso, nx, ny, nz, sx, sy, sz, out_volume, scratch, scratch_bytes))
+        return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
+    if (int rc = r2x::fdk_filter(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, q)) return rc;
+    return r2x::fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx,
+                                cy, cz, out_volume);
+}
+
+int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, float tan_fovx, float tan_fovy,
+                   int mode, float dso, float* filtered) {
+    if (n_views < 1 || H < 1 || W < 1 || W > r2x::FDK_MAX_W || (long long)n_views * H > 0x7fffffffLL)
+        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_filter: bad N/H/W");
+    if (mode != 0 && mode != 1) return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_filter: bad mode");
+    if (mode == 1 && !(dso > 0.0f && tan_fovx > 0.0f && tan_fovy > 0.0f))
+        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_filter: bad DSO / tan_fov");
+    if (!projs || !filtered) return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_filter: bad pointer (NULL)");
+    return r2x::fdk_filter((cudaStream_t)stream, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, filtered);
+}
+
+int r2x_fdk_backproject(void* stream, int n_views, int H, int W, const float* filtered, const float* viewmatrices,
+                        const float* projmatrices, int mode, float dso, int nx, int ny, int nz, float sx, float sy,
+                        float sz, float cx, float cy, float cz, float* out_volume) {
+    if (int rc = r2x::fdk_validate(n_views, H, W, filtered, viewmatrices, projmatrices, 1.0f, 1.0f,
+                                   mode, dso, nx, ny, nz, sx, sy, sz, out_volume, filtered, (size_t)-1))
+        return rc;
+    return r2x::fdk_backproject((cudaStream_t)stream, n_views, H, W, filtered, viewmatrices, projmatrices, mode, dso, nx,
+                                ny, nz, sx, sy, sz, cx, cy, cz, out_volume);
+}
+
+}  // extern "C"

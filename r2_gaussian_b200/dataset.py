@@ -8,8 +8,9 @@
 * `Camera` exposes the attributes render() reads (`dataset/cameras.py:20-84`); `Scene` the reference's
   (`dataset/__init__.py:26-99`): `getTrainCameras()`, `getTestCameras()`, `vol_gt`, `scanner_cfg`, `bbox`, `save`;
 * `init_point_cloud` = `initialize_pcd.py:41-91` (random cloud, or voxels of a given reconstruction above a threshold
-  -- the reconstruction itself, FDK via TIGRE in the reference, is passed in);
-* `write_blender` writes a dataset in that format (used by the tests and for synthetic scenes: no TIGRE here).
+  -- the reconstruction itself is passed in: `fdk.fdk` on the GPU, TIGRE's FDK in the reference);
+* `write_blender` writes a dataset in that format (used by the tests and for synthetic scenes; generating projections
+  with TIGRE is not part of this project).
 
 Device is a parameter everywhere ("cuda" by default like the reference; the CPU tests pass "cpu").
 """

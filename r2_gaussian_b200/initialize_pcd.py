@@ -1,15 +1,19 @@
-"""Initial point cloud for a scene -- the CPU-only plumbing of the reference's `initialize_pcd.py:26-172`
-(BASELINE.json configs[0]: `--recon_method random --n_points 1000` on a synthetic phantom).
+"""Initial point cloud for a scene -- the reference's `initialize_pcd.py:26-172`.
 
     python -m r2_gaussian_b200.initialize_pcd --data <scene dir | NAF pickle> [--output init.npy]
-        [--recon_method random|volume] [--recon recon.npy] [--n_points 50000] [--density_thresh 0.05]
-        [--density_rescale 0.15] [--random_density_max 1.0]
+        [--recon_method random|fdk|volume] [--recon recon.npy] [--n_points 50000] [--density_thresh 0.05]
+        [--density_rescale 0.15] [--random_density_max 1.0] [--evaluate]
 
 `random` draws positions uniformly in the volume and densities in [0, random_density_max) with numpy's global
-generator seeded with 0, exactly like the reference.  The reference's other mode reconstructs a volume with TIGRE's
-FDK first; TIGRE is not available here, so `volume` takes that reconstruction from `--recon` (an .npy in the scene's
-voxel grid, e.g. produced elsewhere) and then samples it the reference's way.  Writes [n_points, 4] = (x, y, z,
-density) in the scene's normalised [-1,1]^3 coordinates to `<scene>/init_<name>.npy` unless `--output` is given.
+generator seeded with 0, exactly like the reference.  `fdk` reconstructs the volume from the train views with the
+GPU FDK of `r2_gaussian_b200.fdk` (the reference calls TIGRE's `algs.fdk`), then samples `n_points` voxels above
+`density_thresh` and scales their densities by `density_rescale`, the reference's way; it needs a CUDA device and at
+least MIN_FDK_VIEWS train views.  `volume` samples a reconstruction made elsewhere (`--recon`, an .npy in the scene's
+voxel grid) the same way.  Writes [n_points, 4] = (x, y, z, density) in the scene's normalised [-1,1]^3 coordinates to
+`<scene>/init_<name>.npy` unless `--output` is given.  `--evaluate` builds the Gaussians from the written cloud, queries
+them on the scene grid and prints their 3D PSNR against the ground-truth volume (`initialize_pcd.py:135-156`).
+
+The default `--recon_method` is `random` (the reference defaults to `fdk`).
 """
 from __future__ import annotations
 
@@ -20,6 +24,55 @@ import numpy as np
 
 from .dataset import init_point_cloud, read_scene
 from .trainer import default_init_path
+
+# A filtered backprojection from a handful of views is dominated by streaks, and thresholding it gives no useful
+# initialisation (the reference's sparse-view setups use 25 to 75 views).
+MIN_FDK_VIEWS = 8
+
+
+def _require_cuda_for_fdk():
+    import torch
+
+    if not torch.cuda.is_available():
+        raise SystemExit("--recon_method fdk needs a CUDA device: the FDK reconstruction runs on the GPU and has no CPU "
+                         "fallback (use --recon_method random, or --recon_method volume --recon <vol.npy>)")
+
+
+def fdk_volume(info) -> np.ndarray:
+    """FDK reconstruction of the train views of a `read_scene` result, as a host float32 [nx, ny, nz] array."""
+    import torch
+
+    from .fdk import fdk
+
+    projs = torch.from_numpy(np.stack([np.asarray(c.image, np.float32) for c in info.train_cameras])).cuda()
+    vol = fdk(projs, [c.angle for c in info.train_cameras], info.scanner_cfg)
+    return vol.cpu().numpy()
+
+
+def evaluate_init(data: str, init_path: str) -> float:
+    """3D PSNR of the Gaussians created from `init_path` against the scene's ground-truth volume."""
+    import torch
+
+    from .dataset import Scene
+    from .gaussian_model import GaussianModel
+    from .metrics import metric_vol
+    from .render_query import query
+    from .trainer import ModelParams, PipelineParams
+
+    model, pipe = ModelParams(), PipelineParams()
+    with torch.no_grad():
+        scene = Scene(data, eval=False, shuffle=False, device="cuda")
+        cfg = scene.scanner_cfg
+        scale_bound = None
+        if model.scale_min and model.scale_max:
+            scale_bound = np.array([model.scale_min, model.scale_max]) * max(cfg["sVoxel"])
+        gaussians = GaussianModel(scale_bound)
+        pts = np.load(init_path)
+        gaussians.create_from_pcd(pts[:, :3], pts[:, 3:4], 1.0)
+        vol_pred = query(gaussians, cfg["offOrigin"], cfg["nVoxel"], cfg["sVoxel"], pipe)["vol"]
+        psnr_3d, _ = metric_vol(scene.vol_gt, vol_pred, "psnr")
+    print(f"3D PSNR for initial Gaussians: {psnr_3d}")
+    return float(psnr_3d)
 
 
 def main(argv=None) -> str:
@@ -32,10 +85,11 @@ def main(argv=None) -> str:
     ap.add_argument("--density_thresh", type=float, default=0.05)
     ap.add_argument("--density_rescale", type=float, default=0.15)
     ap.add_argument("--random_density_max", type=float, default=1.0)
+    ap.add_argument("--evaluate", default=False, action="store_true",
+                    help="Add this flag to evaluate quality (given GT volume, for debug only)")
     a = ap.parse_args(argv)
     if a.recon_method == "fdk":
-        raise SystemExit("--recon_method fdk needs TIGRE (absent here): reconstruct elsewhere and pass "
-                         "--recon_method volume --recon <vol.npy>")
+        _require_cuda_for_fdk()
     np.random.seed(0)                                    # initialize_pcd.py:23
     info = read_scene(os.path.abspath(a.data), eval=False)
     recon = None
@@ -43,14 +97,21 @@ def main(argv=None) -> str:
         if not a.recon:
             raise SystemExit("--recon_method volume needs --recon <vol.npy>")
         recon = np.load(a.recon)
+    if a.recon_method == "fdk" and len(info.train_cameras) < MIN_FDK_VIEWS:
+        raise SystemExit(f"--recon_method fdk needs at least {MIN_FDK_VIEWS} train views, the scene has "
+                         f"{len(info.train_cameras)}: use --recon_method random")
     out = a.output or default_init_path(os.path.abspath(a.data))
     if os.path.exists(out):
         raise SystemExit(f"Initialization file {out} exists! Delete it first.")
     os.makedirs(os.path.dirname(out) or ".", exist_ok=True)
+    if a.recon_method == "fdk":
+        recon = fdk_volume(info)                         # no draws from numpy's generator before np.random.choice
     pts = init_point_cloud(info.scanner_cfg, a.n_points, recon=recon, density_thresh=a.density_thresh,
                            density_rescale=a.density_rescale, random_density_max=a.random_density_max)
     np.save(out, pts)
     print(f"Initialization saved in {out}.")
+    if a.evaluate:
+        evaluate_init(os.path.abspath(a.data), out)
     return out
 
 

@@ -5,6 +5,8 @@
                    B_vox = 56 P + 44 V + 68 R + 4 N (SURVEY.md 8d)
   TV crop          32^3 sub-volume of the 100k cloud, forward + backward (train.py:128-144)
   train iteration  render + fused L1/D-SSIM + 32^3 TV crop query + backward + fused Adam on the headline scene
+  fdk              FDK reconstruction, 50 cone-beam views of 512^2 -> 256^3: filter, backprojection, whole call and
+                   voxel-view updates/s (no reference arm: the reference uses TIGRE, which is not part of this build)
 
 each for ours and, where the compiled reference (oracle/_ref/libr2ref.so) is present, for the reference's own CUDA
 kernels with the identical protocol (CUDA events per step, L2 flushed between steps).  `python scripts/secondary.py`
@@ -240,7 +242,53 @@ def measure(dev=None, peak_gbs: float = 3350.0, quick: bool = False, trace=lambd
                               "autograd_path_api": "GaussianModel / render() / query() / losses / FusedAdam behind autograd",
                               "repeated_iterations": native.repeats}
     trace("secondary: training iteration")
+
+    # ---- FDK reconstruction: 50 views of 512^2 -> 256^3, the reference's cone-beam dataset geometry ----
+    out["fdk"] = measure_fdk(dev, timed)
+    trace("secondary: fdk")
     return out
+
+
+def measure_fdk(dev, timed) -> dict:
+    """Filter, backprojection and the whole r2x_fdk call on 50 seeded 512^2 cone-beam views into a 256^3 grid."""
+    import torch
+
+    from r2_gaussian_b200 import _lib, scene
+
+    lib = _lib.load()
+    sc = scene.cone_beam_scanner(512, 256)
+    views = scene.make_views(sc, 50)
+    N, H, W, n = 50, 512, 512, 256
+    projs = torch.rand(N, H, W, device=dev, generator=torch.Generator(dev).manual_seed(0))
+    vm = torch.tensor(np.stack([v.viewmatrix.reshape(16) for v in views]), device=dev)
+    pm = torch.tensor(np.stack([v.projmatrix.reshape(16) for v in views]), device=dev)
+    q = torch.empty_like(projs)
+    vol = torch.empty(n, n, n, device=dev)
+    nbytes = int(lib.r2x_fdk_scratch_bytes(N, H, W))
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    stream = lambda: torch.cuda.current_stream(dev).cuda_stream
+    tx, ty, dso = float(views[0].tanfovx), float(views[0].tanfovy), float(sc["DSO"])
+    grid = (n, n, n, 2.0, 2.0, 2.0, 0.0, 0.0, 0.0)
+
+    def filt(_i):
+        _lib.check(lib.r2x_fdk_filter(stream(), N, H, W, projs.data_ptr(), tx, ty, 1, dso, q.data_ptr()), "r2x_fdk_filter")
+
+    def backproject(_i):
+        _lib.check(lib.r2x_fdk_backproject(stream(), N, H, W, q.data_ptr(), vm.data_ptr(), pm.data_ptr(), 1, dso, *grid,
+                                           vol.data_ptr()), "r2x_fdk_backproject")
+
+    def total(_i):
+        _lib.check(lib.r2x_fdk(stream(), N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), tx, ty, 1, dso, *grid,
+                               vol.data_ptr(), scratch.data_ptr(), nbytes), "r2x_fdk")
+
+    row = {"workload": "FDK, 50 cone-beam views of 512x512 (DSD 7, DSO 5) -> 256^3 volume, Ram-Lak filter + voxel-driven "
+                       "backprojection (r2x_fdk)",
+           "filter_ms": timed(filt), "backproject_ms": timed(backproject), "ours_ms": timed(total),
+           "sample_fetch": "__ldg through L1/L2",
+           "reference": "none: the reference reconstructs with TIGRE's algs.fdk, which is not part of this build"}
+    row["voxel_view_updates_per_s"] = float(n) ** 3 * N / (row["ours_ms"] * 1e-3)
+    row["backproject_voxel_view_updates_per_s"] = float(n) ** 3 * N / (row["backproject_ms"] * 1e-3)
+    return row
 
 
 if __name__ == "__main__":
