@@ -280,6 +280,26 @@ int r2x_fdk_backproject(void* stream, int n_views, int H, int W, const float* fi
                         const float* projmatrices, int mode, float dso, int nx, int ny, int nz, float sx, float sy,
                         float sz, float cx, float cy, float cz, float* out_volume);
 
+/* ---- forward projection of a voxel volume (synthetic projection data) --------------------------- */
+/* Replaces TIGRE's `Ax` (data_generator/synthetic_dataset/generate_data.py).  Lengths in the scene-scaled units of the
+ * dataset readers.  volume[nx,ny,nz] (index x*ny*nz + y*nz + z) with size (sx,sy,sz) centred at (cx,cy,cz);
+ * viewmatrices[N,16] are the rasterizer's per-view matrices, tan_fovx / tan_fovy the values render() passes (parallel
+ * beam: 1); out_projs[N,H,W] (rows = v, columns = u).  For every detector pixel (row i, column j):
+ *   ray    ndc = ((2j+1)/W - 1, (2i+1)/H - 1); cone beam: from the camera centre along camera-frame
+ *          (ndc_x tan_fovx, ndc_y tan_fovy, 1); parallel beam: from camera-frame (ndc_x, ndc_y, 0) along (0, 0, 1); both
+ *          taken to world space by the rigid inverse of the viewmatrix; unit direction d, so t is a length.
+ *   field  f = trilinear interpolation between the voxel centres c - s/2 + (i + 1/2) s/n, every lattice point outside
+ *          [0,n) having value 0: continuous, nonzero only inside the box c +- (s/2 + s/(2n)).
+ *   value  step * sum_k f(o + (t_c + k step) d) over the integers k whose sample lies inside that box (cone beam also
+ *          t > 0), with t_c = (c - o).d the ray's closest approach to the volume centre, summed in k order in float32.
+ *          A ray that misses the box gives exactly 0.  The callers pass step = accuracy * min(s/n).
+ * The sample positions do not depend on where the ray enters or leaves the box, so samples that rounding moves across
+ * its boundary sit where the field is ~0.  Deterministic (no atomics).  Asynchronous on `stream`.
+ * Limits: H <= 2097120 (grid.y), W and N up to INT_MAX (views are launched 65535 at a time), N*H*W indexed in 64 bits. */
+int r2x_volume_project(void* stream, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
+                       float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
+                       float tan_fovx, float tan_fovy, int mode, float step, float* out_projs);
+
 /* ---- multi-GPU exchange step: one-shot sum over NVLink peer memory ------------------------------ */
 /* The Gaussian-sharded projector (one process per GPU, every rank renders its index shard) needs ONE exchange per
  * projection: the sum of the per-rank partial detector images (BASELINE north_star; the reference itself is

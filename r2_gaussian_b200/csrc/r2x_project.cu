@@ -1,0 +1,169 @@
+// r2x_project.cu -- ray-driven forward projection of a voxel volume (line integrals of its trilinear field).
+//
+// The reference makes its synthetic datasets with TIGRE's `Ax` (data_generator/synthetic_dataset/generate_data.py).
+// This is the same operator, defined so that it agrees with render() by construction: the rays are the rasterizer's
+// (scene.make_view geometry, ndc of the pixel centres), the field is the trilinear interpolation of the volume between
+// voxel centres (0 at every lattice point outside the grid), and the integral is a Riemann sum at a fixed spacing
+// whose sample positions are anchored at the ray's closest approach to the volume centre:
+//
+//   volume_project_kernel  one thread per detector pixel, a CTA is 32 detector rows (v) x 8 columns (u) of one view.
+//                          On a circular scan v runs along world z, the volume's contiguous axis, so the 32 lanes of a
+//                          warp read neighbouring z and most of each sample's 8 corner loads fall in one or two 128-byte
+//                          lines.  Per-thread setup in float64 (rigid inverse of the viewmatrix, ray, closest approach
+//                          t_c, index-space position g_c and step, k range from a slab test); samples
+//                          g_k = fma(k, step, g_c) in float32, floor, 8 predicated __ldg loads, float32 sum in k order.
+//                          The 32 x 8 tile is staged in shared memory so the [N,H,W] rows are stored in whole sectors.
+//                          No atomics: the projections are bitwise reproducible.
+//
+// The float64 NumPy statement of the same definition is oracle/projector_oracle.py.
+#include <cmath>
+#include <cstdint>
+
+#include "../../include/r2x.h"
+#include "r2x_common.cuh"
+
+namespace r2x {
+
+constexpr int PRJ_BV = 32, PRJ_BU = 8;   // CTA: 32 detector rows (lanes) x 8 detector columns
+constexpr int PRJ_MAX_VIEWS = 65535;     // views per launch (grid.z); more are launched in chunks
+
+template <bool CONE>
+__global__ void __launch_bounds__(PRJ_BV * PRJ_BU) volume_project_kernel(
+    const float* __restrict__ vol, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy, float cz,
+    int H, int W, const float* __restrict__ viewm, float tanx, float tany, float step, float* __restrict__ out) {
+    __shared__ float tile[PRJ_BV][PRJ_BU + 1];
+    const int v = blockIdx.y * PRJ_BV + threadIdx.x;   // detector row
+    const int u = blockIdx.x * PRJ_BU + threadIdx.y;   // detector column
+    const int view = blockIdx.z;
+    float acc = 0.0f;
+    if (v < H && u < W) {
+        // world -> camera: rotation Rw[r][c] = m[4c + r], translation T[r] = m[12 + r] (column-major flat)
+        const float* m = viewm + (size_t)view * 16;
+        double Rw[3][3], T[3];
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) Rw[r][c] = (double)__ldg(m + 4 * c + r);
+            T[r] = (double)__ldg(m + 12 + r);
+        }
+        // camera-frame ray of the pixel centre: cone from the source, parallel from (ndc_x, ndc_y, 0), both along +z
+        const double ndx = (2.0 * u + 1.0) / W - 1.0, ndy = (2.0 * v + 1.0) / H - 1.0;
+        const double oc[3] = {CONE ? 0.0 : ndx, CONE ? 0.0 : ndy, 0.0};
+        const double dc[3] = {CONE ? ndx * (double)tanx : 0.0, CONE ? ndy * (double)tany : 0.0, 1.0};
+        // to world through the rigid inverse (Rw^T, -Rw^T T), relative to the volume centre
+        const double ctr[3] = {(double)cx, (double)cy, (double)cz};
+        double o[3], d[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            o[c] = Rw[0][c] * (oc[0] - T[0]) + Rw[1][c] * (oc[1] - T[1]) + Rw[2][c] * (oc[2] - T[2]) - ctr[c];
+            d[c] = Rw[0][c] * dc[0] + Rw[1][c] * dc[1] + Rw[2][c] * dc[2];
+        }
+        const double inv_len = 1.0 / sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+        d[0] *= inv_len; d[1] *= inv_len; d[2] *= inv_len;
+        const double tc = -(o[0] * d[0] + o[1] * d[1] + o[2] * d[2]);   // closest approach to the volume centre
+        // index space: lattice point i (voxel centre) at g = i; the field is nonzero only for g in (-1, n)
+        const int n[3] = {nx, ny, nz};
+        const double s[3] = {(double)sx, (double)sy, (double)sz};
+        double g[3], st[3];
+        double lo = -1e300, hi = 1e300;
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            const double dv = s[a] / n[a];
+            g[a] = (o[a] + tc * d[a]) / dv + 0.5 * (n[a] - 1);
+            st[a] = (double)step * d[a] / dv;
+            if (st[a] != 0.0) {
+                const double k1 = (-1.0 - g[a]) / st[a], k2 = ((double)n[a] - g[a]) / st[a];
+                lo = fmax(lo, fmin(k1, k2));
+                hi = fmin(hi, fmax(k1, k2));
+            } else if (!(g[a] > -1.0 && g[a] < (double)n[a])) {
+                lo = 1.0; hi = 0.0;                                        // parallel to this slab and outside it
+            }
+        }
+        long long k0 = (long long)ceil(fmax(lo, -1e18)), k1 = (long long)floor(fmin(hi, 1e18));
+        if (CONE) k0 = max(k0, (long long)floor(fmin(fmax(-tc / (double)step, -1e18), 1e18)) + 1);   // t > 0
+        const float gx = (float)g[0], gy = (float)g[1], gz = (float)g[2];
+        const float sxk = (float)st[0], syk = (float)st[1], szk = (float)st[2];
+        const long long sy_ = nz, sx_ = (long long)ny * nz;
+        for (long long k = k0; k <= k1; ++k) {
+            const float fk = (float)k;
+            const float px = fmaf(fk, sxk, gx), py = fmaf(fk, syk, gy), pz = fmaf(fk, szk, gz);
+            const float fx0 = floorf(px), fy0 = floorf(py), fz0 = floorf(pz);
+            const int ix = (int)fx0, iy = (int)fy0, iz = (int)fz0;
+            const float fx = px - fx0, fy = py - fy0, fz = pz - fz0;
+            const bool x0 = (unsigned)ix < (unsigned)nx, x1 = (unsigned)(ix + 1) < (unsigned)nx;
+            const bool y0 = (unsigned)iy < (unsigned)ny, y1 = (unsigned)(iy + 1) < (unsigned)ny;
+            const bool z0 = (unsigned)iz < (unsigned)nz, z1 = (unsigned)(iz + 1) < (unsigned)nz;
+            const float* p = vol + (long long)ix * sx_ + (long long)iy * sy_ + iz;
+            const float v000 = (x0 && y0 && z0) ? __ldg(p) : 0.0f;
+            const float v001 = (x0 && y0 && z1) ? __ldg(p + 1) : 0.0f;
+            const float v010 = (x0 && y1 && z0) ? __ldg(p + sy_) : 0.0f;
+            const float v011 = (x0 && y1 && z1) ? __ldg(p + sy_ + 1) : 0.0f;
+            const float v100 = (x1 && y0 && z0) ? __ldg(p + sx_) : 0.0f;
+            const float v101 = (x1 && y0 && z1) ? __ldg(p + sx_ + 1) : 0.0f;
+            const float v110 = (x1 && y1 && z0) ? __ldg(p + sx_ + sy_) : 0.0f;
+            const float v111 = (x1 && y1 && z1) ? __ldg(p + sx_ + sy_ + 1) : 0.0f;
+            const float c00 = fmaf(fz, v001 - v000, v000), c01 = fmaf(fz, v011 - v010, v010);
+            const float c10 = fmaf(fz, v101 - v100, v100), c11 = fmaf(fz, v111 - v110, v110);
+            const float c0 = fmaf(fy, c01 - c00, c00), c1 = fmaf(fy, c11 - c10, c10);
+            acc += fmaf(fx, c1 - c0, c0);
+        }
+        acc *= step;
+    }
+    tile[threadIdx.x][threadIdx.y] = acc;
+    __syncthreads();
+    const int t = threadIdx.y * PRJ_BV + threadIdx.x;
+    const int ro = blockIdx.y * PRJ_BV + t / PRJ_BU, co = blockIdx.x * PRJ_BU + t % PRJ_BU;
+    if (ro < H && co < W) out[((size_t)view * H + ro) * W + co] = tile[t / PRJ_BU][t % PRJ_BU];
+}
+
+static int project_validate(int nx, int ny, int nz, const float* volume, float sx, float sy, float sz, float cx,
+                            float cy, float cz, int N, int H, int W, const float* viewm, float tanx, float tany,
+                            int mode, float step, const float* out) {
+    if (nx < 1 || ny < 1 || nz < 1)
+        return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad grid (each size must be >= 1)");
+    if (N < 1 || H < 1 || W < 1) return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad N/H/W (each must be >= 1)");
+    if ((H + PRJ_BV - 1) / PRJ_BV > 65535)
+        return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad H (more than 2097120 detector rows)");
+    if (mode != 0 && mode != 1) return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad mode (0 = parallel, 1 = cone)");
+    if (!(sx > 0.0f && sy > 0.0f && sz > 0.0f && std::isfinite(sx) && std::isfinite(sy) && std::isfinite(sz)))
+        return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad sVoxel (must be finite and > 0)");
+    if (!(std::isfinite(cx) && std::isfinite(cy) && std::isfinite(cz)))
+        return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad offOrigin (must be finite)");
+    if (!(tanx > 0.0f && tany > 0.0f && std::isfinite(tanx) && std::isfinite(tany)))
+        return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad tan_fov (must be finite and > 0)");
+    if (!(step > 0.0f && std::isfinite(step)))
+        return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad step (must be finite and > 0)");
+    if (!volume || !viewm || !out) return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad pointer (NULL)");
+    return 0;
+}
+
+}  // namespace r2x
+
+extern "C" {
+
+int r2x_volume_project(void* stream, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
+                       float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
+                       float tan_fovx, float tan_fovy, int mode, float step, float* out_projs) {
+    using namespace r2x;
+    if (int rc = project_validate(nx, ny, nz, volume, sx, sy, sz, cx, cy, cz, n_views, H, W, viewmatrices, tan_fovx,
+                                  tan_fovy, mode, step, out_projs))
+        return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const dim3 block(PRJ_BV, PRJ_BU);
+    for (int v0 = 0; v0 < n_views; v0 += PRJ_MAX_VIEWS) {
+        const int nv = min(PRJ_MAX_VIEWS, n_views - v0);
+        const dim3 grid((W + PRJ_BU - 1) / PRJ_BU, (H + PRJ_BV - 1) / PRJ_BV, nv);
+        const float* vm = viewmatrices + (size_t)v0 * 16;
+        float* o = out_projs + (size_t)v0 * H * W;
+        if (mode == 1)
+            volume_project_kernel<true><<<grid, block, 0, st>>>(volume, nx, ny, nz, sx, sy, sz, cx, cy, cz, H, W, vm,
+                                                                tan_fovx, tan_fovy, step, o);
+        else
+            volume_project_kernel<false><<<grid, block, 0, st>>>(volume, nx, ny, nz, sx, sy, sz, cx, cy, cz, H, W, vm,
+                                                                 tan_fovx, tan_fovy, step, o);
+        R2X_CUDA_OK(cudaGetLastError());
+    }
+    return 0;
+}
+
+}  // extern "C"

@@ -9,8 +9,8 @@
   (`dataset/__init__.py:26-99`): `getTrainCameras()`, `getTestCameras()`, `vol_gt`, `scanner_cfg`, `bbox`, `save`;
 * `init_point_cloud` = `initialize_pcd.py:41-91` (random cloud, or voxels of a given reconstruction above a threshold
   -- the reconstruction itself is passed in: `fdk.fdk` on the GPU, TIGRE's FDK in the reference);
-* `write_blender` writes a dataset in that format (used by the tests and for synthetic scenes; generating projections
-  with TIGRE is not part of this project).
+* `write_blender` writes a dataset in that format (used by the tests and by `generate_data`, which makes synthetic
+  scenes from a CT volume with the GPU projector of `projector.py` where the reference uses TIGRE's `Ax`).
 
 Device is a parameter everywhere ("cuda" by default like the reference; the CPU tests pass "cpu").
 """
@@ -75,15 +75,21 @@ def _camera_info(uid, angle, image, name, path, cfg) -> CameraInfo:
                       int(cfg["nDetector"][1]), int(cfg["nDetector"][0]), MODE_ID[cfg["mode"]], cfg)
 
 
-def read_blender(path: str, eval: bool = True) -> SceneInfo:
-    with open(os.path.join(path, "meta_data.json")) as f:
-        meta = json.load(f)
-    cfg = meta["scanner"]
+def scale_scanner(cfg: dict) -> float:
+    """Complete `dVoxel` / `dDetector` of a scanner dict in the reference's file format and rescale it in place to
+    scene units (what `read_blender` does to `meta_data.json`'s scanner); returns scene_scale."""
     if "dVoxel" not in cfg:
         cfg["dVoxel"] = (np.asarray(cfg["sVoxel"], float) / np.asarray(cfg["nVoxel"], float)).tolist()
     if "dDetector" not in cfg:
         cfg["dDetector"] = (np.asarray(cfg["sDetector"], float) / np.asarray(cfg["nDetector"], float)).tolist()
-    scale = _rescale(cfg)
+    return _rescale(cfg)
+
+
+def read_blender(path: str, eval: bool = True) -> SceneInfo:
+    with open(os.path.join(path, "meta_data.json")) as f:
+        meta = json.load(f)
+    cfg = meta["scanner"]
+    scale = scale_scanner(cfg)
     cams = {"train": [], "test": []}
     for split in (("train", "test") if eval else ("train",)):
         offset = len(meta["proj_train"]) if split == "test" else 0

@@ -7,6 +7,9 @@
   train iteration  render + fused L1/D-SSIM + 32^3 TV crop query + backward + fused Adam on the headline scene
   fdk              FDK reconstruction, 50 cone-beam views of 512^2 -> 256^3: filter, backprojection, whole call and
                    voxel-view updates/s (no reference arm: the reference uses TIGRE, which is not part of this build)
+  project          forward projection of a 256^3 volume into 150 cone-beam views of 512^2 (the reference's synthetic
+                   dataset: 50 train + 100 test), samples/s and projections/s, with the card name and power limit
+                   (no reference arm: TIGRE's Ax is not part of this build)
 
 each for ours and, where the compiled reference (oracle/_ref/libr2ref.so) is present, for the reference's own CUDA
 kernels with the identical protocol (CUDA events per step, L2 flushed between steps).  `python scripts/secondary.py`
@@ -246,7 +249,105 @@ def measure(dev=None, peak_gbs: float = 3350.0, quick: bool = False, trace=lambd
     # ---- FDK reconstruction: 50 views of 512^2 -> 256^3, the reference's cone-beam dataset geometry ----
     out["fdk"] = measure_fdk(dev, timed)
     trace("secondary: fdk")
+
+    # ---- volume projection: the reference's synthetic dataset, 50 train + 100 test cone-beam views of 512^2 ----
+    out["project"] = measure_project(dev, timed)
+    trace("secondary: project")
     return out
+
+
+def card(dev) -> dict:
+    """Name and power limit of the device the row was measured on (nvidia-smi query; None if it is unavailable)."""
+    import subprocess
+
+    import torch
+
+    idx = torch.device(dev).index or 0
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(idx)],
+                           capture_output=True, text=True, timeout=20)
+        power = float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        power = None
+    return {"gpu": torch.cuda.get_device_name(idx), "power_limit_w": power}
+
+
+def projector_samples(sc: dict, angles, step: float) -> int:
+    """Samples r2x_volume_project evaluates: per ray, the integers k with t_c + k step inside the support box
+    offOrigin +- (sVoxel/2 + dVoxel/2) (cone beam: t > 0), from the same slab test in float64."""
+    from r2_gaussian_b200 import scene
+
+    n = np.asarray(sc["nVoxel"], np.float64)
+    dv = np.asarray(sc["sVoxel"], np.float64) / n
+    c = np.asarray(sc["offOrigin"], np.float64)
+    total = 0
+    for a in angles:
+        v = scene.make_view(sc, float(a))
+        H, W = v.image_height, v.image_width
+        ndx = (2.0 * np.arange(W) + 1.0) / W - 1.0
+        ndy = (2.0 * np.arange(H) + 1.0) / H - 1.0
+        c2w = np.linalg.inv(v.viewmatrix.astype(np.float64).T)
+        if v.mode == scene.MODE_CONE:
+            d = np.stack(np.broadcast_arrays(ndx[None, :] * v.tanfovx, ndy[:, None] * v.tanfovy, 1.0), -1)
+            o = np.broadcast_to(c2w[:3, 3], d.shape)
+        else:
+            d = np.broadcast_to(np.array([0.0, 0.0, 1.0]), (H, W, 3))
+            o = np.stack(np.broadcast_arrays(ndx[None, :], ndy[:, None], 0.0), -1) @ c2w[:3, :3].T + c2w[:3, 3]
+        d = d @ c2w[:3, :3].T
+        d = d / np.linalg.norm(d, axis=-1, keepdims=True)
+        tc = ((c - o) * d).sum(-1)
+        g = (o + tc[..., None] * d - c) / dv + 0.5 * (n - 1.0)
+        st = step * d / dv
+        lo = np.full(tc.shape, -np.inf)
+        hi = np.full(tc.shape, np.inf)
+        for ax in range(3):
+            nz = st[..., ax] != 0.0
+            s_ = np.where(nz, st[..., ax], 1.0)
+            k1, k2 = (-1.0 - g[..., ax]) / s_, (n[ax] - g[..., ax]) / s_
+            inside = (g[..., ax] > -1.0) & (g[..., ax] < n[ax])
+            lo = np.maximum(lo, np.where(nz, np.minimum(k1, k2), np.where(inside, -np.inf, np.inf)))
+            hi = np.minimum(hi, np.where(nz, np.maximum(k1, k2), np.where(inside, np.inf, -np.inf)))
+        k0 = np.ceil(lo)
+        if v.mode == scene.MODE_CONE:
+            k0 = np.maximum(k0, np.floor(-tc / step) + 1.0)
+        total += int(np.maximum(np.floor(hi) - k0 + 1.0, 0.0).sum())
+    return total
+
+
+def measure_project(dev, timed) -> dict:
+    """r2x_volume_project on the reference's synthetic setting: a seeded 256^3 volume, 50 train views at
+    linspace(0, 2 pi) and 100 sorted random test views, 512^2 cone beam, accuracy 0.5."""
+    import torch
+
+    from r2_gaussian_b200 import _lib, scene
+
+    lib = _lib.load()
+    sc = scene.cone_beam_scanner(512, 256)
+    rng = np.random.RandomState(0)
+    angles = np.concatenate([np.linspace(0.0, 2.0 * np.pi, 51)[:-1], np.sort(rng.rand(100) * 2.0 * np.pi)])
+    views = [scene.make_view(sc, float(a)) for a in angles]
+    N, H, W, n = len(views), 512, 512, 256
+    step = 0.5 * 2.0 / n
+    vol = torch.rand(n, n, n, device=dev, generator=torch.Generator(dev).manual_seed(0))
+    vm = torch.tensor(np.stack([v.viewmatrix.reshape(16) for v in views]), device=dev)
+    projs = torch.empty(N, H, W, device=dev)
+    tx, ty = float(views[0].tanfovx), float(views[0].tanfovy)
+
+    def run(_i):
+        _lib.check(lib.r2x_volume_project(torch.cuda.current_stream(dev).cuda_stream, n, n, n, vol.data_ptr(), 2.0, 2.0,
+                                          2.0, 0.0, 0.0, 0.0, N, H, W, vm.data_ptr(), tx, ty, 1, step,
+                                          projs.data_ptr()), "r2x_volume_project")
+
+    row = {"workload": "forward projection, seeded 256^3 volume -> 150 cone-beam views (50 train + 100 test) of "
+                       "512x512 (DSD 7, DSO 5), accuracy 0.5 (r2x_volume_project)",
+           "ours_ms": timed(run), "sample_fetch": "__ldg through L1/L2",
+           "reference": "none: TIGRE's Ax is not part of this build"}
+    samples = projector_samples(sc, angles, step)
+    row["samples"] = samples
+    row["samples_per_s"] = samples / (row["ours_ms"] * 1e-3)
+    row["projections_per_s"] = N / (row["ours_ms"] * 1e-3)
+    row.update(card(dev))
+    return row
 
 
 def measure_fdk(dev, timed) -> dict:
