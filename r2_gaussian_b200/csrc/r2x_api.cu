@@ -285,9 +285,11 @@ int raster_forward_impl(cudaStream_t st, int P, int W, int H, const float* means
                                      s.geom, direct ? &db : nullptr));
     R2X_TRY(debug_sync(st, debug, "raster preprocess"));
     if (direct) {
-        // tile ranges, work plan and R come straight from the per-CTA tile histograms
+        // tile ranges, work plan and R come straight from the per-CTA tile histograms (the plan's extra-item list,
+        // which lives in the binning buffer, is written by direct_fill)
         const long long cap0 = binning_alloc ? (1ll << 62) : capacity;
-        R2X_TRY(launch_direct_scan(st, db, s.status, cap0, binning_alloc ? nullptr : status_dev));
+        R2X_TRY(launch_direct_scan(st, db, ranges, carve_plan(image_buf, tiles, BinningView{}), s.status, cap0,
+                                   binning_alloc ? nullptr : status_dev));
     } else {
         R2X_TRY(launch_scan(st, P, s.geom.tiles_touched, s.geom.offsets, s.scan_state, s.status));
     }
@@ -309,8 +311,8 @@ int raster_forward_impl(cudaStream_t st, int P, int W, int H, const float* means
     BinningView bv = binning_view(binning_buf, capacity);
     const TilePlan plan = carve_plan(image_buf, tiles, bv);
     if (direct) {
-        R2X_TRY(launch_direct_fill(st, P, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, db, ranges, plan, bv,
-                                   s.geom.gx, s.geom.gy, s.status));
+        R2X_TRY(launch_direct_fill(st, P, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, db, plan, bv, s.geom.gx,
+                                   s.geom.gy, s.status));
     } else {
         status_kernel<<<1, 1, 0, st>>>(s.status, capacity, status_dev);
         R2X_TRY(bin_instances(st, P, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, s.geom.gx, s.geom.gy, tiles,
@@ -365,7 +367,8 @@ int voxel_forward_impl(cudaStream_t st, int P, int nx, int ny, int nz, float sx,
     R2X_TRY(debug_sync(st, debug, "voxel preprocess"));
     if (direct) {
         const long long cap0 = binning_alloc ? (1ll << 62) : capacity;
-        R2X_TRY(launch_direct_scan(st, db, s.status, cap0, binning_alloc ? nullptr : status_dev));
+        R2X_TRY(launch_direct_scan(st, db, ranges, carve_voxel_plan(image_buf, tiles, BinningView{}), s.status,
+                                   cap0, binning_alloc ? nullptr : status_dev));
     } else {
         R2X_TRY(launch_scan(st, P, s.geom.tiles_touched, s.geom.offsets, s.scan_state, s.status));
     }
@@ -386,8 +389,8 @@ int voxel_forward_impl(cudaStream_t st, int P, int nx, int ny, int nz, float sx,
     BinningView bv = binning_view(binning_buf, capacity);
     const TilePlan plan = carve_voxel_plan(image_buf, tiles, bv);
     if (direct) {
-        R2X_TRY(launch_direct_fill(st, P, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, db, ranges, plan, bv, vg.gx,
-                                   vg.gy, s.status));
+        R2X_TRY(launch_direct_fill(st, P, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, db, plan, bv, vg.gx, vg.gy,
+                                   s.status));
     } else if (two_level) {
         status_kernel<<<1, 1, 0, st>>>(s.status, capacity, status_dev);
         const TwoLevel tl = carve_two_level(image_buf, P, vg.gx, vg.gy, vg.gz, bv);

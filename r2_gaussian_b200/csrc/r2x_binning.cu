@@ -491,7 +491,8 @@ __global__ void __launch_bounds__(256) tile_ranges_kernel(const uint32_t* __rest
 size_t directbin_bytes(int P, int num_tiles) {
     const size_t nb = (size_t)((P > 0 ? P : 1) + DIRECT_BLOCK - 1) / DIRECT_BLOCK;
     const size_t t = (size_t)num_tiles;
-    return align_up(t * nb * sizeof(uint32_t), 256) + align_up(t * sizeof(uint32_t), 256) +
+    return align_up(t * nb * sizeof(uint32_t), 256) +
+           align_up((size_t)(1 + direct_scan_ctas(num_tiles)) * sizeof(unsigned long long), 256) +
            2 * align_up(nb * sizeof(uint32_t), 256) + 512;
 }
 
@@ -501,7 +502,8 @@ DirectBin directbin_view(void* buf, int P, int num_tiles) {
     const size_t t = (size_t)num_tiles;
     char* p = (char*)align_up((size_t)buf, 256);
     db.table = (uint32_t*)p; p += align_up(t * nb * sizeof(uint32_t), 256);
-    db.tile_count = (uint32_t*)p; p += align_up(t * sizeof(uint32_t), 256);
+    db.lookback = (unsigned long long*)p;
+    p += align_up((size_t)(1 + direct_scan_ctas(num_tiles)) * sizeof(unsigned long long), 256);
     db.block_total = (uint32_t*)p; p += align_up(nb * sizeof(uint32_t), 256);
     db.block_base = (uint32_t*)p; p += align_up(nb * sizeof(uint32_t), 256);
     db.num_tiles = num_tiles;
@@ -509,199 +511,235 @@ DirectBin directbin_view(void* buf, int P, int num_tiles) {
     return db;
 }
 
-// block-wide exclusive scan helper for the single finishing CTA (256 threads), arbitrary length, in order
-template <typename Load, typename Store>
-__device__ __forceinline__ uint32_t cta_exclusive_scan(int n, Load load, Store store, uint32_t* s_w, uint32_t* s_carry) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) *s_carry = 0;
-    __syncthreads();
-    for (int base = 0; base < n; base += 256) {
-        const int i = base + tid;
-        const uint32_t a = i < n ? load(i) : 0u;
-        uint32_t ia = a;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(0xffffffffu, ia, o);
-            if (lane >= o) ia += t;
-        }
-        if (lane == 31) s_w[warp] = ia;
-        __syncthreads();
-        uint32_t wpre = 0;
-#pragma unroll
-        for (int w = 0; w < 8; ++w)
-            if (w < warp) wpre += s_w[w];
-        const uint32_t ex = *s_carry + wpre + ia - a;
-        if (i < n) store(i, ex, a);
-        __syncthreads();
-        if (tid == 255) *s_carry = ex + a;
-        __syncthreads();
-    }
-    return *s_carry;
-}
+// direct_scan: CTA k (in ticket order) owns the DSCAN_COLS tile columns [8k, 8k + 8) of table[nb][T].  Thread
+// (seg, col) sums a run of consecutive rows of one column (a warp reads 4 rows x 32 bytes, whole sectors); the run
+// sums are scanned over the segments, which gives every tile's total and every row's prefix inside the column.  The
+// tile starts -- an exclusive scan of the tile totals in tile order -- and the extra-chunk offsets of the work plan
+// come from a decoupled look-back over the CTAs in ticket order (one 64-bit state per CTA: flag | extra chunks |
+// instances).  The column is then rewritten as absolute list positions, ranges[t].x + prefix[b][t], and the CTA
+// publishes ranges, extra_off and the zeroed arrival counters of its tiles.  Every CTA also reduces block_total,
+// so R, the overflow flag and the chunk size C are known before any tile start is; CTA 0 writes block_base,
+// status and the queue counters.  The kernel is a chain of dependent round trips (ticket, loads, look-back, stores);
+// small CTAs run it fastest (H100 at 700 W, headline scene: 5.5 / 6.2 / 8.1 us with 256 / 512 / 1024 threads).
+constexpr int DSCAN_THREADS = 256;
+constexpr int DSCAN_WARPS = DSCAN_THREADS / 32;
+constexpr int DSCAN_SEGS = DSCAN_THREADS / DSCAN_COLS;   // 32 row segments
+constexpr int DSCAN_KEEP = 16;                           // rows of a segment kept in registers between the passes
+static_assert(DSCAN_COLS == 8, "a warp is 4 row segments x 8 columns");
+constexpr unsigned long long LB_AGG = 1ull << 62, LB_INCL = 2ull << 62, LB_VALUE = (1ull << 62) - 1;
 
-// One-pass variant for n <= 16 * 256: thread t owns the K = ceil(n/256) consecutive elements [tK, tK+K), so the
-// whole scan costs one round of loads, one warp scan and two barriers (the strip-mined version above pays a
-// dependent global load + three barriers per 256 elements, which dominated direct_fill's prologue).
-template <typename V, typename Load, typename Store>
-__device__ __forceinline__ V cta_exclusive_scan_1pass(int n, Load load, Store store, V* s_w) {
+__global__ void __launch_bounds__(DSCAN_THREADS) direct_scan_kernel(DirectBin db, uint2* __restrict__ ranges, TilePlan pl,
+                                                                    uint32_t* __restrict__ status, long long capacity,
+                                                                    uint32_t* __restrict__ status_out) {
+    pdl_prologue();
+    __shared__ uint32_t s_w[DSCAN_WARPS];
+    __shared__ uint32_t s_wcol[DSCAN_WARPS][DSCAN_COLS];
+    __shared__ uint32_t s_tot[DSCAN_COLS];
+    __shared__ uint32_t s_bid;
+    __shared__ unsigned long long s_excl;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int K = (n + 255) >> 8;
-    V val[16], sum = 0;
-#pragma unroll
-    for (int k = 0; k < 16; ++k) {
+    const int T = db.num_tiles, nb = db.nb, nctas = gridDim.x;
+    if (tid == 0) s_bid = (uint32_t)atomicAdd(&db.lookback[0], 1ull);
+
+    // ---- R = sum of the CTA instance totals (every CTA); CTA 0 also writes their exclusive prefix, block_base
+    const int K = (nb + DSCAN_THREADS - 1) / DSCAN_THREADS;
+    uint32_t mine = 0;
+    for (int k = 0; k < K; ++k) {
         const int i = tid * K + k;
-        val[k] = (k < K && i < n) ? load(i) : V(0);
-        sum += val[k];
+        if (i < nb) mine += db.block_total[i];
     }
-    V ia = sum;
+    uint32_t incl = mine;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
-        const V t = __shfl_up_sync(0xffffffffu, ia, o);
-        if (lane >= o) ia += t;
+        const uint32_t x = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += x;
     }
-    __syncthreads();            // s_w may still be read by a previous scan
-    if (lane == 31) s_w[warp] = ia;
+    if (lane == 31) s_w[warp] = incl;
     __syncthreads();
-    V wpre = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) {
-        const V x = s_w[w];
-        if (w < warp) wpre += x;
-        total += x;
+    uint32_t R = 0, wpre = 0;
+#pragma unroll 8
+    for (int w = 0; w < DSCAN_WARPS; ++w) {
+        const uint32_t x = s_w[w];
+        wpre += (w < warp) ? x : 0u;
+        R += x;
     }
-    V ex = wpre + ia - sum;
-#pragma unroll
-    for (int k = 0; k < 16; ++k) {
-        const int i = tid * K + k;
-        if (k < K && i < n) store(i, ex, val[k], total);
-        ex += val[k];
-    }
-    return total;
-}
-
-// Column scan of table[nb][T]: CTA = 32 tiles x 32 row segments (1024 threads); every thread sums its rows of
-// one tile column (coalesced 128-byte row pieces), the segment sums are scanned through shared memory, then the
-// rows are re-read (L2) and replaced by the exclusive prefix over the CTAs.  CTA 0 also publishes
-// R = sum of the CTA instance totals and the overflow flag.
-constexpr int SCAN_SEGS = 32;
-__global__ void __launch_bounds__(1024) direct_scan_kernel(DirectBin db, uint32_t* __restrict__ status,
-                                                           long long capacity, uint32_t* __restrict__ status_out) {
-    pdl_prologue();
-    __shared__ uint32_t s_seg[SCAN_SEGS][33];
-    __shared__ uint32_t s_red[32];
-    const int lane = threadIdx.x & 31, seg = threadIdx.x >> 5;
-    const int T = db.num_tiles, nb = db.nb;
-    const int t = blockIdx.x * 32 + lane;
-    const int rps = (nb + SCAN_SEGS - 1) / SCAN_SEGS;
-    const int r0 = min(seg * rps, nb), r1 = min(r0 + rps, nb);
-    uint32_t sum = 0;
-    if (t < T) {
-        const uint32_t* col = db.table + t;
-        int r = r0;
-        for (; r + 4 <= r1; r += 4) {
-            const uint32_t a0 = col[(size_t)r * T], a1 = col[(size_t)(r + 1) * T], a2 = col[(size_t)(r + 2) * T],
-                           a3 = col[(size_t)(r + 3) * T];
-            sum += (a0 + a1) + (a2 + a3);
-        }
-        for (; r < r1; ++r) sum += col[(size_t)r * T];
-    }
-    s_seg[seg][lane] = sum;
-    __syncthreads();
-    uint32_t pre = 0;
-    for (int k = 0; k < seg; ++k) pre += s_seg[k][lane];
-    if (t < T) {
-        if (seg == SCAN_SEGS - 1) db.tile_count[t] = pre + sum;
-        uint32_t* col = db.table + t;
-        int r = r0;
-        for (; r + 4 <= r1; r += 4) {
-            const uint32_t a0 = col[(size_t)r * T], a1 = col[(size_t)(r + 1) * T], a2 = col[(size_t)(r + 2) * T],
-                           a3 = col[(size_t)(r + 3) * T];
-            col[(size_t)r * T] = pre;
-            col[(size_t)(r + 1) * T] = pre + a0;
-            col[(size_t)(r + 2) * T] = pre + a0 + a1;
-            col[(size_t)(r + 3) * T] = pre + a0 + a1 + a2;
-            pre += (a0 + a1) + (a2 + a3);
-        }
-        for (; r < r1; ++r) {
-            const uint32_t a = col[(size_t)r * T];
-            col[(size_t)r * T] = pre;
-            pre += a;
-        }
-    }
+    const bool ov = (long long)R > capacity;
+    const uint32_t C = plan_chunk_for(R, pl.chunk_override, pl.chunk_cap);
     if (blockIdx.x == 0) {
-        // instance base of every preprocess CTA (exclusive prefix of the CTA totals), R and the overflow flag
-        __shared__ uint32_t s_carry;
-        if (threadIdx.x == 0) s_carry = 0;
-        __syncthreads();
-        for (int base = 0; base < nb; base += 1024) {
-            const int i = base + threadIdx.x;
-            const uint32_t a = i < nb ? db.block_total[i] : 0u;
-            uint32_t ia = a;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t x = __shfl_up_sync(0xffffffffu, ia, o);
-                if (lane >= o) ia += x;
+        uint32_t run = wpre + incl - mine;
+        for (int k = 0; k < K; ++k) {
+            const int i = tid * K + k;
+            if (i < nb) {
+                const uint32_t v = db.block_total[i];
+                db.block_base[i] = run;
+                run += v;
             }
-            if (lane == 31) s_red[seg] = ia;
-            __syncthreads();
-            uint32_t wpre = 0;
-            for (int w = 0; w < seg; ++w) wpre += s_red[w];
-            const uint32_t ex = s_carry + wpre + ia - a;
-            if (i < nb) db.block_base[i] = ex;
-            __syncthreads();
-            if (threadIdx.x == 1023) s_carry = ex + a;
-            __syncthreads();
         }
-        if (threadIdx.x == 0) {
-            const uint32_t R = s_carry;
-            const uint32_t ov = ((long long)R > capacity) ? 1u : 0u;
+        if (tid == 0) {
             status[0] = R;
-            status[1] = ov;
-            if (status_out) { status_out[0] = R; status_out[1] = ov; }
+            status[1] = ov ? 1u : 0u;
+            if (status_out) { status_out[0] = R; status_out[1] = ov ? 1u : 0u; }
+            pl.counter[0] = pl.counter[1] = pl.counter[3] = 0;
+            pl.counter[2] = C;
         }
     }
+
+    // ---- column sums
+    const int bid = (int)s_bid;
+    const int col = tid & (DSCAN_COLS - 1), seg = tid / DSCAN_COLS;
+    const int t = bid * DSCAN_COLS + col;
+    const int rps = (nb + DSCAN_SEGS - 1) / DSCAN_SEGS;
+    const int r0 = min(seg * rps, nb), r1 = min(r0 + rps, nb);
+    uint32_t* cp = db.table + t;
+    const bool live = t < T;
+    uint32_t keep[DSCAN_KEEP];
+    uint32_t sum = 0;
+#pragma unroll
+    for (int k = 0; k < DSCAN_KEEP; ++k) {
+        keep[k] = (live && r0 + k < r1) ? cp[(size_t)(r0 + k) * T] : 0u;
+        sum += keep[k];
+    }
+    if (live)
+        for (int r = r0 + DSCAN_KEEP; r < r1; ++r) sum += cp[(size_t)r * T];
+    // prefix over the segments: 4 segments per warp (lanes 8 apart), then over the warps
+    uint32_t sincl = sum;
+#pragma unroll
+    for (int o = DSCAN_COLS; o < 32; o <<= 1) {
+        const uint32_t x = __shfl_up_sync(0xffffffffu, sincl, o);
+        if (lane >= o) sincl += x;
+    }
+    if (lane >= 32 - DSCAN_COLS) s_wcol[warp][col] = sincl;
+    __syncthreads();
+    uint32_t pre = sincl - sum, tot = 0;
+#pragma unroll 8
+    for (int w = 0; w < DSCAN_WARPS; ++w) {
+        const uint32_t x = s_wcol[w][col];
+        pre += (w < warp) ? x : 0u;
+        tot += x;
+    }
+    if (tid < DSCAN_COLS) s_tot[tid] = tot;   // warp 0: tot of column tid
+    __syncthreads();
+    // the CTA's tiles in order: instances and extra chunks before column `col`, and in all 8 columns
+    uint32_t cnt_before = 0, ext_before = 0, cnt_all = 0, ext_all = 0;
+#pragma unroll
+    for (int c = 0; c < DSCAN_COLS; ++c) {
+        const uint32_t n = s_tot[c];
+        const uint32_t e = n ? (n - 1) / C : 0u;
+        cnt_before += (c < col) ? n : 0u;
+        ext_before += (c < col) ? e : 0u;
+        cnt_all += n;
+        ext_all += e;
+    }
+
+    // ---- decoupled look-back over the CTAs in ticket order, one warp, 32 predecessors per probe
+    if (warp == 0) {
+        volatile unsigned long long* st = db.lookback + 1;
+        const unsigned long long agg = ((unsigned long long)ext_all << 32) | cnt_all;
+        unsigned long long excl = 0;
+        if (bid == 0) {
+            if (lane == 0) st[0] = LB_INCL | agg;
+        } else {
+            if (lane == 0) st[bid] = LB_AGG | agg;
+            int top = bid - 1;
+            while (true) {
+                const int q = top - lane;
+                const unsigned long long s = q >= 0 ? (unsigned long long)st[q] : LB_INCL;
+                const uint32_t incl_lanes = __ballot_sync(0xffffffffu, (s >> 62) == 2ull);
+                const uint32_t wait_lanes = __ballot_sync(0xffffffffu, (s >> 62) == 0ull);
+                const int stop = incl_lanes ? __ffs(incl_lanes) - 1 : 31;   // nearest inclusive state
+                const uint32_t upto = stop == 31 ? 0xffffffffu : ((2u << stop) - 1u);
+                if (wait_lanes & upto) continue;                          // a predecessor has not published yet
+                unsigned long long v = (lane <= stop) ? (s & LB_VALUE) : 0ull;
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+                excl += v;
+                if (incl_lanes) break;
+                top -= 32;
+            }
+            if (lane == 0) st[bid] = LB_INCL | (excl + agg);
+        }
+        if (lane == 0) s_excl = excl;
+    }
+    __syncthreads();
+    const uint32_t start = (uint32_t)s_excl + cnt_before;              // first list position of tile t
+    const uint32_t eoff = (uint32_t)(s_excl >> 32) + ext_before;       // its first extra work item
+    if (live) {
+        uint32_t pos = start + pre;
+#pragma unroll
+        for (int k = 0; k < DSCAN_KEEP; ++k)
+            if (r0 + k < r1) {
+                cp[(size_t)(r0 + k) * T] = pos;
+                pos += keep[k];
+            }
+        for (int r = r0 + DSCAN_KEEP; r < r1; ++r) {
+            const uint32_t a = cp[(size_t)r * T];
+            cp[(size_t)r * T] = pos;
+            pos += a;
+        }
+        // Overflow (asynchronous variant only): the binning buffer cannot hold the lists, so EMPTY ranges are
+        // published -- the render then produces zeros without touching unwritten list entries -- and the host sees
+        // status[1] = 1 and re-runs with a larger buffer.
+        if (seg == 0) {
+            ranges[t] = ov ? make_uint2(0u, 0u) : make_uint2(start, start + tot);
+            pl.extra_off[t] = ov ? 0u : eoff;
+        }
+    }
+    if (tid < DSCAN_COLS * PLAN_DONE_SLOTS) {
+        const size_t i = (size_t)bid * DSCAN_COLS * PLAN_DONE_SLOTS + tid;
+        if (i < (size_t)T * PLAN_DONE_SLOTS) pl.tile_done[i] = 0;
+    }
+    if (bid == nctas - 1 && tid == 0) pl.extra_off[T] = ov ? 0u : (uint32_t)(s_excl >> 32) + ext_all;
 }
 
-int launch_direct_scan(cudaStream_t st, const DirectBin& db, uint32_t* status, long long capacity,
-                       uint32_t* status_out) {
-    R2X_CUDA_OK(pdl_launch(direct_scan_kernel, dim3((db.num_tiles + 31) / 32), dim3(1024), 0, st, db, status, capacity,
-                           status_out));
+int launch_direct_scan(cudaStream_t st, const DirectBin& db, uint2* ranges, const TilePlan& plan, uint32_t* status,
+                       long long capacity, uint32_t* status_out) {
+    R2X_CUDA_OK(pdl_launch(direct_scan_kernel, dim3(direct_scan_ctas(db.num_tiles)), dim3(DSCAN_THREADS), 0, st, db,
+                           ranges, plan, status, capacity, status_out));
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }
 
 // CTA b places the instances of Gaussians [256 b, 256 b + 256).  It marks, per tile, WHICH of its Gaussians touch
 // the tile (a 256-bit mask per tile, word w = warp w's 32 Gaussians, one ATOMS.OR per instance), turns the word
-// populations into per-word ranks, and then every thread walks the tiles of ITS OWN Gaussian again (lane per
-// instance, the same loop as the marking) and writes the Gaussian id to
-//     range[t].x + prefix[b][t] + rank of the Gaussian among the CTA's Gaussians on tile t
-//                                 = wrank[w][t] + popc(mask[w][t] & lanes below)
+// populations into per-word ranks, and then every thread walks the tiles of ITS OWN Gaussian again (lane per instance,
+// the same loop as the marking); the instance goes to
+//     table[b][t] (direct_scan: where CTA b's run of tile t starts in point_list)
+//       + rank of the Gaussian among the CTA's Gaussians on tile t = wrank[w][t] + popc(mask[w][t] & lanes below)
 // => every tile list is ascending in Gaussian id (the stable order) without any search, sort or warp match, and the
-// instance's emission-order slot (backward moments) follows from offsets[] (emission_slot(), r2x_binning.cuh).  Every CTA derives the tile ranges and its
-// instance base itself (exclusive scans of tile_count / block_total: small and L2-hot), so nothing serial sits between
-// the column scan and this kernel; the publication of the ranges and of the work plan for the render is spread over
-// the CTAs.  Dynamic shared memory: mask[8][T] u32 | base[T] u32 | wrank[8][T] u8.
+// instance's emission-order slot (backward moments) follows from offsets[] (emission_slot(), r2x_binning.cuh).
+// Written one by one, the ids would be one scattered 4-byte store each, and those stores are what the kernel's time
+// goes to.  So when the CTA's instances fit `stage_cap`, they are first put in shared memory in (tile, rank) order --
+// the order of their positions inside each run -- and then stored with consecutive threads on consecutive entries, so
+// a warp's store covers whole runs.  The CTA also writes the extra-item list of the work plan for its slice of the
+// tiles (the list lives in the binning buffer; see launch_direct_scan).
+// Dynamic shared memory: mask[8][T] u32 | base[T] u32 | wrank[8][T] u8 | (staged:) loc[T] u32 | pos[cap] u32 | id[cap] u8
+// (the Gaussian's index inside the CTA).
+constexpr int FILL_STAGE_TILES = 4 * DIRECT_BLOCK;   // staging when T <= 1024 ...
+constexpr int FILL_STAGE_CAP = 4608;                 // ... for up to 4608 instances per CTA: 70.5 KB, 3 CTAs per SM
+
 __global__ void __launch_bounds__(DIRECT_BLOCK) direct_fill_kernel(int P, const uint16_t* __restrict__ cube,
                                                                    const uint32_t* __restrict__ tiles_touched,
                                                                    uint32_t* __restrict__ offsets, DirectBin db,
-                                                                   uint2* __restrict__ ranges, TilePlan pl,
-                                                                   uint32_t* __restrict__ point_list,
-                                                                   uint32_t* __restrict__ inst_pos, long long capacity,
-                                                                   int gx, int gy, const uint32_t* __restrict__ status) {
-    pdl_prologue();
+                                                                   TilePlan pl, uint32_t* __restrict__ point_list,
+                                                                   int gx, int gy, const uint32_t* __restrict__ status,
+                                                                   int stage_cap) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    __shared__ unsigned long long s_w[8];
+    __shared__ uint32_t s_w8[8];
+    __shared__ uint32_t s_ct[4][8];
     const int T = db.num_tiles;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t* tc = db.tile_count;
     uint32_t* s_mask = reinterpret_cast<uint32_t*>(smem_raw);                    // [8][T]
     uint32_t* s_base = s_mask + 8 * (size_t)T;                                    // [T]
     unsigned char* s_wrank = reinterpret_cast<unsigned char*>(s_base + T);        // [8][T]
-    __shared__ uint32_t s_w8[8];
+    uint32_t* s_loc = reinterpret_cast<uint32_t*>(s_wrank + 8 * (size_t)T);      // [T]
+    uint32_t* s_pos = s_loc + T;                                                  // [stage_cap]
+    unsigned char* s_id = reinterpret_cast<unsigned char*>(s_pos + stage_cap);   // [stage_cap]
+    // shared memory only: done while direct_scan may still be running
+    for (int i = tid; i < 2 * T; i += DIRECT_BLOCK) reinterpret_cast<uint4*>(s_mask)[i] = make_uint4(0u, 0u, 0u, 0u);
+    pdl_prologue();
 
     const int b = blockIdx.x;
     const int g = b * DIRECT_BLOCK + tid;
-    for (int i = tid; i < 2 * T; i += DIRECT_BLOCK) reinterpret_cast<uint4*>(s_mask)[i] = make_uint4(0u, 0u, 0u, 0u);
     uint32_t n = 0, c01 = 0, c23 = 0, c45 = 0;
     if (g < P) {
         n = tiles_touched[g];
@@ -709,6 +747,9 @@ __global__ void __launch_bounds__(DIRECT_BLOCK) direct_fill_kernel(int P, const 
         c01 = c[0]; c23 = c[1]; c45 = c[2];
     }
     const uint32_t bbase = db.block_base[b];   // instance base of this CTA (direct_scan)
+    const bool ov = status[1] != 0u;           // overflow (direct_scan): nothing may be written to point_list
+    const uint32_t* row = db.table + (size_t)b * T;   // rewritten by direct_scan even on overflow
+    for (int t = tid; t < T; t += DIRECT_BLOCK) s_base[t] = row[t];
     // CTA-exclusive scan of n
     uint32_t ia = n;
 #pragma unroll
@@ -717,52 +758,26 @@ __global__ void __launch_bounds__(DIRECT_BLOCK) direct_fill_kernel(int P, const 
         if (lane >= o) ia += x;
     }
     if (lane == 31) s_w8[warp] = ia;
-    // where this CTA's run starts inside every tile list
-    const uint32_t* row = db.table + (size_t)b * T;
-    // One pass over the tile counts gives, per tile, the start of its list (low word) and of its extra work items
-    // (high word: chunks beyond the first).  Besides its own bases every CTA publishes a slice of the tile ranges
-    // and of the work plan for the render -- thread tid of CTA b owns the K tiles [tid K, tid K + K) iff
-    // tid == b (mod npub) -- so no serial tail is left.
-    // Overflow (asynchronous variant only): the binning buffer cannot hold the lists, so EMPTY ranges are
-    // published -- the render then produces zeros without touching unwritten list entries -- and the host sees
-    // status[1] = 1 (direct_scan) and re-runs with a larger buffer.
-    const uint32_t C = plan_chunk_for(status[0], pl.chunk_override, pl.chunk_cap);   // status[0] = R (direct_scan)
-    const int npub = db.nb < DIRECT_BLOCK ? db.nb : DIRECT_BLOCK;
-    const bool pub = (b < npub) && (tid % npub == b);
-    const unsigned long long tot = cta_exclusive_scan_1pass<unsigned long long>(
-        T,
-        [&](int i) {
-            const uint32_t c = tc[i];
-            return ((unsigned long long)(c ? (c - 1) / C : 0u) << 32) | c;
-        },
-        [&](int i, unsigned long long ex64, unsigned long long v64, unsigned long long total) {
-            const uint32_t ex = (uint32_t)ex64, cnt = (uint32_t)v64;
-            s_base[i] = ex + row[i];
-            if (pub) {
-                const bool ov = (long long)(uint32_t)total > capacity;
-                const uint32_t eo = ov ? 0u : (uint32_t)(ex64 >> 32), ne = ov ? 0u : (uint32_t)(v64 >> 32);
-                ranges[i] = ov ? make_uint2(0u, 0u) : make_uint2(ex, ex + cnt);
-                pl.extra_off[i] = eo;
+    __syncthreads();
+    uint32_t wpre = 0, total = 0;
 #pragma unroll
-                for (int k = 0; k < PLAN_DONE_SLOTS; ++k) pl.tile_done[(size_t)i * PLAN_DONE_SLOTS + k] = 0;
-                for (uint32_t c = 0; c < ne; ++c)
-                    if ((long long)(eo + c) < pl.max_extra) pl.extra_item[eo + c] = make_uint2((uint32_t)i, c + 1);
-            }
-        },
-        s_w);
-    const uint32_t R = (uint32_t)tot;
-    if (b == 0 && tid == 0) {
-        pl.extra_off[T] = ((long long)R > capacity) ? 0u : (uint32_t)(tot >> 32);
-        pl.counter[0] = pl.counter[1] = pl.counter[3] = 0;
-        pl.counter[2] = C;
+    for (int w = 0; w < 8; ++w) {
+        const uint32_t x = s_w8[w];
+        wpre += (w < warp) ? x : 0u;
+        total += x;
     }
-    uint32_t wpre = 0;
-#pragma unroll
-    for (int w = 0; w < 8; ++w)
-        if (w < warp) wpre += s_w8[w];
-    const uint32_t lex = wpre + ia - n;
-    if (g < P) offsets[g] = bbase + lex + n;     // inclusive scan, same meaning as the reference's point_offsets
-    if ((long long)R > capacity) return;         // overflow: nothing may be written (uniform across the grid)
+    if (g < P) offsets[g] = bbase + wpre + ia;    // inclusive scan, same meaning as the reference's point_offsets
+    if (ov) return;                                // uniform across the grid
+    // extra work items of the tiles [b K, b K + K): (tile, chunk >= 1)
+    {
+        const int K = (T + (int)gridDim.x - 1) / (int)gridDim.x;
+        const int t1 = min(T, (b + 1) * K);
+        for (int t = b * K + tid; t < t1; t += DIRECT_BLOCK) {
+            const uint32_t eo = pl.extra_off[t], ne = pl.extra_off[t + 1] - eo;
+            for (uint32_t c = 0; c < ne; ++c)
+                if ((long long)(eo + c) < pl.max_extra) pl.extra_item[eo + c] = make_uint2((uint32_t)t, c + 1);
+        }
+    }
     const uint32_t x0 = c01 & 0xffff, y0 = c01 >> 16, z0 = c23 & 0xffff, x1 = c23 >> 16, y1 = c45 & 0xffff, z1 = c45 >> 16;
     // mark
     {
@@ -776,14 +791,50 @@ __global__ void __launch_bounds__(DIRECT_BLOCK) direct_fill_kernel(int P, const 
                 }
     }
     __syncthreads();
-    // rank of word w inside its tile's run = population of the words below it
-    for (int t = tid; t < T; t += DIRECT_BLOCK) {
+    // rank of word w inside its tile's run = population of the words below it; returns the CTA's count on tile t
+    auto word_ranks = [&](int t) -> uint32_t {
         uint32_t run = 0;
 #pragma unroll
         for (int w = 0; w < 8; ++w) {
             s_wrank[(size_t)w * T + t] = (unsigned char)run;    // <= 224
             run += __popc(s_mask[(size_t)w * T + t]);
         }
+        return run;
+    };
+    const bool staged = stage_cap > 0 && total <= (uint32_t)stage_cap;   // uniform; stage_cap > 0 only when T <= 1024
+    if (staged) {
+        // loc[t] = where tile t's run starts in the staging buffer: exclusive scan of the counts in tile order
+        // (tile t = k * 256 + tid: K <= 4 interleaved scans at once)
+        uint32_t cnt[4], inc[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const int t = k * DIRECT_BLOCK + tid;
+            cnt[k] = t < T ? word_ranks(t) : 0u;
+            inc[k] = cnt[k];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const uint32_t x = __shfl_up_sync(0xffffffffu, inc[k], o);
+                if (lane >= o) inc[k] += x;
+            }
+            if (lane == 31) s_ct[k][warp] = inc[k];
+        }
+        __syncthreads();
+        uint32_t carry = 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            uint32_t before = 0, all = 0;
+#pragma unroll
+            for (int w = 0; w < 8; ++w) {
+                const uint32_t x = s_ct[k][w];
+                before += (w < warp) ? x : 0u;
+                all += x;
+            }
+            const int t = k * DIRECT_BLOCK + tid;
+            if (t < T) s_loc[t] = carry + before + inc[k] - cnt[k];
+            carry += all;
+        }
+    } else {
+        for (int t = tid; t < T; t += DIRECT_BLOCK) word_ranks(t);
     }
     __syncthreads();
     // place: lane per instance, tiles of this thread's Gaussian in emission order (z, y, x ascending)
@@ -796,22 +847,37 @@ __global__ void __launch_bounds__(DIRECT_BLOCK) direct_fill_kernel(int P, const 
                 const uint32_t rowb = (z * (uint32_t)gy + y) * (uint32_t)gx;
                 for (uint32_t x = x0; x < x1; ++x) {
                     const uint32_t t = rowb + x;
-                    const uint32_t pos = s_base[t] + wr[t] + __popc(plane[t] & below);
-                    point_list[pos] = (uint32_t)g;
+                    const uint32_t r = wr[t] + __popc(plane[t] & below);
+                    if (staged) {
+                        const uint32_t slot = s_loc[t] + r;
+                        s_pos[slot] = s_base[t] + r;
+                        s_id[slot] = (unsigned char)tid;
+                    } else {
+                        point_list[s_base[t] + r] = (uint32_t)g;
+                    }
                 }
             }
+    }
+    if (staged) {
+        __syncthreads();
+        const uint32_t g0 = (uint32_t)b * DIRECT_BLOCK;
+        for (uint32_t i = tid; i < total; i += DIRECT_BLOCK) point_list[s_pos[i]] = g0 + s_id[i];
     }
 }
 
 int launch_direct_fill(cudaStream_t st, int P, const uint16_t* cube, const uint32_t* tiles_touched, uint32_t* offsets,
-                       const DirectBin& db, uint2* ranges, const TilePlan& plan, const BinningView& bv, int gx,
-                       int gy, const uint32_t* status) {
-    const size_t smem = (size_t)db.num_tiles * 44;
-    if (smem > 40 * 1024)
+                       const DirectBin& db, const TilePlan& plan, const BinningView& bv, int gx, int gy,
+                       const uint32_t* status) {
+    static_assert(FILL_STAGE_TILES <= 4 * DIRECT_BLOCK, "the staging scan handles at most 4 tiles per thread");
+    static_assert(FILL_STAGE_TILES * 48 + FILL_STAGE_CAP * 5 <= DIRECT_MAX_TILES * 44, "one attribute covers both layouts");
+    const int T = db.num_tiles;
+    const int cap = T <= FILL_STAGE_TILES ? FILL_STAGE_CAP : 0;
+    const size_t smem = (size_t)T * (cap ? 48 : 44) + (size_t)cap * 5;
+    if (smem > 48 * 1024)
         R2X_CUDA_OK(cudaFuncSetAttribute(direct_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          DIRECT_MAX_TILES * 44));
     R2X_CUDA_OK(pdl_launch(direct_fill_kernel, dim3(db.nb), dim3(DIRECT_BLOCK), smem, st, P, cube, tiles_touched, offsets,
-                           db, ranges, plan, bv.point_list, bv.inst_pos, bv.capacity, gx, gy, status));
+                           db, plan, bv.point_list, gx, gy, status, cap));
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }

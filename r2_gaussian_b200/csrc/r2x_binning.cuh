@@ -120,19 +120,22 @@ BinningView binning_view(void* buf, long long R);
 // ---- direct binning (tile counts up to DIRECT_MAX_TILES) ----------------------------------------
 // No instance list is materialised and nothing is sorted.  The preprocess CTA b (256 consecutive
 // Gaussians) histograms its own instances per tile (`block_tile_histogram`, shared memory) into row b of
-// `table`; `direct_scan` turns every tile's column into exclusive prefixes over the CTAs (= where CTA b's
-// instances of tile t start inside the tile's list) and publishes R; `direct_fill` derives the tile ranges
-// and the work plan and writes each CTA's Gaussian ids straight to their final, stable positions (ascending
-// Gaussian id inside a tile).  4 kernels per forward in total.
+// `table`; `direct_scan` does everything that needs grid-wide totals: it turns every tile's column into
+// absolute list positions (where CTA b's instances of tile t start in point_list), and publishes the tile
+// ranges, the work plan, the CTA instance bases and R; `direct_fill` writes each CTA's Gaussian ids straight
+// to their final, stable positions (ascending Gaussian id inside a tile).  4 kernels per forward in total.
 constexpr int DIRECT_MAX_TILES = 4096;
 constexpr int DIRECT_BLOCK = 256;       // Gaussians per preprocess CTA (== its thread count)
+constexpr int DSCAN_COLS = 8;           // tile columns per direct_scan CTA
 struct DirectBin {
-    uint32_t* table;        // [nb][T]  row b = CTA b's per-tile counts -> exclusive prefix down each column
-    uint32_t* tile_count;   // [T]
+    uint32_t* table;        // [nb][T]  row b = CTA b's per-tile counts -> absolute list position (direct_scan)
+    unsigned long long* lookback;  // [1 + ceil(T / DSCAN_COLS)]  direct_scan's ticket + per-CTA prefix states,
+                                   // zeroed by block_tile_histogram
     uint32_t* block_total;  // [nb]  instances of CTA b
     uint32_t* block_base;   // [nb]  exclusive prefix of block_total (direct_scan)
     int num_tiles, nb;
 };
+__host__ __device__ __forceinline__ int direct_scan_ctas(int num_tiles) { return (num_tiles + DSCAN_COLS - 1) / DSCAN_COLS; }
 size_t directbin_bytes(int P, int num_tiles);
 DirectBin directbin_view(void* buf, int P, int num_tiles);
 inline bool direct_ok(int num_tiles) { return num_tiles <= DIRECT_MAX_TILES; }
@@ -143,6 +146,8 @@ __device__ __forceinline__ void block_tile_histogram(uint32_t* hist_s, const Dir
                                                      uint32_t c45, uint32_t n, int gx, int gy) {
     const int tid = threadIdx.x;
     for (int t = tid; t < db.num_tiles; t += DIRECT_BLOCK) hist_s[t] = 0;
+    if (blockIdx.x == 0)   // direct_scan's look-back state (it waits for this grid to finish before reading it)
+        for (int i = tid; i <= direct_scan_ctas(db.num_tiles); i += DIRECT_BLOCK) db.lookback[i] = 0ull;
     __syncthreads();
     if (n) {
         const uint32_t x0 = c01 & 0xffff, y0 = c01 >> 16, z0 = c23 & 0xffff, x1 = c23 >> 16, y1 = c45 & 0xffff,
@@ -193,11 +198,14 @@ int launch_two_level(cudaStream_t st, int P, const uint16_t* cube, const uint32_
                      const uint32_t* status, const TwoLevel& tl, const BinningView& bv, uint2* ranges,
                      const TilePlan& plan);
 
-int launch_direct_scan(cudaStream_t st, const DirectBin& db, uint32_t* status, long long capacity,
-                       uint32_t* status_out);
+// direct_scan writes ranges[T] and the image-buffer part of the work plan (extra_off, tile_done, counter); the
+// extra-item list lives in the binning buffer, which the synchronous variant only allocates once R is known, so
+// direct_fill writes it.
+int launch_direct_scan(cudaStream_t st, const DirectBin& db, uint2* ranges, const TilePlan& plan, uint32_t* status,
+                       long long capacity, uint32_t* status_out);
 int launch_direct_fill(cudaStream_t st, int P, const uint16_t* cube, const uint32_t* tiles_touched, uint32_t* offsets,
-                       const DirectBin& db, uint2* ranges, const TilePlan& plan, const BinningView& bv, int gx,
-                       int gy, const uint32_t* status);
+                       const DirectBin& db, const TilePlan& plan, const BinningView& bv, int gx, int gy,
+                       const uint32_t* status);
 
 // Exclusive->inclusive scan of tiles_touched[P] into offsets[P]; total (R) is written to *d_total
 // (device) -- single pass, decoupled look-back.  scan_state needs scan_state_bytes(P) bytes, zeroed

@@ -8,7 +8,7 @@
 // level-1 work plan -- over the supertile's 64 tiles:
 //
 //   super_cube      per Gaussian: supertile cube + count, per-block supertile histogram row           (level 1)
-//   direct_scan / direct_fill  (r2x_binning.cu, unchanged)  -> ranges1[S], list1: Gaussian ids, ascending, per supertile
+//   direct_scan / direct_fill  (r2x_binning.cu)  -> ranges1[S], list1: Gaussian ids, ascending, per supertile
 //   fine_count      per item: the 64 per-tile counts of its entries (one ballot per tile transposes the warp's
 //                   32 x 64 membership matrix; a count is the population of a column)              -> table2[item][64]
 //   fine_scan       per supertile: running prefix over its items, tile totals into tile_count[T]
@@ -303,11 +303,11 @@ int launch_two_level(cudaStream_t st, int P, const uint16_t* cube, const uint32_
     super_cube_kernel<<<tl.db1.nb, DIRECT_BLOCK, (size_t)tl.T1 * sizeof(uint32_t), st>>>(P, cube, tiles_touched, tl.cube1,
                                                                                           tl.tiles1, tl.db1, tl.gx1, tl.gy1);
     R2X_CUDA_OK(cudaGetLastError());
-    R2X_PASS(launch_direct_scan(st, tl.db1, tl.status1, bv.capacity, nullptr));
+    R2X_PASS(launch_direct_scan(st, tl.db1, tl.ranges1, tl.plan1, tl.status1, bv.capacity, nullptr));
     BinningView b1 = bv;
     b1.point_list = tl.list1;
-    R2X_PASS(launch_direct_fill(st, P, tl.cube1, tl.tiles1, tl.offsets1, tl.db1, tl.ranges1, tl.plan1, b1, tl.gx1, tl.gy1,
-                           tl.status1));
+    R2X_PASS(launch_direct_fill(st, P, tl.cube1, tl.tiles1, tl.offsets1, tl.db1, tl.plan1, b1, tl.gx1, tl.gy1,
+                                tl.status1));
     // ---- level 2: supertile lists -> tile lists
     int sms;
     R2X_CUDA_OK(sm_count(&sms));
