@@ -300,6 +300,25 @@ int r2x_volume_project(void* stream, int nx, int ny, int nz, const float* volume
                        float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
                        float tan_fovx, float tan_fovy, int mode, float step, float* out_projs);
 
+/* ---- matched backprojection: the transpose of r2x_volume_project (iterative reconstruction) ------------------- */
+/* Replaces TIGRE's `Atb` inside `algs.cgls` / `algs.sart` / `algs.ossart` (r2_gaussian/utils/ct_utils.py).  Same
+ * geometry arguments and units as r2x_volume_project, plus the per-view projmatrices (the rasterizer's, as for r2x_fdk)
+ * for each voxel's detector footprint.  projs[N,H,W] (rows = v, columns = u); out_volume / out_weight [nx,ny,nz]:
+ *   out_volume[x] = step * sum over views (index order) of sum over pixels of projs[v,i,j] * sum_{k in K} h_x(p_k)
+ *   out_weight[x] = the same with projs = 1 (optional: NULL skips it)
+ * where p_k = fmaf(k, s, g) is r2x_volume_project's own float32 index-space sample of pixel (i, j), K its own k range
+ * (the box test, and t > 0 for cone beam), and h_x(p) the trilinear weight the projector gives lattice point x at p:
+ * per axis 1 - f at floor(p) and f at floor(p) + 1, f = p - floor(p).  So out_volume = A^T projs over exactly the
+ * (ray, sample, voxel) triples of r2x_volume_project; only the float32 rounding of the sums differs.  Both outputs are
+ * written in full (no memset needed).  Deterministic (no atomics).  `scratch` holds
+ * r2x_volume_backproject_scratch_bytes(N, H, W) (the projector's ray setup for up to 32 views at a time).
+ * Asynchronous on `stream`.  Limits: nx <= 65535, ny <= 262140, fewer than 2^24 samples per half ray. */
+size_t r2x_volume_backproject_scratch_bytes(int n_views, int H, int W);
+int r2x_volume_backproject(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                           const float* projmatrices, float tan_fovx, float tan_fovy, int mode, int nx, int ny, int nz,
+                           float sx, float sy, float sz, float cx, float cy, float cz, float step, float* out_volume,
+                           float* out_weight, void* scratch, size_t scratch_bytes);
+
 /* ---- multi-GPU exchange step: one-shot sum over NVLink peer memory ------------------------------ */
 /* The Gaussian-sharded projector (one process per GPU, every rank renders its index shard) needs ONE exchange per
  * projection: the sum of the per-rank partial detector images (BASELINE north_star; the reference itself is

@@ -70,6 +70,9 @@ PROTOTYPES = {
     "r2x_fdk_filter": (_i, [_vp, _i, _i, _i, _vp, _f, _f, _i, _f, _vp]),
     "r2x_fdk_backproject": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _i, _f, _i, _i, _i, _f, _f, _f, _f, _f, _f, _vp]),
     "r2x_volume_project": (_i, [_vp, _i, _i, _i, _vp, _f, _f, _f, _f, _f, _f, _i, _i, _i, _vp, _f, _f, _i, _f, _vp]),
+    "r2x_volume_backproject_scratch_bytes": (_sz, [_i, _i, _i]),
+    "r2x_volume_backproject": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _i, _i, _i, _f, _f, _f, _f, _f, _f, _f,
+                                    _vp, _vp, _vp, _sz]),
     "r2x_peer_alloc": (_i, [_sz, C.POINTER(_vp)]),
     "r2x_peer_free": (_i, [_vp]),
     "r2x_ipc_export": (_i, [_vp, _vp]),

@@ -21,6 +21,7 @@
 
 #include "../../include/r2x.h"
 #include "r2x_common.cuh"
+#include "r2x_project.cuh"
 
 namespace r2x {
 
@@ -37,56 +38,12 @@ __global__ void __launch_bounds__(PRJ_BV * PRJ_BU) volume_project_kernel(
     const int view = blockIdx.z;
     float acc = 0.0f;
     if (v < H && u < W) {
-        // world -> camera: rotation Rw[r][c] = m[4c + r], translation T[r] = m[12 + r] (column-major flat)
-        const float* m = viewm + (size_t)view * 16;
-        double Rw[3][3], T[3];
-#pragma unroll
-        for (int r = 0; r < 3; ++r) {
-#pragma unroll
-            for (int c = 0; c < 3; ++c) Rw[r][c] = (double)__ldg(m + 4 * c + r);
-            T[r] = (double)__ldg(m + 12 + r);
-        }
-        // camera-frame ray of the pixel centre: cone from the source, parallel from (ndc_x, ndc_y, 0), both along +z
-        const double ndx = (2.0 * u + 1.0) / W - 1.0, ndy = (2.0 * v + 1.0) / H - 1.0;
-        const double oc[3] = {CONE ? 0.0 : ndx, CONE ? 0.0 : ndy, 0.0};
-        const double dc[3] = {CONE ? ndx * (double)tanx : 0.0, CONE ? ndy * (double)tany : 0.0, 1.0};
-        // to world through the rigid inverse (Rw^T, -Rw^T T), relative to the volume centre
-        const double ctr[3] = {(double)cx, (double)cy, (double)cz};
-        double o[3], d[3];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            o[c] = Rw[0][c] * (oc[0] - T[0]) + Rw[1][c] * (oc[1] - T[1]) + Rw[2][c] * (oc[2] - T[2]) - ctr[c];
-            d[c] = Rw[0][c] * dc[0] + Rw[1][c] * dc[1] + Rw[2][c] * dc[2];
-        }
-        const double inv_len = 1.0 / sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-        d[0] *= inv_len; d[1] *= inv_len; d[2] *= inv_len;
-        const double tc = -(o[0] * d[0] + o[1] * d[1] + o[2] * d[2]);   // closest approach to the volume centre
-        // index space: lattice point i (voxel centre) at g = i; the field is nonzero only for g in (-1, n)
-        const int n[3] = {nx, ny, nz};
-        const double s[3] = {(double)sx, (double)sy, (double)sz};
-        double g[3], st[3];
-        double lo = -1e300, hi = 1e300;
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            const double dv = s[a] / n[a];
-            g[a] = (o[a] + tc * d[a]) / dv + 0.5 * (n[a] - 1);
-            st[a] = (double)step * d[a] / dv;
-            if (st[a] != 0.0) {
-                const double k1 = (-1.0 - g[a]) / st[a], k2 = ((double)n[a] - g[a]) / st[a];
-                lo = fmax(lo, fmin(k1, k2));
-                hi = fmin(hi, fmax(k1, k2));
-            } else if (!(g[a] > -1.0 && g[a] < (double)n[a])) {
-                lo = 1.0; hi = 0.0;                                        // parallel to this slab and outside it
-            }
-        }
-        long long k0 = (long long)ceil(fmax(lo, -1e18)), k1 = (long long)floor(fmin(hi, 1e18));
-        if (CONE) k0 = max(k0, (long long)floor(fmin(fmax(-tc / (double)step, -1e18), 1e18)) + 1);   // t > 0
-        const float gx = (float)g[0], gy = (float)g[1], gz = (float)g[2];
-        const float sxk = (float)st[0], syk = (float)st[1], szk = (float)st[2];
+        const ProjRay ray = project_ray_setup<CONE>(viewm, view, u, v, H, W, nx, ny, nz, sx, sy, sz, cx, cy, cz, tanx,
+                                                    tany, step);
         const long long sy_ = nz, sx_ = (long long)ny * nz;
-        for (long long k = k0; k <= k1; ++k) {
+        for (long long k = ray.k0; k <= ray.k1; ++k) {
             const float fk = (float)k;
-            const float px = fmaf(fk, sxk, gx), py = fmaf(fk, syk, gy), pz = fmaf(fk, szk, gz);
+            const float px = fmaf(fk, ray.sx, ray.gx), py = fmaf(fk, ray.sy, ray.gy), pz = fmaf(fk, ray.sz, ray.gz);
             const float fx0 = floorf(px), fy0 = floorf(py), fz0 = floorf(pz);
             const int ix = (int)fx0, iy = (int)fy0, iz = (int)fz0;
             const float fx = px - fx0, fy = py - fy0, fz = pz - fz0;

@@ -1,14 +1,19 @@
 """Forward projection of a voxel volume on the GPU over the C ABI (r2x_volume_project) -- what the reference obtains from
-TIGRE's `Ax` to synthesise its datasets (`data_generator/synthetic_dataset/generate_data.py`).
+TIGRE's `Ax` to synthesise its datasets (`data_generator/synthetic_dataset/generate_data.py`) -- and its exact
+transpose (r2x_volume_backproject), TIGRE's `Atb` inside the iterative reconstructions of `r2_gaussian_b200.recon`.
 
-    projs = project(volume, angles, scanner_cfg)        # [N, H, W], rows = v, columns = u
+    projs = project(volume, angles, scanner_cfg)                 # [N, H, W], rows = v, columns = u
+    vol = backproject(projs, angles, scanner_cfg)                # [nx, ny, nz] = A^T projs
+    vol, weight = backproject(projs, angles, scanner_cfg, weights=True)   # weight = A^T 1, from the same launch
 
 `volume` is a CUDA float32 [nx, ny, nz] tensor in the voxelizer's layout; `scanner_cfg` is the scaled dict of
 `dataset.read_scene` / `Scene.scanner_cfg`, and the result is in the same scene-scaled units (what the readers hand to
 training).  The per-view geometry is the rasterizer's (`scene.make_view`), so the projections agree with render() by
 construction.  Each pixel is the line integral of the volume's trilinear field, sampled every
 `accuracy * min(dVoxel)` along the ray (`accuracy` defaults to 0.5, as in the reference's scanner files); the exact
-definition is in include/r2x.h.  Runs on the current stream; no CPU fallback.
+definition is in include/r2x.h.  `backproject` sums every (ray, sample, voxel) triple `project` uses, with the same
+weight, so <project(x), y> = <x, backproject(y)> up to float32 rounding.  Both run on the current stream; no CPU
+fallback.  `CTOperator` binds the pair to one set of angles for repeated use (the iterative solvers).
 """
 from __future__ import annotations
 
@@ -21,21 +26,27 @@ from .scene import make_view
 DEFAULT_ACCURACY = 0.5
 
 
+def _check_geometry(what: str, scanner_cfg: dict) -> float:
+    """The scanner settings the projector pair supports; returns `accuracy`."""
+    accuracy = float(scanner_cfg.get("accuracy", DEFAULT_ACCURACY))
+    if not accuracy > 0.0:
+        raise ValueError(f"{what}: accuracy must be > 0, got {accuracy}")
+    if np.any(np.asarray(scanner_cfg.get("offDetector", [0.0, 0.0]), np.float64) != 0.0):
+        raise ValueError(f"{what}: offDetector must be [0, 0]: render() has no detector offset, so such projections "
+                         "would not match training")
+    if scanner_cfg["mode"] != "cone" and not np.allclose(np.asarray(scanner_cfg["sDetector"], np.float64), 2.0,
+                                                         rtol=1e-6, atol=0.0):
+        raise ValueError(f"{what}: a parallel-beam detector must span the scene's [-1, 1] (scaled sDetector [2, 2]), "
+                         f"got {list(scanner_cfg['sDetector'])}: render() could not reproduce that geometry")
+    return accuracy
+
+
 def project(volume: torch.Tensor, angles, scanner_cfg: dict) -> torch.Tensor:
     nvox = tuple(int(v) for v in scanner_cfg["nVoxel"])
     if tuple(getattr(volume, "shape", ())) != nvox:
         raise ValueError(f"project: volume shape {tuple(getattr(volume, 'shape', ()))} is not the scanner's nVoxel "
                          f"{list(nvox)}")
-    accuracy = float(scanner_cfg.get("accuracy", DEFAULT_ACCURACY))
-    if not accuracy > 0.0:
-        raise ValueError(f"project: accuracy must be > 0, got {accuracy}")
-    if np.any(np.asarray(scanner_cfg.get("offDetector", [0.0, 0.0]), np.float64) != 0.0):
-        raise ValueError("project: offDetector must be [0, 0]: render() has no detector offset, so such projections "
-                         "would not match training")
-    if scanner_cfg["mode"] != "cone" and not np.allclose(np.asarray(scanner_cfg["sDetector"], np.float64), 2.0,
-                                                         rtol=1e-6, atol=0.0):
-        raise ValueError(f"project: a parallel-beam detector must span the scene's [-1, 1] (scaled sDetector [2, 2]), "
-                         f"got {list(scanner_cfg['sDetector'])}: render() could not reproduce that geometry")
+    accuracy = _check_geometry("project", scanner_cfg)
     if not isinstance(volume, torch.Tensor) or volume.device.type != "cuda":
         raise RuntimeError("project: volume must be a CUDA tensor (this build has no CPU fallback; "
                            f"got {getattr(volume, 'device', type(volume))})")
@@ -58,3 +69,85 @@ def project(volume: torch.Tensor, angles, scanner_cfg: dict) -> torch.Tensor:
                                     float(views[0].tanfovy), int(views[0].mode), step, out.data_ptr())
     check(rc, "r2x_volume_project")
     return out
+
+
+class CTOperator:
+    """A = r2x_volume_project and A^T = r2x_volume_backproject for fixed angles and scanner on one CUDA device, with the
+    per-view matrices uploaded once.  `A(x, views)` projects a [nx, ny, nz] volume into the views `views` (a slice of
+    the angle list) and `At(y, views, weights)` backprojects their [n, H, W] projections, returning (A_views^T y,
+    A_views^T 1) when `weights` is true.  Inputs are used as float32 contiguous tensors on the operator's device."""
+
+    def __init__(self, angles, scanner_cfg: dict, device):
+        accuracy = _check_geometry("backproject", scanner_cfg)
+        angles = np.asarray(angles, dtype=np.float64).reshape(-1)
+        if len(angles) == 0:
+            raise ValueError("backproject: no angles")
+        views = [make_view(scanner_cfg, float(a)) for a in angles]
+        self.device = torch.device(device)
+        self.nvox = tuple(int(v) for v in scanner_cfg["nVoxel"])
+        self.N, self.H, self.W = len(views), views[0].image_height, views[0].image_width
+        self.size = tuple(float(v) for v in scanner_cfg["sVoxel"])
+        self.centre = tuple(float(v) for v in scanner_cfg["offOrigin"])
+        self.step = accuracy * min(s / n for s, n in zip(self.size, self.nvox))
+        self.mode, self.tanx, self.tany = int(views[0].mode), float(views[0].tanfovx), float(views[0].tanfovy)
+        self.vm = torch.from_numpy(np.stack([v.viewmatrix.reshape(16) for v in views])).to(self.device)
+        self.pm = torch.from_numpy(np.stack([v.projmatrix.reshape(16) for v in views])).to(self.device)
+        self.lib = load()
+
+    def _views(self, views: slice) -> tuple[int, int]:
+        v0, v1, stride = views.indices(self.N)
+        if stride != 1 or v1 <= v0:
+            raise ValueError(f"CTOperator: views must be a non-empty contiguous slice, got {views}")
+        return v0, v1 - v0
+
+    def A(self, x: torch.Tensor, views: slice = slice(None)) -> torch.Tensor:
+        v0, n = self._views(views)
+        with torch.cuda.device(self.device):
+            vol = x.detach().to(self.device, torch.float32).contiguous()
+            if tuple(vol.shape) != self.nvox:
+                raise ValueError(f"project: volume shape {tuple(vol.shape)} is not the scanner's nVoxel {list(self.nvox)}")
+            out = torch.empty((n, self.H, self.W), dtype=torch.float32, device=self.device)
+            rc = self.lib.r2x_volume_project(torch.cuda.current_stream(self.device).cuda_stream, *self.nvox,
+                                             vol.data_ptr(), *self.size, *self.centre, n, self.H, self.W,
+                                             self.vm[v0].data_ptr(), self.tanx, self.tany, self.mode, self.step,
+                                             out.data_ptr())
+        check(rc, "r2x_volume_project")
+        return out
+
+    def At(self, y: torch.Tensor, views: slice = slice(None), weights: bool = False):
+        v0, n = self._views(views)
+        with torch.cuda.device(self.device):
+            projs = y.detach().to(self.device, torch.float32).contiguous()
+            if tuple(projs.shape) != (n, self.H, self.W):
+                raise ValueError(f"backproject: expected projections of shape {[n, self.H, self.W]}, "
+                                 f"got {list(projs.shape)}")
+            vol = torch.empty(self.nvox, dtype=torch.float32, device=self.device)
+            wgt = torch.empty(self.nvox, dtype=torch.float32, device=self.device) if weights else None
+            nbytes = int(self.lib.r2x_volume_backproject_scratch_bytes(n, self.H, self.W))
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            rc = self.lib.r2x_volume_backproject(torch.cuda.current_stream(self.device).cuda_stream, n, self.H, self.W,
+                                                 projs.data_ptr(), self.vm[v0].data_ptr(), self.pm[v0].data_ptr(),
+                                                 self.tanx, self.tany, self.mode, *self.nvox, *self.size, *self.centre,
+                                                 self.step, vol.data_ptr(), wgt.data_ptr() if weights else None,
+                                                 scratch.data_ptr(), nbytes)
+        check(rc, "r2x_volume_backproject")
+        return (vol, wgt) if weights else vol
+
+
+def backproject(projections: torch.Tensor, angles, scanner_cfg: dict, weights: bool = False):
+    """A^T projections for the projector of `project(., angles, scanner_cfg)`: [nx, ny, nz], or (volume, A^T 1) when
+    `weights` is true."""
+    shape = tuple(getattr(projections, "shape", ()))
+    if len(shape) != 3:
+        raise ValueError(f"backproject: expected projections of shape [N, H, W], got {shape}")
+    n_angles = np.asarray(angles, dtype=np.float64).reshape(-1).size
+    if shape[0] != n_angles:
+        raise ValueError(f"backproject: {shape[0]} projections but {n_angles} angles")
+    det = (int(scanner_cfg["nDetector"][0]), int(scanner_cfg["nDetector"][1]))
+    if shape[1:] != det:
+        raise ValueError(f"backproject: projections are {shape[1]}x{shape[2]}, scanner nDetector is {list(det)}")
+    _check_geometry("backproject", scanner_cfg)
+    if not isinstance(projections, torch.Tensor) or projections.device.type != "cuda":
+        raise RuntimeError("backproject: projections must be a CUDA tensor (this build has no CPU fallback; "
+                           f"got {getattr(projections, 'device', type(projections))})")
+    return CTOperator(angles, scanner_cfg, projections.device).At(projections, slice(None), weights)

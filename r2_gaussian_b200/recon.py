@@ -1,0 +1,216 @@
+"""Traditional CT reconstructions on the GPU -- FDK, SART / OS-SART and CGLS, what the reference obtains from TIGRE's
+`algs` (`r2_gaussian/utils/ct_utils.py::recon_volume` / `run_ct_recon_algs`, `scripts/run_traditional_methods.py`).
+
+    x, l2 = cgls(projs, angles, scanner_cfg, niter=60)
+    x = sart(projs, angles, scanner_cfg, niter=20, lmbda=1.0, lmbda_red=0.999, blocksize=1, nonneg=True)
+    x = recon_volume(projs, angles, scanner_cfg, method)           # fdk | cgls | sart | ossart
+
+`projs` is a CUDA [N, H, W] tensor in the dataset layout (scene units, as the readers return it) and `scanner_cfg` the
+scaled dict of `dataset.read_scene`; volumes are [nx, ny, nz] in the voxelizer's layout.  A is `projector.project`
+(r2x_volume_project) and A^T its exact transpose `projector.backproject` (r2x_volume_backproject), so CGLS runs on a
+matched pair.  The solvers (`cgls_solve`, `sart_solve`) are written over two callables, A(x, views) and
+At(y, views, weights), with `views` a contiguous slice of the view list.  Norms and dot products are float64
+reductions without atomics, so every solve is bitwise reproducible.
+
+CGLS (TIGRE's recurrence), from x = 0:
+    r = b - A x,  p = A^T r,  gamma = |p|^2;
+    per iteration:  q = A p,  alpha = gamma / |q|^2,  x += alpha p,  r -= alpha q,  s = A^T r,  beta = |s|^2 / gamma,
+                    gamma = |s|^2,  p = s + beta p.
+    l2[i] = |r| after iteration i (TIGRE's computel2 evaluates |b - A x| with one more projection; it is the same
+    quantity in exact arithmetic).
+
+SART (blocksize 1) / OS-SART (blocksize > 1), from x = 0:
+    W = 1 / (A 1) where A 1 > 0, else 0, computed once;
+    each sweep takes the views in index order, in consecutive blocks B of `blocksize`:
+        r = W * (b_B - A_B x);  (num, den) = (A_B^T r, A_B^T 1) from one fused backprojection;
+        x += lmbda * num / den where den > 0;  x = max(x, 0) if nonneg;
+    after each sweep lmbda *= lmbda_red.
+
+Parity with TIGRE's binaries is not pinned (as for FDK and the projector).  ASD-POCS / OS-ASD-POCS are not built.
+
+    python -m r2_gaussian_b200.recon -s <scene> -m <output> [--methods fdk,sart,cgls]
+
+mirrors `scripts/run_traditional_methods.py`: it reconstructs the scene's train views with each method, scores the
+volume against `vol_gt` with `metrics.metric_vol` and writes, per method, `<output>/<method>/ct_gt.npy`, `ct_pred.npy`,
+`eval_3d.yml` (method, psnr_3d, ssim_3d, ssim_3d_x/y/z, duration (sec), duration (min)) and the test views
+`projs/{i:05d}_render.npy` (projections of the reconstruction) and `projs/{i:05d}_gt.npy`, plus `<output>/eval_3d.yml`
+keyed by method.  PNG slices and projections are not written (matplotlib is not a dependency of this project).
+"""
+from __future__ import annotations
+
+import argparse
+import os
+import sys
+import time
+
+import numpy as np
+import torch
+
+METHODS = ("fdk", "sart", "ossart", "cgls")
+NOT_BUILT = ("asd_pocs", "os_asd_pocs")
+# iteration counts and parameters of ct_utils.recon_volume / run_ct_recon_algs
+CGLS_NITER = 60
+SART_NITER = 20
+OSSART_BLOCKSIZE = 10
+
+
+def _dot(a: torch.Tensor, b: torch.Tensor) -> float:
+    return float((a * b).sum(dtype=torch.float64))
+
+
+def cgls_solve(b: torch.Tensor, A, At, niter: int):
+    """CGLS from x = 0 over the callables A(x, views) / At(y, views, weights); returns (x, l2 per iteration)."""
+    everything = slice(None)
+    r = b.clone()                                         # b - A 0
+    p = At(r, everything, False)
+    x = torch.zeros_like(p)
+    gamma = _dot(p, p)
+    l2 = []
+    for _ in range(niter):
+        if gamma == 0.0:                                  # A^T r = 0: x is a least-squares solution
+            break
+        q = A(p, everything)
+        alpha = gamma / _dot(q, q)
+        x.add_(p, alpha=alpha)
+        r.sub_(q, alpha=alpha)
+        l2.append(_dot(r, r) ** 0.5)
+        s = At(r, everything, False)
+        gamma_new = _dot(s, s)
+        p = s.add_(p, alpha=gamma_new / gamma)
+        gamma = gamma_new
+    return x, l2
+
+
+def sart_solve(b: torch.Tensor, A, At, shape, niter: int, lmbda: float = 1.0, lmbda_red: float = 0.999,
+               blocksize: int = 1, nonneg: bool = True) -> torch.Tensor:
+    """SART / OS-SART from x = 0 over the callables A(x, views) / At(y, views, weights); `shape` is the volume's."""
+    if blocksize < 1:
+        raise ValueError(f"sart: blocksize must be >= 1, got {blocksize}")
+    n = int(b.shape[0])
+    x = torch.zeros(tuple(shape), dtype=b.dtype, device=b.device)
+    w = A(torch.ones_like(x), slice(None))
+    w = torch.where(w > 0, 1.0 / w, torch.zeros_like(w))
+    blocks = [slice(v, min(v + blocksize, n)) for v in range(0, n, blocksize)]
+    for _ in range(niter):
+        for views in blocks:
+            r = w[views] * (b[views] - A(x, views))
+            num, den = At(r, views, True)
+            x.add_(torch.where(den > 0, num / den, torch.zeros_like(num)), alpha=lmbda)
+            if nonneg:
+                x.clamp_(min=0.0)
+        lmbda *= lmbda_red
+    return x
+
+
+def _operator(projs, angles, scanner_cfg):
+    from .projector import CTOperator
+
+    if not isinstance(projs, torch.Tensor) or projs.device.type != "cuda":
+        raise RuntimeError("recon: projections must be a CUDA tensor (this build has no CPU fallback; "
+                           f"got {getattr(projs, 'device', type(projs))})")
+    op = CTOperator(angles, scanner_cfg, projs.device)
+    b = projs.detach().to(torch.float32).contiguous()
+    if tuple(b.shape) != (op.N, op.H, op.W):
+        raise ValueError(f"recon: projections {list(b.shape)} do not match {op.N} angles of {op.H}x{op.W} pixels")
+    return op, b
+
+
+def cgls(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = CGLS_NITER):
+    """CGLS on the GPU projector pair; returns (volume, l2 per iteration)."""
+    op, b = _operator(projs, angles, scanner_cfg)
+    return cgls_solve(b, op.A, op.At, niter)
+
+
+def sart(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = SART_NITER, lmbda: float = 1.0,
+         lmbda_red: float = 0.999, blocksize: int = 1, nonneg: bool = True) -> torch.Tensor:
+    """SART (blocksize 1) or OS-SART on the GPU projector pair."""
+    op, b = _operator(projs, angles, scanner_cfg)
+    return sart_solve(b, op.A, op.At, op.nvox, niter, lmbda, lmbda_red, blocksize, nonneg)
+
+
+def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str) -> torch.Tensor:
+    """The reconstructions of ct_utils.recon_volume / run_ct_recon_algs with their iteration counts."""
+    if method == "fdk":
+        from .fdk import fdk
+
+        return fdk(projs, angles, scanner_cfg)
+    if method == "cgls":
+        return cgls(projs, angles, scanner_cfg, CGLS_NITER)[0]
+    if method == "sart":
+        return sart(projs, angles, scanner_cfg, SART_NITER)
+    if method == "ossart":
+        return sart(projs, angles, scanner_cfg, SART_NITER, blocksize=OSSART_BLOCKSIZE)
+    raise ValueError(f"recon_volume: unknown method {method!r} (supported: {', '.join(METHODS)})")
+
+
+def _parse_methods(text: str) -> list[str]:
+    methods = [m.strip() for m in text.split(",") if m.strip()]
+    for m in methods:
+        if m in NOT_BUILT:
+            raise SystemExit(f"method {m} is not built (TV-regularised ASD-POCS is not part of this project); "
+                             f"supported: {', '.join(METHODS)}")
+        if m not in METHODS:
+            raise SystemExit(f"unknown method {m!r}; supported: {', '.join(METHODS)}")
+    if not methods:
+        raise SystemExit(f"no methods given; supported: {', '.join(METHODS)}")
+    return methods
+
+
+def main(argv=None) -> dict:
+    ap = argparse.ArgumentParser(description="Traditional CT reconstructions (FDK, SART, OS-SART, CGLS) of a scene")
+    ap.add_argument("-s", "--source_path", required=True, help="scene directory or NAF pickle")
+    ap.add_argument("-m", "--model_path", required=True, help="output directory")
+    ap.add_argument("--methods", default="fdk,sart,cgls", help=f"comma-separated subset of {','.join(METHODS)}")
+    a = ap.parse_args(argv)
+    methods = _parse_methods(a.methods)
+    if not torch.cuda.is_available():
+        raise SystemExit("the reconstructions need a CUDA device: they run on the GPU and have no CPU fallback")
+    import yaml
+
+    from .dataset import read_scene
+    from .metrics import metric_vol
+    from .projector import project
+
+    source = os.path.abspath(a.source_path)
+    info = read_scene(source, eval=True)
+    cfg = info.scanner_cfg
+    projs_train = torch.from_numpy(np.stack([np.asarray(c.image, np.float32) for c in info.train_cameras])).cuda()
+    train_angles = [c.angle for c in info.train_cameras]
+    test_angles = [c.angle for c in info.test_cameras]
+    vol_gt = np.asarray(info.vol, np.float32)
+    out = {}
+    print(f"Run traditional algorithms on {os.path.basename(source)}")
+    for method in methods:
+        print(f"Run {method}...")
+        save = os.path.join(a.model_path, method)
+        os.makedirs(os.path.join(save, "projs"), exist_ok=True)
+        torch.cuda.synchronize()
+        t0 = time.time()
+        pred = recon_volume(projs_train, train_angles, cfg, method)
+        torch.cuda.synchronize()
+        duration = time.time() - t0
+        ct_pred = pred.cpu().numpy()
+        psnr_3d, _ = metric_vol(vol_gt, ct_pred, "psnr")
+        ssim_3d, ssim_axis = metric_vol(vol_gt, ct_pred, "ssim")
+        np.save(os.path.join(save, "ct_gt.npy"), vol_gt)
+        np.save(os.path.join(save, "ct_pred.npy"), ct_pred)
+        report = {"method": method, "psnr_3d": float(psnr_3d), "ssim_3d": float(ssim_3d),
+                  "ssim_3d_x": float(ssim_axis[0]), "ssim_3d_y": float(ssim_axis[1]), "ssim_3d_z": float(ssim_axis[2]),
+                  "duration (sec)": duration, "duration (min)": duration / 60}
+        with open(os.path.join(save, "eval_3d.yml"), "w") as f:
+            yaml.dump(report, f, default_flow_style=False, sort_keys=False)
+        if test_angles:
+            render = project(pred, test_angles, cfg).cpu().numpy()
+            for i, cam in enumerate(info.test_cameras):
+                np.save(os.path.join(save, "projs", f"{i:05d}_render.npy"), render[i])
+                np.save(os.path.join(save, "projs", f"{i:05d}_gt.npy"), np.asarray(cam.image, np.float32))
+        out[method] = report
+        print(f"[{method}] psnr_3d: {psnr_3d}, ssim_3d: {ssim_3d}")
+    with open(os.path.join(a.model_path, "eval_3d.yml"), "w") as f:
+        yaml.dump(out, f, default_flow_style=False, sort_keys=False)
+    print(f"Run traditional algorithms on {os.path.basename(source)} complete")
+    return out
+
+
+if __name__ == "__main__":
+    main(sys.argv[1:])

@@ -10,6 +10,11 @@
   project          forward projection of a 256^3 volume into 150 cone-beam views of 512^2 (the reference's synthetic
                    dataset: 50 train + 100 test), samples/s and projections/s, with the card name and power limit
                    (no reference arm: TIGRE's Ax is not part of this build)
+  backproject      the matched backprojection (r2x_volume_backproject) of the fdk row's 50 cone-beam views of 512^2
+                   into 256^3, with and without its weight output, per view next to the projector's per view on the
+                   same views, with the card name and power limit (no reference arm: TIGRE's Atb)
+  recon            one CGLS iteration and one SART sweep (50 single-view updates) on the same workload (no reference
+                   arm: TIGRE's algs)
 
 each for ours and, where the compiled reference (oracle/_ref/libr2ref.so) is present, for the reference's own CUDA
 kernels with the identical protocol (CUDA events per step, L2 flushed between steps).  `python scripts/secondary.py`
@@ -253,6 +258,12 @@ def measure(dev=None, peak_gbs: float = 3350.0, quick: bool = False, trace=lambd
     # ---- volume projection: the reference's synthetic dataset, 50 train + 100 test cone-beam views of 512^2 ----
     out["project"] = measure_project(dev, timed)
     trace("secondary: project")
+
+    # ---- matched backprojection and the iterative reconstructions on the fdk row's workload ----
+    out["backproject"] = measure_backproject(dev, timed)
+    trace("secondary: backproject")
+    out["recon"] = measure_recon(dev, timed)
+    trace("secondary: recon")
     return out
 
 
@@ -389,6 +400,59 @@ def measure_fdk(dev, timed) -> dict:
            "reference": "none: the reference reconstructs with TIGRE's algs.fdk, which is not part of this build"}
     row["voxel_view_updates_per_s"] = float(n) ** 3 * N / (row["ours_ms"] * 1e-3)
     row["backproject_voxel_view_updates_per_s"] = float(n) ** 3 * N / (row["backproject_ms"] * 1e-3)
+    return row
+
+
+def _recon_workload(dev):
+    """The fdk row's geometry (50 cone-beam views of 512^2 at linspace(0, 2 pi), 256^3 grid, accuracy 0.5) with seeded
+    projections of a seeded volume, bound to the GPU projector pair."""
+    import torch
+
+    from r2_gaussian_b200 import scene
+    from r2_gaussian_b200.projector import CTOperator
+
+    sc = dict(scene.cone_beam_scanner(512, 256), accuracy=0.5)
+    op = CTOperator(np.linspace(0.0, 2.0 * np.pi, 51)[:-1], sc, dev)
+    vol = torch.rand(256, 256, 256, device=dev, generator=torch.Generator(dev).manual_seed(0))
+    return op, op.A(vol)
+
+
+def measure_backproject(dev, timed) -> dict:
+    """r2x_volume_backproject with and without out_weight, and r2x_volume_project on the same 50 views."""
+    op, b = _recon_workload(dev)
+    n = op.N
+    row = {"workload": "matched backprojection, 50 cone-beam views of 512x512 (DSD 7, DSO 5) -> 256^3, accuracy 0.5 "
+                       "(r2x_volume_backproject: ray table + voxel-driven gather)",
+           "ours_ms": timed(lambda _i: op.At(b)), "with_weight_ms": timed(lambda _i: op.At(b, weights=True), 10, 2),
+           "project_same_views_ms": timed(lambda _i: op.A(b.new_zeros(op.nvox)), 10, 2),
+           "reference": "none: TIGRE's Atb is not part of this build"}
+    row["per_view_ms"] = row["ours_ms"] / n
+    row["project_per_view_ms"] = row["project_same_views_ms"] / n
+    row["backproject_over_project_per_view"] = row["per_view_ms"] / row["project_per_view_ms"]
+    row.update(card(dev))
+    return row
+
+
+def measure_recon(dev, timed) -> dict:
+    """One CGLS iteration (A, A^T and three float64 reductions) and one SART sweep (50 single-view updates, each a
+    one-view projection and a fused one-view backprojection) on the backproject row's workload."""
+    import torch
+
+    from r2_gaussian_b200 import recon
+
+    op, b = _recon_workload(dev)
+    one = lambda x, views: op.A(torch.ones_like(x), views)
+    row = {"workload": "one CGLS iteration and one SART sweep (blocksize 1: 50 view updates) on 50 cone-beam views of "
+                       "512x512 -> 256^3 (recon.cgls_solve / recon.sart_solve over projector.CTOperator)",
+           "cgls_iteration_ms": timed(lambda _i: recon.cgls_solve(b, op.A, op.At, 1), 5, 1),
+           "cgls_setup_ms": timed(lambda _i: recon.cgls_solve(b, op.A, op.At, 0), 5, 1),
+           "sart_sweep_ms": timed(lambda _i: recon.sart_solve(b, op.A, op.At, op.nvox, 1), 5, 1),
+           "sart_setup_ms": timed(lambda _i: one(b.new_zeros(op.nvox), slice(None)), 5, 1),
+           "reference": "none: TIGRE's algs.cgls / algs.sart are not part of this build"}
+    # cgls_solve(niter=1) is setup (A^T b) + one iteration; sart_solve(niter=1) is W = 1 / A 1 + one sweep
+    row["cgls_iteration_ms"] -= row["cgls_setup_ms"]
+    row["sart_sweep_ms"] -= row["sart_setup_ms"]
+    row.update(card(dev))
     return row
 
 
