@@ -7,12 +7,20 @@ sits exactly on the alpha = 1e-5 cut may flip and moves a pixel by 1e-5 absolute
 import numpy as np
 import pytest
 
+import regime_cases
 import util
 
 pytestmark = pytest.mark.gpu
 
 CASES = ["cone_init_small", "cone_trained_small", "parallel_trained_small", "cone_trained_ragged", "cone_trained_mid",
-         "cone_trained_bigdet"]
+         "cone_trained_bigdet", "det_16", "det_7x5", "det_656x400", "det_768", "det_1024", "det_256x4096", "det_272x3856",
+         "det_65536x16", "det_16x65536"]
+# the binning each case is meant to take (tests/regime_cases.py): tile counts on both sides of DIRECT_MAX_TILES and of
+# direct_fill's staging limit FILL_STAGE_TILES, a single tile, a single tile row / column
+PATHS = {"cone_trained_mid": ("direct", 256), "cone_trained_bigdet": ("radix", 4225), "det_16": ("direct", 1),
+         "det_7x5": ("direct", 1), "det_656x400": ("direct", 1025), "det_768": ("direct", 2304),
+         "det_1024": ("direct", 4096), "det_256x4096": ("direct", 4096), "det_272x3856": ("radix", 4097),
+         "det_65536x16": ("direct", 4096), "det_16x65536": ("direct", 4096)}
 
 
 @pytest.mark.parametrize("name", CASES)
@@ -42,9 +50,15 @@ def test_forward_matches_oracle(name):
     scale = float(np.abs(orc["image"]).max())
     err = np.abs(ours["image"].astype(np.float64) - orc["image"]).max()
     assert err <= 1e-5 * scale + 1e-7, f"image error {err} vs scale {scale}"
+    if name in PATHS:
+        reg = regime_cases.regime(orc, (view.image_height, view.image_width))
+        assert (reg["path"], reg["T"]) == PATHS[name] and reg["R"] > 0
+        if reg["path"] == "direct":
+            assert reg["staged"].all() == (reg["T"] <= regime_cases.K["FILL_STAGE_TILES"])
 
 
-@pytest.mark.parametrize("name", ["cone_trained_small", "parallel_trained_small", "cone_trained_ragged", "cone_trained_bigdet"])
+@pytest.mark.parametrize("name", ["cone_trained_small", "parallel_trained_small", "cone_trained_ragged", "cone_trained_bigdet",
+                                  "det_7x5", "det_656x400", "det_1024", "det_272x3856", "det_65536x16"])
 def test_backward_matches_oracle(name):
     cloud, view = util.case(name)
     ours = util.ours_raster_forward(cloud, view, export=False)

@@ -2,6 +2,7 @@
 import numpy as np
 import pytest
 
+import regime_cases
 import util
 from r2_gaussian_b200 import scene
 
@@ -16,7 +17,22 @@ GRIDS = {
     "manytiles": ((144, 136, 136), (2.0, 2.0, 2.0), (0.0, 0.0, 0.0), 1200, "trained"),
     # the same grid through the radix-sort binning (R2X_VOXEL_BINNING=radix; also what grids beyond 512^3 take)
     "manytiles_radix": ((144, 136, 136), (2.0, 2.0, 2.0), (0.0, 0.0, 0.0), 1200, "trained"),
+    # around the tile-count switches (tests/regime_cases.py): a single tile; direct binning beyond direct_fill's staging
+    # limit up to exactly DIRECT_MAX_TILES; one tile more (two-level); thin grids whose supertile count T1 is exactly
+    # DIRECT_MAX_TILES (two-level) and one more (radix)
+    "t1": ((5, 3, 7), (1.0, 0.6, 1.4), (0.0, 0.0, 0.0), 300, "trained"),
+    "direct96": ((96, 96, 96), (2.0, 2.0, 2.0), (0.0, 0.0, 0.0), 3000, "trained"),
+    "direct128": ((128, 128, 128), (2.0, 2.0, 2.0), (0.0, 0.0, 0.0), 3000, "trained"),
+    "twolevel_4097": ((136, 1928, 8), (2.0, 2.0, 2.0), (0.0, 0.0, 0.0), 1500, "trained"),
+    "thin_t1_4096": ((8, 8, 131072), (2.0, 2.0, 2.0), (0.0, 0.0, 0.0), 400, "trained"),
+    "thin_t1_4097": ((8, 8, 131104), (2.0, 2.0, 2.0), (0.0, 0.0, 0.0), 400, "trained"),
 }
+# largest scale of the added grids' clouds: keeps their instance counts (and the oracle's time) small
+SCALE_MAX = {"direct96": 0.03, "direct128": 0.03, "twolevel_4097": 0.02, "thin_t1_4096": 0.02, "thin_t1_4097": 0.02}
+# binning path and tile count (T, or T1 supertiles past DIRECT_MAX_TILES) each added grid is meant to take
+PATHS = {"t1": ("direct", 1), "direct96": ("direct", 1728), "direct128": ("direct", 4096),
+         "twolevel_4097": ("two_level", 4097), "thin_t1_4096": ("two_level", 16384), "thin_t1_4097": ("radix", 16388)}
+T1 = {"thin_t1_4096": 4096, "thin_t1_4097": 4097}
 
 
 @pytest.fixture(autouse=True)
@@ -28,14 +44,16 @@ def _binning_mode(request, monkeypatch):
         monkeypatch.delenv("R2X_VOXEL_BINNING", raising=False)
 
 
-def _cloud(P, kind, seed):
+def _cloud(P, kind, seed, name=""):
+    if name in SCALE_MAX:
+        return scene.make_cloud(P, kind=kind, seed=seed, scale_bound=(0.001, SCALE_MAX[name]))
     return scene.make_cloud(P, kind=kind, seed=seed)
 
 
 @pytest.mark.parametrize("name", list(GRIDS))
 def test_forward_matches_oracle(name):
     nV, sV, ctr, P, kind = GRIDS[name]
-    cloud = _cloud(P, kind, len(name))
+    cloud = _cloud(P, kind, len(name), name)
     ours = util.ours_voxel_forward(cloud, nV, sV, ctr)
     orc = util.oracle_voxel_forward(cloud, nV, sV, ctr)
     assert ours["R"] == orc["R"]
@@ -50,12 +68,19 @@ def test_forward_matches_oracle(name):
     scale = float(np.abs(orc["vol"]).max()) if orc["R"] else 1.0
     err = np.abs(ours["vol"].astype(np.float64) - orc["vol"]).max()
     assert err <= 1e-5 * scale + 1e-7, f"volume error {err} vs scale {scale}"
+    if name in PATHS:
+        reg = regime_cases.regime(orc, nV)
+        assert (reg["path"], reg["T"]) == PATHS[name] and reg["R"] > 0
+        assert name not in T1 or reg["T1"] == T1[name]
+        if reg["path"] == "direct":
+            assert reg["staged"].all() == (reg["T"] <= regime_cases.K["FILL_STAGE_TILES"])
 
 
-@pytest.mark.parametrize("name", ["full32", "ragged", "tvcrop", "manytiles", "manytiles_radix"])
+@pytest.mark.parametrize("name", ["full32", "ragged", "tvcrop", "manytiles", "manytiles_radix", "t1", "direct128",
+                                  "twolevel_4097", "thin_t1_4096", "thin_t1_4097"])
 def test_backward_matches_oracle(name):
     nV, sV, ctr, P, kind = GRIDS[name]
-    cloud = _cloud(P, kind, len(name))
+    cloud = _cloud(P, kind, len(name), name)
     ours = util.ours_voxel_forward(cloud, nV, sV, ctr, export=False)
     orc = util.oracle_voxel_forward(cloud, nV, sV, ctr)
     dL = np.random.RandomState(11).randn(*nV).astype(np.float32)

@@ -30,8 +30,24 @@ def case(name: str):
         "cone_trained_mid": ("trained", "cone", 20000, 256),
         "cone_init_mid": ("init", "cone", 50000, 256),
         "cone_trained_bigdet": ("trained", "cone", 1500, 1040),  # 65 x 65 = 4225 tiles > DIRECT_MAX_TILES: radix path
+        # detectors of (H, W) pixels at the 512-pixel baseline's pitch, around the tile-count switches of the binning
+        # (tests/regime_cases.py states and checks which side each lands on)
+        "det_16": ("trained", "cone", 600, (16, 16)),            # T = 1
+        "det_7x5": ("trained", "cone", 600, (5, 7)),             # T = 1, a partial tile
+        "det_656x400": ("trained", "cone", 3000, (400, 656)),    # T = 1025: direct, unstaged
+        "det_768": ("trained", "cone", 3000, (768, 768)),        # T = 2304
+        "det_1024": ("trained", "cone", 3000, (1024, 1024)),     # T = 4096 = DIRECT_MAX_TILES
+        "det_256x4096": ("trained", "cone", 3000, (4096, 256)),  # T = 4096, 16 x 256 tiles
+        "det_272x3856": ("trained", "cone", 3000, (3856, 272)),  # T = 4097: radix
+        "det_65536x16": ("trained", "cone", 2000, (16, 65536)),  # T = 4096, one tile row
+        "det_16x65536": ("trained", "cone", 2000, (65536, 16)),  # T = 4096, one tile column
     }[name]
-    sc = scene.cone_beam_scanner(n, 64) if beam == "cone" else scene.parallel_beam_scanner(n, 64)
+    if isinstance(n, tuple):
+        sc = scene.cone_beam_scanner(max(n), 64)
+        sc["nDetector"] = list(n)
+        sc["sDetector"] = [4.0 * n[0] / 512, 4.0 * n[1] / 512]
+    else:
+        sc = scene.cone_beam_scanner(n, 64) if beam == "cone" else scene.parallel_beam_scanner(n, 64)
     view = scene.make_view(sc, 0.37 + 0.1 * len(name))
     cloud = scene.make_cloud(P, kind=kind, seed=len(name))
     return cloud, view
