@@ -1,6 +1,7 @@
 // r2x_api.cu -- the C ABI declared in include/r2x.h: buffer carving, stage orchestration, error
-// reporting.  Stage order (both pipelines): preprocess -> scan(tiles_touched) -> [sync variant: read R,
-// obtain the binning buffer] -> emit instances -> stable tile-id sort + ranges -> render.
+// reporting.  Stage order (both pipelines): preprocess -> binning (bin_forward: scan -> [sync variant: read R,
+// obtain the binning buffer] -> direct fill | two-level | emit + stable tile-id sort + ranges, and the work plan)
+// -> render.
 #include <atomic>
 #include <cstdio>
 #include <cstring>
@@ -113,26 +114,54 @@ VoxelState carve_voxel(const void* buf, int P) {
     return s;
 }
 
-// image buffer = ranges[T] | work plan | direct-binning table (when T <= DIRECT_MAX_TILES)
-TilePlan carve_plan(const void* image_buf, int tiles, const BinningView& bv) {
-    char* p = (char*)al((size_t)image_buf) + al((size_t)tiles * sizeof(uint2));
-    return plan_view(p, tiles, bv);
+// ---- binning front-end shared by both pipelines --------------------------------------------------
+// What the front-end needs to know about a pipeline: its tile grid, whether it has a two-level binning path, and the
+// largest work-plan chunk its render kernels take.
+struct Pipeline {
+    const char* name;   // "raster" | "voxel": error messages, debug stages
+    int gx, gy, gz;
+    bool two_level;
+    int chunk_cap;
+    int tiles() const { return gx * gy * gz; }
+    BinPath path() const { return bin_path(gx, gy, gz, two_level); }
+};
+Pipeline raster_pipeline(int W, int H) {
+    return {"raster", (W + R2X_TILE - 1) / R2X_TILE, (H + R2X_TILE - 1) / R2X_TILE, 1, false, PLAN_CHUNK};
 }
-// voxelizer: work items may hold up to VOX_CHUNK_CAP instances (walked in segments), see plan_chunk_for
-TilePlan carve_voxel_plan(const void* image_buf, int tiles, const BinningView& bv) {
-    TilePlan pl = carve_plan(image_buf, tiles, bv);
-    pl.chunk_cap = VOX_CHUNK_CAP;
-    return pl;
-}
-DirectBin carve_directbin(const void* image_buf, int P, int tiles) {
-    char* p = (char*)al((size_t)image_buf) + al((size_t)tiles * sizeof(uint2)) + plan_bytes(tiles);
-    return directbin_view(p, P, tiles);
+// voxelizer work items may hold up to VOX_CHUNK_CAP instances (walked in segments), see plan_chunk_for
+Pipeline voxel_pipeline(int nx, int ny, int nz) {
+    return {"voxel", (nx + R2X_VTILE - 1) / R2X_VTILE, (ny + R2X_VTILE - 1) / R2X_VTILE, (nz + R2X_VTILE - 1) / R2X_VTILE,
+            true, VOX_CHUNK_CAP};
 }
 
-TwoLevel carve_two_level(const void* image_buf, int P, int gx, int gy, int gz, const BinningView& bv) {
-    const int tiles = gx * gy * gz;
-    char* p = (char*)al((size_t)image_buf) + al((size_t)tiles * sizeof(uint2)) + plan_bytes(tiles);
-    return two_level_view(p, P, gx, gy, gz, bv);
+struct ImageViews {
+    uint2* ranges;   // [T]
+    TilePlan plan;   // its extra-item list and partial sums live in the binning buffer
+    DirectBin db;    // direct binning only
+    TwoLevel tl;     // two-level binning only
+};
+// image buffer = ranges[T] | work plan | direct-binning table (T <= DIRECT_MAX_TILES) or two-level scratch (sized by the
+// geometry alone, whatever R2X_VOXEL_BINNING says).  Returns the size r2x_*_image_bytes reports; carves *v when given.
+size_t image_layout(const void* buf, int P, const Pipeline& pp, const BinningView& bv, ImageViews* v) {
+    const size_t t = (size_t)pp.gx * pp.gy * pp.gz;
+    const int T = (int)t;
+    const size_t head = al(t * sizeof(uint2)) + plan_bytes(T);
+    const bool direct = pp.path() == BinPath::Direct;
+    const size_t tail = direct ? directbin_bytes(P, T) : pp.two_level ? two_level_bytes(P, pp.gx, pp.gy, pp.gz) : 0;
+    if (v) {
+        char* base = (char*)al((size_t)buf);
+        v->ranges = (uint2*)base;
+        v->plan = plan_view(base + al(t * sizeof(uint2)), T, bv);
+        v->plan.chunk_cap = pp.chunk_cap;
+        v->db = direct ? directbin_view(base + head, P, T) : DirectBin{};
+        v->tl = (!direct && tail) ? two_level_view(base + head, P, pp.gx, pp.gy, pp.gz, bv) : TwoLevel{};
+    }
+    return head + tail + 1024;
+}
+ImageViews image_views(const void* buf, int P, const Pipeline& pp, const BinningView& bv) {
+    ImageViews v;
+    image_layout(buf, P, pp, bv, &v);
+    return v;
 }
 
 // sorted position -> tile id through the ranges (direct binning keeps no per-instance tile array)
@@ -153,12 +182,6 @@ __global__ void export_keys_ranges_kernel(long long R, const uint32_t* d_total, 
         keys[s] = ((uint64_t)(uint32_t)lo << 32) | (uint64_t)__float_as_uint(d);
     }
     if (point_list_out) point_list_out[s] = g;
-}
-
-int sort_passes(int num_tiles) {
-    int bits = 1;
-    while ((1ll << bits) < (long long)num_tiles) ++bits;
-    return (bits + 7) / 8;
 }
 
 __global__ void status_kernel(uint32_t* status, long long capacity, uint32_t* status_out) {
@@ -226,8 +249,7 @@ __global__ void voxel_export_geom_kernel(int P, VoxelGeom geom, float* means3D_n
     if (tiles_touched) tiles_touched[g] = geom.tiles_touched[g];
     if (point_offsets) point_offsets[g] = geom.offsets[g];
 }
-// keys[s] = (tile << 32) | float_bits(depth of point_list[s]); depth lives at float index depth_idx of
-// the Gaussian's record (record stride rec_stride float4).
+// keys[s] = (tile << 32) | float_bits(depth of point_list[s]); the depth of Gaussian g is depth[depth_stride * g]
 __global__ void export_keys_kernel(long long R, const uint32_t* d_total, const uint32_t* sorted_tiles,
                                    const uint32_t* point_list, const float* depth, int depth_stride,
                                    uint64_t* keys, uint32_t* point_list_out) {
@@ -241,13 +263,87 @@ __global__ void export_keys_kernel(long long R, const uint32_t* d_total, const u
     if (point_list_out) point_list_out[s] = g;
 }
 
-// ---- shared forward tail: emit -> sort -> ranges ---------------------------------------------
-int bin_instances(cudaStream_t st, int P, const uint16_t* cube, const uint32_t* tiles_touched,
-                  const uint32_t* offsets, int gx, int gy, int num_tiles, const uint32_t* d_total,
-                  const BinningView& bv, long long R_launch, uint2* ranges) {
-    if (R_launch > 0) R2X_TRY(launch_emit(st, P, cube, tiles_touched, offsets, gx, gy, d_total, bv));
-    R2X_TRY(launch_sort_and_ranges(st, R_launch, num_tiles, d_total, bv, ranges, nullptr));
+// the voxelizer's view-space depth of Gaussian g is rec[4 g + 3].y: float 13 of its 16-float record
+const float* voxel_depth(const VoxelGeom& geom) { return reinterpret_cast<const float*>(geom.rec + 3) + 1; }
+constexpr int VOX_DEPTH_STRIDE = 4 * sizeof(float4) / sizeof(float);
+
+// ranges (reference convention), keys and point_list of a forward's binning; the depth of Gaussian g is
+// depth[depth_stride * g]
+void export_binning(cudaStream_t st, int P, const Pipeline& pp, long long R, const void* binning_buf,
+                    const void* image_buf, const uint32_t* status, const float* depth, int depth_stride, uint64_t* keys,
+                    uint32_t* point_list, uint32_t* ranges) {
+    const int T = pp.tiles();
+    const ImageViews img = image_views(image_buf, P, pp, BinningView{});
+    if (ranges) export_ranges_kernel<<<(unsigned)((T + 255) / 256), 256, 0, st>>>(T, img.ranges, ranges);
+    if (R <= 0 || (!keys && !point_list)) return;
+    const BinningView bv = binning_view((void*)binning_buf, R);
+    const unsigned grid = (unsigned)((R + 255) / 256);
+    if (pp.path() == BinPath::Radix)
+        export_keys_kernel<<<grid, 256, 0, st>>>(R, status, sorted_tile_ids(bv, T), bv.point_list, depth, depth_stride,
+                                                 keys, point_list);
+    else
+        export_keys_ranges_kernel<<<grid, 256, 0, st>>>(R, status, img.ranges, T, bv.point_list, depth, depth_stride,
+                                                        keys, point_list);
+}
+
+// P == 0: zero output, empty ranges, R = 0 and no overflow
+int forward_empty(cudaStream_t st, const Pipeline& pp, float* out, size_t out_elems, const void* image_buf,
+                  uint32_t* status, uint32_t* status_dev) {
+    R2X_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float) * out_elems, st));
+    R2X_CUDA_OK(cudaMemsetAsync(image_views(image_buf, 0, pp, BinningView{}).ranges, 0, sizeof(uint2) * (size_t)pp.tiles(), st));
+    R2X_CUDA_OK(cudaMemsetAsync(status, 0, 16, st));
+    if (status_dev) R2X_CUDA_OK(cudaMemsetAsync(status_dev, 0, 8, st));
     return 0;
+}
+
+// The binning sequence of both forwards, after their preprocess: scan (direct binning: direct_scan, which also publishes
+// the ranges, the work plan and R); [synchronous variant (binning_alloc): read R back, allocate the binning buffer];
+// then direct fill, two-level binning, or emit + sort + ranges and the plan.  R and the overflow flag go to status
+// (and, asynchronous variant, to status_dev); on overflow the ranges are empty.  The render then reads *bv (its
+// capacity sizes the render grid) and *img.
+int bin_forward(cudaStream_t st, const Pipeline& pp, BinPath path, int P, const uint16_t* cube,
+                const uint32_t* tiles_touched, uint32_t* offsets, void* scan_state, uint32_t* status,
+                const void* image_buf, r2x_alloc_fn binning_alloc, void* alloc_user, void* binning_buf,
+                long long capacity, uint32_t* status_dev, int debug, int* num_rendered, BinningView* bv,
+                ImageViews* img) {
+    const std::string fn = std::string("r2x_") + pp.name + "_forward";
+    if (path == BinPath::Direct) {
+        // tile ranges, work plan and R come straight from the per-CTA tile histograms (the plan's extra-item list,
+        // which lives in the binning buffer, is written by direct_fill)
+        const ImageViews pre = image_views(image_buf, P, pp, BinningView{});
+        const long long cap0 = binning_alloc ? (1ll << 62) : capacity;
+        R2X_TRY(launch_direct_scan(st, pre.db, pre.ranges, pre.plan, status, cap0, binning_alloc ? nullptr : status_dev));
+    } else {
+        R2X_TRY(launch_scan(st, P, tiles_touched, offsets, scan_state, status));
+    }
+    R2X_TRY(debug_sync(st, debug, (std::string(pp.name) + " scan").c_str()));
+    if (binning_alloc) {  // synchronous variant: learn R, size the binning buffer exactly
+        uint32_t R = 0;
+        R2X_CUDA_OK(cudaMemcpyAsync(&R, status, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        R2X_CUDA_OK(cudaStreamSynchronize(st));
+        if (num_rendered) *num_rendered = (int)R;
+        binning_buf = binning_alloc(binning_bytes((long long)R), alloc_user);
+        if (!binning_buf) return fail_msg(R2X_ERR_INVALID, (fn + ": binning allocator returned NULL").c_str());
+        capacity = R;
+    } else if (!binning_buf || capacity < 0) {
+        return fail_msg(R2X_ERR_INVALID, (fn + "_async: no binning buffer").c_str());
+    }
+    *bv = binning_view(binning_buf, capacity);
+    *img = image_views(image_buf, P, pp, *bv);
+    if (path == BinPath::Direct) {
+        R2X_TRY(launch_direct_fill(st, P, cube, tiles_touched, offsets, img->db, img->plan, *bv, pp.gx, pp.gy, status));
+    } else {
+        status_kernel<<<1, 1, 0, st>>>(status, capacity, status_dev);
+        if (path == BinPath::TwoLevel) {
+            R2X_TRY(launch_two_level(st, P, cube, tiles_touched, pp.gx, pp.gy, pp.gz, status, img->tl, *bv, img->ranges,
+                                     img->plan));
+        } else {
+            if (capacity > 0) R2X_TRY(launch_emit(st, P, cube, tiles_touched, offsets, pp.gx, pp.gy, status, *bv));
+            R2X_TRY(launch_sort_and_ranges(st, capacity, pp.tiles(), status, *bv, img->ranges));
+            R2X_TRY(launch_plan(st, img->ranges, img->plan));
+        }
+    }
+    return debug_sync(st, debug, (std::string(pp.name) + " binning").c_str());
 }
 
 int raster_forward_impl(cudaStream_t st, int P, int W, int H, const float* means3D, const float* opacities,
@@ -261,66 +357,24 @@ int raster_forward_impl(cudaStream_t st, int P, int W, int H, const float* means
     if (mode != 0 && mode != 1) return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward: mode must be 0 (parallel) or 1 (cone)");
     if (num_rendered) *num_rendered = 0;
     RasterState s = carve_raster(geom_buf, P, W, H);
-    const int tiles = s.geom.gx * s.geom.gy;
     if (s.geom.gx > 65535 || s.geom.gy > 65535) return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward: detector too large");
-    uint2* ranges = (uint2*)al((size_t)image_buf);
-    if (P == 0) {
-        R2X_CUDA_OK(cudaMemsetAsync(out_color, 0, sizeof(float) * (size_t)W * H, st));
-        R2X_CUDA_OK(cudaMemsetAsync(ranges, 0, sizeof(uint2) * tiles, st));
-        R2X_CUDA_OK(cudaMemsetAsync(s.status, 0, 16, st));
-        if (status_dev) R2X_CUDA_OK(cudaMemsetAsync(status_dev, 0, 8, st));
-        return 0;
-    }
+    const Pipeline pp = raster_pipeline(W, H);
+    if (P == 0) return forward_empty(st, pp, out_color, (size_t)W * H, image_buf, s.status, status_dev);
     if (!means3D || !opacities || !radii || !viewmatrix || !projmatrix)
         return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward: null input");
     if (!cov3D_precomp && (!scales || !rotations))
         return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward: need scales+rotations or cov3D_precomp");
-    const bool direct = direct_ok(tiles);
-    DirectBin db{};
-    if (direct) {
-        db = carve_directbin(image_buf, P, tiles);
-    }
+    const BinPath path = pp.path();
+    ImageViews img = image_views(image_buf, P, pp, BinningView{});
     R2X_TRY(launch_raster_preprocess(st, P, means3D, scales, scale_modifier, rotations, opacities, cov3D_precomp,
                                      viewmatrix, projmatrix, W, H, tan_fovx, tan_fovy, mode, prefiltered, radii,
-                                     s.geom, direct ? &db : nullptr));
+                                     s.geom, path == BinPath::Direct ? &img.db : nullptr));
     R2X_TRY(debug_sync(st, debug, "raster preprocess"));
-    if (direct) {
-        // tile ranges, work plan and R come straight from the per-CTA tile histograms (the plan's extra-item list,
-        // which lives in the binning buffer, is written by direct_fill)
-        const long long cap0 = binning_alloc ? (1ll << 62) : capacity;
-        R2X_TRY(launch_direct_scan(st, db, ranges, carve_plan(image_buf, tiles, BinningView{}), s.status, cap0,
-                                   binning_alloc ? nullptr : status_dev));
-    } else {
-        R2X_TRY(launch_scan(st, P, s.geom.tiles_touched, s.geom.offsets, s.scan_state, s.status));
-    }
-    R2X_TRY(debug_sync(st, debug, "raster scan"));
-    long long R_launch;
-    if (binning_alloc) {  // synchronous variant: learn R, size the binning buffer exactly
-        uint32_t R = 0;
-        R2X_CUDA_OK(cudaMemcpyAsync(&R, s.status, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-        R2X_CUDA_OK(cudaStreamSynchronize(st));
-        if (num_rendered) *num_rendered = (int)R;
-        binning_buf = binning_alloc(binning_bytes((long long)R), alloc_user);
-        if (!binning_buf) return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward: binning allocator returned NULL");
-        capacity = R;
-        R_launch = R;
-    } else {
-        if (!binning_buf || capacity < 0) return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward_async: no binning buffer");
-        R_launch = capacity;
-    }
-    BinningView bv = binning_view(binning_buf, capacity);
-    const TilePlan plan = carve_plan(image_buf, tiles, bv);
-    if (direct) {
-        R2X_TRY(launch_direct_fill(st, P, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, db, plan, bv, s.geom.gx,
-                                   s.geom.gy, s.status));
-    } else {
-        status_kernel<<<1, 1, 0, st>>>(s.status, capacity, status_dev);
-        R2X_TRY(bin_instances(st, P, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, s.geom.gx, s.geom.gy, tiles,
-                              s.status, bv, R_launch, ranges));
-        R2X_TRY(launch_plan(st, ranges, plan));
-    }
-    R2X_TRY(debug_sync(st, debug, "raster binning"));
-    R2X_TRY(launch_raster_render(st, W, H, s.geom, ranges, bv.point_list, plan, R_launch, out_color));
+    BinningView bv;
+    R2X_TRY(bin_forward(st, pp, path, P, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, s.scan_state, s.status,
+                        image_buf, binning_alloc, alloc_user, binning_buf, capacity, status_dev, debug, num_rendered, &bv,
+                        &img));
+    R2X_TRY(launch_raster_render(st, W, H, s.geom, img.ranges, bv.point_list, img.plan, bv.capacity, out_color));
     R2X_TRY(debug_sync(st, debug, "raster render"));
     return 0;
 }
@@ -339,16 +393,9 @@ int voxel_forward_impl(cudaStream_t st, int P, int nx, int ny, int nz, float sx,
     if (vg.gx > 65535 || vg.gy > 65535 || vg.gz > 65535) return fail_msg(R2X_ERR_INVALID, "r2x_voxel_forward: grid too large");
     const long long tiles_ll = (long long)vg.gx * vg.gy * vg.gz;
     if (tiles_ll > (1ll << 30)) return fail_msg(R2X_ERR_INVALID, "r2x_voxel_forward: too many tiles");
-    const int tiles = (int)tiles_ll;
     VoxelState s = carve_voxel(geom_buf, P);
-    uint2* ranges = (uint2*)al((size_t)image_buf);
-    if (P == 0) {
-        R2X_CUDA_OK(cudaMemsetAsync(out_volume, 0, sizeof(float) * (size_t)nx * ny * nz, st));
-        R2X_CUDA_OK(cudaMemsetAsync(ranges, 0, sizeof(uint2) * (size_t)tiles, st));
-        R2X_CUDA_OK(cudaMemsetAsync(s.status, 0, 16, st));
-        if (status_dev) R2X_CUDA_OK(cudaMemsetAsync(status_dev, 0, 8, st));
-        return 0;
-    }
+    const Pipeline pp = voxel_pipeline(nx, ny, nz);
+    if (P == 0) return forward_empty(st, pp, out_volume, (size_t)nx * ny * nz, image_buf, s.status, status_dev);
     if (!means3D || !opacities || !radii_x || !radii_y || !radii_z)
         return fail_msg(R2X_ERR_INVALID, "r2x_voxel_forward: null input");
     if (!scales)
@@ -356,54 +403,16 @@ int voxel_forward_impl(cudaStream_t st, int P, int nx, int ny, int nz, float sx,
                         "r2x_voxel_forward: scales are required (the bounding radius is 3*max(scale)/dVoxel even "
                         "with cov3D_precomp; the reference dereferences scales unconditionally, VOX/forward.cu:137)");
     if (!cov3D_precomp && !rotations) return fail_msg(R2X_ERR_INVALID, "r2x_voxel_forward: need rotations or cov3D_precomp");
-    const bool direct = direct_ok(tiles);
-    const bool two_level = two_level_ok(vg.gx, vg.gy, vg.gz);   // more tiles than the direct table holds
-    DirectBin db{};
-    if (direct) {
-        db = carve_directbin(image_buf, P, tiles);
-    }
+    const BinPath path = pp.path();
+    ImageViews img = image_views(image_buf, P, pp, BinningView{});
     R2X_TRY(launch_voxel_preprocess(st, P, means3D, scales, scale_modifier, rotations, opacities, cov3D_precomp, vg,
-                                    radii_x, radii_y, radii_z, s.geom, direct ? &db : nullptr));
+                                    radii_x, radii_y, radii_z, s.geom, path == BinPath::Direct ? &img.db : nullptr));
     R2X_TRY(debug_sync(st, debug, "voxel preprocess"));
-    if (direct) {
-        const long long cap0 = binning_alloc ? (1ll << 62) : capacity;
-        R2X_TRY(launch_direct_scan(st, db, ranges, carve_voxel_plan(image_buf, tiles, BinningView{}), s.status,
-                                   cap0, binning_alloc ? nullptr : status_dev));
-    } else {
-        R2X_TRY(launch_scan(st, P, s.geom.tiles_touched, s.geom.offsets, s.scan_state, s.status));
-    }
-    long long R_launch;
-    if (binning_alloc) {
-        uint32_t R = 0;
-        R2X_CUDA_OK(cudaMemcpyAsync(&R, s.status, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-        R2X_CUDA_OK(cudaStreamSynchronize(st));
-        if (num_rendered) *num_rendered = (int)R;
-        binning_buf = binning_alloc(binning_bytes((long long)R), alloc_user);
-        if (!binning_buf) return fail_msg(R2X_ERR_INVALID, "r2x_voxel_forward: binning allocator returned NULL");
-        capacity = R;
-        R_launch = R;
-    } else {
-        if (!binning_buf || capacity < 0) return fail_msg(R2X_ERR_INVALID, "r2x_voxel_forward_async: no binning buffer");
-        R_launch = capacity;
-    }
-    BinningView bv = binning_view(binning_buf, capacity);
-    const TilePlan plan = carve_voxel_plan(image_buf, tiles, bv);
-    if (direct) {
-        R2X_TRY(launch_direct_fill(st, P, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, db, plan, bv, vg.gx, vg.gy,
-                                   s.status));
-    } else if (two_level) {
-        status_kernel<<<1, 1, 0, st>>>(s.status, capacity, status_dev);
-        const TwoLevel tl = carve_two_level(image_buf, P, vg.gx, vg.gy, vg.gz, bv);
-        R2X_TRY(launch_two_level(st, P, s.geom.cube, s.geom.tiles_touched, vg.gx, vg.gy, vg.gz, s.status, tl, bv, ranges,
-                                 plan));
-    } else {
-        status_kernel<<<1, 1, 0, st>>>(s.status, capacity, status_dev);
-        R2X_TRY(bin_instances(st, P, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, vg.gx, vg.gy, tiles, s.status,
-                              bv, R_launch, ranges));
-        R2X_TRY(launch_plan(st, ranges, plan));
-    }
-    R2X_TRY(debug_sync(st, debug, "voxel binning"));
-    R2X_TRY(launch_voxel_render(st, vg, s.geom, ranges, bv.point_list, plan, R_launch, out_volume));
+    BinningView bv;
+    R2X_TRY(bin_forward(st, pp, path, P, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, s.scan_state, s.status,
+                        image_buf, binning_alloc, alloc_user, binning_buf, capacity, status_dev, debug, num_rendered, &bv,
+                        &img));
+    R2X_TRY(launch_voxel_render(st, vg, s.geom, img.ranges, bv.point_list, img.plan, bv.capacity, out_volume));
     R2X_TRY(debug_sync(st, debug, "voxel render"));
     return 0;
 }
@@ -420,14 +429,11 @@ int r2x_version(void) { return 100; }
 
 size_t r2x_raster_geom_bytes(int P) { return raster_geom_bytes(P); }
 size_t r2x_raster_image_bytes(int P, int W, int H) {
-    size_t t = (size_t)((W + R2X_TILE - 1) / R2X_TILE) * ((H + R2X_TILE - 1) / R2X_TILE);
-    return al(t * sizeof(uint2)) + plan_bytes((int)t) + (direct_ok((int)t) ? directbin_bytes(P, (int)t) : 0) + 1024;
+    return image_layout(nullptr, P, raster_pipeline(W, H), BinningView{}, nullptr);
 }
 size_t r2x_voxel_geom_bytes(int P) { return voxel_geom_bytes(P); }
 size_t r2x_voxel_image_bytes(int P, int nx, int ny, int nz) {
-    size_t t = (size_t)((nx + 7) / 8) * ((ny + 7) / 8) * ((nz + 7) / 8);
-    return al(t * sizeof(uint2)) + plan_bytes((int)t) + (direct_ok((int)t) ? directbin_bytes(P, (int)t) : 0) +
-           two_level_bytes(P, (nx + 7) / 8, (ny + 7) / 8, (nz + 7) / 8) + 1024;
+    return image_layout(nullptr, P, voxel_pipeline(nx, ny, nz), BinningView{}, nullptr);
 }
 size_t r2x_binning_bytes(long long R) { return binning_bytes(R); }
 size_t r2x_raster_bwd_scratch_bytes(long long R) { return al((size_t)(R > 0 ? R : 1) * 32) + 256; }
@@ -466,12 +472,9 @@ int r2x_raster_render_only(void* stream, int P, int W, int H, long long R, const
         return fail_msg(R2X_ERR_INVALID, "r2x_raster_render_only: bad args");
     RasterState s = carve_raster(geom_buf, P, W, H);
     BinningView bv = binning_view((void*)binning_buf, R);
-    const uint2* ranges = (const uint2*)al((size_t)image_buf);
-    const TilePlan plan = carve_plan(image_buf, s.geom.gx * s.geom.gy, bv);
-    // the work plan of the forward is still valid: only the queue head and the arrival counters are rewound
-    R2X_CUDA_OK(cudaMemsetAsync(plan.counter, 0, sizeof(uint32_t), (cudaStream_t)stream));
-    R2X_CUDA_OK(cudaMemsetAsync(plan.tile_done, 0, sizeof(uint32_t) * PLAN_DONE_SLOTS * (size_t)plan.num_tiles, (cudaStream_t)stream));
-    return launch_raster_render((cudaStream_t)stream, W, H, s.geom, ranges, bv.point_list, plan, R, out_color);
+    const ImageViews img = image_views(image_buf, P, raster_pipeline(W, H), bv);
+    R2X_TRY(rewind_plan((cudaStream_t)stream, img.plan));
+    return launch_raster_render((cudaStream_t)stream, W, H, s.geom, img.ranges, bv.point_list, img.plan, R, out_color);
 }
 
 int r2x_voxel_render_only(void* stream, int P, int nx, int ny, int nz, long long R, const void* geom_buf,
@@ -481,11 +484,9 @@ int r2x_voxel_render_only(void* stream, int P, int nx, int ny, int nz, long long
     const VoxelGrid vg = make_voxel_grid(nx, ny, nz, 1.f, 1.f, 1.f, 0.f, 0.f, 0.f);  // render needs the tile grid only
     VoxelState s = carve_voxel(geom_buf, P);
     BinningView bv = binning_view((void*)binning_buf, R);
-    const uint2* ranges = (const uint2*)al((size_t)image_buf);
-    const TilePlan plan = carve_voxel_plan(image_buf, vg.gx * vg.gy * vg.gz, bv);
-    R2X_CUDA_OK(cudaMemsetAsync(plan.counter, 0, sizeof(uint32_t), (cudaStream_t)stream));
-    R2X_CUDA_OK(cudaMemsetAsync(plan.tile_done, 0, sizeof(uint32_t) * PLAN_DONE_SLOTS * (size_t)plan.num_tiles, (cudaStream_t)stream));
-    return launch_voxel_render((cudaStream_t)stream, vg, s.geom, ranges, bv.point_list, plan, R, out_volume);
+    const ImageViews img = image_views(image_buf, P, voxel_pipeline(nx, ny, nz), bv);
+    R2X_TRY(rewind_plan((cudaStream_t)stream, img.plan));
+    return launch_voxel_render((cudaStream_t)stream, vg, s.geom, img.ranges, bv.point_list, img.plan, R, out_volume);
 }
 
 int r2x_raster_backward(void* stream, int P, long long R, int W, int H, const float* means3D, const float* scales,
@@ -504,12 +505,13 @@ int r2x_raster_backward(void* stream, int P, long long R, int W, int H, const fl
         return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward: null pointer");
     if (R > 0 && (!binning_buf || !scratch)) return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward: null binning/scratch");
     RasterState s = carve_raster(geom_buf, P, W, H);
-    const uint2* ranges = (const uint2*)al((size_t)image_buf);
+    const Pipeline pp = raster_pipeline(W, H);
     BinningView bv = binning_view((void*)binning_buf, R);
+    const ImageViews img = image_views(image_buf, P, pp, bv);
     float4* inst_grad = (float4*)al((size_t)scratch);
-    const TilePlan plan = carve_plan(image_buf, s.geom.gx * s.geom.gy, bv);
-    const uint32_t* inst_pos = direct_ok(s.geom.gx * s.geom.gy) ? nullptr : bv.inst_pos;   // direct binning: slots are derived
-    if (R > 0) R2X_TRY(launch_raster_render_bwd(st, W, H, s.geom, ranges, bv.point_list, inst_pos, plan, R, dL_dpix, inst_grad));
+    const uint32_t* inst_pos = pp.path() == BinPath::Radix ? bv.inst_pos : nullptr;   // otherwise slots are derived
+    if (R > 0)
+        R2X_TRY(launch_raster_render_bwd(st, W, H, s.geom, img.ranges, bv.point_list, inst_pos, img.plan, dL_dpix, inst_grad));
     R2X_TRY(debug_sync(st, debug, "raster render backward"));
     R2X_TRY(launch_raster_gauss_bwd(st, P, means3D, radii, scales, scale_modifier, rotations, cov3D_precomp, viewmatrix,
                                     projmatrix, W, H, tan_fovx, tan_fovy, mode, s.geom, R, bv.inst_pos, inst_grad,
@@ -534,18 +536,8 @@ int r2x_raster_export(void* stream, int P, int W, int H, long long R, const void
     RasterState s = carve_raster(geom_buf, P, W, H);
     raster_export_geom_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, s.geom, means2D, depths, conic_opacity, mus,
                                                                 tiles_touched, point_offsets);
-    const int tiles = s.geom.gx * s.geom.gy;
-    if (ranges) export_ranges_kernel<<<(tiles + 255) / 256, 256, 0, st>>>(tiles, (const uint2*)al((size_t)image_buf), ranges);
-    if (R > 0 && (keys || point_list)) {
-        BinningView bv = binning_view((void*)binning_buf, R);
-        if (direct_ok(tiles)) {
-            export_keys_ranges_kernel<<<(unsigned)((R + 255) / 256), 256, 0, st>>>(
-                R, s.status, (const uint2*)al((size_t)image_buf), tiles, bv.point_list, s.geom.depth, 1, keys, point_list);
-        } else {
-            const uint32_t* sorted = bv.keys[sort_passes(tiles) & 1];
-            export_keys_kernel<<<(unsigned)((R + 255) / 256), 256, 0, st>>>(R, s.status, sorted, bv.point_list, s.geom.depth, 1, keys, point_list);
-        }
-    }
+    export_binning(st, P, raster_pipeline(W, H), R, binning_buf, image_buf, s.status, s.geom.depth, 1, keys, point_list,
+                   ranges);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -590,13 +582,13 @@ int r2x_voxel_backward(void* stream, int P, long long R, int nx, int ny, int nz,
     if (R > 0 && (!binning_buf || !scratch)) return fail_msg(R2X_ERR_INVALID, "r2x_voxel_backward: null binning/scratch");
     const VoxelGrid vg = make_voxel_grid(nx, ny, nz, sx, sy, sz, cx, cy, cz);
     VoxelState s = carve_voxel(geom_buf, P);
-    const uint2* ranges = (const uint2*)al((size_t)image_buf);
+    const Pipeline pp = voxel_pipeline(nx, ny, nz);
     BinningView bv = binning_view((void*)binning_buf, R);
+    const ImageViews img = image_views(image_buf, P, pp, bv);
     float4* inst_grad = (float4*)al((size_t)scratch);
-    const TilePlan plan = carve_voxel_plan(image_buf, vg.gx * vg.gy * vg.gz, bv);
-    // direct and two-level binning keep no per-instance slot array: the slots are derived (emission_slot())
-    const uint32_t* inst_pos = (direct_ok(vg.gx * vg.gy * vg.gz) || two_level_ok(vg.gx, vg.gy, vg.gz)) ? nullptr : bv.inst_pos;
-    if (R > 0) R2X_TRY(launch_voxel_render_bwd(st, vg, s.geom, ranges, bv.point_list, inst_pos, plan, R, dL_dvol, inst_grad));
+    const uint32_t* inst_pos = pp.path() == BinPath::Radix ? bv.inst_pos : nullptr;   // otherwise slots are derived
+    if (R > 0)
+        R2X_TRY(launch_voxel_render_bwd(st, vg, s.geom, img.ranges, bv.point_list, inst_pos, img.plan, R, dL_dvol, inst_grad));
     R2X_TRY(debug_sync(st, debug, "voxel render backward"));
     R2X_TRY(launch_voxel_gauss_bwd(st, P, radii_x, radii_y, radii_z, scales, scale_modifier, rotations, cov3D_precomp, vg,
                                    s.geom, R, bv.inst_pos, inst_grad, dL_dopacity, dL_dmean3D, dL_dcov3D, dL_dscale,
@@ -614,18 +606,8 @@ int r2x_voxel_export(void* stream, int P, int nx, int ny, int nz, long long R, c
     VoxelState s = carve_voxel(geom_buf, P);
     voxel_export_geom_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, s.geom, means3D_norm, depths, conic_opacity,
                                                                tiles_touched, point_offsets);
-    const size_t tiles = (size_t)((nx + 7) / 8) * ((ny + 7) / 8) * ((nz + 7) / 8);
-    if (ranges) export_ranges_kernel<<<(unsigned)((tiles + 255) / 256), 256, 0, st>>>((int)tiles, (const uint2*)al((size_t)image_buf), ranges);
-    if (R > 0 && (keys || point_list)) {
-        BinningView bv = binning_view((void*)binning_buf, R);
-        if (direct_ok((int)tiles) || two_level_ok((nx + 7) / 8, (ny + 7) / 8, (nz + 7) / 8)) {
-            export_keys_ranges_kernel<<<(unsigned)((R + 255) / 256), 256, 0, st>>>(
-                R, s.status, (const uint2*)al((size_t)image_buf), (int)tiles, bv.point_list, reinterpret_cast<const float*>(s.geom.rec) + 13, 16, keys, point_list);
-        } else {
-            const uint32_t* sorted = bv.keys[sort_passes((int)tiles) & 1];
-            export_keys_kernel<<<(unsigned)((R + 255) / 256), 256, 0, st>>>(R, s.status, sorted, bv.point_list, reinterpret_cast<const float*>(s.geom.rec) + 13, 16, keys, point_list);
-        }
-    }
+    export_binning(st, P, voxel_pipeline(nx, ny, nz), R, binning_buf, image_buf, s.status, voxel_depth(s.geom),
+                   VOX_DEPTH_STRIDE, keys, point_list, ranges);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }

@@ -1,5 +1,4 @@
 // r2x_binning.cu -- see r2x_binning.cuh for the design.
-#include <cstdlib>
 #include "r2x_binning.cuh"
 
 namespace r2x {
@@ -7,16 +6,6 @@ namespace r2x {
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 static size_t plan_items(long long R) { return (size_t)(R > 0 ? R : 1) / PLAN_MIN_CHUNK + 1; }
-
-int plan_chunk_override() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("R2X_CHUNK");
-        v = e ? atoi(e) : 0;
-        if (v < 0) v = 0;
-    }
-    return v;
-}
 
 size_t binning_bytes(long long R) {
     size_t r = (size_t)(R > 0 ? R : 1);
@@ -62,7 +51,7 @@ TilePlan plan_view(void* buf, int num_tiles, const BinningView& bv) {
     pl.extra_item = bv.extra_item;
     pl.partial = bv.partial;
     pl.num_tiles = num_tiles;
-    pl.chunk_override = plan_chunk_override();
+    pl.chunk_override = 0;
     pl.chunk_cap = PLAN_CHUNK;
     pl.max_extra = (long long)plan_items(bv.capacity);
     return pl;
@@ -149,8 +138,9 @@ int launch_plan(cudaStream_t st, const uint2* ranges, const TilePlan& plan) {
     return 0;
 }
 
-int reset_plan_counter(cudaStream_t st, const TilePlan& plan, int which) {
-    R2X_CUDA_OK(cudaMemsetAsync(plan.counter + which, 0, sizeof(uint32_t), st));
+int rewind_plan(cudaStream_t st, const TilePlan& plan) {
+    R2X_CUDA_OK(cudaMemsetAsync(plan.counter, 0, sizeof(uint32_t), st));
+    R2X_CUDA_OK(cudaMemsetAsync(plan.tile_done, 0, sizeof(uint32_t) * PLAN_DONE_SLOTS * (size_t)plan.num_tiles, st));
     return 0;
 }
 
@@ -882,14 +872,20 @@ int launch_direct_fill(cudaStream_t st, int P, const uint16_t* cube, const uint3
     return 0;
 }
 
-int launch_sort_and_ranges(cudaStream_t st, long long R_launch, int num_tiles, const uint32_t* d_total,
-                           const BinningView& bv, uint2* ranges, uint32_t** sorted_keys_out) {
-    R2X_CUDA_OK(cudaMemsetAsync(ranges, 0, sizeof(uint2) * (size_t)num_tiles, st));
-    if (sorted_keys_out) *sorted_keys_out = bv.keys[0];
-    if (R_launch <= 0) return 0;
+// 8-bit passes over the ceil(log2 T) bits of a tile id
+static int sort_passes(int num_tiles) {
     int bits = 1;
     while ((1ll << bits) < (long long)num_tiles) ++bits;
-    const int passes = (bits + 7) / 8;
+    return (bits + 7) / 8;
+}
+
+const uint32_t* sorted_tile_ids(const BinningView& bv, int num_tiles) { return bv.keys[sort_passes(num_tiles) & 1]; }
+
+int launch_sort_and_ranges(cudaStream_t st, long long R_launch, int num_tiles, const uint32_t* d_total,
+                           const BinningView& bv, uint2* ranges) {
+    R2X_CUDA_OK(cudaMemsetAsync(ranges, 0, sizeof(uint2) * (size_t)num_tiles, st));
+    if (R_launch <= 0) return 0;
+    const int passes = sort_passes(num_tiles);
     long long nbl = (R_launch + SORT_CHUNK - 1) / SORT_CHUNK;
     const int nb = (int)(nbl < SORT_MAX_BLOCKS ? nbl : SORT_MAX_BLOCKS);
     int cur = 0;
@@ -910,7 +906,6 @@ int launch_sort_and_ranges(cudaStream_t st, long long R_launch, int num_tiles, c
         R2X_CUDA_OK(cudaGetLastError());
         cur ^= 1;
     }
-    if (sorted_keys_out) *sorted_keys_out = bv.keys[cur];
     long long nbr = (R_launch + 255) / 256;
     int sms;
     R2X_CUDA_OK(sm_count(&sms));

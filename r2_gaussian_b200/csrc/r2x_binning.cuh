@@ -38,9 +38,8 @@ constexpr int SORT_CHUNK = SORT_THREADS * SORT_ITEMS;  // 4096
 constexpr int SORT_MAX_BLOCKS = 264;                   // 2 CTAs per SM on the 132 SMs of an H100 SXM
 
 // ---- work plan for the per-tile kernels -------------------------------------------------------
-// Per-tile lists are cut into chunks of at most C instances (C = the launch's chunk size, 64..PLAN_CHUNK, decided ON
-// THE DEVICE by plan_chunk_for: PLAN_CHUNK unless overridden); a tile of n instances gets ceil(n / C) chunks of EQUAL
-// length (+-1).  A (tile, chunk) pair is one
+// Per-tile lists are cut into chunks of at most C instances (C = the launch's chunk size, decided ON THE DEVICE by
+// plan_chunk_for); a tile of n instances gets ceil(n / C) chunks of EQUAL length (+-1).  A (tile, chunk) pair is one
 // work item of the render kernels, handed out through an atomic counter, so that SM load is balanced no matter how
 // uneven the per-tile counts are.  Items [0,T) are chunk 0 of every tile (also of empty tiles: they write the
 // zeros); items [T, T+E) are the extra chunks, looked up in `extra_item`.  A tile with several chunks combines its
@@ -55,7 +54,7 @@ struct TilePlan {
     uint2* extra_item;    // [R/PLAN_MIN_CHUNK + 1] (tile, chunk >= 1) of extra item j   (binning buffer)
     float* partial;       // [R/PLAN_MIN_CHUNK + 1][512] partial sums of extra chunks      (binning buffer)
     int num_tiles;
-    int chunk_override;   // 0 = automatic (plan_chunk_for); else the chunk size to use (R2X_CHUNK, experiments)
+    int chunk_override;   // 0 = automatic (plan_chunk_for); else the chunk size to use (two-level binning's level 1)
     int chunk_cap;        // largest chunk the consumer kernels take: PLAN_CHUNK (rasterizer: records staged per item),
                           // VOX_CHUNK_CAP (voxelizer: an item is walked in segments of PLAN_CHUNK records)
     long long max_extra;  // entries in extra_item / partial
@@ -74,12 +73,12 @@ __host__ __device__ __forceinline__ uint32_t plan_chunk_for(uint32_t R, int chun
     const uint32_t want = (R / 4096u + (uint32_t)PLAN_CHUNK - 1u) / (uint32_t)PLAN_CHUNK * (uint32_t)PLAN_CHUNK;
     return want < (uint32_t)PLAN_CHUNK ? (uint32_t)PLAN_CHUNK : (want > cap ? cap : want);
 }
-int plan_chunk_override();   // R2X_CHUNK from the environment (0 when unset)
 size_t plan_bytes(int num_tiles);
 struct BinningView;
 TilePlan plan_view(void* image_buf_after_ranges, int num_tiles, const BinningView& bv);
 int launch_plan(cudaStream_t st, const uint2* ranges, const TilePlan& plan);
-int reset_plan_counter(cudaStream_t st, const TilePlan& plan, int which);
+// a forward's plan stays valid for another render of the same lists: rewinds the queue head and the arrival counters
+int rewind_plan(cudaStream_t st, const TilePlan& plan);
 
 // Emission-order slot of instance (Gaussian g, tile (tx,ty,tz)): the instances of a Gaussian are contiguous in emission
 // order, [offsets[g] - n_g, offsets[g]), tiles of its cube row-major (z, y, x).  Direct binning does not materialise
@@ -117,6 +116,14 @@ __device__ __forceinline__ void plan_decode(const TilePlan& pl, const uint2* __r
 size_t binning_bytes(long long R);
 BinningView binning_view(void* buf, long long R);
 
+// ---- which binning a tile grid takes -------------------------------------------------------------
+//   Direct    T <= DIRECT_MAX_TILES: per-CTA tile histograms, no instance list, no sort (below)
+//   TwoLevel  pipelines that have it (the voxelizer), when the supertile grid fits the direct table (r2x_binning2.cu)
+//   Radix     otherwise, or when R2X_VOXEL_BINNING=radix (read per call): emit, stable sort by tile id, ranges
+// Only the radix path materialises inst_pos; the others derive emission slots (emission_slot()).
+enum class BinPath { Direct, TwoLevel, Radix };
+BinPath bin_path(int gx, int gy, int gz, bool has_two_level);
+
 // ---- direct binning (tile counts up to DIRECT_MAX_TILES) ----------------------------------------
 // No instance list is materialised and nothing is sorted.  The preprocess CTA b (256 consecutive
 // Gaussians) histograms its own instances per tile (`block_tile_histogram`, shared memory) into row b of
@@ -138,7 +145,6 @@ struct DirectBin {
 __host__ __device__ __forceinline__ int direct_scan_ctas(int num_tiles) { return (num_tiles + DSCAN_COLS - 1) / DSCAN_COLS; }
 size_t directbin_bytes(int P, int num_tiles);
 DirectBin directbin_view(void* buf, int P, int num_tiles);
-inline bool direct_ok(int num_tiles) { return num_tiles <= DIRECT_MAX_TILES; }
 
 // Called by all 256 threads of a preprocess CTA.  hist_s: shared uint32[T] scratch.  (c01,c23,c45) is
 // the packed tile cube of this thread's Gaussian, n its instance count (0 if culled).
@@ -191,8 +197,7 @@ struct TwoLevel {
     uint32_t* tile_incl;        // [T]    inclusive scan of tile_count in tile-id order
     void* scan_state;
 };
-bool two_level_ok(int gx, int gy, int gz);   // false when the grid fits the direct table, is too large, or R2X_VOXEL_BINNING=radix
-size_t two_level_bytes(int P, int gx, int gy, int gz);
+size_t two_level_bytes(int P, int gx, int gy, int gz);   // 0 unless the grid takes two-level binning by its geometry
 TwoLevel two_level_view(void* buf, int P, int gx, int gy, int gz, const BinningView& bv);
 int launch_two_level(cudaStream_t st, int P, const uint16_t* cube, const uint32_t* tiles_touched, int gx, int gy, int gz,
                      const uint32_t* status, const TwoLevel& tl, const BinningView& bv, uint2* ranges,
@@ -221,7 +226,9 @@ int launch_emit(cudaStream_t st, int P, const uint16_t* cube, const uint32_t* ti
 // Stable sort by tile id + per-tile ranges.  `R_launch` sizes the grids (R itself is read on the device
 // from d_total so that the same launch sequence works when the host does not know R).
 int launch_sort_and_ranges(cudaStream_t st, long long R_launch, int num_tiles, const uint32_t* d_total,
-                           const BinningView& bv, uint2* ranges, uint32_t** sorted_keys_out);
+                           const BinningView& bv, uint2* ranges);
+// the sort's output: tile id per sorted position (keys[0] or keys[1], by the parity of the pass count)
+const uint32_t* sorted_tile_ids(const BinningView& bv, int num_tiles);
 
 // exact 3-NN mean squared distance (r2x_knn.cu)
 size_t knn_scratch_bytes(int P);

@@ -253,7 +253,10 @@ static bool two_level_fits(int gx, int gy, int gz) {
     return T > DIRECT_MAX_TILES && T1 <= DIRECT_MAX_TILES;
 }
 
-bool two_level_ok(int gx, int gy, int gz) { return two_level_fits(gx, gy, gz) && !radix_forced(); }
+BinPath bin_path(int gx, int gy, int gz, bool has_two_level) {
+    if ((long long)gx * gy * gz <= DIRECT_MAX_TILES) return BinPath::Direct;
+    return has_two_level && two_level_fits(gx, gy, gz) && !radix_forced() ? BinPath::TwoLevel : BinPath::Radix;
+}
 
 size_t two_level_bytes(int P, int gx, int gy, int gz) {
     if (!two_level_fits(gx, gy, gz)) return 0;   // sized by the geometry alone, whatever R2X_VOXEL_BINNING says

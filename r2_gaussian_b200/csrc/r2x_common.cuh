@@ -211,15 +211,6 @@ inline cudaError_t pdl_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
-// atomicAdd with release semantics at gpu scope: everything this thread (and, through a preceding warp/CTA
-// barrier, its peers) wrote before is visible to whoever observes the incremented value.  Cheaper than
-// __threadfence() + atomicAdd, and it does not invalidate the SM's L1.
-__device__ __forceinline__ uint32_t atom_add_release_gpu(uint32_t* addr, uint32_t v) {
-    uint32_t old;
-    asm volatile("atom.add.release.gpu.global.u32 %0, [%1], %2;" : "=r"(old) : "l"(addr), "r"(v) : "memory");
-    return old;
-}
-
 // FP32 pairs carried in one 64-bit register pair.  Hopper has no packed FP32 arithmetic, so each operation is two
 // scalar FMUL / FADD / FFMA with the same round-to-nearest, no-flush semantics per lane; pack2 / unpack2 are register
 // renames that the compiler removes.

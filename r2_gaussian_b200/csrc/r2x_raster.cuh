@@ -25,7 +25,7 @@ int launch_raster_render(cudaStream_t st, int W, int H, const RasterGeom& geom, 
                          const uint32_t* point_list, const TilePlan& plan, long long R_launch, float* out_color);
 int launch_raster_render_bwd(cudaStream_t st, int W, int H, const RasterGeom& geom, const uint2* ranges,
                              const uint32_t* point_list, const uint32_t* inst_pos, const TilePlan& plan,
-                             long long R_launch, const float* dL_dpix, float4* inst_grad);
+                             const float* dL_dpix, float4* inst_grad);
 int launch_raster_gauss_bwd(cudaStream_t st, int P, const float* means, const int* radii, const float* scales,
                             float scale_modifier, const float* rots, const float* cov3D_precomp, const float* view,
                             const float* proj, int W, int H, float tan_fovx, float tan_fovy, int mode,
