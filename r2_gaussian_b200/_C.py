@@ -54,24 +54,57 @@ def _require_cuda(t: torch.Tensor, name: str):
         )
 
 
+def _u8(nbytes: int, dev) -> torch.Tensor:
+    return torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
+
+
+class _Kind:
+    """What the rasterizer's and the voxelizer's forward state differ in: the library's size functions, and `seed`,
+    the instances per Gaussian provisioned for a shape that has no capacity hint yet."""
+
+    def __init__(self, name: str, seed: int):
+        self.name, self.seed = name, seed
+
+    def state(self, P: int, grid, dev) -> tuple[torch.Tensor, torch.Tensor]:
+        """(geom, image) buffers of one forward over `grid`: (W, H) for raster, (nx, ny, nz) for voxel."""
+        lib = load()
+        return (_u8(getattr(lib, f"r2x_{self.name}_geom_bytes")(P), dev),
+                _u8(getattr(lib, f"r2x_{self.name}_image_bytes")(P, *grid), dev))
+
+    def bwd_scratch(self, capacity: int, dev) -> torch.Tensor:
+        """Scratch of a backward over a binning buffer carved for `capacity` instances."""
+        return _u8(getattr(load(), f"r2x_{self.name}_bwd_scratch_bytes")(capacity), dev)
+
+
+RASTER, VOXEL = _Kind("raster", 12), _Kind("voxel", 8)
+
+
+def binning_buffer(capacity: int, dev) -> torch.Tensor:
+    """Binning buffer for `capacity` (Gaussian, tile) instances (the same layout for both kinds)."""
+    return _u8(load().r2x_binning_bytes(capacity), dev)
+
+
+def raster_key(dev: torch.device, P: int, W: int, H: int) -> tuple:
+    """Capacity-hint key of a raster shape (`dev` with its index, as a CUDA tensor's device has)."""
+    return ("raster", dev.index, int(P), int(W), int(H))
+
+
+def voxel_key(dev: torch.device, P: int, nx: int, ny: int, nz: int, sVoxel_x: float) -> tuple:
+    """Capacity-hint key of a voxel shape: the instance count depends strongly on the voxel pitch, so it is part of it."""
+    return ("voxel", dev.index, int(P), int(nx), int(ny), int(nz), round(float(sVoxel_x) / int(nx), 6))
+
+
 class _Workspace:
-    """Per-(device, kind, size) instance-capacity hints so that the binning buffer can be provisioned
-    BEFORE the forward runs: the whole pipeline is then enqueued without a host round trip in the middle,
-    and the one synchronisation the reference API needs anyway (num_rendered is a Python int) happens at
-    the end.  If a call needs more instances than provisioned it is simply re-run with a larger buffer.
-    Capacities are rounded to a coarse grid so that torch's caching allocator sees repeating sizes."""
+    """The instance capacity of the binning buffer, decided here for every caller in the package.
+
+    Per-shape hints (keys from `raster_key` / `voxel_key`) let the binning buffer be provisioned BEFORE the forward
+    runs: the whole pipeline is then enqueued without a host round trip in the middle, and the one synchronisation the
+    reference API needs anyway (num_rendered is a Python int) happens at the end.  If a call needs more instances than
+    provisioned it is simply re-run with a larger buffer.  Capacities are rounded to a coarse grid so that torch's
+    caching allocator sees repeating sizes."""
 
     hints: dict = {}
     _pinned: list = []
-
-    @classmethod
-    def pinned_status(cls):
-        return cls._pinned.pop() if cls._pinned else torch.zeros(2, dtype=torch.int32).pin_memory()
-
-    @classmethod
-    def release(cls, t):
-        if len(cls._pinned) < 16:
-            cls._pinned.append(t)
 
     @staticmethod
     def _round(n: int) -> int:
@@ -79,15 +112,45 @@ class _Workspace:
         return (int(n) + step - 1) // step * step
 
     @classmethod
-    def capacity(cls, key, P: int, per_gaussian: int) -> int:
-        return cls.hints.get(key) or cls._round(max(per_gaussian * P, 1 << 14))
+    def first(cls, P: int, seed: int) -> int:
+        """Capacity for a shape without a hint: `seed` instances per Gaussian, at least 16384."""
+        return cls._round(max(seed * P, 1 << 14))
+
+    @classmethod
+    def grown(cls, R: int) -> int:
+        """Capacity for a forward that needed R instances: 20 % headroom plus 1024."""
+        return cls._round(int(R * 1.2) + 1024)
+
+    @classmethod
+    def provision(cls, key, P: int, seed: int, speculative: bool = False) -> int:
+        cap = cls.hints.get(key) or cls.first(P, seed)
+        if speculative:     # generous: an overflow needs the instance count to double between two calls of this shape
+            cap = cls._round(max(2 * cap, seed * P))
+        return cap
 
     @classmethod
     def update(cls, key, R: int):
-        want = cls._round(int(R * 1.2) + 1024)
+        want = cls.grown(R)
         cur = cls.hints.get(key, 0)
         # grow immediately, shrink slowly (keeps sizes stable while the cloud changes during training)
         cls.hints[key] = want if want > cur or want < cur // 2 else cur
+
+    @classmethod
+    def to_host(cls, status: torch.Tensor) -> torch.Tensor:
+        """Start copying the device status word {R, overflow} to pinned host memory (no host wait).  Record an event
+        after this call and `read` the returned tensor once the event has completed."""
+        host = cls._pinned.pop() if cls._pinned else torch.zeros(2, dtype=torch.int32).pin_memory()
+        host.copy_(status, non_blocking=True)
+        return host
+
+    @classmethod
+    def read(cls, host: torch.Tensor, key) -> tuple[int, int]:
+        """-> (R, overflow) of a status word from `to_host`; updates the hint of `key` and returns `host` to the pool."""
+        R, overflow = int(host[0]), int(host[1])
+        cls.update(key, R)
+        if len(cls._pinned) < 16:
+            cls._pinned.append(host)
+        return R, overflow
 
 
 class CapacityOverflow(RuntimeError):
@@ -119,10 +182,8 @@ class NumRendered(int):
             return int(self)
         host, event, key = self.pending
         event.synchronize()
-        R, overflow = int(host[0]), int(host[1])
         self.pending = None
-        _Workspace.update(key, R)
-        _Workspace.release(host)
+        R, overflow = _Workspace.read(host, key)
         if overflow:
             raise CapacityOverflow(f"forward needed {R} instances, binning buffer provisioned for {self.capacity}; "
                                    "the capacity hint has been raised -- repeat the iteration")
@@ -132,15 +193,15 @@ class NumRendered(int):
 class speculative:
     """Context manager used by the autograd bridges in training mode: inside it the forward entry points do NOT
     synchronise with the host (the one sync of the reference API, `num_rendered` being a Python int, is what
-    serialises host and device twice per training iteration).  The binning buffer is provisioned from the instance
-    count of the previous call with the same shape (+20 %), the status word travels to pinned host memory behind an
-    event, and the check happens in the backward.  Disabled by R2X_SPECULATIVE=0, by debug=True, under no_grad, and
-    for the first call of a shape (no hint yet)."""
+    serialises host and device twice per training iteration).  `_forward` provisions the binning buffer from the
+    instance count of the previous call with the same shape (`_Workspace.provision`), the status word travels to pinned
+    host memory behind an event, and the check happens in the backward.  Disabled by R2X_SPECULATIVE=0 (read by
+    `active()` only), by debug=True, under no_grad, and for the first call of a shape (no hint yet)."""
 
     _tls = threading.local()
 
     def __init__(self, on: bool = True):
-        self.on = bool(on) and os.environ.get("R2X_SPECULATIVE", "1") != "0"
+        self.on = bool(on)
 
     def __enter__(self):
         self.prev = getattr(self._tls, "on", False)
@@ -153,26 +214,40 @@ class speculative:
 
     @classmethod
     def active(cls) -> bool:
-        return bool(getattr(cls._tls, "on", False))
+        return bool(getattr(cls._tls, "on", False)) and os.environ.get("R2X_SPECULATIVE", "1") != "0"
+
+
+def _forward(launch, key, P: int, seed: int, dev) -> tuple[NumRendered, torch.Tensor]:
+    """Run one asynchronous forward; `launch(binning, capacity, status)` enqueues it.  -> (NumRendered, binning).
+
+    Inside `speculative`, once the shape has a hint, the call returns at once: the status word travels to pinned host
+    memory behind an event and `NumRendered.resolve()` reads it.  Otherwise the status is read here (the one host
+    synchronisation of the call) and the forward is re-run with the raised hint until it fits."""
+    spec = speculative.active() and key in _Workspace.hints
+    cap = _Workspace.provision(key, P, seed, spec)
+    status = torch.empty(2, dtype=torch.int32, device=dev)
+    while True:
+        binning = binning_buffer(cap, dev)
+        launch(binning, cap, status)
+        if spec:
+            host = _Workspace.to_host(status)
+            event = torch.cuda.Event()
+            event.record(torch.cuda.current_stream(dev))
+            return NumRendered(cap, cap, (host, event, key)), binning
+        R, overflow = status.tolist()
+        _Workspace.update(key, R)
+        if not overflow:
+            return NumRendered(R, cap), binning
+        cap = _Workspace.provision(key, P, seed)
 
 
 def _carved_capacity(binning: torch.Tensor, R) -> int:
-    """Instance count the binning buffer was carved for (what the backward must carve with)."""
+    """Backward prologue: resolve a pending `num_rendered` (raises CapacityOverflow if its speculative forward did not
+    fit), then return the instance count `binning` was carved for, which the backward must carve with.  The count
+    travels with R (`NumRendered.capacity`); the buffer itself is not read."""
+    if getattr(R, "pending", None) is not None:
+        R.resolve()
     return int(getattr(R, "capacity", R))
-
-
-def _pending(status, cap, key, dev) -> NumRendered:
-    """Ship the device status word {R, overflow} to pinned host memory behind an event (no host wait)."""
-    host = _Workspace.pinned_status()
-    host.copy_(status, non_blocking=True)
-    ev = torch.cuda.Event()
-    ev.record(torch.cuda.current_stream(dev))
-    return NumRendered(cap, cap, (host, ev, key))
-
-
-def _status_pair(dev):
-    st = torch.empty(2, dtype=torch.int32, device=dev)
-    return st
 
 
 def rasterize_gaussians(means3D, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
@@ -192,13 +267,9 @@ def rasterize_gaussians(means3D, opacity, scales, rotations, scale_modifier, cov
         means3D = _f32(means3D, dev); opacity = _f32(opacity, dev)
         scales = _f32(scales, dev); rotations = _f32(rotations, dev); cov3D_precomp = _f32(cov3D_precomp, dev)
         viewmatrix = _f32(viewmatrix, dev); projmatrix = _f32(projmatrix, dev); campos = _f32(campos, dev)
-        u8 = dict(dtype=torch.uint8, device=dev)
         out_color = torch.empty((1, H, W), dtype=torch.float32, device=dev)
         radii = torch.empty((P,), dtype=torch.int32, device=dev)
-        geom = torch.empty(lib.r2x_raster_geom_bytes(P), **u8)
-        img = torch.empty(lib.r2x_raster_image_bytes(P, W, H), **u8)
-        status = _status_pair(dev)
-        key = ("raster", dev.index, P, W, H)
+        geom, img = RASTER.state(P, (W, H), dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
         if debug or P == 0:
             alloc = _BinningAlloc(dev)
@@ -210,26 +281,17 @@ def rasterize_gaussians(means3D, opacity, scales, rotations, scale_modifier, cov
                 alloc.cb, None, int(bool(debug)), C.byref(nr))
             check(rc, "r2x_raster_forward")
             return NumRendered(nr.value), out_color, radii, geom, alloc.tensor, img
-        cap = _Workspace.capacity(key, P, 12)
-        spec = speculative.active() and key in _Workspace.hints
-        if spec:    # generous: an overflow needs the instance count to double between two calls of this shape
-            cap = _Workspace._round(max(2 * cap, 12 * P))
-        while True:
-            binning = torch.empty(lib.r2x_binning_bytes(cap), **u8)
+
+        def launch(binning, cap, status):
             rc = lib.r2x_raster_forward_async(
                 stream, P, W, H, _ptr(means3D), _ptr(opacity), _ptr(scales), float(scale_modifier), _ptr(rotations),
                 _ptr(cov3D_precomp), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), float(tan_fovx), float(tan_fovy),
                 int(bool(prefiltered)), int(mode), out_color.data_ptr(), _ptr(radii), geom.data_ptr(), img.data_ptr(),
                 binning.data_ptr(), cap, status.data_ptr())
             check(rc, "r2x_raster_forward_async")
-            if spec:
-                return (_pending(status, cap, key, dev), out_color, radii, geom, binning, img)
-            R, overflow = status.tolist()      # the one host synchronisation of the call
-            _Workspace.update(key, R)
-            if not overflow:
-                break
-            cap = _Workspace.capacity(key, P, 12)
-    return NumRendered(R, cap), out_color, radii, geom, binning, img
+
+        R, binning = _forward(launch, raster_key(dev, P, W, H), P, RASTER.seed, dev)
+    return R, out_color, radii, geom, binning, img
 
 
 class _BinningAlloc:
@@ -263,12 +325,10 @@ def rasterize_gaussians_backward(means3D, radii, scales, rotations, scale_modifi
         g_mean2D = torch.empty((P, 3), **opts); g_op = torch.empty((P, 1), **opts); g_mu = torch.empty((P, 1), **opts)
         g_mean3D = torch.empty((P, 3), **opts); g_cov = torch.empty((P, 6), **opts)
         g_scale = torch.empty((P, 3), **opts); g_rot = torch.empty((P, 4), **opts)
-        if getattr(R, "pending", None) is not None:
-            R.resolve()                         # raises CapacityOverflow if the speculative forward did not fit
         R = _carved_capacity(binningBuffer, R)
-        scratch = torch.empty(lib.r2x_raster_bwd_scratch_bytes(int(R)), dtype=torch.uint8, device=dev)
+        scratch = RASTER.bwd_scratch(R, dev)
         rc = lib.r2x_raster_backward(
-            torch.cuda.current_stream(dev).cuda_stream, P, int(R), W, H, _ptr(means3D), _ptr(scales),
+            torch.cuda.current_stream(dev).cuda_stream, P, R, W, H, _ptr(means3D), _ptr(scales),
             float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(viewmatrix), _ptr(projmatrix),
             _ptr(campos), float(tan_fovx), float(tan_fovy), _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer),
             _ptr(imageBuffer), scratch.data_ptr(), _ptr(dL), _ptr(g_mean2D), _ptr(g_op), _ptr(g_mu),
@@ -305,12 +365,10 @@ def voxelize_gaussians(means3D, opacity, scales, rotations, scale_modifier, cov3
     with torch.cuda.device(dev):
         means3D = _f32(means3D, dev); opacity = _f32(opacity, dev)
         scales = _f32(scales, dev); rotations = _f32(rotations, dev); cov3D_precomp = _f32(cov3D_precomp, dev)
-        u8 = dict(dtype=torch.uint8, device=dev)
         vol = torch.empty((nx, ny, nz), dtype=torch.float32, device=dev)
         rx = torch.empty((P,), dtype=torch.int32, device=dev)
         ry = torch.empty_like(rx); rz = torch.empty_like(rx)
-        geom = torch.empty(lib.r2x_voxel_geom_bytes(P), **u8)
-        img = torch.empty(lib.r2x_voxel_image_bytes(P, nx, ny, nz), **u8)
+        geom, img = VOXEL.state(P, (nx, ny, nz), dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
         grid_args = (nx, ny, nz, float(sVoxel_x), float(sVoxel_y), float(sVoxel_z), float(center_x), float(center_y),
                      float(center_z))
@@ -323,27 +381,15 @@ def voxelize_gaussians(means3D, opacity, scales, rotations, scale_modifier, cov3
                                        geom.data_ptr(), img.data_ptr(), alloc.cb, None, int(bool(debug)), C.byref(nr))
             check(rc, "r2x_voxel_forward")
             return NumRendered(nr.value), vol, rx, ry, rz, geom, alloc.tensor, img
-        # the instance count depends strongly on the voxel pitch: key the hint on the grid as well
-        key = ("voxel", dev.index, P, nx, ny, nz, round(float(sVoxel_x) / nx, 6))
-        status = _status_pair(dev)
-        cap = _Workspace.capacity(key, P, 8)
-        spec = speculative.active() and key in _Workspace.hints
-        if spec:    # (random TV crops see very different instance counts: keep at least 8 per Gaussian)
-            cap = _Workspace._round(max(2 * cap, 8 * P))
-        while True:
-            binning = torch.empty(lib.r2x_binning_bytes(cap), **u8)
+
+        def launch(binning, cap, status):
             rc = lib.r2x_voxel_forward_async(stream, P, *grid_args, *in_args, vol.data_ptr(), _ptr(rx), _ptr(ry),
                                              _ptr(rz), geom.data_ptr(), img.data_ptr(), binning.data_ptr(), cap,
                                              status.data_ptr())
             check(rc, "r2x_voxel_forward_async")
-            if spec:
-                return (_pending(status, cap, key, dev), vol, rx, ry, rz, geom, binning, img)
-            R, overflow = status.tolist()
-            _Workspace.update(key, R)
-            if not overflow:
-                break
-            cap = _Workspace.capacity(key, P, 8)
-    return NumRendered(R, cap), vol, rx, ry, rz, geom, binning, img
+
+        R, binning = _forward(launch, voxel_key(dev, P, nx, ny, nz, sVoxel_x), P, VOXEL.seed, dev)
+    return R, vol, rx, ry, rz, geom, binning, img
 
 
 def voxelize_gaussians_backward(means3D, radii_x, radii_y, radii_z, scales, rotations, scale_modifier,
@@ -361,12 +407,10 @@ def voxelize_gaussians_backward(means3D, radii_x, radii_y, radii_z, scales, rota
         opts = dict(dtype=torch.float32, device=dev)
         g_op = torch.empty((P, 1), **opts); g_mean = torch.empty((P, 3), **opts); g_cov = torch.empty((P, 6), **opts)
         g_scale = torch.empty((P, 3), **opts); g_rot = torch.empty((P, 4), **opts)
-        if getattr(R, "pending", None) is not None:
-            R.resolve()
         R = _carved_capacity(binningBuffer, R)
-        scratch = torch.empty(lib.r2x_voxel_bwd_scratch_bytes(int(R)), dtype=torch.uint8, device=dev)
+        scratch = VOXEL.bwd_scratch(R, dev)
         rc = lib.r2x_voxel_backward(
-            torch.cuda.current_stream(dev).cuda_stream, P, int(R), int(nVoxel_x), int(nVoxel_y), int(nVoxel_z),
+            torch.cuda.current_stream(dev).cuda_stream, P, R, int(nVoxel_x), int(nVoxel_y), int(nVoxel_z),
             float(sVoxel_x), float(sVoxel_y), float(sVoxel_z), float(center_x), float(center_y), float(center_z),
             _ptr(means3D), _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(radii_x),
             _ptr(radii_y), _ptr(radii_z), _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imageBuffer),

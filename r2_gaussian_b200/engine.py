@@ -11,6 +11,7 @@ from __future__ import annotations
 
 import torch
 
+from . import _C
 from ._lib import check, load
 
 
@@ -18,27 +19,55 @@ def _ptr(t):
     return None if t is None or t.numel() == 0 else t.data_ptr()
 
 
-class RasterEngine:
-    """Forward X-ray projector for a fixed (P, W, H) with preallocated state."""
+class _Engine:
+    """State kept across calls and the capacity check shared by both engines; capacities follow `_C._Workspace`."""
 
-    def __init__(self, P: int, W: int, H: int, device="cuda", capacity: int | None = None):
+    def __init__(self, kind, P: int, grid, device, capacity: int | None):
         self.lib = load()
-        self.P, self.W, self.H = int(P), int(W), int(H)
+        self.P = int(P)
         self.device = torch.device(device)
         with torch.cuda.device(self.device):
-            u8 = dict(dtype=torch.uint8, device=self.device)
-            self.geom = torch.empty(self.lib.r2x_raster_geom_bytes(self.P), **u8)
-            self.img = torch.empty(self.lib.r2x_raster_image_bytes(self.P, self.W, self.H), **u8)
-            self.radii = torch.empty(self.P, dtype=torch.int32, device=self.device)
-            self.out = torch.empty((1, self.H, self.W), dtype=torch.float32, device=self.device)
+            self.geom, self.img = kind.state(self.P, grid, self.device)
             self.status = torch.zeros(2, dtype=torch.int32, device=self.device)
-            self.capacity = 0
-            self.binning = None
-            self._reserve(capacity if capacity is not None else max(16 * self.P, 1 << 16))
+            self._reserve(capacity if capacity is not None else _C._Workspace.first(self.P, kind.seed))
 
     def _reserve(self, capacity: int):
         self.capacity = int(capacity)
-        self.binning = torch.empty(self.lib.r2x_binning_bytes(self.capacity), dtype=torch.uint8, device=self.device)
+        self.binning = _C.binning_buffer(self.capacity, self.device)
+
+    def grow(self, R: int):
+        """Re-provision the binning buffer for a forward that needed R instances."""
+        self._reserve(_C._Workspace.grown(R))
+
+    def num_rendered(self) -> int:
+        """Synchronises; instance count of the last forward."""
+        return int(self.status.cpu()[0].item())
+
+    def check(self) -> bool:
+        """Synchronises; True if the last forward fitted the capacity, else grows it (caller re-runs)."""
+        R, ov = (int(v) for v in self.status.cpu().tolist())
+        if ov:
+            self.grow(R)
+            return False
+        return True
+
+    def fit(self, *fwd_args, **fwd_kw):
+        """Run forward until it fits.  Returns R."""
+        while True:
+            self.forward(*fwd_args, **fwd_kw)
+            if self.check():
+                break
+        return self.num_rendered()
+
+
+class RasterEngine(_Engine):
+    """Forward X-ray projector for a fixed (P, W, H) with preallocated state."""
+
+    def __init__(self, P: int, W: int, H: int, device="cuda", capacity: int | None = None):
+        self.W, self.H = int(W), int(H)
+        super().__init__(_C.RASTER, P, (self.W, self.H), device, capacity)
+        self.radii = torch.empty(self.P, dtype=torch.int32, device=self.device)
+        self.out = torch.empty((1, self.H, self.W), dtype=torch.float32, device=self.device)
 
     def forward(self, means, dens, scales, rots, viewmatrix, projmatrix, campos, tanfovx, tanfovy, mode,
                 scale_modifier: float = 1.0, cov3D_precomp=None, out=None):
@@ -61,50 +90,15 @@ class RasterEngine:
         check(rc, "r2x_raster_render_only")
         return out
 
-    def num_rendered(self) -> int:
-        """Synchronises; instance count of the last forward."""
-        return int(self.status.cpu()[0].item())
 
-    def check(self) -> bool:
-        """Synchronises; True if the last forward fitted the capacity, else grows it (caller re-runs)."""
-        R, ov = (int(v) for v in self.status.cpu().tolist())
-        if ov:
-            self._reserve(int(R * 1.25) + 1024)
-            return False
-        return True
-
-    def fit(self, *fwd_args, **fwd_kw):
-        """Run forward until it fits, then trim the capacity to 1.25x the need.  Returns R."""
-        while True:
-            self.forward(*fwd_args, **fwd_kw)
-            if self.check():
-                break
-        R = self.num_rendered()
-        return R
-
-
-class VoxelEngine:
+class VoxelEngine(_Engine):
     """Forward density-volume query for a fixed (P, grid) with preallocated state."""
 
     def __init__(self, P: int, nVoxel, device="cuda", capacity: int | None = None):
-        self.lib = load()
-        self.P = int(P)
         self.nx, self.ny, self.nz = (int(v) for v in nVoxel)
-        self.device = torch.device(device)
-        with torch.cuda.device(self.device):
-            u8 = dict(dtype=torch.uint8, device=self.device)
-            self.geom = torch.empty(self.lib.r2x_voxel_geom_bytes(self.P), **u8)
-            self.img = torch.empty(self.lib.r2x_voxel_image_bytes(self.P, self.nx, self.ny, self.nz), **u8)
-            self.radii = torch.empty((3, self.P), dtype=torch.int32, device=self.device)
-            self.out = torch.empty((self.nx, self.ny, self.nz), dtype=torch.float32, device=self.device)
-            self.status = torch.zeros(2, dtype=torch.int32, device=self.device)
-            self.capacity = 0
-            self.binning = None
-            self._reserve(capacity if capacity is not None else max(32 * self.P, 1 << 16))
-
-    def _reserve(self, capacity: int):
-        self.capacity = int(capacity)
-        self.binning = torch.empty(self.lib.r2x_binning_bytes(self.capacity), dtype=torch.uint8, device=self.device)
+        super().__init__(_C.VOXEL, P, (self.nx, self.ny, self.nz), device, capacity)
+        self.radii = torch.empty((3, self.P), dtype=torch.int32, device=self.device)
+        self.out = torch.empty((self.nx, self.ny, self.nz), dtype=torch.float32, device=self.device)
 
     def forward(self, means, dens, scales, rots, sVoxel, center, scale_modifier: float = 1.0, cov3D_precomp=None,
                 out=None):
@@ -125,23 +119,6 @@ class VoxelEngine:
                                             self.img.data_ptr(), out.data_ptr())
         check(rc, "r2x_voxel_render_only")
         return out
-
-    def num_rendered(self) -> int:
-        return int(self.status.cpu()[0].item())
-
-    def check(self) -> bool:
-        R, ov = (int(v) for v in self.status.cpu().tolist())
-        if ov:
-            self._reserve(int(R * 1.25) + 1024)
-            return False
-        return True
-
-    def fit(self, *fwd_args, **fwd_kw):
-        while True:
-            self.forward(*fwd_args, **fwd_kw)
-            if self.check():
-                break
-        return self.num_rendered()
 
 
 class HostProjector:
@@ -209,7 +186,7 @@ class HostProjector:
         self.e_out[k].synchronize()
         if int(self.h_status[k][1]) != 0:              # capacity overflow: grow and redo this request, in order
             torch.cuda.synchronize(self.device)
-            self.engine._reserve(int(int(self.h_status[k][0]) * 1.25) + 1024)
+            self.engine.grow(int(self.h_status[k][0]))
             t = self.submit(*req)
             return self.wait(t)
         return req[-1]

@@ -33,27 +33,6 @@ def _act(params) -> ActivationDesc:
     return a
 
 
-def _forward_loop(run, key, P, per_gaussian, dev, training):
-    """Provision the binning buffer, run the forward; training: speculative (capacity resolved in the backward),
-    otherwise synchronise and grow on overflow.  Returns (NumRendered, binning)."""
-    lib = load()
-    cap = _C._Workspace.capacity(key, P, per_gaussian)
-    spec = training and key in _C._Workspace.hints and os.environ.get("R2X_SPECULATIVE", "1") != "0"
-    if spec:
-        cap = _C._Workspace._round(max(2 * cap, per_gaussian * P))
-    status = torch.empty(2, dtype=torch.int32, device=dev)
-    while True:
-        binning = torch.empty(lib.r2x_binning_bytes(cap), dtype=torch.uint8, device=dev)
-        run(binning, cap, status)
-        if spec:
-            return _C._pending(status, cap, key, dev), binning
-        R, overflow = status.tolist()
-        _C._Workspace.update(key, R)
-        if not overflow:
-            return _C.NumRendered(R, cap), binning
-        cap = _C._Workspace.capacity(key, P, per_gaussian)
-
-
 class _RasterizeRaw(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, raw_density, raw_scales, raw_rotations, settings, act):
@@ -64,12 +43,10 @@ class _RasterizeRaw(torch.autograd.Function):
         f = lambda t: _C._f32(t, dev)
         means3D, raw_density, raw_scales, raw_rotations = f(means3D), f(raw_density), f(raw_scales), f(raw_rotations)
         view, proj, campos = f(s.viewmatrix), f(s.projmatrix), f(s.campos)
-        with torch.cuda.device(dev):
-            u8 = dict(dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev), _C.speculative(any(ctx.needs_input_grad)):
             color = torch.empty((1, H, W), dtype=torch.float32, device=dev)
             radii = torch.empty((P,), dtype=torch.int32, device=dev)
-            geom = torch.empty(lib.r2x_raster_geom_bytes(P), **u8)
-            img = torch.empty(lib.r2x_raster_image_bytes(P, W, H), **u8)
+            geom, img = _C.RASTER.state(P, (W, H), dev)
             stream = torch.cuda.current_stream(dev).cuda_stream
 
             def run(binning, cap, status):
@@ -80,7 +57,7 @@ class _RasterizeRaw(torch.autograd.Function):
                     status.data_ptr(), C.byref(act))
                 check(rc, "r2x_raster_forward_async_raw")
 
-            R, binning = _forward_loop(run, ("raster", dev.index, P, W, H), P, 12, dev, any(ctx.needs_input_grad))
+            R, binning = _C._forward(run, _C.raster_key(dev, P, W, H), P, _C.RASTER.seed, dev)
         ctx.settings, ctx.act, ctx.num_rendered = s, act, R
         ctx.save_for_backward(means3D, raw_scales, raw_rotations, radii, geom, binning, img, view, proj, campos)
         ctx.mark_non_differentiable(radii)
@@ -91,8 +68,6 @@ class _RasterizeRaw(torch.autograd.Function):
         lib = load()
         s, act, R = ctx.settings, ctx.act, ctx.num_rendered
         means3D, raw_scales, raw_rotations, radii, geom, binning, img, view, proj, campos = ctx.saved_tensors
-        if getattr(R, "pending", None) is not None:
-            R.resolve()
         cap = _C._carved_capacity(binning, R)
         dev = means3D.device
         P, H, W = int(means3D.shape[0]), int(s.image_height), int(s.image_width)
@@ -100,7 +75,7 @@ class _RasterizeRaw(torch.autograd.Function):
             opts = dict(dtype=torch.float32, device=dev)
             g2 = torch.empty((P, 3), **opts); gd = torch.empty((P, 1), **opts); g3 = torch.empty((P, 3), **opts)
             gcov = torch.empty((P, 6), **opts); gs = torch.empty((P, 3), **opts); gr = torch.empty((P, 4), **opts)
-            scratch = torch.empty(lib.r2x_raster_bwd_scratch_bytes(cap), dtype=torch.uint8, device=dev)
+            scratch = _C.RASTER.bwd_scratch(cap, dev)
             dL = _C._f32(grad_color, dev)
             rc = lib.r2x_raster_backward_raw(
                 torch.cuda.current_stream(dev).cuda_stream, P, cap, W, H, _C._ptr(means3D), _C._ptr(raw_scales),
@@ -124,12 +99,10 @@ class _VoxelizeRaw(torch.autograd.Function):
         means3D, raw_density, raw_scales, raw_rotations = f(means3D), f(raw_density), f(raw_scales), f(raw_rotations)
         grid = (nx, ny, nz, float(s.sVoxel_x), float(s.sVoxel_y), float(s.sVoxel_z), float(s.center_x), float(s.center_y),
                 float(s.center_z))
-        with torch.cuda.device(dev):
-            u8 = dict(dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev), _C.speculative(any(ctx.needs_input_grad)):
             vol = torch.empty((nx, ny, nz), dtype=torch.float32, device=dev)
             rx = torch.empty((P,), dtype=torch.int32, device=dev); ry = torch.empty_like(rx); rz = torch.empty_like(rx)
-            geom = torch.empty(lib.r2x_voxel_geom_bytes(P), **u8)
-            img = torch.empty(lib.r2x_voxel_image_bytes(P, nx, ny, nz), **u8)
+            geom, img = _C.VOXEL.state(P, (nx, ny, nz), dev)
             stream = torch.cuda.current_stream(dev).cuda_stream
 
             def run(binning, cap, status):
@@ -139,8 +112,7 @@ class _VoxelizeRaw(torch.autograd.Function):
                     img.data_ptr(), binning.data_ptr(), cap, status.data_ptr(), C.byref(act))
                 check(rc, "r2x_voxel_forward_async_raw")
 
-            key = ("voxel", dev.index, P, nx, ny, nz, round(float(s.sVoxel_x) / nx, 6))
-            R, binning = _forward_loop(run, key, P, 8, dev, any(ctx.needs_input_grad))
+            R, binning = _C._forward(run, _C.voxel_key(dev, P, nx, ny, nz, s.sVoxel_x), P, _C.VOXEL.seed, dev)
         ctx.settings, ctx.act, ctx.num_rendered, ctx.grid = s, act, R, grid
         ctx.save_for_backward(means3D, raw_scales, raw_rotations, rx, ry, rz, geom, binning, img)
         return vol, (rx, ry, rz)
@@ -150,8 +122,6 @@ class _VoxelizeRaw(torch.autograd.Function):
         lib = load()
         s, act, R, grid = ctx.settings, ctx.act, ctx.num_rendered, ctx.grid
         means3D, raw_scales, raw_rotations, rx, ry, rz, geom, binning, img = ctx.saved_tensors
-        if getattr(R, "pending", None) is not None:
-            R.resolve()
         cap = _C._carved_capacity(binning, R)
         dev = means3D.device
         P = int(means3D.shape[0])
@@ -159,7 +129,7 @@ class _VoxelizeRaw(torch.autograd.Function):
             opts = dict(dtype=torch.float32, device=dev)
             gd = torch.empty((P, 1), **opts); g3 = torch.empty((P, 3), **opts); gcov = torch.empty((P, 6), **opts)
             gs = torch.empty((P, 3), **opts); gr = torch.empty((P, 4), **opts)
-            scratch = torch.empty(lib.r2x_voxel_bwd_scratch_bytes(cap), dtype=torch.uint8, device=dev)
+            scratch = _C.VOXEL.bwd_scratch(cap, dev)
             dL = _C._f32(grad_vol, dev)
             rc = lib.r2x_voxel_backward_raw(
                 torch.cuda.current_stream(dev).cuda_stream, P, cap, *grid, _C._ptr(means3D), _C._ptr(raw_scales),

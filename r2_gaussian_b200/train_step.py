@@ -15,9 +15,10 @@ issues the same kernels directly:
     Adam on the four parameter tensors   r2x_adam_step_sum  (gradient = raster part + voxel part)
 
 No autograd graph, no per-iteration allocation, no host synchronisation: both forwards are speculative (instance
-capacity provisioned from the previous call of the same shape, `_C._Workspace`), and the statistics / Adam launches
+capacity from `_C._Workspace.provision`, after the previous call of the same shape), and the statistics / Adam launches
 are GUARDED by the forwards' overflow flags on the device, so an overflowed iteration changes nothing; the host reads
-the flags one iteration late (`check()`), raises the capacity and repeats that iteration.
+the flags one iteration late (`check()`, through `_C._Workspace.read`, which raises the hint) and repeats that
+iteration.
 
 The model's tensors are updated in place: `GaussianModel._xyz/_density/_scaling/_rotation`, the `FusedAdam` state of
 `gaussians.optimizer` (same `exp_avg`, `exp_avg_sq`, `step`, so checkpoints and the densification surgery are
@@ -76,10 +77,9 @@ class NativeTrainStep:
             self.image = self.image_ext[:H * W].view(1, H, W)
             self.flag_r = self.image_ext[H * W:H * W + 1]
             self.radii = torch.empty((P,), **i32)
-            self.geom = torch.empty(lib.r2x_raster_geom_bytes(P), **u8)
-            self.img = torch.empty(lib.r2x_raster_image_bytes(P, W, H), **u8)
+            self.geom, self.img = _C.RASTER.state(P, (W, H), dev)
             self.status_r = torch.zeros(2, **i32)
-            self.key_r = ("raster", dev.index, P, W, H)
+            self.key_r = _C.raster_key(dev, P, W, H)
             self.g2 = torch.empty((P, 3), **f32); self.gd = torch.empty((P, 1), **f32); self.g3 = torch.empty((P, 3), **f32)
             self.gcov = torch.empty((P, 6), **f32); self.gs = torch.empty((P, 3), **f32); self.gr = torch.empty((P, 4), **f32)
             # image loss
@@ -94,10 +94,9 @@ class NativeTrainStep:
                 self.vol = self.vol_ext[:nx * ny * nz].view(nx, ny, nz)
                 self.flag_v = self.vol_ext[nx * ny * nz:nx * ny * nz + 1]
                 self.rx = torch.empty((P,), **i32); self.ry = torch.empty((P,), **i32); self.rz = torch.empty((P,), **i32)
-                self.geom_v = torch.empty(lib.r2x_voxel_geom_bytes(P), **u8)
-                self.img_v = torch.empty(lib.r2x_voxel_image_bytes(P, nx, ny, nz), **u8)
+                self.geom_v, self.img_v = _C.VOXEL.state(P, self.tv_n, dev)
                 self.status_v = torch.zeros(2, **i32)
-                self.key_v = ("voxel", dev.index, P, nx, ny, nz, round(self.tv_s[0] / nx, 6))
+                self.key_v = _C.voxel_key(dev, P, nx, ny, nz, self.tv_s[0])
                 self.tv_scratch_bytes = int(lib.r2x_tv3d_scratch_bytes(nx, ny, nz))
                 self.tv_scratch = torch.empty(self.tv_scratch_bytes, **u8)
                 self.tv_out = torch.zeros(1, **f32)
@@ -137,20 +136,17 @@ class NativeTrainStep:
         self._bound = self._signature(H, W)
 
     def _provision(self):
-        """Instance capacities for this iteration (generous: an overflow needs the count to double between two calls)."""
-        lib, dev = self.lib, self.dev
-        W_ = _C._Workspace
-        want_r = W_._round(max(2 * W_.capacity(self.key_r, self.P, 12), 12 * self.P))
+        """Instance capacities for this iteration: both forwards are speculative.  The buffers only ever grow."""
+        dev = self.dev
+        want_r = _C._Workspace.provision(self.key_r, self.P, _C.RASTER.seed, speculative=True)
         if want_r > self.cap_r:
             self.cap_r = want_r
-            self.binning_r = torch.empty(lib.r2x_binning_bytes(want_r), dtype=torch.uint8, device=dev)
-            self.scratch_r = torch.empty(lib.r2x_raster_bwd_scratch_bytes(want_r), dtype=torch.uint8, device=dev)
+            self.binning_r, self.scratch_r = _C.binning_buffer(want_r, dev), _C.RASTER.bwd_scratch(want_r, dev)
         if self.use_tv:
-            want_v = W_._round(max(2 * W_.capacity(self.key_v, self.P, 8), 8 * self.P))
+            want_v = _C._Workspace.provision(self.key_v, self.P, _C.VOXEL.seed, speculative=True)
             if want_v > self.cap_v:
                 self.cap_v = want_v
-                self.binning_v = torch.empty(lib.r2x_binning_bytes(want_v), dtype=torch.uint8, device=dev)
-                self.scratch_v = torch.empty(lib.r2x_voxel_bwd_scratch_bytes(want_v), dtype=torch.uint8, device=dev)
+                self.binning_v, self.scratch_v = _C.binning_buffer(want_v, dev), _C.VOXEL.bwd_scratch(want_v, dev)
 
     # ------------------------------------------------------------------ one iteration
     def __call__(self, cam, gt, tv_centre=None, apply_update: bool = True):
@@ -247,10 +243,7 @@ class NativeTrainStep:
                                             float(b2), float(self.adam[0][0]["eps"]), steps.pop(), self.status_r.data_ptr(),
                                             guard_v), "r2x_adam_step_sum")
             # the status words travel to pinned host memory behind an event; read one iteration late
-            host = _C._Workspace.pinned_status(), (_C._Workspace.pinned_status() if self.use_tv else None)
-            host[0].copy_(self.status_r, non_blocking=True)
-            if self.use_tv:
-                host[1].copy_(self.status_v, non_blocking=True)
+            host = _C._Workspace.to_host(self.status_r), (_C._Workspace.to_host(self.status_v) if self.use_tv else None)
             ev = torch.cuda.Event()
             ev.record(torch.cuda.current_stream(dev))
         self._pending = (host, ev, (cam, gt, tv_centre, apply_update))
@@ -270,14 +263,8 @@ class NativeTrainStep:
         host, ev, args = self._pending
         self._pending = None
         ev.synchronize()
-        Rr, ov_r = int(host[0][0]), int(host[0][1])
-        _C._Workspace.update(self.key_r, Rr)
-        _C._Workspace.release(host[0])
-        ov_v = 0
-        if self.use_tv:
-            Rv, ov_v = int(host[1][0]), int(host[1][1])
-            _C._Workspace.update(self.key_v, Rv)
-            _C._Workspace.release(host[1])
+        ov_r = _C._Workspace.read(host[0], self.key_r)[1]
+        ov_v = _C._Workspace.read(host[1], self.key_v)[1] if self.use_tv else 0
         if ov_r or ov_v:
             self.repeats += 1
             if self.repeats > 8:

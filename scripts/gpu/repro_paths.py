@@ -9,7 +9,7 @@ from r2_gaussian_b200 import scene, _C
 
 def voxel(P, nV, kind="trained", bwd=True, hint=None):
     cloud = scene.make_cloud(P, kind=kind, seed=3)
-    key = ("voxel", 0, P, *nV, round(2.0 / nV[0], 6))
+    key = _C.voxel_key(torch.device("cuda", 0), P, *nV, 2.0)
     if hint is not None:
         _C._Workspace.hints[key] = hint          # force a capacity overflow on the first attempt
     f = util.ours_voxel_forward(cloud, nV, (2.0, 2.0, 2.0), (0.0, 0.0, 0.0))
@@ -26,7 +26,7 @@ def voxel(P, nV, kind="trained", bwd=True, hint=None):
 def raster(P, n, kind="trained", hint=None):
     cloud = scene.make_cloud(P, kind=kind, seed=4)
     view = scene.make_view(scene.cone_beam_scanner(n, 64), 0.7)
-    key = ("raster", 0, P, n, n)
+    key = _C.raster_key(torch.device("cuda", 0), P, n, n)
     if hint is not None:
         _C._Workspace.hints[key] = hint
     f = util.ours_raster_forward(cloud, view)
@@ -45,7 +45,7 @@ raster(1500, 1040)                           # 4225 tiles: radix path
 raster(1500, 1040, hint=4096)                # radix path, overflow then re-run
 voxel(1500, (32, 32, 32))
 voxel(1500, (32, 32, 32), hint=4096)
-voxel(1200, (144, 136, 136))                 # 5202 tiles: radix path
+voxel(1200, (144, 136, 136))                 # 5202 tiles, 125 supertiles: two-level binning
 voxel(1200, (144, 136, 136), hint=4096)
 voxel(20000, (96, 96, 96), kind="init")      # 1728 tiles, many instances per tile (multi-chunk tiles)
 print("ALL OK")

@@ -197,7 +197,7 @@ def test_speculative_training_forward_defers_the_capacity_check():
         img, radii = GaussianRasterizer(s)(t["means"], m2, t["dens"], t["scales"], t["rots"])
         return t, img
 
-    key = ("raster", 0, cloud.P, view.image_width, view.image_height)
+    key = _C.raster_key(torch.device("cuda", 0), cloud.P, view.image_width, view.image_height)
     _C._Workspace.hints.pop(key, None)
     t1, img1 = run(cloud)                          # first call of the shape: synchronous, sets the hint
     assert key in _C._Workspace.hints
