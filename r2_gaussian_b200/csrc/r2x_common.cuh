@@ -48,15 +48,17 @@ __device__ __forceinline__ float act_scale_grad(const Activation& a, float x) { 
     const float sg = act_sigmoid(x);
     return (a.hi - a.lo) * sg * (1.0f - sg);
 }
+// norm receives the unclamped |q|
 __device__ __forceinline__ float4 act_normalize(float4 q, float& norm) {
-    norm = fmaxf(sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w), 1e-12f);
-    const float inv = 1.0f / norm;
+    norm = sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
+    const float inv = 1.0f / fmaxf(norm, 1e-12f);
     return make_float4(q.x * inv, q.y * inv, q.z * inv, q.w * inv);
 }
-// gradient of q_hat = q / |q| pulled back to q:  (dq_hat - q_hat (q_hat . dq_hat)) / |q|
+// gradient of q_hat = q / max(|q|, 1e-12) pulled back to q:  (dq_hat - q_hat (q_hat . dq_hat)) / |q|; below the clamp
+// the denominator is a constant (torch's clamp_min passes no gradient to |q|), so the gradient is dq_hat / 1e-12
 __device__ __forceinline__ void act_normalize_grad(float4 qn, float norm, float* dr) {
-    const float dot = qn.x * dr[0] + qn.y * dr[1] + qn.z * dr[2] + qn.w * dr[3];
-    const float inv = 1.0f / norm;
+    const float dot = norm >= 1e-12f ? qn.x * dr[0] + qn.y * dr[1] + qn.z * dr[2] + qn.w * dr[3] : 0.0f;
+    const float inv = 1.0f / fmaxf(norm, 1e-12f);
     dr[0] = (dr[0] - qn.x * dot) * inv; dr[1] = (dr[1] - qn.y * dot) * inv;
     dr[2] = (dr[2] - qn.z * dot) * inv; dr[3] = (dr[3] - qn.w * dot) * inv;
 }

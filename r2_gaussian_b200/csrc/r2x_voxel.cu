@@ -602,7 +602,7 @@ __global__ void __launch_bounds__(256) voxel_gauss_bwd_kernel(
         float inv[6];
         voxel_inverse(vc, inv);
         // VOX/backward.cu:348-370 with the per-pair sums factored into moments
-        dop = act.enabled ? S0 * (1.0f - expf(-rho)) : S0;     // raw density: softplus' = 1 - exp(-rho)
+        dop = act.enabled ? S0 * -expm1f(-rho) : S0;     // raw density: softplus' = 1 - exp(-rho) = -expm1(-rho)
         dmean[0] = rho * (-inv[0] * Sx - inv[1] * Sy - inv[2] * Sz) * vg.dvx;   // note: x dVoxel, as the reference
         dmean[1] = rho * (-inv[3] * Sy - inv[1] * Sx - inv[4] * Sz) * vg.dvy;
         dmean[2] = rho * (-inv[5] * Sz - inv[2] * Sx - inv[4] * Sy) * vg.dvz;

@@ -70,10 +70,9 @@ def to_torch(cloud, view, device="cuda", requires_grad=False):
     return t
 
 
-def ours_raster_forward(cloud, view, export=True, cov3D_precomp=None, debug=False):
+def ours_raster_forward(cloud, view, export=True, cov3D_precomp=None, debug=False, scale_modifier=1.0):
     import torch
     from r2_gaussian_b200 import _C
-    from r2_gaussian_b200._lib import load, check
 
     t = to_torch(cloud, view)
     empty = torch.Tensor([])
@@ -81,36 +80,42 @@ def ours_raster_forward(cloud, view, export=True, cov3D_precomp=None, debug=Fals
     if cov3D_precomp is not None:
         scales, rots, cov = empty, empty, torch.tensor(cov3D_precomp, device="cuda")
     R, color, radii, geom, binning, img = _C.rasterize_gaussians(
-        t["means"], t["dens"], scales, rots, 1.0, cov, t["view"], t["proj"], view.tanfovx, view.tanfovy,
+        t["means"], t["dens"], scales, rots, scale_modifier, cov, t["view"], t["proj"], view.tanfovx, view.tanfovy,
         view.image_height, view.image_width, t["campos"], False, view.mode, debug)
     t["scales_in"], t["rots_in"], t["cov_in"] = scales, rots, cov
-    out = dict(R=R, image=color[0].cpu().numpy(), radii=radii.cpu().numpy(), state=(geom, binning, img), t=t)
+    out = dict(R=R, image=color[0].cpu().numpy(), radii=radii.cpu().numpy(), state=(geom, binning, img), t=t,
+               scale_modifier=scale_modifier)
     if export:
-        lib = load()
-        P, W, H = cloud.P, view.image_width, view.image_height
-        T = ((W + 15) // 16) * ((H + 15) // 16)
-        dev = "cuda"
-        xy = torch.empty((P, 2), device=dev); depth = torch.empty(P, device=dev)
-        co = torch.empty((P, 4), device=dev); mu = torch.empty(P, device=dev)
-        tt = torch.empty(P, dtype=torch.int32, device=dev); po = torch.empty(P, dtype=torch.int32, device=dev)
-        keys = torch.empty(max(R, 1), dtype=torch.int64, device=dev)
-        pl = torch.empty(max(R, 1), dtype=torch.int32, device=dev)
-        ranges = torch.empty((T, 2), dtype=torch.int32, device=dev)
-        from r2_gaussian_b200._C import _carved_capacity
-        cap = _carved_capacity(binning, R)
-        keys = torch.empty(max(cap, 1), dtype=torch.int64, device=dev)
-        pl = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
-        rc = lib.r2x_raster_export(torch.cuda.current_stream().cuda_stream, P, W, H, cap, geom.data_ptr(),
-                                   binning.data_ptr() if binning.numel() else None, img.data_ptr(), xy.data_ptr(),
-                                   depth.data_ptr(), co.data_ptr(), mu.data_ptr(), tt.data_ptr(), po.data_ptr(),
-                                   keys.data_ptr(), pl.data_ptr(), ranges.data_ptr())
-        check(rc, "r2x_raster_export")
-        torch.cuda.synchronize()
-        out.update(xy=xy.cpu().numpy(), depth=depth.cpu().numpy(), conic_opacity=co.cpu().numpy(), mu=mu.cpu().numpy(),
-                   tiles_touched=tt.cpu().numpy().astype(np.uint32), point_offsets=po.cpu().numpy().astype(np.uint32),
-                   keys=keys.cpu().numpy().astype(np.uint64)[:R], point_list=pl.cpu().numpy().astype(np.uint32)[:R],
-                   ranges=ranges.cpu().numpy().astype(np.uint32))
+        out.update(raster_export(cloud.P, view.image_width, view.image_height, R, geom, binning, img))
     return out
+
+
+def raster_export(P, W, H, R, geom, binning, img):
+    """The stage outputs a rasterizer forward left in its buffers (r2x_raster_export), as host arrays."""
+    import torch
+    from r2_gaussian_b200._C import _carved_capacity
+    from r2_gaussian_b200._lib import load, check
+
+    lib = load()
+    T = ((W + 15) // 16) * ((H + 15) // 16)
+    dev = "cuda"
+    xy = torch.empty((P, 2), device=dev); depth = torch.empty(P, device=dev)
+    co = torch.empty((P, 4), device=dev); mu = torch.empty(P, device=dev)
+    tt = torch.empty(P, dtype=torch.int32, device=dev); po = torch.empty(P, dtype=torch.int32, device=dev)
+    ranges = torch.empty((T, 2), dtype=torch.int32, device=dev)
+    cap = _carved_capacity(binning, R)
+    keys = torch.empty(max(cap, 1), dtype=torch.int64, device=dev)
+    pl = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+    rc = lib.r2x_raster_export(torch.cuda.current_stream().cuda_stream, P, W, H, cap, geom.data_ptr(),
+                               binning.data_ptr() if binning.numel() else None, img.data_ptr(), xy.data_ptr(),
+                               depth.data_ptr(), co.data_ptr(), mu.data_ptr(), tt.data_ptr(), po.data_ptr(),
+                               keys.data_ptr(), pl.data_ptr(), ranges.data_ptr())
+    check(rc, "r2x_raster_export")
+    torch.cuda.synchronize()
+    return dict(xy=xy.cpu().numpy(), depth=depth.cpu().numpy(), conic_opacity=co.cpu().numpy(), mu=mu.cpu().numpy(),
+                tiles_touched=tt.cpu().numpy().astype(np.uint32), point_offsets=po.cpu().numpy().astype(np.uint32),
+                keys=keys.cpu().numpy().astype(np.uint64)[:R], point_list=pl.cpu().numpy().astype(np.uint32)[:R],
+                ranges=ranges.cpu().numpy().astype(np.uint32))
 
 
 def ours_raster_backward(cloud, view, fwd, dL, debug=False):
@@ -121,8 +126,9 @@ def ours_raster_backward(cloud, view, fwd, dL, debug=False):
     geom, binning, img = fwd["state"]
     radii = torch.tensor(fwd["radii"], device="cuda")
     g = _C.rasterize_gaussians_backward(
-        t["means"], radii, t["scales_in"], t["rots_in"], 1.0, t["cov_in"], t["view"], t["proj"], view.tanfovx,
-        view.tanfovy, torch.tensor(dL, device="cuda")[None], t["campos"], geom, fwd["R"], binning, img, view.mode, debug)
+        t["means"], radii, t["scales_in"], t["rots_in"], fwd["scale_modifier"], t["cov_in"], t["view"], t["proj"],
+        view.tanfovx, view.tanfovy, torch.tensor(dL, device="cuda")[None], t["campos"], geom, fwd["R"], binning, img,
+        view.mode, debug)
     names = ["dL_dmean2D", "dL_dopacity", "dL_dmu", "dL_dmean3D", "dL_dcov3D", "dL_dscale", "dL_drot"]
     return {n: x.cpu().numpy() for n, x in zip(names, g)}
 
@@ -135,18 +141,17 @@ def oracle_raster_forward(cloud, view, **kw):
                               view.mode, **kw)
 
 
-def oracle_raster_backward(cloud, view, fwd, dL):
+def oracle_raster_backward(cloud, view, fwd, dL, **kw):
     from oracle import r2_oracle as orc
 
     return orc.raster_backward(fwd, cloud.means, cloud.scales, cloud.rotations, view.viewmatrix, view.projmatrix,
-                               view.image_width, view.image_height, view.tanfovx, view.tanfovy, view.mode, dL)
+                               view.image_width, view.image_height, view.tanfovx, view.tanfovy, view.mode, dL, **kw)
 
 
 # ---- voxelizer ------------------------------------------------------------------------------
-def ours_voxel_forward(cloud, nVoxel, sVoxel, center, export=True, cov3D_precomp=None, debug=False):
+def ours_voxel_forward(cloud, nVoxel, sVoxel, center, export=True, cov3D_precomp=None, debug=False, scale_modifier=1.0):
     import torch
     from r2_gaussian_b200 import _C
-    from r2_gaussian_b200._lib import load, check
 
     t = to_torch(cloud, None)
     rots, cov = t["rots"], torch.Tensor([])
@@ -154,35 +159,40 @@ def ours_voxel_forward(cloud, nVoxel, sVoxel, center, export=True, cov3D_precomp
         rots, cov = torch.Tensor([]), torch.tensor(cov3D_precomp, device="cuda")
     t["rots_in"], t["cov_in"] = rots, cov
     R, vol, rx, ry, rz, geom, binning, img = _C.voxelize_gaussians(
-        t["means"], t["dens"], t["scales"], rots, 1.0, cov, nVoxel[0], nVoxel[1], nVoxel[2],
+        t["means"], t["dens"], t["scales"], rots, scale_modifier, cov, nVoxel[0], nVoxel[1], nVoxel[2],
         sVoxel[0], sVoxel[1], sVoxel[2], center[0], center[1], center[2], False, debug)
     out = dict(R=R, vol=vol.cpu().numpy(), radii_x=rx.cpu().numpy(), radii_y=ry.cpu().numpy(), radii_z=rz.cpu().numpy(),
-               state=(geom, binning, img), t=t, radii_t=(rx, ry, rz))
+               state=(geom, binning, img), t=t, radii_t=(rx, ry, rz), scale_modifier=scale_modifier)
     if export:
-        lib = load()
-        P = cloud.P
-        nx, ny, nz = nVoxel
-        T = ((nx + 7) // 8) * ((ny + 7) // 8) * ((nz + 7) // 8)
-        dev = "cuda"
-        xyz = torch.empty((P, 3), device=dev); depth = torch.empty(P, device=dev); co = torch.empty((P, 7), device=dev)
-        tt = torch.empty(P, dtype=torch.int32, device=dev); po = torch.empty(P, dtype=torch.int32, device=dev)
-        keys = torch.empty(max(R, 1), dtype=torch.int64, device=dev)
-        pl = torch.empty(max(R, 1), dtype=torch.int32, device=dev)
-        ranges = torch.empty((T, 2), dtype=torch.int32, device=dev)
-        from r2_gaussian_b200._C import _carved_capacity
-        cap = _carved_capacity(binning, R)
-        keys = torch.empty(max(cap, 1), dtype=torch.int64, device=dev)
-        pl = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
-        rc = lib.r2x_voxel_export(torch.cuda.current_stream().cuda_stream, P, nx, ny, nz, cap, geom.data_ptr(),
-                                  binning.data_ptr() if binning.numel() else None, img.data_ptr(), xyz.data_ptr(),
-                                  depth.data_ptr(), co.data_ptr(), tt.data_ptr(), po.data_ptr(), keys.data_ptr(),
-                                  pl.data_ptr(), ranges.data_ptr())
-        check(rc, "r2x_voxel_export")
-        torch.cuda.synchronize()
-        out.update(xyz_vol=xyz.cpu().numpy(), depth=depth.cpu().numpy(), conic_opacity=co.cpu().numpy(),
-                   tiles_touched=tt.cpu().numpy().astype(np.uint32), keys=keys.cpu().numpy().astype(np.uint64)[:R],
-                   point_list=pl.cpu().numpy().astype(np.uint32)[:R], ranges=ranges.cpu().numpy().astype(np.uint32))
+        out.update(voxel_export(cloud.P, nVoxel, R, geom, binning, img))
     return out
+
+
+def voxel_export(P, nVoxel, R, geom, binning, img):
+    """The stage outputs a voxelizer forward left in its buffers (r2x_voxel_export), as host arrays."""
+    import torch
+    from r2_gaussian_b200._C import _carved_capacity
+    from r2_gaussian_b200._lib import load, check
+
+    lib = load()
+    nx, ny, nz = nVoxel
+    T = ((nx + 7) // 8) * ((ny + 7) // 8) * ((nz + 7) // 8)
+    dev = "cuda"
+    xyz = torch.empty((P, 3), device=dev); depth = torch.empty(P, device=dev); co = torch.empty((P, 7), device=dev)
+    tt = torch.empty(P, dtype=torch.int32, device=dev); po = torch.empty(P, dtype=torch.int32, device=dev)
+    ranges = torch.empty((T, 2), dtype=torch.int32, device=dev)
+    cap = _carved_capacity(binning, R)
+    keys = torch.empty(max(cap, 1), dtype=torch.int64, device=dev)
+    pl = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+    rc = lib.r2x_voxel_export(torch.cuda.current_stream().cuda_stream, P, nx, ny, nz, cap, geom.data_ptr(),
+                              binning.data_ptr() if binning.numel() else None, img.data_ptr(), xyz.data_ptr(),
+                              depth.data_ptr(), co.data_ptr(), tt.data_ptr(), po.data_ptr(), keys.data_ptr(),
+                              pl.data_ptr(), ranges.data_ptr())
+    check(rc, "r2x_voxel_export")
+    torch.cuda.synchronize()
+    return dict(xyz_vol=xyz.cpu().numpy(), depth=depth.cpu().numpy(), conic_opacity=co.cpu().numpy(),
+                tiles_touched=tt.cpu().numpy().astype(np.uint32), keys=keys.cpu().numpy().astype(np.uint64)[:R],
+                point_list=pl.cpu().numpy().astype(np.uint32)[:R], ranges=ranges.cpu().numpy().astype(np.uint32))
 
 
 def ours_voxel_backward(cloud, nVoxel, sVoxel, center, fwd, dL, debug=False):
@@ -193,8 +203,8 @@ def ours_voxel_backward(cloud, nVoxel, sVoxel, center, fwd, dL, debug=False):
     geom, binning, img = fwd["state"]
     rx, ry, rz = fwd["radii_t"]
     g = _C.voxelize_gaussians_backward(
-        t["means"], rx, ry, rz, t["scales"], t["rots_in"], 1.0, t["cov_in"], torch.tensor(dL, device="cuda"), geom,
-        fwd["R"], binning, img, nVoxel[0], nVoxel[1], nVoxel[2], sVoxel[0], sVoxel[1], sVoxel[2], center[0], center[1],
+        t["means"], rx, ry, rz, t["scales"], t["rots_in"], fwd["scale_modifier"], t["cov_in"],
+        torch.tensor(dL, device="cuda"), geom, fwd["R"], binning, img, nVoxel[0], nVoxel[1], nVoxel[2], sVoxel[0], sVoxel[1], sVoxel[2], center[0], center[1],
         center[2], debug)
     names = ["dL_dopacity", "dL_dmean3D", "dL_dcov3D", "dL_dscale", "dL_drot"]
     return {n: x.cpu().numpy() for n, x in zip(names, g)}
@@ -206,10 +216,10 @@ def oracle_voxel_forward(cloud, nVoxel, sVoxel, center, **kw):
     return orc.voxel_forward(cloud.means, cloud.scales, cloud.rotations, cloud.density, nVoxel, sVoxel, center, **kw)
 
 
-def oracle_voxel_backward(cloud, nVoxel, sVoxel, fwd, dL):
+def oracle_voxel_backward(cloud, nVoxel, sVoxel, fwd, dL, **kw):
     from oracle import r2_oracle as orc
 
-    return orc.voxel_backward(fwd, cloud.scales, cloud.rotations, nVoxel, sVoxel, dL)
+    return orc.voxel_backward(fwd, cloud.scales, cloud.rotations, nVoxel, sVoxel, dL, **kw)
 
 
 # ---- comparison helpers ---------------------------------------------------------------------
