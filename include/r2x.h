@@ -223,6 +223,27 @@ int r2x_raster_backward_raw(void* stream, int P, long long R, int W, int H, cons
                             const void* geom_buf, const void* binning_buf, const void* image_buf, void* scratch,
                             const float* dL_dpix, float* dL_dmean2D, float* dL_draw_density, float* dL_dmean3D,
                             float* dL_dcov3D, float* dL_draw_scale, float* dL_draw_rot, int mode, const r2x_activation* act);
+
+/* ---- view- and projection-matrix gradients of the rasterizer backward (per-view pose refinement) -------------- */
+/* r2x_raster_backward (act == NULL) or r2x_raster_backward_raw (act != NULL: raw scales / rotations, dL_dopacity is the
+ * raw density gradient, cov3D_precomp must be NULL) with the same per-Gaussian outputs, bit for bit, that also writes
+ * dL_dviewmatrix[16] / dL_dprojmatrix[16] (device): the gradient with respect to the 16 floats exactly as passed
+ * (column-major flat, as the reference stores them).  Every discrete decision of the forward is held fixed (cull,
+ * radius, tile rectangles, alpha cut, the clamp of the view-space point, the 1e-7 regularisations), the convention of
+ * the per-Gaussian gradients.  Entries the rasterizer never reads get 0: viewmatrix[3, 7, 11, 15] and
+ * projmatrix[2, 6, 10, 14].  One row of partial sums per 256 Gaussians goes to `pose_scratch`
+ * (>= r2x_raster_backward_pose_scratch_bytes(P) bytes), summed in a fixed order in float64: no atomics, bitwise
+ * reproducible.  Arguments are checked before any CUDA work. */
+size_t r2x_raster_backward_pose_scratch_bytes(int P);
+int r2x_raster_backward_pose(void* stream, int P, long long R, int W, int H, const float* means3D, const float* scales,
+                             float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                             const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
+                             float tan_fovy, const int* radii, const void* geom_buf, const void* binning_buf,
+                             const void* image_buf, void* scratch, const float* dL_dpix, float* dL_dmean2D,
+                             float* dL_dopacity, float* dL_dmu, float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale,
+                             float* dL_drot, int mode, int debug, const r2x_activation* act, float* dL_dviewmatrix,
+                             float* dL_dprojmatrix, void* pose_scratch, size_t pose_scratch_bytes);
+
 int r2x_voxel_forward_async_raw(void* stream, int P, int nx, int ny, int nz, float sx, float sy, float sz, float cx,
                                 float cy, float cz, const float* means3D, const float* raw_density,
                                 const float* raw_scales, float scale_modifier, const float* raw_rotations,

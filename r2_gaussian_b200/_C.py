@@ -337,6 +337,46 @@ def rasterize_gaussians_backward(means3D, radii, scales, rotations, scale_modifi
     return g_mean2D, g_op, g_mu, g_mean3D, g_cov, g_scale, g_rot
 
 
+def rasterize_gaussians_backward_matrices(means3D, radii, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
+                                          projmatrix, tan_fovx, tan_fovy, dL_dout_color, campos, geomBuffer, R,
+                                          binningBuffer, imageBuffer, mode, debug, act=None):
+    """`rasterize_gaussians_backward` that also returns the gradients with respect to the two matrices ->
+    (dL_dmeans2D, dL_dopacity, dL_dmu, dL_dmeans3D, dL_dcov3D, dL_dscales, dL_drotations, dL_dviewmatrix[4,4],
+    dL_dprojmatrix[4,4]).  With `act` (an `ActivationDesc`) scales / rotations are the raw parameters and dL_dopacity
+    is the raw density gradient (dL_dmu is then None), as `fused` passes them.  The matrix gradients are laid out like
+    the matrices (element [i, j] is dL / d matrix[i, j])."""
+    _require_cuda(means3D, "means3D")
+    lib = load()
+    dev = means3D.device
+    P = int(means3D.shape[0])
+    H, W = int(dL_dout_color.shape[-2]), int(dL_dout_color.shape[-1])
+    with torch.cuda.device(dev):
+        means3D = _f32(means3D, dev); scales = _f32(scales, dev); rotations = _f32(rotations, dev)
+        cov3D_precomp = None if cov3D_precomp is None else _f32(cov3D_precomp, dev)
+        viewmatrix = _f32(viewmatrix, dev); projmatrix = _f32(projmatrix, dev); campos = _f32(campos, dev)
+        dL = _f32(dL_dout_color, dev)
+        opts = dict(dtype=torch.float32, device=dev)
+        g_mean2D = torch.empty((P, 3), **opts); g_op = torch.empty((P, 1), **opts)
+        g_mu = torch.empty((P, 1), **opts) if act is None else None
+        g_mean3D = torch.empty((P, 3), **opts); g_cov = torch.empty((P, 6), **opts)
+        g_scale = torch.empty((P, 3), **opts); g_rot = torch.empty((P, 4), **opts)
+        g_view = torch.empty((4, 4), **opts); g_proj = torch.empty((4, 4), **opts)
+        R = _carved_capacity(binningBuffer, R)
+        scratch = RASTER.bwd_scratch(R, dev)
+        pose_bytes = lib.r2x_raster_backward_pose_scratch_bytes(P)
+        pose_scratch = _u8(pose_bytes, dev)
+        rc = lib.r2x_raster_backward_pose(
+            torch.cuda.current_stream(dev).cuda_stream, P, R, W, H, _ptr(means3D), _ptr(scales),
+            float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(viewmatrix), _ptr(projmatrix),
+            _ptr(campos), float(tan_fovx), float(tan_fovy), _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer),
+            _ptr(imageBuffer), scratch.data_ptr(), _ptr(dL), _ptr(g_mean2D), _ptr(g_op), _ptr(g_mu),
+            _ptr(g_mean3D), _ptr(g_cov), _ptr(g_scale), _ptr(g_rot), int(mode), int(bool(debug)),
+            None if act is None else C.byref(act), g_view.data_ptr(), g_proj.data_ptr(), pose_scratch.data_ptr(),
+            pose_bytes)
+        check(rc, "r2x_raster_backward_pose")
+    return g_mean2D, g_op, g_mu, g_mean3D, g_cov, g_scale, g_rot, g_view, g_proj
+
+
 def mark_visible(means3D, viewmatrix, projmatrix):
     """-> bool[P]: view-space z > 0.2 (RAS/auxiliary.h:143-168)."""
     _require_cuda(means3D, "means3D")

@@ -489,16 +489,25 @@ int r2x_voxel_render_only(void* stream, int P, int nx, int ny, int nz, long long
     return launch_voxel_render((cudaStream_t)stream, vg, s.geom, img.ranges, bv.point_list, img.plan, R, out_volume);
 }
 
-int r2x_raster_backward(void* stream, int P, long long R, int W, int H, const float* means3D, const float* scales,
-                        float scale_modifier, const float* rotations, const float* cov3D_precomp,
-                        const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
-                        float tan_fovy, const int* radii, const void* geom_buf, const void* binning_buf,
-                        const void* image_buf, void* scratch, const float* dL_dpix, float* dL_dmean2D,
-                        float* dL_dopacity, float* dL_dmu, float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale,
-                        float* dL_drot, int mode, int debug) {
-    (void)campos;
+}  // extern "C"
+
+namespace {
+// r2x_raster_backward, and with pose_scratch != NULL also dL_dview / dL_dproj (r2x_raster_backward_pose)
+int raster_backward_impl(void* stream, int P, long long R, int W, int H, const float* means3D, const float* scales,
+                         float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                         const float* viewmatrix, const float* projmatrix, float tan_fovx, float tan_fovy,
+                         const int* radii, const void* geom_buf, const void* binning_buf, const void* image_buf,
+                         void* scratch, const float* dL_dpix, float* dL_dmean2D, float* dL_dopacity, float* dL_dmu,
+                         float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale, float* dL_drot, int mode, int debug,
+                         void* pose_scratch, float* dL_dview, float* dL_dproj) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (P == 0) return 0;
+    if (P == 0) {   // no Gaussian: the matrix gradients are zero
+        if (pose_scratch) {
+            R2X_CUDA_OK(cudaMemsetAsync(dL_dview, 0, 16 * sizeof(float), st));
+            R2X_CUDA_OK(cudaMemsetAsync(dL_dproj, 0, 16 * sizeof(float), st));
+        }
+        return 0;
+    }
     if (P < 0 || W <= 0 || H <= 0 || R < 0) return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward: bad sizes");
     if (!geom_buf || !image_buf || !dL_dpix || !dL_dmean2D || !dL_dopacity || !dL_dmean3D || !dL_dcov3D ||
         !dL_dscale || !dL_drot || !radii || !means3D)
@@ -515,9 +524,27 @@ int r2x_raster_backward(void* stream, int P, long long R, int W, int H, const fl
     R2X_TRY(debug_sync(st, debug, "raster render backward"));
     R2X_TRY(launch_raster_gauss_bwd(st, P, means3D, radii, scales, scale_modifier, rotations, cov3D_precomp, viewmatrix,
                                     projmatrix, W, H, tan_fovx, tan_fovy, mode, s.geom, R, bv.inst_pos, inst_grad,
-                                    dL_dmean2D, dL_dopacity, dL_dmu, dL_dmean3D, dL_dcov3D, dL_dscale, dL_drot));
+                                    dL_dmean2D, dL_dopacity, dL_dmu, dL_dmean3D, dL_dcov3D, dL_dscale, dL_drot,
+                                    pose_scratch, dL_dview, dL_dproj));
     R2X_TRY(debug_sync(st, debug, "raster per-Gaussian backward"));
     return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int r2x_raster_backward(void* stream, int P, long long R, int W, int H, const float* means3D, const float* scales,
+                        float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                        const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
+                        float tan_fovy, const int* radii, const void* geom_buf, const void* binning_buf,
+                        const void* image_buf, void* scratch, const float* dL_dpix, float* dL_dmean2D,
+                        float* dL_dopacity, float* dL_dmu, float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale,
+                        float* dL_drot, int mode, int debug) {
+    (void)campos;
+    return raster_backward_impl(stream, P, R, W, H, means3D, scales, scale_modifier, rotations, cov3D_precomp, viewmatrix,
+                                projmatrix, tan_fovx, tan_fovy, radii, geom_buf, binning_buf, image_buf, scratch, dL_dpix,
+                                dL_dmean2D, dL_dopacity, dL_dmu, dL_dmean3D, dL_dcov3D, dL_dscale, dL_drot, mode, debug,
+                                nullptr, nullptr, nullptr);
 }
 
 int r2x_mark_visible(void* stream, int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
@@ -647,6 +674,38 @@ int r2x_raster_backward_raw(void* stream, int P, long long R, int W, int H, cons
                                projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buf, binning_buf, image_buf, scratch,
                                dL_dpix, dL_dmean2D, dL_draw_density, nullptr, dL_dmean3D, dL_dcov3D, dL_draw_scale,
                                dL_draw_rot, mode, 0);
+}
+
+size_t r2x_raster_backward_pose_scratch_bytes(int P) { return raster_pose_scratch_bytes(P); }
+
+int r2x_raster_backward_pose(void* stream, int P, long long R, int W, int H, const float* means3D, const float* scales,
+                             float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                             const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
+                             float tan_fovy, const int* radii, const void* geom_buf, const void* binning_buf,
+                             const void* image_buf, void* scratch, const float* dL_dpix, float* dL_dmean2D,
+                             float* dL_dopacity, float* dL_dmu, float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale,
+                             float* dL_drot, int mode, int debug, const r2x_activation* act, float* dL_dviewmatrix,
+                             float* dL_dprojmatrix, void* pose_scratch, size_t pose_scratch_bytes) {
+    (void)campos;
+    if (P < 0 || W <= 0 || H <= 0 || R < 0) return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward_pose: bad sizes");
+    if (!viewmatrix || !projmatrix || !dL_dviewmatrix || !dL_dprojmatrix)
+        return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward_pose: null matrix or matrix gradient");
+    if (!pose_scratch || pose_scratch_bytes < raster_pose_scratch_bytes(P))
+        return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward_pose: pose_scratch is NULL or smaller than "
+                                         "r2x_raster_backward_pose_scratch_bytes(P)");
+    if (act && (cov3D_precomp || !scales || !rotations))
+        return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward_pose: raw parameters need scales and rotations and no "
+                                         "cov3D_precomp");
+    if (!act)
+        return raster_backward_impl(stream, P, R, W, H, means3D, scales, scale_modifier, rotations, cov3D_precomp,
+                                    viewmatrix, projmatrix, tan_fovx, tan_fovy, radii, geom_buf, binning_buf, image_buf,
+                                    scratch, dL_dpix, dL_dmean2D, dL_dopacity, dL_dmu, dL_dmean3D, dL_dcov3D, dL_dscale,
+                                    dL_drot, mode, debug, pose_scratch, dL_dviewmatrix, dL_dprojmatrix);
+    ActScope scope(act);
+    return raster_backward_impl(stream, P, R, W, H, means3D, scales, scale_modifier, rotations, nullptr, viewmatrix,
+                                projmatrix, tan_fovx, tan_fovy, radii, geom_buf, binning_buf, image_buf, scratch, dL_dpix,
+                                dL_dmean2D, dL_dopacity, dL_dmu, dL_dmean3D, dL_dcov3D, dL_dscale, dL_drot, mode, debug,
+                                pose_scratch, dL_dviewmatrix, dL_dprojmatrix);
 }
 
 int r2x_voxel_forward_async_raw(void* stream, int P, int nx, int ny, int nz, float sx, float sy, float sz, float cx,

@@ -31,7 +31,10 @@ int launch_raster_gauss_bwd(cudaStream_t st, int P, const float* means, const in
                             const float* proj, int W, int H, float tan_fovx, float tan_fovy, int mode,
                             const RasterGeom& geom, long long capacity, const uint32_t* inst_pos,
                             const float4* inst_grad, float* dL_dmean2D, float* dL_dopacity, float* dL_dmu, float* dL_dmean3D,
-                            float* dL_dcov3D, float* dL_dscale, float* dL_drot);
+                            float* dL_dcov3D, float* dL_dscale, float* dL_drot, void* pose_scratch = nullptr,
+                            float* dL_dview = nullptr, float* dL_dproj = nullptr);
+// pose_scratch of launch_raster_gauss_bwd (the per-CTA rows of the view / projection matrix gradients)
+size_t raster_pose_scratch_bytes(int P);
 int launch_mark_visible(cudaStream_t st, int P, const float* means, const float* view, unsigned char* present);
 
 }  // namespace r2x

@@ -87,6 +87,27 @@ class _RasterizeRaw(torch.autograd.Function):
         return g3, g2, gd, gs, gr, None, None
 
 
+class _RasterizeRawMatrices(torch.autograd.Function):
+    """`_RasterizeRaw` with the view and projection matrices as differentiable inputs (the settings' own are ignored)."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, raw_density, raw_scales, raw_rotations, viewmatrix, projmatrix, settings, act):
+        s = settings._replace(viewmatrix=viewmatrix.detach(), projmatrix=projmatrix.detach())
+        ctx.matrix_dtypes = (viewmatrix.dtype, projmatrix.dtype)
+        return _RasterizeRaw.forward(ctx, means3D, means2D, raw_density, raw_scales, raw_rotations, s, act)
+
+    @staticmethod
+    def backward(ctx, grad_color, _grad_radii):
+        s, act, R = ctx.settings, ctx.act, ctx.num_rendered
+        means3D, raw_scales, raw_rotations, radii, geom, binning, img, view, proj, campos = ctx.saved_tensors
+        g2, gd, _, g3, _gcov, gs, gr, gv, gp = _C.rasterize_gaussians_backward_matrices(
+            means3D, radii, raw_scales, raw_rotations, s.scale_modifier, None, view, proj, s.tanfovx, s.tanfovy,
+            grad_color, campos, geom, R, binning, img, s.mode, False, act=act)
+        gv = gv.view(s.viewmatrix.shape).to(ctx.matrix_dtypes[0])
+        gp = gp.view(s.projmatrix.shape).to(ctx.matrix_dtypes[1])
+        return g3, g2, gd, gs, gr, gv, gp, None, None
+
+
 class _VoxelizeRaw(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, raw_density, raw_scales, raw_rotations, settings, act):
@@ -143,6 +164,12 @@ class _VoxelizeRaw(torch.autograd.Function):
 def rasterize_raw(means3D, means2D, raw, settings):
     """raw = model.raw_parameters(): {"density", "scaling", "rotation", "scale_bound"} -> (image [1,H,W], radii)."""
     return _RasterizeRaw.apply(means3D, means2D, raw["density"], raw["scaling"], raw["rotation"], settings, _act(raw))
+
+
+def rasterize_raw_matrices(means3D, means2D, raw, viewmatrix, projmatrix, settings):
+    """`rasterize_raw` whose image is also differentiable with respect to `viewmatrix` / `projmatrix`."""
+    return _RasterizeRawMatrices.apply(means3D, means2D, raw["density"], raw["scaling"], raw["rotation"], viewmatrix,
+                                       projmatrix, settings, _act(raw))
 
 
 def voxelize_raw(means3D, raw, settings):

@@ -68,6 +68,43 @@ def rasterize_gaussians(means3D, means2D, opacities, scales, rotations, cov3Ds_p
     return _RasterizeGaussians.apply(means3D, means2D, opacities, scales, rotations, cov3Ds_precomp, raster_settings)
 
 
+class _RasterizeGaussiansMatrices(torch.autograd.Function):
+    """`_RasterizeGaussians` with the view and projection matrices as differentiable inputs (not part of the
+    reference's surface: `GaussianRasterizer` keeps returning no gradient for the settings' matrices).
+    forward inputs:  (means3D, means2D, opacities, scales, rotations, cov3Ds_precomp, viewmatrix, projmatrix, settings)
+    The settings' own matrices are ignored."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, opacities, scales, rotations, cov3Ds_precomp, viewmatrix, projmatrix,
+                raster_settings):
+        s = raster_settings._replace(viewmatrix=viewmatrix.detach(), projmatrix=projmatrix.detach())
+        ctx.matrix_dtypes = (viewmatrix.dtype, projmatrix.dtype)
+        return _RasterizeGaussians.forward(ctx, means3D, means2D, opacities, scales, rotations, cov3Ds_precomp, s)
+
+    @staticmethod
+    def backward(ctx, grad_color, _grad_radii):
+        s = ctx.raster_settings
+        means3D, scales, rotations, cov3Ds_precomp, radii, geom, binning, img = ctx.saved_tensors
+        native_args = (means3D, radii, scales, rotations, s.scale_modifier, cov3Ds_precomp, s.viewmatrix,
+                       s.projmatrix, s.tanfovx, s.tanfovy, grad_color, s.campos, geom, ctx.num_rendered, binning, img,
+                       s.mode, s.debug)
+        g_means2D, g_opac, _g_mu, g_means3D, g_cov, g_scales, g_rots, g_view, g_proj = call_with_snapshot(
+            _C.rasterize_gaussians_backward_matrices, native_args, s.debug, "snapshot_bw.dump", "backward")
+        g_view = g_view.view(s.viewmatrix.shape).to(ctx.matrix_dtypes[0])
+        g_proj = g_proj.view(s.projmatrix.shape).to(ctx.matrix_dtypes[1])
+        return g_means3D, g_means2D, g_opac, g_scales, g_rots, g_cov, g_view, g_proj, None
+
+
+def rasterize_gaussians_matrices(means3D, means2D, opacities, scales, rotations, cov3Ds_precomp, viewmatrix, projmatrix,
+                                 raster_settings):
+    """-> (image [1,H,W], radii); the image is differentiable with respect to `viewmatrix` / `projmatrix` too."""
+    _exactly_one_covariance_source(scales, rotations, cov3Ds_precomp)
+    empty = torch.Tensor([])
+    return _RasterizeGaussiansMatrices.apply(
+        means3D, means2D, opacities, empty if scales is None else scales, empty if rotations is None else rotations,
+        empty if cov3Ds_precomp is None else cov3Ds_precomp, viewmatrix, projmatrix, raster_settings)
+
+
 def _exactly_one_covariance_source(scales, rotations, cov3D_precomp):
     have_sr = scales is not None or rotations is not None
     full_sr = scales is not None and rotations is not None

@@ -7,6 +7,8 @@ world_view_transform, full_proj_transform, camera_center; `pipe` exposes debug a
 After `sharded.enable(group)` (Gaussian-sharded runs: the trainer, bench.py) each rank holds a shard of the
 Gaussians and the image / volume is summed over ranks; the per-Gaussian outputs describe the local shard.
 Without that opt-in an initialised process group changes nothing (data-parallel / multi-scene jobs).
+When the camera's world_view_transform or full_proj_transform requires grad (e.g. `pose.PoseCorrection`), the
+backward also fills their .grad (not with Gaussian sharding); otherwise render() runs exactly as the reference's.
 """
 from __future__ import annotations
 
@@ -14,8 +16,8 @@ import math
 
 import torch
 
-from . import fused
-from .rasterization import GaussianRasterizationSettings, GaussianRasterizer
+from . import fused, sharded
+from .rasterization import GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians_matrices
 from .sharded import sharded_sum
 from .voxelization import GaussianVoxelizationSettings, GaussianVoxelizer
 
@@ -78,13 +80,25 @@ def render(viewpoint_camera, pc, pipe, scaling_modifier=1.0):
         campos=viewpoint_camera.camera_center, prefiltered=False, mode=mode,
         debug=bool(getattr(pipe, "debug", False)))
     raw = _raw_parameters(pc, pipe)
+    view, proj = viewpoint_camera.world_view_transform, viewpoint_camera.full_proj_transform
+    matrices = torch.is_grad_enabled() and (view.requires_grad or proj.requires_grad)
+    if matrices and sharded.enabled():
+        raise RuntimeError("render(): gradients with respect to the camera matrices are not supported with Gaussian "
+                           "sharding (each rank would hold a partial sum over its shard)")
     if raw is not None:
-        image, radii = fused.rasterize_raw(xyz, screenspace_points, raw, settings)
+        if matrices:
+            image, radii = fused.rasterize_raw_matrices(xyz, screenspace_points, raw, view, proj, settings)
+        else:
+            image, radii = fused.rasterize_raw(xyz, screenspace_points, raw, settings)
         return {"render": sharded_sum(image), "viewspace_points": screenspace_points,
                 "visibility_filter": radii > 0, "radii": radii}
     scales, rotations, cov3D = _covariance_inputs(pc, pipe, scaling_modifier)
-    image, radii = GaussianRasterizer(raster_settings=settings)(
-        means3D=xyz, means2D=screenspace_points, opacities=pc.get_density, scales=scales, rotations=rotations,
-        cov3D_precomp=cov3D)
+    if matrices:
+        image, radii = rasterize_gaussians_matrices(xyz, screenspace_points, pc.get_density, scales, rotations, cov3D,
+                                                    view, proj, settings)
+    else:
+        image, radii = GaussianRasterizer(raster_settings=settings)(
+            means3D=xyz, means2D=screenspace_points, opacities=pc.get_density, scales=scales, rotations=rotations,
+            cov3D_precomp=cov3D)
     return {"render": sharded_sum(image), "viewspace_points": screenspace_points,
             "visibility_filter": radii > 0, "radii": radii}
