@@ -244,6 +244,25 @@ int r2x_raster_backward_pose(void* stream, int P, long long R, int W, int H, con
                              float* dL_drot, int mode, int debug, const r2x_activation* act, float* dL_dviewmatrix,
                              float* dL_dprojmatrix, void* pose_scratch, size_t pose_scratch_bytes);
 
+/* ---- per-view pose corrections on the device (pose.PoseCorrection, NativeTrainStep(pose=...)) ------------------ */
+/* omega / nu [n_views, 3] (device): per-view twists xi = (omega, nu), a LEFT perturbation in the camera frame,
+ * T' = exp(xi) T, with world_view_transform = T^T and full_proj_transform = T^T projection_matrix (all 16 floats,
+ * device, row-major as the torch tensors store them).  r2x_pose_apply writes the corrected matrices of view
+ * `view_index`:  out_view = view + view D^T,  out_full = full + (view D^T) proj,  D = exp(xi) - I formed in float64
+ * with the coefficients and the series switch (theta^2 < 1e-2) of pose._coefficients; each entry is the float64 sum,
+ * rounded to float32 once, and a zero increment counts as -0.0, so a zero twist returns both matrices bit for bit.
+ * The camera centre is not an output: the raster kernels never read `campos`, callers pass the camera's own.
+ * r2x_pose_grad writes dL_domega / dL_dnu [n_views, 3] in full: row `view_index` is the chain rule of dL_dview /
+ * dL_dproj (as r2x_raster_backward_pose writes them) through that same float64 expression (exact derivative, forward
+ * mode), rounded once; every other row, and row `anchor` (-1: none) always, is 0.  The base full_proj_transform does
+ * not enter the derivative.  Arguments are checked before any CUDA work; one small launch each, asynchronous. */
+int r2x_pose_apply(void* stream, const float* omega, const float* nu, int n_views, int view_index,
+                   const float* world_view_transform, const float* full_proj_transform, const float* projection_matrix,
+                   float* out_world_view_transform, float* out_full_proj_transform);
+int r2x_pose_grad(void* stream, const float* omega, const float* nu, int n_views, int view_index, int anchor,
+                  const float* world_view_transform, const float* projection_matrix, const float* dL_dview,
+                  const float* dL_dproj, float* dL_domega, float* dL_dnu);
+
 int r2x_voxel_forward_async_raw(void* stream, int P, int nx, int ny, int nz, float sx, float sy, float sz, float cx,
                                 float cy, float cz, const float* means3D, const float* raw_density,
                                 const float* raw_scales, float scale_modifier, const float* raw_rotations,

@@ -23,6 +23,13 @@ the camera frame about its own axes and nu moves it along them, in scene units. 
 both computed with torch ops from (omega_i, nu_i), so autograd carries dL/d(matrices) from the rasterizer to the
 parameters.  With zero correction both matrices equal the camera's bit for bit.
 
+`PoseCorrection.device_camera(cam, i, anchor)` is the same map as two small device kernels (libr2xray's
+`r2x_pose_apply` / `r2x_pose_grad`): the matrices come from a float64 evaluation rounded once, and the backward is the
+exact chain rule through it.  It replaces ~30 torch ops forward and as many backward with one launch each, and it is
+what both training paths use (`NativeTrainStep(pose=...)` calls the kernels directly; `trainer --pose_refine`).  Its
+gradient rows are written in full, with the `anchor` view's row held at 0: a rigid motion of the scene together with
+every camera leaves every image unchanged, so one view fixes the frame.
+
 Pose gradients are not supported together with Gaussian sharding (`sharded.enable`); intrinsics (tan_fovx, detector
 offsets) stay as given.
 """
@@ -32,6 +39,8 @@ import copy
 
 import torch
 from torch import nn
+
+from ._lib import check, load
 
 
 def hat(w: torch.Tensor) -> torch.Tensor:
@@ -107,3 +116,60 @@ class PoseCorrection(nn.Module):
         out.full_proj_transform = full
         out.camera_center = torch.linalg.inv(view.detach())[3, :3].contiguous()
         return out
+
+    def device_camera(self, cam, i: int, anchor: int = 0):
+        """A copy of `cam` whose matrices carry correction `i`, formed by the device kernels (module docstring):
+        differentiable in omega / nu, whose gradient rows other than `i` -- and row `anchor` (-1: none) always -- are
+        0.  float32 CUDA parameters only.  `camera_center` stays the camera's own (the rasterizer never reads it)."""
+        view, full = _DevicePose.apply(self.omega, self.nu, int(i), int(anchor), cam.world_view_transform,
+                                       cam.full_proj_transform, cam.projection_matrix)
+        out = copy.copy(cam)
+        out.world_view_transform = view
+        out.full_proj_transform = full
+        return out
+
+
+def _matrix(t: torch.Tensor, dev) -> torch.Tensor:
+    if t.dtype != torch.float32 or t.device != dev or not t.is_contiguous():
+        t = t.to(device=dev, dtype=torch.float32).contiguous()
+    if t.numel() != 16:
+        raise ValueError("PoseCorrection.device_camera: camera matrices must have 16 entries")
+    return t
+
+
+class _DevicePose(torch.autograd.Function):
+    """(omega, nu) -> (world_view_transform', full_proj_transform') of view i through r2x_pose_apply / r2x_pose_grad."""
+
+    @staticmethod
+    def forward(ctx, omega, nu, i, anchor, wvt, full, proj):
+        for name, p in (("omega", omega), ("nu", nu)):
+            if not p.is_cuda or p.dtype != torch.float32 or not p.is_contiguous() or p.dim() != 2 or p.shape[1] != 3:
+                raise RuntimeError(f"PoseCorrection.device_camera: {name} must be a contiguous float32 CUDA [n_views, 3]")
+        dev = omega.device
+        wvt, full, proj = _matrix(wvt, dev), _matrix(full, dev), _matrix(proj, dev)
+        lib = load()
+        with torch.cuda.device(dev):
+            view_out = torch.empty((4, 4), dtype=torch.float32, device=dev)
+            full_out = torch.empty((4, 4), dtype=torch.float32, device=dev)
+            check(lib.r2x_pose_apply(torch.cuda.current_stream(dev).cuda_stream, omega.data_ptr(), nu.data_ptr(),
+                                     int(omega.shape[0]), i, wvt.data_ptr(), full.data_ptr(), proj.data_ptr(),
+                                     view_out.data_ptr(), full_out.data_ptr()), "r2x_pose_apply")
+        ctx.i, ctx.anchor = i, anchor
+        ctx.save_for_backward(omega, nu, wvt, proj)
+        return view_out, full_out
+
+    @staticmethod
+    def backward(ctx, g_view, g_full):
+        omega, nu, wvt, proj = ctx.saved_tensors
+        dev = omega.device
+        zero = lambda: torch.zeros((4, 4), dtype=torch.float32, device=dev)
+        g_view = zero() if g_view is None else _matrix(g_view, dev)
+        g_full = zero() if g_full is None else _matrix(g_full, dev)
+        lib = load()
+        with torch.cuda.device(dev):
+            g_omega, g_nu = torch.empty_like(omega), torch.empty_like(nu)
+            check(lib.r2x_pose_grad(torch.cuda.current_stream(dev).cuda_stream, omega.data_ptr(), nu.data_ptr(),
+                                    int(omega.shape[0]), ctx.i, ctx.anchor, wvt.data_ptr(), proj.data_ptr(),
+                                    g_view.data_ptr(), g_full.data_ptr(), g_omega.data_ptr(), g_nu.data_ptr()),
+                  "r2x_pose_grad")
+        return g_omega, g_nu, None, None, None, None, None

@@ -20,6 +20,19 @@ are GUARDED by the forwards' overflow flags on the device, so an overflowed iter
 the flags one iteration late (`check()`, through `_C._Workspace.read`, which raises the hint) and repeats that
 iteration.
 
+With `pose=(PoseCorrection, FusedAdam over [omega] and [nu], one group each)` the step also refines the view's pose
+(`pose.py`), still without autograd or host synchronisation:
+
+    corrected matrices of view i         r2x_pose_apply                       (before the raster forward)
+    raster backward + matrix gradients   r2x_raster_backward_pose             (replaces r2x_raster_backward_raw; the
+                                                                               same per-Gaussian gradients bit for bit)
+    twist gradient of view i             r2x_pose_grad                        (row `pose_anchor` held at 0)
+    Adam on omega and nu                 r2x_adam_step_sum                    (after the Gaussians', same guards)
+
+`__call__` then takes the view index; the pose step count is kept like the Gaussians' (undone when `check()` repeats an
+iteration).  Pose refinement with Gaussian sharding is refused at bind time: each rank would hold only a partial sum
+of the matrix gradients.  With `pose=None` the launch sequence is the one above.
+
 The model's tensors are updated in place: `GaussianModel._xyz/_density/_scaling/_rotation`, the `FusedAdam` state of
 `gaussians.optimizer` (same `exp_avg`, `exp_avg_sq`, `step`, so checkpoints and the densification surgery are
 unchanged) and `max_radii2D / xyz_gradient_accum / denom`.  After densification (new tensors) the step re-binds itself.
@@ -42,8 +55,10 @@ def enabled() -> bool:
 
 class NativeTrainStep:
     def __init__(self, gaussians, lambda_dssim: float, lambda_tv: float = 0.0, tv_vol_nVoxel=None, tv_vol_sVoxel=None,
-                 scaling_modifier: float = 1.0):
+                 scaling_modifier: float = 1.0, pose=None, pose_anchor: int = 0):
         self.gm = gaussians
+        self.pose, self.pose_opt = (None, None) if pose is None else pose
+        self.pose_anchor = int(pose_anchor)
         self.lambda_dssim, self.lambda_tv = float(lambda_dssim), float(lambda_tv)
         self.tv_n = None if tv_vol_nVoxel is None else tuple(int(v) for v in tv_vol_nVoxel)
         self.tv_s = None if tv_vol_sVoxel is None else tuple(float(v) for v in tv_vol_sVoxel)
@@ -57,8 +72,11 @@ class NativeTrainStep:
     # ------------------------------------------------------------------ buffers
     def _signature(self, H, W):
         gm = self.gm
-        return (sharded.enabled(), gm._xyz.data_ptr(), gm._density.data_ptr(), gm._scaling.data_ptr(), gm._rotation.data_ptr(),
-                int(gm._xyz.shape[0]), H, W, gm.max_radii2D.data_ptr(), gm.xyz_gradient_accum.data_ptr())
+        sig = (sharded.enabled(), gm._xyz.data_ptr(), gm._density.data_ptr(), gm._scaling.data_ptr(), gm._rotation.data_ptr(),
+               int(gm._xyz.shape[0]), H, W, gm.max_radii2D.data_ptr(), gm.xyz_gradient_accum.data_ptr())
+        if self.pose is not None:
+            sig += (self.pose.omega.data_ptr(), self.pose.nu.data_ptr())
+        return sig
 
     def _bind(self, H, W):
         gm, lib = self.gm, self.lib
@@ -133,7 +151,46 @@ class NativeTrainStep:
             a.numel = p.numel()
             self.adam_grads2[k] = g2.data_ptr() if g2 is not None else None
         self.act = fused._act(gm.raw_parameters())
+        if self.pose is not None:
+            self._bind_pose(P, dev)
         self._bound = self._signature(H, W)
+
+    def _bind_pose(self, P, dev):
+        """Buffers of the pose path: corrected matrices, their gradients, the pose gradients and the two Adam groups
+        (omega, nu) on the pose optimizer's own state tensors."""
+        if self.sharded:
+            raise RuntimeError("NativeTrainStep: pose refinement is not supported with Gaussian sharding (every rank "
+                               "would hold only its shard's part of the matrix gradients)")
+        corr, opt = self.pose, self.pose_opt
+        for name, p in (("omega", corr.omega), ("nu", corr.nu)):
+            if p.device != dev or p.dtype != torch.float32 or not p.is_contiguous():
+                raise RuntimeError(f"NativeTrainStep: pose {name} must be contiguous float32 on {dev}")
+        groups = [(g, g["params"]) for g in opt.param_groups]
+        if len(groups) != 2 or groups[0][1] != [corr.omega] or groups[1][1] != [corr.nu]:
+            raise RuntimeError("NativeTrainStep: the pose optimizer must hold two groups, [omega] and [nu]")
+        self.n_views = int(corr.omega.shape[0])
+        if not -1 <= self.pose_anchor < self.n_views:
+            raise ValueError(f"NativeTrainStep: pose anchor {self.pose_anchor} out of range for {self.n_views} views")
+        f32 = dict(dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            self.pose_view = torch.empty((4, 4), **f32); self.pose_full = torch.empty((4, 4), **f32)
+            self.pose_gview = torch.empty((4, 4), **f32); self.pose_gproj = torch.empty((4, 4), **f32)
+            self.pose_scratch_bytes = int(self.lib.r2x_raster_backward_pose_scratch_bytes(P))
+            self.pose_scratch = torch.empty(self.pose_scratch_bytes, dtype=torch.uint8, device=dev)
+            self.g_omega, self.g_nu = torch.empty_like(corr.omega), torch.empty_like(corr.nu)
+        self.pose_adam = []
+        for (group, _), p, g in zip(groups, (corr.omega, corr.nu), (self.g_omega, self.g_nu)):
+            st = opt.state[p]
+            if len(st) == 0:
+                st["step"] = torch.tensor(0.0, dtype=torch.float32)
+                st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+            self.pose_adam.append((group, p, st, g))
+        self.pose_groups = (AdamGroup * 2)()
+        for k, (group, p, st, g) in enumerate(self.pose_adam):
+            a = self.pose_groups[k]
+            a.param, a.grad, a.exp_avg, a.exp_avg_sq = p.data_ptr(), g.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr()
+            a.numel = p.numel()
 
     def _provision(self):
         """Instance capacities for this iteration: both forwards are speculative.  The buffers only ever grow."""
@@ -149,10 +206,13 @@ class NativeTrainStep:
                 self.binning_v, self.scratch_v = _C.binning_buffer(want_v, dev), _C.VOXEL.bwd_scratch(want_v, dev)
 
     # ------------------------------------------------------------------ one iteration
-    def __call__(self, cam, gt, tv_centre=None, apply_update: bool = True):
+    def __call__(self, cam, gt, tv_centre=None, apply_update: bool = True, view: int | None = None,
+                 pose_update: bool | None = None):
         """Enqueue one iteration.  `cam`: camera (render_query.render's contract); `gt`: [1,H,W] or [H,W] CUDA float32
-        target; `tv_centre`: 3 floats (ignored without TV).  Returns {"render", "radii", "loss" (device [3]: L1, SSIM,
-        image total), "tv" (device [1] or None)} -- views of buffers that the next call overwrites."""
+        target; `tv_centre`: 3 floats (ignored without TV).  With `pose`: `view` is the camera's row of the
+        PoseCorrection and `pose_update` (default: `apply_update`) whether the pose Adam steps.  Returns {"render",
+        "radii", "loss" (device [3]: L1, SSIM, image total), "tv" (device [1] or None)} -- views of buffers that the
+        next call overwrites."""
         self.check()                                            # the previous iteration (one late; no stall)
         H, W = int(cam.image_height), int(cam.image_width)
         if self._bound != self._signature(H, W):
@@ -162,11 +222,16 @@ class NativeTrainStep:
         # an EMPTY SHARD of a Gaussian-sharded run goes through the same sequence: the library calls are no-ops that
         # produce a zero image / volume (and zero status words), and the rank takes part in both exchanges with the same
         # buffer sizes as its peers
-        args = (cam, gt, None if tv_centre is None else tuple(float(v) for v in tv_centre), bool(apply_update))
+        pose_args = None
+        if self.pose is not None:
+            if view is None or not 0 <= int(view) < self.n_views:
+                raise ValueError(f"NativeTrainStep: pose refinement needs the view index (0..{self.n_views - 1}), got {view}")
+            pose_args = (int(view), bool(apply_update if pose_update is None else pose_update))
+        args = (cam, gt, None if tv_centre is None else tuple(float(v) for v in tv_centre), bool(apply_update), pose_args)
         self._enqueue(*args)
         return self.result
 
-    def _enqueue(self, cam, gt, tv_centre, apply_update):
+    def _enqueue(self, cam, gt, tv_centre, apply_update, pose_args):
         gm, lib, dev, P, H, W = self.gm, self.lib, self.dev, self.P, self.H, self.W
         self._provision()
         mode = int(cam.mode)
@@ -185,6 +250,13 @@ class NativeTrainStep:
         xyz, dens, scal, rot = gm._xyz, gm._density, gm._scaling, gm._rotation
         with torch.cuda.device(dev):
             st = torch.cuda.current_stream(dev).cuda_stream
+            if pose_args is not None:
+                # the corrected matrices of this view (the camera centre stays the camera's: the kernels never read it)
+                corr = self.pose
+                check(lib.r2x_pose_apply(st, corr.omega.data_ptr(), corr.nu.data_ptr(), self.n_views, pose_args[0],
+                                         view.data_ptr(), proj.data_ptr(), cam.projection_matrix.data_ptr(),
+                                         self.pose_view.data_ptr(), self.pose_full.data_ptr()), "r2x_pose_apply")
+                view, proj = self.pose_view, self.pose_full
             check(lib.r2x_raster_forward_async_raw(
                 st, P, W, H, xyz.data_ptr(), dens.data_ptr(), scal.data_ptr(), sm, rot.data_ptr(), view.data_ptr(),
                 proj.data_ptr(), campos.data_ptr(), tfx, tfy, mode, self.image.data_ptr(), self.radii.data_ptr(),
@@ -219,12 +291,29 @@ class NativeTrainStep:
                     self.img_v.data_ptr(), self.scratch_v.data_ptr(), self.dL_dvol.data_ptr(), self.gdv.data_ptr(),
                     self.g3v.data_ptr(), self.gcovv.data_ptr(), self.gsv.data_ptr(), self.grv.data_ptr(), act),
                     "r2x_voxel_backward_raw")
-            check(lib.r2x_raster_backward_raw(
-                st, P, self.cap_r, W, H, xyz.data_ptr(), scal.data_ptr(), sm, rot.data_ptr(), view.data_ptr(), proj.data_ptr(),
-                campos.data_ptr(), tfx, tfy, self.radii.data_ptr(), self.geom.data_ptr(), self.binning_r.data_ptr(),
-                self.img.data_ptr(), self.scratch_r.data_ptr(), self.dL_dimage.data_ptr(), self.g2.data_ptr(),
-                self.gd.data_ptr(), self.g3.data_ptr(), self.gcov.data_ptr(), self.gs.data_ptr(), self.gr.data_ptr(), mode,
-                act), "r2x_raster_backward_raw")
+            if pose_args is None:
+                check(lib.r2x_raster_backward_raw(
+                    st, P, self.cap_r, W, H, xyz.data_ptr(), scal.data_ptr(), sm, rot.data_ptr(), view.data_ptr(),
+                    proj.data_ptr(), campos.data_ptr(), tfx, tfy, self.radii.data_ptr(), self.geom.data_ptr(),
+                    self.binning_r.data_ptr(), self.img.data_ptr(), self.scratch_r.data_ptr(), self.dL_dimage.data_ptr(),
+                    self.g2.data_ptr(), self.gd.data_ptr(), self.g3.data_ptr(), self.gcov.data_ptr(), self.gs.data_ptr(),
+                    self.gr.data_ptr(), mode, act), "r2x_raster_backward_raw")
+            else:
+                # the same per-Gaussian gradients, bit for bit, plus dL/d(view, full), chained to the view's twist
+                check(lib.r2x_raster_backward_pose(
+                    st, P, self.cap_r, W, H, xyz.data_ptr(), scal.data_ptr(), sm, rot.data_ptr(), None, view.data_ptr(),
+                    proj.data_ptr(), campos.data_ptr(), tfx, tfy, self.radii.data_ptr(), self.geom.data_ptr(),
+                    self.binning_r.data_ptr(), self.img.data_ptr(), self.scratch_r.data_ptr(), self.dL_dimage.data_ptr(),
+                    self.g2.data_ptr(), self.gd.data_ptr(), None, self.g3.data_ptr(), self.gcov.data_ptr(),
+                    self.gs.data_ptr(), self.gr.data_ptr(), mode, 0, act, self.pose_gview.data_ptr(),
+                    self.pose_gproj.data_ptr(), self.pose_scratch.data_ptr(), self.pose_scratch_bytes),
+                    "r2x_raster_backward_pose")
+                corr = self.pose
+                check(lib.r2x_pose_grad(st, corr.omega.data_ptr(), corr.nu.data_ptr(), self.n_views, pose_args[0],
+                                        self.pose_anchor, cam.world_view_transform.data_ptr(),
+                                        cam.projection_matrix.data_ptr(), self.pose_gview.data_ptr(),
+                                        self.pose_gproj.data_ptr(), self.g_omega.data_ptr(), self.g_nu.data_ptr()),
+                      "r2x_pose_grad")
             guard_v = self.status_v.data_ptr() if self.use_tv else None
             check(lib.r2x_densify_stats(st, P, self.radii.data_ptr(), self.g2.data_ptr(), gm.max_radii2D.data_ptr(),
                                         gm.xyz_gradient_accum.data_ptr(), gm.denom.data_ptr(), self.status_r.data_ptr(),
@@ -242,11 +331,27 @@ class NativeTrainStep:
                                             C.cast(self.adam_grads2, C.c_void_p) if self.use_tv else None, float(b1),
                                             float(b2), float(self.adam[0][0]["eps"]), steps.pop(), self.status_r.data_ptr(),
                                             guard_v), "r2x_adam_step_sum")
+            if pose_args is not None and pose_args[1]:
+                # the pose optimizer's step, guarded by BOTH forwards' status words like the Gaussians' own
+                steps = set()
+                for k, (group, _p, stt, _g) in enumerate(self.pose_adam):
+                    stt["step"] += 1
+                    steps.add(int(stt["step"].item()))
+                    self.pose_groups[k].lr = float(group["lr"])
+                if len(steps) != 1:
+                    raise RuntimeError("NativeTrainStep: the pose parameters' Adam step counts differ")
+                pg = self.pose_adam[0][0]
+                b1, b2 = pg["betas"]
+                if self.pose_adam[1][0]["betas"] != pg["betas"] or self.pose_adam[1][0]["eps"] != pg["eps"]:
+                    raise RuntimeError("NativeTrainStep: the two pose groups must share betas and eps")
+                check(lib.r2x_adam_step_sum(st, 2, C.cast(self.pose_groups, C.c_void_p), None, float(b1), float(b2),
+                                            float(pg["eps"]), steps.pop(), self.status_r.data_ptr(), guard_v),
+                      "r2x_adam_step_sum")
             # the status words travel to pinned host memory behind an event; read one iteration late
             host = _C._Workspace.to_host(self.status_r), (_C._Workspace.to_host(self.status_v) if self.use_tv else None)
             ev = torch.cuda.Event()
             ev.record(torch.cuda.current_stream(dev))
-        self._pending = (host, ev, (cam, gt, tv_centre, apply_update))
+        self._pending = (host, ev, (cam, gt, tv_centre, apply_update, pose_args))
         self.result = {"render": image, "radii": self.radii, "viewspace_grad": self.g2, "loss": self.loss_out,
                        "tv": self.tv_out if self.use_tv else None}
 
@@ -271,6 +376,9 @@ class NativeTrainStep:
                 raise _C.CapacityOverflow("NativeTrainStep: the instance capacity keeps overflowing")
             if args[3]:
                 for _group, _p, stt, _g1, _g2 in self.adam:
+                    stt["step"] -= 1
+            if args[4] is not None and args[4][1]:
+                for _group, _p, stt, _g in self.pose_adam:
                     stt["step"] -= 1
             self._enqueue(*args)
             self.check()

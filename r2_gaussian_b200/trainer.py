@@ -13,6 +13,12 @@ Under `torchrun --nproc-per-node N` the same command trains Gaussian-sharded: ev
 cloud with its own Adam state and densification (budget `max_num_gaussians / N`), `render()` / `query()` sum the
 partial images / volumes over the ranks (NCCL, or the peer-memory kernel with `--peer_exchange`), the host RNG
 streams stay in lock-step (same seed, same draws), rank 0 writes one merged `point_cloud.pickle`.
+
+`--pose_refine` (single GPU only) also learns one rigid correction per train view (`pose.PoseCorrection`, row =
+`cam.uid`, train view 0 held at zero) with its own FusedAdam (`PoseParams` learning rates, log-linear over
+`--iterations`), on both training paths; the poses step wherever the Gaussians would and at densification iterations.
+Train views are then evaluated with their corrected cameras, each save writes `train_poses.npz` and checkpoints carry
+the poses.  Without the switch nothing changes: same launches, settings files, checkpoints and printed keys.
 """
 from __future__ import annotations
 
@@ -30,7 +36,10 @@ from . import losses
 from ._C import CapacityOverflow
 from .dataset import Scene
 from .gaussian_model import GaussianModel
+from .gaussian_utils import get_expon_lr_func
 from .metrics import metric_proj, metric_vol
+from .optim import FusedAdam
+from .pose import PoseCorrection
 from .render_query import query, render
 from . import sharded, train_step
 from .sharded import gather_point_cloud, shard_init_points, world_info
@@ -82,6 +91,21 @@ class OptimizationParams:
     max_num_gaussians: int | None = 500_000
 
 
+@dataclass
+class PoseParams:
+    """`--pose_refine`: learn one rigid correction per train view together with the scene (`pose.PoseCorrection`; train
+    view 0 anchors the frame).  Learning rates decay log-linearly from init to final over `--iterations`.  The defaults
+    are a starting point (rotation in rad, translation in scene units), not tuned on real scans."""
+    pose_refine: bool = False
+    pose_rotation_lr_init: float = 1e-3
+    pose_rotation_lr_final: float = 1e-5
+    pose_translation_lr_init: float = 5e-3
+    pose_translation_lr_final: float = 5e-5
+
+
+POSE_ANCHOR = 0     # the train view whose correction stays exactly zero
+
+
 def default_init_path(source_path: str) -> str:
     """`<scene>/init_<scene>.npy` for directories, `<dir>/init_<stem>.npy` for NAF pickles (`initialize.py:29-41`)."""
     if os.path.exists(os.path.join(source_path, "meta_data.json")):
@@ -107,9 +131,10 @@ def derived_settings(scanner_cfg: dict, model: ModelParams, opt: OptimizationPar
 
 
 @torch.no_grad()
-def evaluate(scene: Scene, gaussians: GaussianModel, pipe, with_ssim: bool = True) -> dict:
+def evaluate(scene: Scene, gaussians: GaussianModel, pipe, with_ssim: bool = True, pose=None) -> dict:
     """3-D PSNR / SSIM of the queried volume and 2-D PSNR / SSIM of the rendered train and test views, with the
-    reference's metric definitions (`train.py:262-330`, `utils/image_utils.py:90-183`)."""
+    reference's metric definitions (`train.py:262-330`, `utils/image_utils.py:90-183`).  `pose` (a PoseCorrection over
+    the train views): train views are rendered with their corrected cameras; test views keep their nominal poses."""
     cfg = scene.scanner_cfg
     vol = query(gaussians, cfg["offOrigin"], cfg["nVoxel"], cfg["sVoxel"], pipe)["vol"]
     out = {"psnr_3d": metric_vol(scene.vol_gt, vol, "psnr")[0]}
@@ -118,6 +143,8 @@ def evaluate(scene: Scene, gaussians: GaussianModel, pipe, with_ssim: bool = Tru
     for name, cams in (("train", scene.getTrainCameras()), ("test", scene.getTestCameras())):
         if not cams:
             continue
+        if name == "train" and pose is not None:
+            cams = [pose.device_camera(c, c.uid, POSE_ANCHOR) for c in cams]
         imgs = torch.concat([render(c, gaussians, pipe)["render"] for c in cams], 0).permute(1, 2, 0)
         gts = torch.concat([c.original_image.to(imgs.device) for c in cams], 0).permute(1, 2, 0)
         out[f"psnr_2d_{name}"] = metric_proj(gts, imgs, "psnr")[0]
@@ -128,8 +155,12 @@ def evaluate(scene: Scene, gaussians: GaussianModel, pipe, with_ssim: bool = Tru
 
 def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, testing_iterations=(),
              saving_iterations=(), checkpoint_iterations=(), checkpoint: str | None = None, init_points=None,
-             log=print) -> dict:
+             log=print, pose_params: PoseParams | None = None) -> dict:
     first_iter = 0
+    refine = pose_params is not None and pose_params.pose_refine
+    if refine and world_info()[1] > 1:
+        raise RuntimeError("--pose_refine is not supported with Gaussian sharding (WORLD_SIZE > 1): every rank would "
+                           "hold only its shard's part of the camera-matrix gradients")
     scene = Scene(model.source_path, model.model_path, eval=model.eval, shuffle=False, device="cuda",
                   data_device=model.data_device)
     cfg = scene.scanner_cfg
@@ -158,6 +189,16 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
     gaussians.create_from_pcd(init_points[:, :3], init_points[:, 3:4], 1.0, dist2=dist2)
     scene.gaussians = gaussians
     gaussians.training_setup(opt)
+    corr = pose_opt = pose_lr = None
+    if refine:
+        # one correction per train camera, row = cam.uid (its position in getTrainCameras())
+        corr = PoseCorrection(len(scene.getTrainCameras()), device="cuda")
+        pose_opt = FusedAdam([{"params": [corr.omega], "lr": 0.0, "name": "omega"},
+                              {"params": [corr.nu], "lr": 0.0, "name": "nu"}], lr=0.0, eps=1e-15)
+        pose_lr = (get_expon_lr_func(pose_params.pose_rotation_lr_init, pose_params.pose_rotation_lr_final,
+                                     max_steps=opt.iterations),
+                   get_expon_lr_func(pose_params.pose_translation_lr_init, pose_params.pose_translation_lr_final,
+                                     max_steps=opt.iterations))
     if checkpoint is not None:
         path = rank_checkpoint_path(checkpoint, rank, world)
         payload = torch.load(path, weights_only=False)
@@ -166,7 +207,19 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
         if (tag["rank"], tag["world"]) != (rank, world):
             raise RuntimeError(f"checkpoint {path} was written by rank {tag['rank']} of {tag['world']}; this process is "
                                f"rank {rank} of {world} (a Gaussian-sharded run resumes with the same number of ranks)")
+        pose_state = payload[3] if len(payload) > 3 else None
+        if refine != (pose_state is not None):
+            raise RuntimeError(f"checkpoint {path} was written {'with' if pose_state is not None else 'without'} "
+                               f"--pose_refine; resume it with the same setting")
         gaussians.restore(model_state, opt)
+        if refine:
+            if tuple(pose_state["omega"].shape) != tuple(corr.omega.shape):
+                raise RuntimeError(f"checkpoint {path} holds poses of {pose_state['omega'].shape[0]} train views, the "
+                                   f"scene has {corr.omega.shape[0]}")
+            with torch.no_grad():
+                corr.omega.copy_(pose_state["omega"])
+                corr.nu.copy_(pose_state["nu"])
+            pose_opt.load_state_dict(pose_state["optimizer"])
         log(f"Load checkpoint {os.path.basename(path)}.")
 
     use_tv = opt.lambda_tv > 0
@@ -180,7 +233,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
     native = None
     if train_step.enabled() and not getattr(pipe, "debug", False) and not getattr(pipe, "compute_cov3D_python", False):
         native = train_step.NativeTrainStep(gaussians, opt.lambda_dssim, opt.lambda_tv if use_tv else 0.0, tv_n,
-                                            [float(v) for v in tv_s])
+                                            [float(v) for v in tv_s],
+                                            **({} if corr is None else dict(pose=(corr, pose_opt), pose_anchor=POSE_ANCHOR)))
     if world > 1:
         # one exchange of each shape before the clock starts: the NCCL communicator / the peer-memory reducers are
         # created on first use (seconds at 8 ranks), which is set-up, not a training step
@@ -214,6 +268,9 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
             torch.cuda.synchronize()
             t_mark = (time.perf_counter(), t_aside, iteration - 1)
         gaussians.update_learning_rate(iteration)
+        if corr is not None:
+            for group, schedule in zip(pose_opt.param_groups, pose_lr):
+                group["lr"] = schedule(iteration)
         if not stack:
             stack = scene.getTrainCameras().copy()
         cam = stack.pop(random.randint(0, len(stack) - 1))
@@ -227,8 +284,10 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
             # fixed launch sequence, no autograd (train_step.py).  At a densification iteration the reference's
             # optimizer.step() comes AFTER the tensors were replaced and therefore applies nothing (their .grad is None,
             # train.py:158-176): the same here.
+            # The pose gradient is valid at a densification iteration too, so the poses step there (both paths).
             gt = cam.original_image.cuda()
-            native(cam, gt, centre, apply_update=(iteration < opt.iterations) and not densify_due)
+            pose_kw = {} if corr is None else dict(view=cam.uid, pose_update=iteration < opt.iterations)
+            native(cam, gt, centre, apply_update=(iteration < opt.iterations) and not densify_due, **pose_kw)
             total = None
             with torch.no_grad():
                 if densify_due:
@@ -236,7 +295,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                     gaussians.densify_and_prune(opt.densify_grad_threshold, opt.density_min_threshold, opt.max_screen_size,
                                                 ds["max_scale"], opt.max_num_gaussians, ds["densify_scale_threshold"], bbox)
         else:
-            pkg = render(cam, gaussians, pipe)
+            view_cam = (lambda: cam) if corr is None else (lambda: corr.device_camera(cam, cam.uid, POSE_ANCHOR))
+            pkg = render(view_cam(), gaussians, pipe)
             gt = cam.original_image.cuda()
             loss = losses.image_loss(pkg["render"], gt, lambda_dssim=opt.lambda_dssim)
             total = loss["total"]
@@ -249,7 +309,9 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                 # a speculative forward (no host sync) ran out of instance capacity: its image was all zeros and this
                 # step's gradients are void.  The capacity hint has been raised; redo the step with the same camera.
                 gaussians.optimizer.zero_grad(set_to_none=True)
-                pkg = render(cam, gaussians, pipe)
+                if pose_opt is not None:
+                    pose_opt.zero_grad(set_to_none=True)
+                pkg = render(view_cam(), gaussians, pipe)
                 total = losses.image_loss(pkg["render"], gt, lambda_dssim=opt.lambda_dssim)["total"]
                 if use_tv:
                     total = total + opt.lambda_tv * losses.tv_3d_loss(query(gaussians, centre, tv_n, tv_s, pipe)["vol"],
@@ -272,6 +334,9 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
             if total is not None and iteration < opt.iterations:
                 gaussians.optimizer.step()
                 gaussians.optimizer.zero_grad(set_to_none=True)
+                if pose_opt is not None:
+                    pose_opt.step()
+                    pose_opt.zero_grad(set_to_none=True)
             if native is not None and (iteration in saving_iterations or iteration in checkpoint_iterations or
                                        iteration in testing_iterations or iteration == opt.iterations):
                 native.flush()       # the last enqueued iteration is checked (and repeated if it had overflowed)
@@ -280,6 +345,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                 with _aside():
                     if world == 1:
                         scene.save(iteration, queryfunc)
+                        if corr is not None:
+                            save_train_poses(scene, corr, iteration)
                     else:
                         save_sharded(scene, gaussians, iteration, queryfunc, rank)
             if scene.model_path and iteration in checkpoint_iterations:
@@ -288,6 +355,10 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                     name = os.path.basename(rank_checkpoint_path(f"chkpnt{iteration}.pth", rank, world))
                     payload = (gaussians.capture(), iteration) if world == 1 else \
                         (gaussians.capture(), iteration, {"rank": rank, "world": world})
+                    if corr is not None:    # (model, iteration, tag, poses): written only with --pose_refine
+                        payload = (payload[0], iteration, {"rank": rank, "world": world},
+                                   {"omega": corr.omega.detach().cpu(), "nu": corr.nu.detach().cpu(),
+                                    "optimizer": pose_opt.state_dict()})
                     torch.save(payload, os.path.join(ckpt_dir, name))
                     if world > 1:
                         torch.distributed.barrier()  # no rank runs ahead into the next exchange while others write
@@ -297,7 +368,7 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                     sharded.check_peer_exchange()    # the loss read-out above synchronised anyway
             if iteration in testing_iterations:
                 with _aside():
-                    history["eval"][iteration] = evaluate(scene, gaussians, pipe)
+                    history["eval"][iteration] = evaluate(scene, gaussians, pipe, pose=corr)
                 log(f"[ITER {iteration}] {history['eval'][iteration]}  points {gaussians.get_xyz.shape[0]}")
                 if world > 1:
                     sharded.check_peer_exchange()
@@ -315,7 +386,20 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
     history["iterations"] = opt.iterations - first_iter
     history["gaussians"] = int(gaussians.get_xyz.shape[0])
     history["scene"], history["model"] = scene, gaussians
+    if corr is not None:
+        history["pose"] = corr
     return history
+
+
+@torch.no_grad()
+def save_train_poses(scene: Scene, corr, iteration: int):
+    """`point_cloud/iteration_<N>/train_poses.npz`: omega / nu [n,3], the corrected world_view_transform [n,4,4] of every
+    train view (row = cam.uid, stored transposed like the camera's) and the nominal angles [n] of the dataset."""
+    cams = scene.getTrainCameras()
+    wvt = torch.stack([corr.device_camera(c, c.uid, POSE_ANCHOR).world_view_transform for c in cams])
+    np.savez(os.path.join(scene.model_path, f"point_cloud/iteration_{iteration}", "train_poses.npz"),
+             omega=corr.omega.detach().cpu().numpy(), nu=corr.nu.detach().cpu().numpy(),
+             world_view_transform=wvt.cpu().numpy(), angle=np.array([float(c.angle) for c in cams]))
 
 
 def rank_checkpoint_path(path: str, rank: int, world: int) -> str:
@@ -353,15 +437,20 @@ def write_eval_yaml(model_path: str, iteration: int, ev: dict):
                 yaml.dump(d2, f, default_flow_style=False, sort_keys=False)
 
 
-def write_cfg_args(model_path: str, model, pipe, opt, extra: dict):
+def write_cfg_args(model_path: str, model, pipe, opt, extra: dict, pose: PoseParams | None = None):
     """`<model_path>/cfg_args`: the Namespace repr the reference's test.py evaluates (`arguments/__init__.py:74-95`,
-    written by `utils/log_utils.py:28-29`), with the reference's field names, next to a JSON copy."""
+    written by `utils/log_utils.py:28-29`), with the reference's field names, next to a JSON copy.  The pose settings
+    are added (flat, and as "pose" in the JSON) only when `pose.pose_refine` is on."""
     from argparse import Namespace
-    flat = {**asdict(model), **asdict(pipe), **asdict(opt), **extra}
+    pose_fields = asdict(pose) if pose is not None and pose.pose_refine else {}
+    flat = {**asdict(model), **asdict(pipe), **asdict(opt), **pose_fields, **extra}
     with open(os.path.join(model_path, "cfg_args"), "w") as f:
         f.write(str(Namespace(**flat)))
+    doc = {"model": asdict(model), "pipe": asdict(pipe), "opt": asdict(opt)}
+    if pose_fields:
+        doc["pose"] = pose_fields
     with open(os.path.join(model_path, "cfg_args.json"), "w") as f:
-        json.dump({"model": asdict(model), "pipe": asdict(pipe), "opt": asdict(opt)}, f, indent=1)
+        json.dump(doc, f, indent=1)
 
 
 def save_sharded(scene: Scene, gaussians: GaussianModel, iteration: int, queryfunc, rank: int):
@@ -396,13 +485,15 @@ def _add_dataclass_args(parser, cls, skip=()):
             parser.add_argument("--" + name, default=default, type=typ)
 
 
-def main(argv=None):
+def parse_args(argv=None):
+    """-> (argparse namespace, ModelParams, PipelineParams, OptimizationParams, PoseParams) of the command line."""
     ap = argparse.ArgumentParser(description="Train R2-Gaussian on one scene (H100-native pipeline)")
     ap.add_argument("-s", "--source_path", required=True)
     ap.add_argument("-m", "--model_path", default="")
     _add_dataclass_args(ap, ModelParams, skip=("source_path", "model_path"))
     _add_dataclass_args(ap, PipelineParams)
     _add_dataclass_args(ap, OptimizationParams)
+    _add_dataclass_args(ap, PoseParams)
     ap.add_argument("--test_iterations", nargs="+", type=int, default=[5000, 10000, 20000, 30000])
     ap.add_argument("--save_iterations", nargs="+", type=int, default=[])
     ap.add_argument("--checkpoint_iterations", nargs="+", type=int, default=[])
@@ -412,7 +503,15 @@ def main(argv=None):
                     help="multi-GPU: sum partial images / volumes with the NVLink peer-memory kernel instead of NCCL")
     a = ap.parse_args(argv)
     pick = lambda cls: cls(**{k: getattr(a, k) for k in cls.__dataclass_fields__})
-    model, pipe, opt = pick(ModelParams), pick(PipelineParams), pick(OptimizationParams)
+    model, pipe, opt, pose = pick(ModelParams), pick(PipelineParams), pick(OptimizationParams), pick(PoseParams)
+    if pose.pose_refine and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        ap.error("--pose_refine is not supported with Gaussian sharding (WORLD_SIZE > 1): every rank would hold only "
+                 "its shard's part of the camera-matrix gradients; train on one GPU")
+    return a, model, pipe, opt, pose
+
+
+def main(argv=None):
+    a, model, pipe, opt, pose = parse_args(argv)
     model.source_path = os.path.abspath(model.source_path)
     if not model.model_path:
         model.model_path = os.path.join("./output", os.path.basename(model.source_path.rstrip("/")))
@@ -421,7 +520,7 @@ def main(argv=None):
         write_cfg_args(model.model_path, model, pipe, opt,
                        {"test_iterations": a.test_iterations, "save_iterations": a.save_iterations,
                         "checkpoint_iterations": a.checkpoint_iterations, "start_checkpoint": a.start_checkpoint,
-                        "quiet": False, "config": None, "detect_anomaly": False})
+                        "quiet": False, "config": None, "detect_anomaly": False}, pose)
     random.seed(a.seed), np.random.seed(a.seed), torch.manual_seed(a.seed)     # safe_state (`general_utils.py:61-63`)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if world > 1:                      # launched by torchrun: one process per GPU, Gaussians sharded by index
@@ -435,7 +534,7 @@ def main(argv=None):
             from .sharded import enable_peer_exchange
             enable_peer_exchange(True)
     hist = training(model, opt, pipe, set(a.test_iterations) | {opt.iterations}, set(a.save_iterations),
-                    set(a.checkpoint_iterations), a.start_checkpoint)
+                    set(a.checkpoint_iterations), a.start_checkpoint, pose_params=pose)
     final = hist["eval"].get(opt.iterations, {})
     if world > 1:
         import torch.distributed as dist
