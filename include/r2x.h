@@ -98,6 +98,34 @@ int r2x_raster_backward(void* stream, int P, long long R, int W, int H, const fl
                         float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale, float* dL_drot, int mode,
                         int debug);
 
+/* ---- batched views: N views of one cloud in one call ---------------------------------------------
+ * All views share W, H, tan_fovx / tan_fovy, mode and scale_modifier; view v has its own
+ * viewmatrices[16 v .. 16 v + 15] / projmatrices[16 v ..] (column-major as the single-view calls).
+ * out_color[N,H,W]; radii[N,P].  Image v and radii[v] are bit for bit what r2x_raster_forward_async
+ * computes for view v alone.  The views are the bands of one stacked tile grid (view v owns tile rows
+ * [v ceil(H/16), (v+1) ceil(H/16))), binned and rendered together; N * ceil(H/16) must be <= 65535.
+ * The instance count R is the sum over the views; capacity / status_dev as r2x_raster_forward_async.
+ * Scales and rotations are required (no cov3D_precomp). */
+size_t r2x_raster_views_geom_bytes(int P, int N);
+size_t r2x_raster_views_image_bytes(int P, int N, int W, int H);
+int r2x_raster_forward_views_async(void* stream, int P, int N, int W, int H, const float* means3D,
+                                   const float* opacities, const float* scales, float scale_modifier,
+                                   const float* rotations, const float* viewmatrices, const float* projmatrices,
+                                   float tan_fovx, float tan_fovy, int mode, float* out_color, int* radii,
+                                   void* geom_buf, void* image_buf, void* binning_buf, long long capacity,
+                                   uint32_t* status_dev);
+/* dL_dpix[N,H,W].  Per-Gaussian gradients are summed over the views in view order in float32
+ * (acc = g[0]; acc = acc + g[v]), where g[v] is what r2x_raster_backward returns for view v alone:
+ * dL_dopacity[P], dL_dmean3D[P,3], dL_dcov3D[P,6], dL_dscale[P,3], dL_drot[P,4].  dL_dmean2D[N,P,3] is
+ * kept per view (densification statistics).  R and scratch as r2x_raster_backward. */
+int r2x_raster_backward_views(void* stream, int P, int N, long long R, int W, int H, const float* means3D,
+                              const float* scales, float scale_modifier, const float* rotations,
+                              const float* viewmatrices, const float* projmatrices, float tan_fovx, float tan_fovy,
+                              const int* radii, const void* geom_buf, const void* binning_buf, const void* image_buf,
+                              void* scratch, const float* dL_dpix, float* dL_dmean2D, float* dL_dopacity,
+                              float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale, float* dL_drot, int mode,
+                              int debug);
+
 /* Stage entry points for measurement (bench.py roofline, ncu): re-run ONLY the per-tile accumulation
  * kernel (the reference's renderCUDA, RAS/forward.cu:294-395 / VOX/forward.cu:183-315) on the state a
  * previous forward left in the three buffers.  `R` = the count the binning buffer was carved for. */

@@ -377,6 +377,91 @@ def rasterize_gaussians_backward_matrices(means3D, radii, scales, rotations, sca
     return g_mean2D, g_op, g_mu, g_mean3D, g_cov, g_scale, g_rot, g_view, g_proj
 
 
+def views_key(dev: torch.device, P: int, N: int, W: int, H: int) -> tuple:
+    """Capacity-hint key of a batched-views shape (its instance count is the sum over the N views)."""
+    return ("raster_views", dev.index, int(P), int(N), int(W), int(H))
+
+
+def views_state(P: int, N: int, W: int, H: int, dev) -> tuple[torch.Tensor, torch.Tensor]:
+    """(geom, image) buffers of one batched forward of N views."""
+    lib = load()
+    return _u8(lib.r2x_raster_views_geom_bytes(P, N), dev), _u8(lib.r2x_raster_views_image_bytes(P, N, W, H), dev)
+
+
+def check_views_args(means3D, viewmatrices, projmatrices) -> int:
+    """Shape checks of a batched-views call (no CUDA call) -> N."""
+    if means3D.ndim != 2 or means3D.shape[1] != 3:
+        raise ValueError("means3D must have dimensions (num_points, 3)")
+    if viewmatrices.ndim != 3 or tuple(viewmatrices.shape[1:]) != (4, 4) or viewmatrices.shape[0] < 1:
+        raise ValueError(f"viewmatrices must have dimensions (N >= 1, 4, 4), got {tuple(viewmatrices.shape)}")
+    if tuple(projmatrices.shape) != tuple(viewmatrices.shape):
+        raise ValueError(f"projmatrices {tuple(projmatrices.shape)} must match viewmatrices {tuple(viewmatrices.shape)}")
+    return int(viewmatrices.shape[0])
+
+
+def rasterize_views(means3D, opacity, scales, rotations, scale_modifier, viewmatrices, projmatrices, tan_fovx, tan_fovy,
+                    image_height, image_width, mode):
+    """N views of one cloud in one call -> (num_rendered, images[N,H,W], radii[N,P] int32, geom, binning, img).
+
+    Image v and radii[v] are bit for bit what `rasterize_gaussians` computes for view v alone.  num_rendered (summed
+    over the views) is a `NumRendered` carrying the binning buffer's capacity, with the same overflow handling as the
+    single-view call."""
+    N = check_views_args(means3D, viewmatrices, projmatrices)
+    for t, name in ((means3D, "means3D"), (viewmatrices, "viewmatrices"), (projmatrices, "projmatrices")):
+        _require_cuda(t, name)
+    lib = load()
+    dev = means3D.device
+    P, H, W = int(means3D.shape[0]), int(image_height), int(image_width)
+    with torch.cuda.device(dev):
+        means3D = _f32(means3D, dev); opacity = _f32(opacity, dev)
+        scales = _f32(scales, dev); rotations = _f32(rotations, dev)
+        viewmatrices = _f32(viewmatrices, dev); projmatrices = _f32(projmatrices, dev)
+        images = torch.empty((N, H, W), dtype=torch.float32, device=dev)
+        radii = torch.empty((N, P), dtype=torch.int32, device=dev)
+        geom, img = views_state(P, N, W, H, dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+
+        def launch(binning, cap, status):
+            rc = lib.r2x_raster_forward_views_async(
+                stream, P, N, W, H, _ptr(means3D), _ptr(opacity), _ptr(scales), float(scale_modifier),
+                _ptr(rotations), _ptr(viewmatrices), _ptr(projmatrices), float(tan_fovx), float(tan_fovy), int(mode),
+                images.data_ptr(), _ptr(radii), geom.data_ptr(), img.data_ptr(), binning.data_ptr(), cap,
+                status.data_ptr())
+            check(rc, "r2x_raster_forward_views_async")
+
+        R, binning = _forward(launch, views_key(dev, P, N, W, H), P * N, RASTER.seed, dev)
+    return R, images, radii, geom, binning, img
+
+
+def rasterize_views_backward(means3D, radii, scales, rotations, scale_modifier, viewmatrices, projmatrices, tan_fovx,
+                             tan_fovy, dL_dimages, geomBuffer, R, binningBuffer, imageBuffer, mode, debug=False):
+    """-> (dL_dmeans2D[N,P,3] per view, dL_dopacity[P,1], dL_dmeans3D[P,3], dL_dcov3D[P,6], dL_dscales[P,3],
+    dL_drotations[P,4]); the per-Gaussian gradients are summed over the views in view order (float32)."""
+    N = check_views_args(means3D, viewmatrices, projmatrices)
+    _require_cuda(means3D, "means3D")
+    lib = load()
+    dev = means3D.device
+    P = int(means3D.shape[0])
+    H, W = int(dL_dimages.shape[-2]), int(dL_dimages.shape[-1])
+    with torch.cuda.device(dev):
+        means3D = _f32(means3D, dev); scales = _f32(scales, dev); rotations = _f32(rotations, dev)
+        viewmatrices = _f32(viewmatrices, dev); projmatrices = _f32(projmatrices, dev); dL = _f32(dL_dimages, dev)
+        opts = dict(dtype=torch.float32, device=dev)
+        g_mean2D = torch.empty((N, P, 3), **opts); g_op = torch.empty((P, 1), **opts)
+        g_mean3D = torch.empty((P, 3), **opts); g_cov = torch.empty((P, 6), **opts)
+        g_scale = torch.empty((P, 3), **opts); g_rot = torch.empty((P, 4), **opts)
+        R = _carved_capacity(binningBuffer, R)
+        scratch = RASTER.bwd_scratch(R, dev)
+        rc = lib.r2x_raster_backward_views(
+            torch.cuda.current_stream(dev).cuda_stream, P, N, R, W, H, _ptr(means3D), _ptr(scales),
+            float(scale_modifier), _ptr(rotations), _ptr(viewmatrices), _ptr(projmatrices), float(tan_fovx),
+            float(tan_fovy), _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imageBuffer), scratch.data_ptr(),
+            _ptr(dL), _ptr(g_mean2D), _ptr(g_op), _ptr(g_mean3D), _ptr(g_cov), _ptr(g_scale), _ptr(g_rot), int(mode),
+            int(bool(debug)))
+        check(rc, "r2x_raster_backward_views")
+    return g_mean2D, g_op, g_mean3D, g_cov, g_scale, g_rot
+
+
 def mark_visible(means3D, viewmatrix, projmatrix):
     """-> bool[P]: view-space z > 0.2 (RAS/auxiliary.h:143-168)."""
     _require_cuda(means3D, "means3D")

@@ -34,6 +34,12 @@ PROTOTYPES = {
                                       _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
     "r2x_raster_backward": (_i, [_vp, _i, _ll, _i, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _f, _f, _vp,
                                  _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i]),
+    "r2x_raster_views_geom_bytes": (_sz, [_i, _i]),
+    "r2x_raster_views_image_bytes": (_sz, [_i, _i, _i, _i]),
+    "r2x_raster_forward_views_async": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _f, _vp, _vp, _vp, _f, _f, _i, _vp, _vp,
+                                            _vp, _vp, _vp, _ll, _vp]),
+    "r2x_raster_backward_views": (_i, [_vp, _i, _i, _ll, _i, _i, _vp, _vp, _f, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _vp,
+                                       _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i]),
     "r2x_raster_render_only": (_i, [_vp, _i, _i, _i, _ll, _vp, _vp, _vp, _vp]),
     "r2x_voxel_render_only": (_i, [_vp, _i, _i, _i, _i, _ll, _vp, _vp, _vp, _vp]),
     "r2x_mark_visible": (_i, [_vp, _i, _vp, _vp, _vp, _vp]),

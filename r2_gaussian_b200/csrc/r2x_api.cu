@@ -142,25 +142,28 @@ struct ImageViews {
 };
 // image buffer = ranges[T] | work plan | direct-binning table (T <= DIRECT_MAX_TILES) or two-level scratch (sized by the
 // geometry alone, whatever R2X_VOXEL_BINNING says).  Returns the size r2x_*_image_bytes reports; carves *v when given.
-size_t image_layout(const void* buf, int P, const Pipeline& pp, const BinningView& bv, ImageViews* v) {
+// With `vb` (batched views; pp is the stacked grid, P the virtual Gaussian count) the direct table is the banded one.
+size_t image_layout(const void* buf, int P, const Pipeline& pp, const BinningView& bv, ImageViews* v,
+                    const ViewBands* vb = nullptr) {
     const size_t t = (size_t)pp.gx * pp.gy * pp.gz;
     const int T = (int)t;
     const size_t head = al(t * sizeof(uint2)) + plan_bytes(T);
     const bool direct = pp.path() == BinPath::Direct;
-    const size_t tail = direct ? directbin_bytes(P, T) : pp.two_level ? two_level_bytes(P, pp.gx, pp.gy, pp.gz) : 0;
+    const size_t tail = direct ? (vb ? directbin_views_bytes(*vb) : directbin_bytes(P, T))
+                        : pp.two_level ? two_level_bytes(P, pp.gx, pp.gy, pp.gz) : 0;
     if (v) {
         char* base = (char*)al((size_t)buf);
         v->ranges = (uint2*)base;
         v->plan = plan_view(base + al(t * sizeof(uint2)), T, bv);
         v->plan.chunk_cap = pp.chunk_cap;
-        v->db = direct ? directbin_view(base + head, P, T) : DirectBin{};
+        v->db = !direct ? DirectBin{} : vb ? directbin_views_view(base + head, *vb) : directbin_view(base + head, P, T);
         v->tl = (!direct && tail) ? two_level_view(base + head, P, pp.gx, pp.gy, pp.gz, bv) : TwoLevel{};
     }
     return head + tail + 1024;
 }
-ImageViews image_views(const void* buf, int P, const Pipeline& pp, const BinningView& bv) {
+ImageViews image_views(const void* buf, int P, const Pipeline& pp, const BinningView& bv, const ViewBands* vb = nullptr) {
     ImageViews v;
-    image_layout(buf, P, pp, bv, &v);
+    image_layout(buf, P, pp, bv, &v, vb);
     return v;
 }
 
@@ -305,14 +308,16 @@ int bin_forward(cudaStream_t st, const Pipeline& pp, BinPath path, int P, const 
                 const uint32_t* tiles_touched, uint32_t* offsets, void* scan_state, uint32_t* status,
                 const void* image_buf, r2x_alloc_fn binning_alloc, void* alloc_user, void* binning_buf,
                 long long capacity, uint32_t* status_dev, int debug, int* num_rendered, BinningView* bv,
-                ImageViews* img) {
+                ImageViews* img, const ViewBands* vb = nullptr) {
     const std::string fn = std::string("r2x_") + pp.name + "_forward";
     if (path == BinPath::Direct) {
         // tile ranges, work plan and R come straight from the per-CTA tile histograms (the plan's extra-item list,
         // which lives in the binning buffer, is written by direct_fill)
-        const ImageViews pre = image_views(image_buf, P, pp, BinningView{});
+        const ImageViews pre = image_views(image_buf, P, pp, BinningView{}, vb);
         const long long cap0 = binning_alloc ? (1ll << 62) : capacity;
-        R2X_TRY(launch_direct_scan(st, pre.db, pre.ranges, pre.plan, status, cap0, binning_alloc ? nullptr : status_dev));
+        uint32_t* sd = binning_alloc ? nullptr : status_dev;
+        if (vb) R2X_TRY(launch_direct_scan_views(st, pre.db, *vb, pre.ranges, pre.plan, status, cap0, sd));
+        else R2X_TRY(launch_direct_scan(st, pre.db, pre.ranges, pre.plan, status, cap0, sd));
     } else {
         R2X_TRY(launch_scan(st, P, tiles_touched, offsets, scan_state, status));
     }
@@ -329,9 +334,13 @@ int bin_forward(cudaStream_t st, const Pipeline& pp, BinPath path, int P, const 
         return fail_msg(R2X_ERR_INVALID, (fn + "_async: no binning buffer").c_str());
     }
     *bv = binning_view(binning_buf, capacity);
-    *img = image_views(image_buf, P, pp, *bv);
+    *img = image_views(image_buf, P, pp, *bv, vb);
     if (path == BinPath::Direct) {
-        R2X_TRY(launch_direct_fill(st, P, cube, tiles_touched, offsets, img->db, img->plan, *bv, pp.gx, pp.gy, status));
+        if (vb)
+            R2X_TRY(launch_direct_fill_views(st, P, cube, tiles_touched, offsets, img->db, *vb, img->plan, *bv, pp.gx, pp.gy,
+                                             status));
+        else
+            R2X_TRY(launch_direct_fill(st, P, cube, tiles_touched, offsets, img->db, img->plan, *bv, pp.gx, pp.gy, status));
     } else {
         status_kernel<<<1, 1, 0, st>>>(status, capacity, status_dev);
         if (path == BinPath::TwoLevel) {
@@ -377,6 +386,89 @@ int raster_forward_impl(cudaStream_t st, int P, int W, int H, const float* means
     R2X_TRY(launch_raster_render(st, W, H, s.geom, img.ranges, bv.point_list, img.plan, bv.capacity, out_color));
     R2X_TRY(debug_sync(st, debug, "raster render"));
     return 0;
+}
+
+// ---- batched views: N views of one cloud as the bands of one stacked tile grid (ViewBands, r2x_binning.cuh) ----------
+struct ViewsShape {
+    int Pv;         // virtual Gaussians N * Pp
+    ViewBands vb;
+    Pipeline pp;    // the stacked grid gx x gy x N (z = view)
+};
+// Checks the sizes (no CUDA call) and derives the layout of a batched forward / backward.
+int views_shape(const char* fn, int P, int N, int W, int H, ViewsShape* s) {
+    if (N < 1) return fail_msg(R2X_ERR_INVALID, (std::string(fn) + ": bad N (need at least one view)").c_str());
+    if (W <= 0 || H <= 0 || P < 0) return fail_msg(R2X_ERR_INVALID, (std::string(fn) + ": bad P/W/H").c_str());
+    const long long gx = (W + R2X_TILE - 1) / R2X_TILE, gy = (H + R2X_TILE - 1) / R2X_TILE;
+    if (gx > 65535 || (long long)N * gy > 65535)
+        return fail_msg(R2X_ERR_INVALID, (std::string(fn) + ": bad N/W/H (too many tile rows: N * ceil(H / 16) and "
+                                                             "ceil(W / 16) must be <= 65535)").c_str());
+    const long long Pp = ((long long)(P > 0 ? P : 1) + DIRECT_BLOCK - 1) / DIRECT_BLOCK * DIRECT_BLOCK;
+    if (Pp * N > (1ll << 31) - 1 || gx * gy * N > (1ll << 30))
+        return fail_msg(R2X_ERR_INVALID, (std::string(fn) + ": bad N/P (too many views x Gaussians or tiles)").c_str());
+    s->Pv = (int)(Pp * N);
+    s->vb = ViewBands{N, (int)(gx * gy), (int)(Pp / DIRECT_BLOCK)};
+    s->pp = Pipeline{"raster_views", (int)gx, (int)gy, N, false, PLAN_CHUNK};
+    return 0;
+}
+
+int raster_views_forward_impl(cudaStream_t st, int P, int N, int W, int H, const float* means3D, const float* opacities,
+                              const float* scales, float scale_modifier, const float* rotations, const float* viewmatrices,
+                              const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float* out, int* radii,
+                              void* geom_buf, void* image_buf, void* binning_buf, long long capacity,
+                              uint32_t* status_dev) {
+    const char* fn = "r2x_raster_forward_views_async";
+    ViewsShape vs;
+    R2X_TRY(views_shape(fn, P, N, W, H, &vs));
+    if (!out || !geom_buf || !image_buf) return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward_views_async: null output/state buffer");
+    if (mode != 0 && mode != 1)
+        return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward_views_async: mode must be 0 (parallel) or 1 (cone)");
+    if (!binning_buf || capacity < 0) return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward_views_async: no binning buffer");
+    if (P > 0 && (!means3D || !opacities || !scales || !rotations || !radii || !viewmatrices || !projmatrices))
+        return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward_views_async: null input");
+    RasterState s = carve_raster(geom_buf, vs.Pv, W, H);   // the tile grid of one view
+    if (P == 0) return forward_empty(st, vs.pp, out, (size_t)N * W * H, image_buf, s.status, status_dev);
+    const BinPath path = vs.pp.path();
+    ImageViews img = image_views(image_buf, vs.Pv, vs.pp, BinningView{}, &vs.vb);
+    R2X_TRY(launch_raster_preprocess_views(st, P, N, means3D, scales, scale_modifier, rotations, opacities, viewmatrices,
+                                           projmatrices, W, H, tan_fovx, tan_fovy, mode, radii, s.geom,
+                                           path == BinPath::Direct ? &img.db : nullptr, vs.vb));
+    BinningView bv;
+    R2X_TRY(bin_forward(st, vs.pp, path, vs.Pv, s.geom.cube, s.geom.tiles_touched, s.geom.offsets, s.scan_state, s.status,
+                        image_buf, nullptr, nullptr, binning_buf, capacity, status_dev, 0, nullptr, &bv, &img, &vs.vb));
+    return launch_raster_render_views(st, W, H, s.geom.gy, s.geom, img.ranges, bv.point_list, img.plan, bv.capacity, out);
+}
+
+int raster_views_backward_impl(cudaStream_t st, int P, int N, long long R, int W, int H, const float* means3D,
+                               const float* scales, float scale_modifier, const float* rotations,
+                               const float* viewmatrices, const float* projmatrices, float tan_fovx, float tan_fovy,
+                               const int* radii, const void* geom_buf, const void* binning_buf, const void* image_buf,
+                               void* scratch, const float* dL_dpix, float* dL_dmean2D, float* dL_dopacity,
+                               float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale, float* dL_drot, int mode,
+                               int debug) {
+    const char* fn = "r2x_raster_backward_views";
+    ViewsShape vs;
+    R2X_TRY(views_shape(fn, P, N, W, H, &vs));
+    if (R < 0) return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward_views: bad R");
+    if (mode != 0 && mode != 1) return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward_views: mode must be 0 or 1");
+    if (P == 0) return 0;
+    if (!geom_buf || !image_buf || !dL_dpix || !dL_dmean2D || !dL_dopacity || !dL_dmean3D || !dL_dcov3D || !dL_dscale ||
+        !dL_drot || !radii || !means3D || !scales || !rotations || !viewmatrices || !projmatrices)
+        return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward_views: null pointer");
+    if (R > 0 && (!binning_buf || !scratch))
+        return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward_views: null binning/scratch");
+    RasterState s = carve_raster(geom_buf, vs.Pv, W, H);
+    BinningView bv = binning_view((void*)binning_buf, R);
+    const ImageViews img = image_views(image_buf, vs.Pv, vs.pp, bv, &vs.vb);
+    float4* inst_grad = (float4*)al((size_t)scratch);
+    const uint32_t* inst_pos = vs.pp.path() == BinPath::Radix ? bv.inst_pos : nullptr;   // otherwise slots are derived
+    if (R > 0)
+        R2X_TRY(launch_raster_render_bwd_views(st, W, H, s.geom.gy, s.geom, img.ranges, bv.point_list, inst_pos, img.plan,
+                                               dL_dpix, inst_grad));
+    R2X_TRY(debug_sync(st, debug, "raster views render backward"));
+    R2X_TRY(launch_raster_gauss_bwd_views(st, P, N, vs.vb.band_ctas * DIRECT_BLOCK, means3D, radii, scales, scale_modifier,
+                                          rotations, viewmatrices, projmatrices, W, H, tan_fovx, tan_fovy, mode, s.geom, R,
+                                          inst_grad, dL_dmean2D, dL_dopacity, dL_dmean3D, dL_dcov3D, dL_dscale, dL_drot));
+    return debug_sync(st, debug, "raster views per-Gaussian backward");
 }
 
 int voxel_forward_impl(cudaStream_t st, int P, int nx, int ny, int nz, float sx, float sy, float sz, float cx,
@@ -464,6 +556,40 @@ int r2x_raster_forward_async(void* stream, int P, int W, int H, const float* mea
                                cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, prefiltered, mode,
                                out_color, radii, geom_buf, image_buf, nullptr, nullptr, binning_buf, capacity,
                                status_dev, 0, nullptr);
+}
+
+size_t r2x_raster_views_geom_bytes(int P, int N) {
+    ViewsShape vs;
+    return views_shape("r2x_raster_views_geom_bytes", P, N, 1, 1, &vs) ? 0 : raster_geom_bytes(vs.Pv);
+}
+size_t r2x_raster_views_image_bytes(int P, int N, int W, int H) {
+    ViewsShape vs;
+    if (views_shape("r2x_raster_views_image_bytes", P, N, W, H, &vs)) return 0;
+    return image_layout(nullptr, vs.Pv, vs.pp, BinningView{}, nullptr, &vs.vb);
+}
+
+int r2x_raster_forward_views_async(void* stream, int P, int N, int W, int H, const float* means3D,
+                                   const float* opacities, const float* scales, float scale_modifier,
+                                   const float* rotations, const float* viewmatrices, const float* projmatrices,
+                                   float tan_fovx, float tan_fovy, int mode, float* out_color, int* radii,
+                                   void* geom_buf, void* image_buf, void* binning_buf, long long capacity,
+                                   uint32_t* status_dev) {
+    return raster_views_forward_impl((cudaStream_t)stream, P, N, W, H, means3D, opacities, scales, scale_modifier,
+                                     rotations, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode, out_color, radii,
+                                     geom_buf, image_buf, binning_buf, capacity, status_dev);
+}
+
+int r2x_raster_backward_views(void* stream, int P, int N, long long R, int W, int H, const float* means3D,
+                              const float* scales, float scale_modifier, const float* rotations,
+                              const float* viewmatrices, const float* projmatrices, float tan_fovx, float tan_fovy,
+                              const int* radii, const void* geom_buf, const void* binning_buf, const void* image_buf,
+                              void* scratch, const float* dL_dpix, float* dL_dmean2D, float* dL_dopacity,
+                              float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale, float* dL_drot, int mode,
+                              int debug) {
+    return raster_views_backward_impl((cudaStream_t)stream, P, N, R, W, H, means3D, scales, scale_modifier, rotations,
+                                      viewmatrices, projmatrices, tan_fovx, tan_fovy, radii, geom_buf, binning_buf,
+                                      image_buf, scratch, dL_dpix, dL_dmean2D, dL_dopacity, dL_dmean3D, dL_dcov3D,
+                                      dL_dscale, dL_drot, mode, debug);
 }
 
 int r2x_raster_render_only(void* stream, int P, int W, int H, long long R, const void* geom_buf,

@@ -478,26 +478,41 @@ __global__ void __launch_bounds__(256) tile_ranges_kernel(const uint32_t* __rest
 // ------------------------------------------------------------------------------------------------
 // Direct binning
 // ------------------------------------------------------------------------------------------------
-size_t directbin_bytes(int P, int num_tiles) {
-    const size_t nb = (size_t)((P > 0 ? P : 1) + DIRECT_BLOCK - 1) / DIRECT_BLOCK;
-    const size_t t = (size_t)num_tiles;
-    return align_up(t * nb * sizeof(uint32_t), 256) +
-           align_up((size_t)(1 + direct_scan_ctas(num_tiles)) * sizeof(unsigned long long), 256) +
-           2 * align_up(nb * sizeof(uint32_t), 256) + 512;
+// table [nb][row_tiles] | look-back [1 + ceil(num_tiles / DSCAN_COLS)] | block_total [nb] | block_base [nb]
+static size_t directbin_layout(void* buf, size_t nb, int num_tiles, int row_tiles, DirectBin* db) {
+    const size_t t = (size_t)row_tiles;
+    const size_t table = align_up(t * nb * sizeof(uint32_t), 256);
+    const size_t lookback = align_up((size_t)(1 + direct_scan_ctas(num_tiles)) * sizeof(unsigned long long), 256);
+    const size_t per_cta = align_up(nb * sizeof(uint32_t), 256);
+    if (db) {
+        char* p = (char*)align_up((size_t)buf, 256);
+        db->table = (uint32_t*)p; p += table;
+        db->lookback = (unsigned long long*)p; p += lookback;
+        db->block_total = (uint32_t*)p; p += per_cta;
+        db->block_base = (uint32_t*)p;
+        db->num_tiles = num_tiles;
+        db->nb = (int)nb;
+    }
+    return table + lookback + 2 * per_cta + 512;
 }
+
+static size_t direct_ctas(int P) { return (size_t)((P > 0 ? P : 1) + DIRECT_BLOCK - 1) / DIRECT_BLOCK; }
+
+size_t directbin_bytes(int P, int num_tiles) { return directbin_layout(nullptr, direct_ctas(P), num_tiles, num_tiles, nullptr); }
 
 DirectBin directbin_view(void* buf, int P, int num_tiles) {
     DirectBin db;
-    const size_t nb = (size_t)((P > 0 ? P : 1) + DIRECT_BLOCK - 1) / DIRECT_BLOCK;
-    const size_t t = (size_t)num_tiles;
-    char* p = (char*)align_up((size_t)buf, 256);
-    db.table = (uint32_t*)p; p += align_up(t * nb * sizeof(uint32_t), 256);
-    db.lookback = (unsigned long long*)p;
-    p += align_up((size_t)(1 + direct_scan_ctas(num_tiles)) * sizeof(unsigned long long), 256);
-    db.block_total = (uint32_t*)p; p += align_up(nb * sizeof(uint32_t), 256);
-    db.block_base = (uint32_t*)p; p += align_up(nb * sizeof(uint32_t), 256);
-    db.num_tiles = num_tiles;
-    db.nb = (int)nb;
+    directbin_layout(buf, direct_ctas(P), num_tiles, num_tiles, &db);
+    return db;
+}
+
+size_t directbin_views_bytes(const ViewBands& vb) {
+    return directbin_layout(nullptr, (size_t)vb.views * vb.band_ctas, vb.views * vb.band_tiles, vb.band_tiles, nullptr);
+}
+
+DirectBin directbin_views_view(void* buf, const ViewBands& vb) {
+    DirectBin db;
+    directbin_layout(buf, (size_t)vb.views * vb.band_ctas, vb.views * vb.band_tiles, vb.band_tiles, &db);
     return db;
 }
 
@@ -518,9 +533,12 @@ constexpr int DSCAN_KEEP = 16;                           // rows of a segment ke
 static_assert(DSCAN_COLS == 8, "a warp is 4 row segments x 8 columns");
 constexpr unsigned long long LB_AGG = 1ull << 62, LB_INCL = 2ull << 62, LB_VALUE = (1ull << 62) - 1;
 
-__global__ void __launch_bounds__(DSCAN_THREADS) direct_scan_kernel(DirectBin db, uint2* __restrict__ ranges, TilePlan pl,
-                                                                    uint32_t* __restrict__ status, long long capacity,
-                                                                    uint32_t* __restrict__ status_out) {
+// VIEWS = true (batched views): the column of tile t is made of the band_ctas rows of its view's CTAs, rows
+// band_tiles long (ViewBands); all other rows are zero for t and are neither stored nor read.
+template <bool VIEWS>
+__device__ __forceinline__ void direct_scan_body(DirectBin db, ViewBands vb, uint2* __restrict__ ranges, TilePlan pl,
+                                                 uint32_t* __restrict__ status, long long capacity,
+                                                 uint32_t* __restrict__ status_out) {
     pdl_prologue();
     __shared__ uint32_t s_w[DSCAN_WARPS];
     __shared__ uint32_t s_wcol[DSCAN_WARPS][DSCAN_COLS];
@@ -578,19 +596,26 @@ __global__ void __launch_bounds__(DSCAN_THREADS) direct_scan_kernel(DirectBin db
     const int bid = (int)s_bid;
     const int col = tid & (DSCAN_COLS - 1), seg = tid / DSCAN_COLS;
     const int t = bid * DSCAN_COLS + col;
-    const int rps = (nb + DSCAN_SEGS - 1) / DSCAN_SEGS;
-    const int r0 = min(seg * rps, nb), r1 = min(r0 + rps, nb);
+    int rows = nb, stride = T;
     uint32_t* cp = db.table + t;
+    if constexpr (VIEWS) {
+        const int v = t / vb.band_tiles;
+        rows = vb.band_ctas;
+        stride = vb.band_tiles;
+        cp = db.table + (size_t)v * vb.band_ctas * vb.band_tiles + (t - v * vb.band_tiles);
+    }
+    const int rps = (rows + DSCAN_SEGS - 1) / DSCAN_SEGS;
+    const int r0 = min(seg * rps, rows), r1 = min(r0 + rps, rows);
     const bool live = t < T;
     uint32_t keep[DSCAN_KEEP];
     uint32_t sum = 0;
 #pragma unroll
     for (int k = 0; k < DSCAN_KEEP; ++k) {
-        keep[k] = (live && r0 + k < r1) ? cp[(size_t)(r0 + k) * T] : 0u;
+        keep[k] = (live && r0 + k < r1) ? cp[(size_t)(r0 + k) * stride] : 0u;
         sum += keep[k];
     }
     if (live)
-        for (int r = r0 + DSCAN_KEEP; r < r1; ++r) sum += cp[(size_t)r * T];
+        for (int r = r0 + DSCAN_KEEP; r < r1; ++r) sum += cp[(size_t)r * stride];
     // prefix over the segments: 4 segments per warp (lanes 8 apart), then over the warps
     uint32_t sincl = sum;
 #pragma unroll
@@ -658,12 +683,12 @@ __global__ void __launch_bounds__(DSCAN_THREADS) direct_scan_kernel(DirectBin db
 #pragma unroll
         for (int k = 0; k < DSCAN_KEEP; ++k)
             if (r0 + k < r1) {
-                cp[(size_t)(r0 + k) * T] = pos;
+                cp[(size_t)(r0 + k) * stride] = pos;
                 pos += keep[k];
             }
         for (int r = r0 + DSCAN_KEEP; r < r1; ++r) {
-            const uint32_t a = cp[(size_t)r * T];
-            cp[(size_t)r * T] = pos;
+            const uint32_t a = cp[(size_t)r * stride];
+            cp[(size_t)r * stride] = pos;
             pos += a;
         }
         // Overflow (asynchronous variant only): the binning buffer cannot hold the lists, so EMPTY ranges are
@@ -681,10 +706,32 @@ __global__ void __launch_bounds__(DSCAN_THREADS) direct_scan_kernel(DirectBin db
     if (bid == nctas - 1 && tid == 0) pl.extra_off[T] = ov ? 0u : (uint32_t)(s_excl >> 32) + ext_all;
 }
 
+__global__ void __launch_bounds__(DSCAN_THREADS) direct_scan_kernel(DirectBin db, uint2* __restrict__ ranges, TilePlan pl,
+                                                                    uint32_t* __restrict__ status, long long capacity,
+                                                                    uint32_t* __restrict__ status_out) {
+    direct_scan_body<false>(db, ViewBands{1, db.num_tiles, db.nb}, ranges, pl, status, capacity, status_out);
+}
+
+__global__ void __launch_bounds__(DSCAN_THREADS) direct_scan_views_kernel(DirectBin db, ViewBands vb,
+                                                                          uint2* __restrict__ ranges, TilePlan pl,
+                                                                          uint32_t* __restrict__ status,
+                                                                          long long capacity,
+                                                                          uint32_t* __restrict__ status_out) {
+    direct_scan_body<true>(db, vb, ranges, pl, status, capacity, status_out);
+}
+
 int launch_direct_scan(cudaStream_t st, const DirectBin& db, uint2* ranges, const TilePlan& plan, uint32_t* status,
                        long long capacity, uint32_t* status_out) {
     R2X_CUDA_OK(pdl_launch(direct_scan_kernel, dim3(direct_scan_ctas(db.num_tiles)), dim3(DSCAN_THREADS), 0, st, db,
                            ranges, plan, status, capacity, status_out));
+    R2X_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int launch_direct_scan_views(cudaStream_t st, const DirectBin& db, const ViewBands& vb, uint2* ranges,
+                             const TilePlan& plan, uint32_t* status, long long capacity, uint32_t* status_out) {
+    R2X_CUDA_OK(pdl_launch(direct_scan_views_kernel, dim3(direct_scan_ctas(db.num_tiles)), dim3(DSCAN_THREADS), 0, st, db,
+                           vb, ranges, plan, status, capacity, status_out));
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -707,16 +754,20 @@ int launch_direct_scan(cudaStream_t st, const DirectBin& db, uint2* ranges, cons
 constexpr int FILL_STAGE_TILES = 4 * DIRECT_BLOCK;   // staging when T <= 1024 ...
 constexpr int FILL_STAGE_CAP = 4608;                 // ... for up to 4608 instances per CTA: 70.5 KB, 3 CTAs per SM
 
-__global__ void __launch_bounds__(DIRECT_BLOCK) direct_fill_kernel(int P, const uint16_t* __restrict__ cube,
-                                                                   const uint32_t* __restrict__ tiles_touched,
-                                                                   uint32_t* __restrict__ offsets, DirectBin db,
-                                                                   TilePlan pl, uint32_t* __restrict__ point_list,
-                                                                   int gx, int gy, const uint32_t* __restrict__ status,
-                                                                   int stage_cap) {
+// VIEWS = true (batched views): CTA b belongs to one view, its table row and its shared tables cover that view's band
+// (T = band_tiles, tiles numbered band-locally: the tile cube's z, the view, is dropped); the work plan's extra items
+// cover the whole grid (T_all = db.num_tiles).
+template <bool VIEWS>
+__device__ __forceinline__ void direct_fill_body(int P, const uint16_t* __restrict__ cube,
+                                                 const uint32_t* __restrict__ tiles_touched,
+                                                 uint32_t* __restrict__ offsets, DirectBin db, TilePlan pl,
+                                                 uint32_t* __restrict__ point_list, int gx, int gy,
+                                                 const uint32_t* __restrict__ status, int stage_cap, int band_tiles) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ uint32_t s_w8[8];
     __shared__ uint32_t s_ct[4][8];
-    const int T = db.num_tiles;
+    const int T = VIEWS ? band_tiles : db.num_tiles;
+    const int T_all = db.num_tiles;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint32_t* s_mask = reinterpret_cast<uint32_t*>(smem_raw);                    // [8][T]
     uint32_t* s_base = s_mask + 8 * (size_t)T;                                    // [T]
@@ -760,15 +811,16 @@ __global__ void __launch_bounds__(DIRECT_BLOCK) direct_fill_kernel(int P, const 
     if (ov) return;                                // uniform across the grid
     // extra work items of the tiles [b K, b K + K): (tile, chunk >= 1)
     {
-        const int K = (T + (int)gridDim.x - 1) / (int)gridDim.x;
-        const int t1 = min(T, (b + 1) * K);
+        const int K = (T_all + (int)gridDim.x - 1) / (int)gridDim.x;
+        const int t1 = min(T_all, (b + 1) * K);
         for (int t = b * K + tid; t < t1; t += DIRECT_BLOCK) {
             const uint32_t eo = pl.extra_off[t], ne = pl.extra_off[t + 1] - eo;
             for (uint32_t c = 0; c < ne; ++c)
                 if ((long long)(eo + c) < pl.max_extra) pl.extra_item[eo + c] = make_uint2((uint32_t)t, c + 1);
         }
     }
-    const uint32_t x0 = c01 & 0xffff, y0 = c01 >> 16, z0 = c23 & 0xffff, x1 = c23 >> 16, y1 = c45 & 0xffff, z1 = c45 >> 16;
+    const uint32_t x0 = c01 & 0xffff, y0 = c01 >> 16, x1 = c23 >> 16, y1 = c45 & 0xffff;
+    const uint32_t z0 = VIEWS ? 0u : (c23 & 0xffff), z1 = VIEWS ? 1u : (c45 >> 16);
     // mark
     {
         uint32_t* plane = s_mask + (size_t)warp * T;
@@ -853,6 +905,37 @@ __global__ void __launch_bounds__(DIRECT_BLOCK) direct_fill_kernel(int P, const 
         const uint32_t g0 = (uint32_t)b * DIRECT_BLOCK;
         for (uint32_t i = tid; i < total; i += DIRECT_BLOCK) point_list[s_pos[i]] = g0 + s_id[i];
     }
+}
+
+__global__ void __launch_bounds__(DIRECT_BLOCK) direct_fill_kernel(int P, const uint16_t* __restrict__ cube,
+                                                                   const uint32_t* __restrict__ tiles_touched,
+                                                                   uint32_t* __restrict__ offsets, DirectBin db,
+                                                                   TilePlan pl, uint32_t* __restrict__ point_list,
+                                                                   int gx, int gy, const uint32_t* __restrict__ status,
+                                                                   int stage_cap) {
+    direct_fill_body<false>(P, cube, tiles_touched, offsets, db, pl, point_list, gx, gy, status, stage_cap, 0);
+}
+
+__global__ void __launch_bounds__(DIRECT_BLOCK) direct_fill_views_kernel(
+    int P, const uint16_t* __restrict__ cube, const uint32_t* __restrict__ tiles_touched, uint32_t* __restrict__ offsets,
+    DirectBin db, TilePlan pl, uint32_t* __restrict__ point_list, int gx, int gy, const uint32_t* __restrict__ status,
+    int stage_cap, int band_tiles) {
+    direct_fill_body<true>(P, cube, tiles_touched, offsets, db, pl, point_list, gx, gy, status, stage_cap, band_tiles);
+}
+
+int launch_direct_fill_views(cudaStream_t st, int P, const uint16_t* cube, const uint32_t* tiles_touched,
+                             uint32_t* offsets, const DirectBin& db, const ViewBands& vb, const TilePlan& plan,
+                             const BinningView& bv, int gx, int gy, const uint32_t* status) {
+    const int T = vb.band_tiles;   // a CTA's shared tables cover its view's band
+    const int cap = T <= FILL_STAGE_TILES ? FILL_STAGE_CAP : 0;
+    const size_t smem = (size_t)T * (cap ? 48 : 44) + (size_t)cap * 5;
+    if (smem > 48 * 1024)
+        R2X_CUDA_OK(cudaFuncSetAttribute(direct_fill_views_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         DIRECT_MAX_TILES * 44));
+    R2X_CUDA_OK(pdl_launch(direct_fill_views_kernel, dim3(db.nb), dim3(DIRECT_BLOCK), smem, st, P, cube, tiles_touched,
+                           offsets, db, plan, bv.point_list, gx, gy, status, cap, T));
+    R2X_CUDA_OK(cudaGetLastError());
+    return 0;
 }
 
 int launch_direct_fill(cudaStream_t st, int P, const uint16_t* cube, const uint32_t* tiles_touched, uint32_t* offsets,

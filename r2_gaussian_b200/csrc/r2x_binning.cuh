@@ -146,10 +146,25 @@ __host__ __device__ __forceinline__ int direct_scan_ctas(int num_tiles) { return
 size_t directbin_bytes(int P, int num_tiles);
 DirectBin directbin_view(void* buf, int P, int num_tiles);
 
-// Called by all 256 threads of a preprocess CTA.  hist_s: shared uint32[T] scratch.  (c01,c23,c45) is
-// the packed tile cube of this thread's Gaussian, n its instance count (0 if culled).
-__device__ __forceinline__ void block_tile_histogram(uint32_t* hist_s, const DirectBin& db, uint32_t c01, uint32_t c23,
-                                                     uint32_t c45, uint32_t n, int gx, int gy) {
+// ---- batched views: N views of one cloud binned as one stacked tile grid --------------------------------------------
+// View v owns tile rows [v gy, (v + 1) gy) of a gx x N gy grid (a 3-D grid gx x gy x N: the z of a tile is its view) and
+// the virtual Gaussians [v Pp, (v + 1) Pp), Pp = P rounded up to DIRECT_BLOCK.  So every direct-binning CTA belongs to
+// one view and only counts the band_tiles = gx gy tiles of its band: table is [nb][band_tiles] (db.num_tiles is the
+// whole grid's N band_tiles, db.nb = N band_ctas), which keeps the table linear in N.
+struct ViewBands {
+    int views;        // N
+    int band_tiles;   // gx * gy of one view
+    int band_ctas;    // Pp / DIRECT_BLOCK
+};
+size_t directbin_views_bytes(const ViewBands& vb);
+DirectBin directbin_views_view(void* buf, const ViewBands& vb);
+
+// Called by all 256 threads of a preprocess CTA.  hist_s: shared uint32[T] scratch, s_wsum: shared uint32[8]
+// (the block total's warp sums).  (c01,c23,c45) is the packed tile cube of this thread's Gaussian, n its instance
+// count (0 if culled).
+__device__ __forceinline__ void block_tile_histogram_into(uint32_t* hist_s, uint32_t* s_wsum, const DirectBin& db,
+                                                          uint32_t c01, uint32_t c23, uint32_t c45, uint32_t n, int gx,
+                                                          int gy) {
     const int tid = threadIdx.x;
     for (int t = tid; t < db.num_tiles; t += DIRECT_BLOCK) hist_s[t] = 0;
     if (blockIdx.x == 0)   // direct_scan's look-back state (it waits for this grid to finish before reading it)
@@ -165,7 +180,6 @@ __device__ __forceinline__ void block_tile_histogram(uint32_t* hist_s, const Dir
             }
     }
     // block total of n (fixed-order tree, result identical for every thread that reads it)
-    __shared__ uint32_t s_wsum[DIRECT_BLOCK / 32];
     uint32_t v = n;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -178,6 +192,11 @@ __device__ __forceinline__ void block_tile_histogram(uint32_t* hist_s, const Dir
         for (int w = 0; w < DIRECT_BLOCK / 32; ++w) tot += s_wsum[w];
         db.block_total[blockIdx.x] = tot;
     }
+}
+__device__ __forceinline__ void block_tile_histogram(uint32_t* hist_s, const DirectBin& db, uint32_t c01, uint32_t c23,
+                                                     uint32_t c45, uint32_t n, int gx, int gy) {
+    __shared__ uint32_t s_wsum[DIRECT_BLOCK / 32];
+    block_tile_histogram_into(hist_s, s_wsum, db, c01, c23, c45, n, gx, gy);
 }
 
 // ---- two-level direct binning (voxel grids with more than DIRECT_MAX_TILES tiles; r2x_binning2.cu) --------------
@@ -211,6 +230,12 @@ int launch_direct_scan(cudaStream_t st, const DirectBin& db, uint2* ranges, cons
 int launch_direct_fill(cudaStream_t st, int P, const uint16_t* cube, const uint32_t* tiles_touched, uint32_t* offsets,
                        const DirectBin& db, const TilePlan& plan, const BinningView& bv, int gx, int gy,
                        const uint32_t* status);
+// the same two stages over the banded table of batched views (P = N Pp virtual Gaussians, gy = one view's tile rows)
+int launch_direct_scan_views(cudaStream_t st, const DirectBin& db, const ViewBands& vb, uint2* ranges,
+                             const TilePlan& plan, uint32_t* status, long long capacity, uint32_t* status_out);
+int launch_direct_fill_views(cudaStream_t st, int P, const uint16_t* cube, const uint32_t* tiles_touched,
+                             uint32_t* offsets, const DirectBin& db, const ViewBands& vb, const TilePlan& plan,
+                             const BinningView& bv, int gx, int gy, const uint32_t* status);
 
 // Exclusive->inclusive scan of tiles_touched[P] into offsets[P]; total (R) is written to *d_total
 // (device) -- single pass, decoupled look-back.  scan_state needs scan_state_bytes(P) bytes, zeroed

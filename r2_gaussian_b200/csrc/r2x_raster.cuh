@@ -33,6 +33,24 @@ int launch_raster_gauss_bwd(cudaStream_t st, int P, const float* means, const in
                             const float4* inst_grad, float* dL_dmean2D, float* dL_dopacity, float* dL_dmu, float* dL_dmean3D,
                             float* dL_dcov3D, float* dL_dscale, float* dL_drot, void* pose_scratch = nullptr,
                             float* dL_dview = nullptr, float* dL_dproj = nullptr);
+// batched views (r2x_raster_forward_views_async / r2x_raster_backward_views): `geom` is carved for vb.views * Pp
+// virtual Gaussians (Pp = vb.band_ctas * DIRECT_BLOCK) with the tile grid of ONE view (geom.gx, geom.gy = band rows);
+// `db` (direct binning) is the views layout of directbin_views_view; out / dL_dpix are [views][H][W]
+int launch_raster_preprocess_views(cudaStream_t st, int P, int views, const float* means, const float* scales,
+                                   float scale_modifier, const float* rots, const float* opac, const float* viewmats,
+                                   const float* projmats, int W, int H, float tan_fovx, float tan_fovy, int mode,
+                                   int* radii, const RasterGeom& geom, const DirectBin* db, const ViewBands& vb);
+int launch_raster_render_views(cudaStream_t st, int W, int H, int band_rows, const RasterGeom& geom, const uint2* ranges,
+                               const uint32_t* point_list, const TilePlan& plan, long long R_launch, float* out);
+int launch_raster_render_bwd_views(cudaStream_t st, int W, int H, int band_rows, const RasterGeom& geom,
+                                   const uint2* ranges, const uint32_t* point_list, const uint32_t* inst_pos,
+                                   const TilePlan& plan, const float* dL_dpix, float4* inst_grad);
+int launch_raster_gauss_bwd_views(cudaStream_t st, int P, int views, int Pp, const float* means, const int* radii,
+                                  const float* scales, float scale_modifier, const float* rots, const float* viewmats,
+                                  const float* projmats, int W, int H, float tan_fovx, float tan_fovy, int mode,
+                                  const RasterGeom& geom, long long capacity, const float4* inst_grad, float* dL_dmean2D,
+                                  float* dL_dopacity, float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale,
+                                  float* dL_drot);
 // pose_scratch of launch_raster_gauss_bwd (the per-CTA rows of the view / projection matrix gradients)
 size_t raster_pose_scratch_bytes(int P);
 int launch_mark_visible(cudaStream_t st, int P, const float* means, const float* view, unsigned char* present);

@@ -68,6 +68,7 @@ class RasterEngine(_Engine):
         super().__init__(_C.RASTER, P, (self.W, self.H), device, capacity)
         self.radii = torch.empty(self.P, dtype=torch.int32, device=self.device)
         self.out = torch.empty((1, self.H, self.W), dtype=torch.float32, device=self.device)
+        self._views = {}   # N -> (geom, image, radii[N,P], images[N,H,W]) of forward_views
 
     def forward(self, means, dens, scales, rots, viewmatrix, projmatrix, campos, tanfovx, tanfovy, mode,
                 scale_modifier: float = 1.0, cov3D_precomp=None, out=None):
@@ -80,6 +81,32 @@ class RasterEngine(_Engine):
             self.geom.data_ptr(), self.img.data_ptr(), self.binning.data_ptr(), self.capacity, self.status.data_ptr())
         check(rc, "r2x_raster_forward_async")
         return out
+
+    def forward_views(self, means, dens, scales, rots, viewmatrices, projmatrices, tanfovx, tanfovy, mode,
+                      scale_modifier: float = 1.0, out=None):
+        """Enqueue the projections of N = len(viewmatrices) views in one batched call on the current stream; returns
+        the [N,H,W] output (image v is bit for bit `forward` of view v).  The views' state buffers are kept per N; the
+        binning buffer, its capacity and the status word are the engine's (`check()` / `grow()` as for `forward`)."""
+        N = int(viewmatrices.shape[0])
+        if N not in self._views:
+            with torch.cuda.device(self.device):
+                geom, img = _C.views_state(self.P, N, self.W, self.H, self.device)
+                radii = torch.empty((N, self.P), dtype=torch.int32, device=self.device)
+                images = torch.empty((N, self.H, self.W), dtype=torch.float32, device=self.device)
+            self._views[N] = (geom, img, radii, images)
+        geom, img, radii, images = self._views[N]
+        out = images if out is None else out
+        rc = self.lib.r2x_raster_forward_views_async(
+            torch.cuda.current_stream(self.device).cuda_stream, self.P, N, self.W, self.H, _ptr(means), _ptr(dens),
+            _ptr(scales), float(scale_modifier), _ptr(rots), _ptr(viewmatrices), _ptr(projmatrices), float(tanfovx),
+            float(tanfovy), int(mode), out.data_ptr(), radii.data_ptr(), geom.data_ptr(), img.data_ptr(),
+            self.binning.data_ptr(), self.capacity, self.status.data_ptr())
+        check(rc, "r2x_raster_forward_views_async")
+        return out
+
+    def views_radii(self, N: int) -> torch.Tensor:
+        """radii[N,P] of the last `forward_views` of N views."""
+        return self._views[int(N)][2]
 
     def render_only(self, out=None):
         """Re-run only the per-tile accumulation kernel on the state of the last forward (profiling)."""

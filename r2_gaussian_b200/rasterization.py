@@ -105,6 +105,55 @@ def rasterize_gaussians_matrices(means3D, means2D, opacities, scales, rotations,
         empty if cov3Ds_precomp is None else cov3Ds_precomp, viewmatrix, projmatrix, raster_settings)
 
 
+class _RasterizeViews(torch.autograd.Function):
+    """N views of one cloud in one native call (not part of the reference's surface).
+    forward inputs:  (means3D, means2D[N,P,3], opacities, scales, rotations, viewmatrices[N,4,4], projmatrices[N,4,4],
+    settings) -> (images[N,H,W], radii[N,P]); the settings' own matrices are ignored.  The backward sums the Gaussian
+    gradients over the views and hands means2D the per-view screen-space gradients."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, opacities, scales, rotations, viewmatrices, projmatrices, raster_settings):
+        s = raster_settings
+        with _C.speculative(any(ctx.needs_input_grad) and not s.debug):
+            num_rendered, images, radii, geom, binning, img = _C.rasterize_views(
+                means3D, opacities, scales, rotations, s.scale_modifier, viewmatrices, projmatrices, s.tanfovx,
+                s.tanfovy, s.image_height, s.image_width, s.mode)
+        ctx.raster_settings = s
+        ctx.num_rendered = num_rendered
+        ctx.save_for_backward(means3D, scales, rotations, viewmatrices, projmatrices, radii, geom, binning, img)
+        ctx.mark_non_differentiable(radii)
+        return images, radii
+
+    @staticmethod
+    def backward(ctx, grad_images, _grad_radii):
+        s = ctx.raster_settings
+        means3D, scales, rotations, viewmatrices, projmatrices, radii, geom, binning, img = ctx.saved_tensors
+        g_means2D, g_opac, g_means3D, _g_cov, g_scales, g_rots = _C.rasterize_views_backward(
+            means3D, radii, scales, rotations, s.scale_modifier, viewmatrices, projmatrices, s.tanfovx, s.tanfovy,
+            grad_images, geom, ctx.num_rendered, binning, img, s.mode, s.debug)
+        return g_means3D, g_means2D, g_opac, g_scales, g_rots, None, None, None
+
+
+def rasterize_views(means3D, opacities, scales, rotations, viewmatrices, projmatrices, raster_settings, means2D=None):
+    """Project one cloud into N views at once -> (images[N,H,W], radii[N,P] int32).
+
+    All views share the settings' image size, tanfovx / tanfovy, scale_modifier and mode; view v has its own
+    viewmatrices[v] / projmatrices[v] (the settings' viewmatrix / projmatrix / campos are not used).  Image v is bit
+    for bit the single-view render of view v.  Gradients flow to means3D, opacities, scales and rotations (summed over
+    the views); `means2D` (a [N,P,3] tensor, e.g. zeros with requires_grad) receives the per-view screen-space
+    gradients, as `viewspace_points` does in `render()`.  Scales and rotations are required (no precomputed 3-D
+    covariance); the camera matrices get no gradient."""
+    N = _C.check_views_args(means3D, viewmatrices, projmatrices)
+    if scales is None or rotations is None:
+        raise ValueError("rasterize_views needs scales and rotations (cov3D_precomp is not supported)")
+    if means2D is None:
+        means2D = torch.zeros((N, means3D.shape[0], 3), dtype=means3D.dtype, device=means3D.device)
+    elif tuple(means2D.shape) != (N, means3D.shape[0], 3):
+        raise ValueError(f"means2D must have dimensions ({N}, {means3D.shape[0]}, 3), got {tuple(means2D.shape)}")
+    return _RasterizeViews.apply(means3D, means2D, opacities, scales, rotations, viewmatrices.detach(),
+                                 projmatrices.detach(), raster_settings)
+
+
 def _exactly_one_covariance_source(scales, rotations, cov3D_precomp):
     have_sr = scales is not None or rotations is not None
     full_sr = scales is not None and rotations is not None

@@ -17,7 +17,8 @@ import math
 import torch
 
 from . import fused, sharded
-from .rasterization import GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians_matrices
+from .rasterization import (GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians_matrices,
+                            rasterize_views)
 from .sharded import sharded_sum
 from .voxelization import GaussianVoxelizationSettings, GaussianVoxelizer
 
@@ -53,6 +54,52 @@ def query(pc, center, nVoxel, sVoxel, pipe, scaling_modifier=1.0):
     vol, radii = GaussianVoxelizer(voxel_settings=settings)(
         means3D=pc.get_xyz, opacities=pc.get_density, scales=scales, rotations=rotations, cov3D_precomp=cov3D)
     return {"vol": sharded_sum(vol), "radii": radii}
+
+
+def _tan_fov(camera) -> tuple[float, float]:
+    mode = int(camera.mode)
+    if mode == 0:
+        return 1.0, 1.0
+    if mode == 1:
+        return math.tan(camera.FoVx * 0.5), math.tan(camera.FoVy * 0.5)
+    raise ValueError("Unsupported mode!")
+
+
+def render_views(cameras, pc, pipe, scaling_modifier=1.0):
+    """X-ray projections of the model for N cameras in one batched call -> the `render()` dict with a leading view
+    axis: {"render": [N,1,H,W], "viewspace_points": [N,P,3] (receives the per-view dL/dmean2D), "visibility_filter":
+    bool[N,P], "radii": int[N,P]}.  render["render"][v] is bit for bit render(cameras[v], ...)["render"] (activated
+    parameters).  The cameras must share image size, field of view and mode; they are not differentiated, the
+    covariance is never precomputed in Python, and Gaussian sharding is not supported."""
+    cameras = list(cameras)
+    if not cameras:
+        raise ValueError("render_views(): no camera")
+    c0 = cameras[0]
+    shape = lambda c: (int(c.image_height), int(c.image_width), int(c.mode), _tan_fov(c))
+    if any(shape(c) != shape(c0) for c in cameras[1:]):
+        raise ValueError("render_views(): all cameras must share image size, field of view and mode")
+    if getattr(pipe, "compute_cov3D_python", False):
+        raise ValueError("render_views(): compute_cov3D_python is not supported (needs scales and rotations)")
+    if sharded.enabled():
+        raise RuntimeError("render_views(): Gaussian sharding is not supported")
+    tanfovx, tanfovy = _tan_fov(c0)
+    views = torch.stack([c.world_view_transform.detach() for c in cameras])
+    projs = torch.stack([c.full_proj_transform.detach() for c in cameras])
+    xyz = pc.get_xyz
+    screenspace_points = torch.zeros((len(cameras),) + tuple(xyz.shape), dtype=xyz.dtype, device=xyz.device,
+                                     requires_grad=True) + 0
+    try:
+        screenspace_points.retain_grad()
+    except Exception:
+        pass
+    settings = GaussianRasterizationSettings(
+        image_height=int(c0.image_height), image_width=int(c0.image_width), tanfovx=tanfovx, tanfovy=tanfovy,
+        scale_modifier=scaling_modifier, viewmatrix=views[0], projmatrix=projs[0], campos=c0.camera_center,
+        prefiltered=False, mode=int(c0.mode), debug=bool(getattr(pipe, "debug", False)))
+    images, radii = rasterize_views(xyz, pc.get_density, pc.get_scaling, pc.get_rotation, views, projs, settings,
+                                    means2D=screenspace_points)
+    return {"render": images.unsqueeze(1), "viewspace_points": screenspace_points, "visibility_filter": radii > 0,
+            "radii": radii}
 
 
 def render(viewpoint_camera, pc, pipe, scaling_modifier=1.0):
