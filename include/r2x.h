@@ -194,6 +194,11 @@ int r2x_knn3_mean_dist2(void* stream, int P, const float* points, float* mean_di
 size_t r2x_image_loss_scratch_bytes(int H, int W);
 int r2x_image_loss(void* stream, int H, int W, const float* image, const float* target, float w_l1,
                    float w_dssim, float* loss_out, float* grad_out, void* scratch, size_t scratch_bytes);
+/* The same for N images (1 <= N <= 65535) in the same three launches: images / targets / grad_out [N,H,W],
+ * loss_out[N,3]; row v is bit for bit r2x_image_loss of image v.  scratch: r2x_image_loss_views_scratch_bytes. */
+size_t r2x_image_loss_views_scratch_bytes(int N, int H, int W);
+int r2x_image_loss_views(void* stream, int N, int H, int W, const float* images, const float* targets, float w_l1,
+                         float w_dssim, float* loss_out, float* grad_out, void* scratch, size_t scratch_bytes);
 
 /* 3-D total variation of vol[nx][ny][nz] (`tv_3d_loss`, loss_utils.py:19-34): sum of absolute forward
  * differences along the three axes, divided by their number when reduction_mean != 0.  loss_out[1] (device),
@@ -228,6 +233,10 @@ int r2x_adam_step_sum(void* stream, int ngroups, const r2x_adam_group* groups, c
  * dL_dmean2D is [P,3]; the other arrays [P] float32.  Guards as above. */
 int r2x_densify_stats(void* stream, int P, const int* radii, const float* dL_dmean2D, float* max_radii2D,
                       float* xyz_gradient_accum, float* denom, const uint32_t* guard0, const uint32_t* guard1);
+/* The statistics of N >= 1 views in one launch: radii[N,P], dL_dmean2D[N,P,3]; bit for bit N r2x_densify_stats calls
+ * in view order, with the same guards. */
+int r2x_densify_stats_views(void* stream, int N, int P, const int* radii, const float* dL_dmean2D, float* max_radii2D,
+                            float* xyz_gradient_accum, float* denom, const uint32_t* guard0, const uint32_t* guard1);
 
 /* ---- folded parameter activations (SURVEY 8(f) rank 2) ------------------------------------------ */
 /* The reference applies softplus (density), a bounded sigmoid or exp (scale) and normalize (rotation) as separate torch
@@ -251,6 +260,23 @@ int r2x_raster_backward_raw(void* stream, int P, long long R, int W, int H, cons
                             const void* geom_buf, const void* binning_buf, const void* image_buf, void* scratch,
                             const float* dL_dpix, float* dL_dmean2D, float* dL_draw_density, float* dL_dmean3D,
                             float* dL_dcov3D, float* dL_draw_scale, float* dL_draw_rot, int mode, const r2x_activation* act);
+/* Batched views on raw parameters: the arguments and buffers of r2x_raster_forward_views_async /
+ * r2x_raster_backward_views (no debug flag).  image[v] and radii[v] are bit for bit r2x_raster_forward_async_raw of view
+ * v; each raw gradient is the view-order float32 sum (acc = g[0]; acc = acc + g[v]) of r2x_raster_backward_raw's per
+ * view, and dL_dmean2D[N,P,3] is kept per view. */
+int r2x_raster_forward_views_async_raw(void* stream, int P, int N, int W, int H, const float* means3D,
+                                       const float* raw_density, const float* raw_scales, float scale_modifier,
+                                       const float* raw_rotations, const float* viewmatrices, const float* projmatrices,
+                                       float tan_fovx, float tan_fovy, int mode, float* out_color, int* radii,
+                                       void* geom_buf, void* image_buf, void* binning_buf, long long capacity,
+                                       uint32_t* status_dev, const r2x_activation* act);
+int r2x_raster_backward_views_raw(void* stream, int P, int N, long long R, int W, int H, const float* means3D,
+                                  const float* raw_scales, float scale_modifier, const float* raw_rotations,
+                                  const float* viewmatrices, const float* projmatrices, float tan_fovx, float tan_fovy,
+                                  const int* radii, const void* geom_buf, const void* binning_buf, const void* image_buf,
+                                  void* scratch, const float* dL_dpix, float* dL_dmean2D, float* dL_draw_density,
+                                  float* dL_dmean3D, float* dL_dcov3D, float* dL_draw_scale, float* dL_draw_rot, int mode,
+                                  const r2x_activation* act);
 
 /* ---- view- and projection-matrix gradients of the rasterizer backward (per-view pose refinement) -------------- */
 /* r2x_raster_backward (act == NULL) or r2x_raster_backward_raw (act != NULL: raw scales / rotations, dL_dopacity is the

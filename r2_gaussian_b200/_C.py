@@ -400,12 +400,13 @@ def check_views_args(means3D, viewmatrices, projmatrices) -> int:
 
 
 def rasterize_views(means3D, opacity, scales, rotations, scale_modifier, viewmatrices, projmatrices, tan_fovx, tan_fovy,
-                    image_height, image_width, mode):
+                    image_height, image_width, mode, act=None):
     """N views of one cloud in one call -> (num_rendered, images[N,H,W], radii[N,P] int32, geom, binning, img).
 
     Image v and radii[v] are bit for bit what `rasterize_gaussians` computes for view v alone.  num_rendered (summed
     over the views) is a `NumRendered` carrying the binning buffer's capacity, with the same overflow handling as the
-    single-view call."""
+    single-view call.  With `act` (an `ActivationDesc`) opacity / scales / rotations are the RAW parameters
+    (`rasterize_views_raw`)."""
     N = check_views_args(means3D, viewmatrices, projmatrices)
     for t, name in ((means3D, "means3D"), (viewmatrices, "viewmatrices"), (projmatrices, "projmatrices")):
         _require_cuda(t, name)
@@ -422,21 +423,25 @@ def rasterize_views(means3D, opacity, scales, rotations, scale_modifier, viewmat
         stream = torch.cuda.current_stream(dev).cuda_stream
 
         def launch(binning, cap, status):
-            rc = lib.r2x_raster_forward_views_async(
-                stream, P, N, W, H, _ptr(means3D), _ptr(opacity), _ptr(scales), float(scale_modifier),
-                _ptr(rotations), _ptr(viewmatrices), _ptr(projmatrices), float(tan_fovx), float(tan_fovy), int(mode),
-                images.data_ptr(), _ptr(radii), geom.data_ptr(), img.data_ptr(), binning.data_ptr(), cap,
-                status.data_ptr())
-            check(rc, "r2x_raster_forward_views_async")
+            args = (stream, P, N, W, H, _ptr(means3D), _ptr(opacity), _ptr(scales), float(scale_modifier),
+                    _ptr(rotations), _ptr(viewmatrices), _ptr(projmatrices), float(tan_fovx), float(tan_fovy), int(mode),
+                    images.data_ptr(), _ptr(radii), geom.data_ptr(), img.data_ptr(), binning.data_ptr(), cap,
+                    status.data_ptr())
+            if act is None:
+                check(lib.r2x_raster_forward_views_async(*args), "r2x_raster_forward_views_async")
+            else:
+                check(lib.r2x_raster_forward_views_async_raw(*args, C.byref(act)), "r2x_raster_forward_views_async_raw")
 
         R, binning = _forward(launch, views_key(dev, P, N, W, H), P * N, RASTER.seed, dev)
     return R, images, radii, geom, binning, img
 
 
 def rasterize_views_backward(means3D, radii, scales, rotations, scale_modifier, viewmatrices, projmatrices, tan_fovx,
-                             tan_fovy, dL_dimages, geomBuffer, R, binningBuffer, imageBuffer, mode, debug=False):
+                             tan_fovy, dL_dimages, geomBuffer, R, binningBuffer, imageBuffer, mode, debug=False, act=None):
     """-> (dL_dmeans2D[N,P,3] per view, dL_dopacity[P,1], dL_dmeans3D[P,3], dL_dcov3D[P,6], dL_dscales[P,3],
-    dL_drotations[P,4]); the per-Gaussian gradients are summed over the views in view order (float32)."""
+    dL_drotations[P,4]); the per-Gaussian gradients are summed over the views in view order (float32).  With `act`
+    scales / rotations are the raw parameters and the gradients are those of the raw density / scales / rotations
+    (`rasterize_views_raw_backward`)."""
     N = check_views_args(means3D, viewmatrices, projmatrices)
     _require_cuda(means3D, "means3D")
     lib = load()
@@ -452,14 +457,33 @@ def rasterize_views_backward(means3D, radii, scales, rotations, scale_modifier, 
         g_scale = torch.empty((P, 3), **opts); g_rot = torch.empty((P, 4), **opts)
         R = _carved_capacity(binningBuffer, R)
         scratch = RASTER.bwd_scratch(R, dev)
-        rc = lib.r2x_raster_backward_views(
-            torch.cuda.current_stream(dev).cuda_stream, P, N, R, W, H, _ptr(means3D), _ptr(scales),
-            float(scale_modifier), _ptr(rotations), _ptr(viewmatrices), _ptr(projmatrices), float(tan_fovx),
-            float(tan_fovy), _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imageBuffer), scratch.data_ptr(),
-            _ptr(dL), _ptr(g_mean2D), _ptr(g_op), _ptr(g_mean3D), _ptr(g_cov), _ptr(g_scale), _ptr(g_rot), int(mode),
-            int(bool(debug)))
-        check(rc, "r2x_raster_backward_views")
+        args = (torch.cuda.current_stream(dev).cuda_stream, P, N, R, W, H, _ptr(means3D), _ptr(scales),
+                float(scale_modifier), _ptr(rotations), _ptr(viewmatrices), _ptr(projmatrices), float(tan_fovx),
+                float(tan_fovy), _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imageBuffer),
+                scratch.data_ptr(), _ptr(dL), _ptr(g_mean2D), _ptr(g_op), _ptr(g_mean3D), _ptr(g_cov), _ptr(g_scale),
+                _ptr(g_rot), int(mode))
+        if act is None:
+            check(lib.r2x_raster_backward_views(*args, int(bool(debug))), "r2x_raster_backward_views")
+        else:
+            check(lib.r2x_raster_backward_views_raw(*args, C.byref(act)), "r2x_raster_backward_views_raw")
     return g_mean2D, g_op, g_mean3D, g_cov, g_scale, g_rot
+
+
+def rasterize_views_raw(means3D, raw_density, raw_scales, raw_rotations, scale_modifier, viewmatrices, projmatrices,
+                        tan_fovx, tan_fovy, image_height, image_width, mode, act):
+    """`rasterize_views` on the RAW parameters (the activations of `act`, an `ActivationDesc`, run in the kernels):
+    image v and radii[v] are bit for bit the single-view raw render (`fused.rasterize_raw`) of view v."""
+    return rasterize_views(means3D, raw_density, raw_scales, raw_rotations, scale_modifier, viewmatrices, projmatrices,
+                           tan_fovx, tan_fovy, image_height, image_width, mode, act=act)
+
+
+def rasterize_views_raw_backward(means3D, radii, raw_scales, raw_rotations, scale_modifier, viewmatrices, projmatrices,
+                                 tan_fovx, tan_fovy, dL_dimages, geomBuffer, R, binningBuffer, imageBuffer, mode, act):
+    """-> (dL_dmeans2D[N,P,3] per view, dL_draw_density[P,1], dL_dmeans3D[P,3], dL_dcov3D[P,6], dL_draw_scales[P,3],
+    dL_draw_rotations[P,4]): each gradient is the view-order float32 sum of the single-view raw backward's."""
+    return rasterize_views_backward(means3D, radii, raw_scales, raw_rotations, scale_modifier, viewmatrices,
+                                    projmatrices, tan_fovx, tan_fovy, dL_dimages, geomBuffer, R, binningBuffer,
+                                    imageBuffer, mode, act=act)
 
 
 def mark_visible(means3D, viewmatrix, projmatrix):

@@ -55,15 +55,22 @@ PROTOTYPES = {
     "r2x_knn3_mean_dist2": (_i, [_vp, _i, _vp, _vp, _vp, _sz]),
     "r2x_image_loss_scratch_bytes": (_sz, [_i, _i]),
     "r2x_image_loss": (_i, [_vp, _i, _i, _vp, _vp, _f, _f, _vp, _vp, _vp, _sz]),
+    "r2x_image_loss_views_scratch_bytes": (_sz, [_i, _i, _i]),
+    "r2x_image_loss_views": (_i, [_vp, _i, _i, _i, _vp, _vp, _f, _f, _vp, _vp, _vp, _sz]),
     "r2x_tv3d_scratch_bytes": (_sz, [_i, _i, _i]),
     "r2x_tv3d_loss": (_i, [_vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _sz]),
     "r2x_adam_step": (_i, [_vp, _i, _vp, C.c_double, C.c_double, C.c_double, _ll]),
     "r2x_adam_step_sum": (_i, [_vp, _i, _vp, _vp, C.c_double, C.c_double, C.c_double, _ll, _vp, _vp]),
     "r2x_densify_stats": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "r2x_densify_stats_views": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "r2x_raster_forward_async_raw": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _f, _i, _vp, _vp, _vp, _vp,
                                           _vp, _ll, _vp, _vp]),
     "r2x_raster_backward_raw": (_i, [_vp, _i, _ll, _i, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _vp, _vp,
                                      _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    "r2x_raster_forward_views_async_raw": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _f, _vp, _vp, _vp, _f, _f, _i, _vp,
+                                                _vp, _vp, _vp, _vp, _ll, _vp, _vp]),
+    "r2x_raster_backward_views_raw": (_i, [_vp, _i, _i, _ll, _i, _i, _vp, _vp, _f, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp,
+                                           _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     "r2x_raster_backward_pose_scratch_bytes": (_sz, [_i]),
     "r2x_raster_backward_pose": (_i, [_vp, _i, _ll, _i, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _f, _f, _vp,
                                       _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i,

@@ -16,6 +16,11 @@ int launch_adam(cudaStream_t st, int ngroups, const r2x_adam_group* groups, doub
                 long long step, const float* const* grads2, const uint32_t* guard0, const uint32_t* guard1);
 int launch_densify_stats(cudaStream_t st, int P, const int* radii, const float* grad2d, float* max_radii, float* accum,
                          float* denom, const uint32_t* guard0, const uint32_t* guard1);
+int launch_densify_stats_views(cudaStream_t st, int N, int P, const int* radii, const float* grad2d, float* max_radii,
+                               float* accum, float* denom, const uint32_t* guard0, const uint32_t* guard1);
+size_t image_loss_views_scratch_bytes(int N, int H, int W);
+int launch_image_loss_views(cudaStream_t st, int N, int H, int W, const float* images, const float* targets, float w_l1,
+                            float w_dssim, float* loss_out, float* grad_out, void* scratch, size_t scratch_bytes);
 
 static thread_local std::string g_err;
 static thread_local Activation g_act = {0, 0, 0.f, 0.f};
@@ -802,6 +807,34 @@ int r2x_raster_backward_raw(void* stream, int P, long long R, int W, int H, cons
                                dL_draw_rot, mode, 0);
 }
 
+int r2x_raster_forward_views_async_raw(void* stream, int P, int N, int W, int H, const float* means3D,
+                                       const float* raw_density, const float* raw_scales, float scale_modifier,
+                                       const float* raw_rotations, const float* viewmatrices, const float* projmatrices,
+                                       float tan_fovx, float tan_fovy, int mode, float* out_color, int* radii,
+                                       void* geom_buf, void* image_buf, void* binning_buf, long long capacity,
+                                       uint32_t* status_dev, const r2x_activation* act) {
+    if (!act) return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward_views_async_raw: null activation");
+    ActScope scope(act);
+    return raster_views_forward_impl((cudaStream_t)stream, P, N, W, H, means3D, raw_density, raw_scales, scale_modifier,
+                                     raw_rotations, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode, out_color, radii,
+                                     geom_buf, image_buf, binning_buf, capacity, status_dev);
+}
+
+int r2x_raster_backward_views_raw(void* stream, int P, int N, long long R, int W, int H, const float* means3D,
+                                  const float* raw_scales, float scale_modifier, const float* raw_rotations,
+                                  const float* viewmatrices, const float* projmatrices, float tan_fovx, float tan_fovy,
+                                  const int* radii, const void* geom_buf, const void* binning_buf, const void* image_buf,
+                                  void* scratch, const float* dL_dpix, float* dL_dmean2D, float* dL_draw_density,
+                                  float* dL_dmean3D, float* dL_dcov3D, float* dL_draw_scale, float* dL_draw_rot, int mode,
+                                  const r2x_activation* act) {
+    if (!act) return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward_views_raw: null activation");
+    ActScope scope(act);
+    return raster_views_backward_impl((cudaStream_t)stream, P, N, R, W, H, means3D, raw_scales, scale_modifier,
+                                      raw_rotations, viewmatrices, projmatrices, tan_fovx, tan_fovy, radii, geom_buf,
+                                      binning_buf, image_buf, scratch, dL_dpix, dL_dmean2D, dL_draw_density, dL_dmean3D,
+                                      dL_dcov3D, dL_draw_scale, dL_draw_rot, mode, 0);
+}
+
 size_t r2x_raster_backward_pose_scratch_bytes(int P) { return raster_pose_scratch_bytes(P); }
 
 int r2x_raster_backward_pose(void* stream, int P, long long R, int W, int H, const float* means3D, const float* scales,
@@ -876,6 +909,14 @@ int r2x_image_loss(void* stream, int H, int W, const float* image, const float* 
                                   scratch_bytes);
 }
 
+size_t r2x_image_loss_views_scratch_bytes(int N, int H, int W) { return r2x::image_loss_views_scratch_bytes(N, H, W); }
+
+int r2x_image_loss_views(void* stream, int N, int H, int W, const float* images, const float* targets, float w_l1,
+                         float w_dssim, float* loss_out, float* grad_out, void* scratch, size_t scratch_bytes) {
+    return r2x::launch_image_loss_views((cudaStream_t)stream, N, H, W, images, targets, w_l1, w_dssim, loss_out, grad_out,
+                                        scratch, scratch_bytes);
+}
+
 size_t r2x_tv3d_scratch_bytes(int nx, int ny, int nz) { return r2x::tv3d_scratch_bytes(nx, ny, nz); }
 
 int r2x_tv3d_loss(void* stream, int nx, int ny, int nz, const float* vol, int reduction_mean, float* loss_out,
@@ -902,6 +943,15 @@ int r2x_densify_stats(void* stream, int P, const int* radii, const float* dL_dme
         return fail_msg(R2X_ERR_INVALID, "r2x_densify_stats: null pointer");
     return r2x::launch_densify_stats((cudaStream_t)stream, P, radii, dL_dmean2D, max_radii2D, xyz_gradient_accum, denom,
                                      guard0, guard1);
+}
+
+int r2x_densify_stats_views(void* stream, int N, int P, const int* radii, const float* dL_dmean2D, float* max_radii2D,
+                            float* xyz_gradient_accum, float* denom, const uint32_t* guard0, const uint32_t* guard1) {
+    if (N < 1 || P < 0) return fail_msg(R2X_ERR_INVALID, "r2x_densify_stats_views: bad N/P");
+    if (P > 0 && (!radii || !dL_dmean2D || !max_radii2D || !xyz_gradient_accum || !denom))
+        return fail_msg(R2X_ERR_INVALID, "r2x_densify_stats_views: null pointer");
+    return r2x::launch_densify_stats_views((cudaStream_t)stream, N, P, radii, dL_dmean2D, max_radii2D, xyz_gradient_accum,
+                                           denom, guard0, guard1);
 }
 
 }  // extern "C"

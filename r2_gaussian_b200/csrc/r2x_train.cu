@@ -39,10 +39,12 @@ static SsimWindow make_window() {
 }
 
 // Stage 1: per pixel SSIM statistics -> the three maps the gradient needs + per-CTA partial sums.
-__global__ void __launch_bounds__(LT * LT) ssim_stats_kernel(int H, int W, const float* __restrict__ x,
-                                                            const float* __restrict__ y, SsimWindow win,
-                                                            float* __restrict__ maps,       // [3][H][W] or NULL
-                                                            float* __restrict__ partial) {  // [nblk][2]
+// The *_body functions are shared by the one-image kernels and the batched ones (*_views_kernel: blockIdx.z or, for the
+// reduction, blockIdx.x is the image, whose pointers are shifted before the body runs).
+__device__ __forceinline__ void ssim_stats_body(int H, int W, const float* __restrict__ x, const float* __restrict__ y,
+                                                const SsimWindow& win,
+                                                float* __restrict__ maps,       // [3][H][W] or NULL
+                                                float* __restrict__ partial) {  // [nblk][2]
     __shared__ float sx[LE][LE + 1], sy[LE][LE + 1];
     __shared__ float hx[LE][LT], hy[LE][LT], hxx[LE][LT], hyy[LE][LT], hxy[LE][LT];
     __shared__ float s_red[2][LT * LT / 32];
@@ -113,9 +115,24 @@ __global__ void __launch_bounds__(LT * LT) ssim_stats_kernel(int H, int W, const
     }
 }
 
+__global__ void __launch_bounds__(LT * LT) ssim_stats_kernel(int H, int W, const float* __restrict__ x,
+                                                            const float* __restrict__ y, SsimWindow win,
+                                                            float* __restrict__ maps, float* __restrict__ partial) {
+    ssim_stats_body(H, W, x, y, win, maps, partial);
+}
+
+// image v = blockIdx.z: its maps and partials live in slab v (`slab` floats apart) of the scratch
+__global__ void __launch_bounds__(LT * LT) ssim_stats_views_kernel(int H, int W, const float* __restrict__ x,
+                                                                  const float* __restrict__ y, SsimWindow win,
+                                                                  float* __restrict__ maps, float* __restrict__ partial,
+                                                                  size_t slab) {
+    const size_t v = blockIdx.z, n = (size_t)H * W;
+    ssim_stats_body(H, W, x + v * n, y + v * n, win, maps ? maps + v * slab : nullptr, partial + v * slab);
+}
+
 // fixed-order final reduction of the per-CTA partials: out = {mean |x-y|, mean SSIM, total loss}
-__global__ void __launch_bounds__(1024) ssim_reduce_kernel(int nblk, const float* __restrict__ partial, float inv_n,
-                                                           float w_l1, float w_dssim, float* __restrict__ out) {
+__device__ __forceinline__ void ssim_reduce_body(int nblk, const float* __restrict__ partial, float inv_n, float w_l1,
+                                                 float w_dssim, float* __restrict__ out) {
     __shared__ double s_a[32], s_b[32];
     double a = 0.0, b = 0.0;
     for (int i = threadIdx.x; i < nblk; i += 1024) { a += (double)partial[2 * i]; b += (double)partial[2 * i + 1]; }
@@ -134,11 +151,22 @@ __global__ void __launch_bounds__(1024) ssim_reduce_kernel(int nblk, const float
     }
 }
 
+__global__ void __launch_bounds__(1024) ssim_reduce_kernel(int nblk, const float* __restrict__ partial, float inv_n,
+                                                           float w_l1, float w_dssim, float* __restrict__ out) {
+    ssim_reduce_body(nblk, partial, inv_n, w_l1, w_dssim, out);
+}
+
+// image v = blockIdx.x -> out[3 v .. 3 v + 2]
+__global__ void __launch_bounds__(1024) ssim_reduce_views_kernel(int nblk, const float* __restrict__ partial,
+                                                                 size_t slab, float inv_n, float w_l1, float w_dssim,
+                                                                 float* __restrict__ out) {
+    ssim_reduce_body(nblk, partial + blockIdx.x * slab, inv_n, w_l1, w_dssim, out + 3 * (size_t)blockIdx.x);
+}
+
 // Stage 2: d loss / d x = w_l1 sign(x-y)/N - w_dssim/N [ conv(M1) + 2 x conv(M2) + y conv(M3) ]
-__global__ void __launch_bounds__(LT * LT) ssim_grad_kernel(int H, int W, const float* __restrict__ x,
-                                                           const float* __restrict__ y, SsimWindow win,
-                                                           const float* __restrict__ maps, float w_l1, float w_dssim,
-                                                           float inv_n, float* __restrict__ grad) {
+__device__ __forceinline__ void ssim_grad_body(int H, int W, const float* __restrict__ x, const float* __restrict__ y,
+                                               const SsimWindow& win, const float* __restrict__ maps, float w_l1,
+                                               float w_dssim, float inv_n, float* __restrict__ grad) {
     __shared__ float sm[3][LE][LE + 1];
     __shared__ float hm[3][LE][LT];
     const int tid = threadIdx.y * LT + threadIdx.x;
@@ -182,6 +210,21 @@ __global__ void __launch_bounds__(LT * LT) ssim_grad_kernel(int H, int W, const 
     grad[o] = inv_n * (w_l1 * sgn - w_dssim * dssim);
 }
 
+__global__ void __launch_bounds__(LT * LT) ssim_grad_kernel(int H, int W, const float* __restrict__ x,
+                                                           const float* __restrict__ y, SsimWindow win,
+                                                           const float* __restrict__ maps, float w_l1, float w_dssim,
+                                                           float inv_n, float* __restrict__ grad) {
+    ssim_grad_body(H, W, x, y, win, maps, w_l1, w_dssim, inv_n, grad);
+}
+
+__global__ void __launch_bounds__(LT * LT) ssim_grad_views_kernel(int H, int W, const float* __restrict__ x,
+                                                                 const float* __restrict__ y, SsimWindow win,
+                                                                 const float* __restrict__ maps, size_t slab, float w_l1,
+                                                                 float w_dssim, float inv_n, float* __restrict__ grad) {
+    const size_t v = blockIdx.z, n = (size_t)H * W;
+    ssim_grad_body(H, W, x + v * n, y + v * n, win, maps + v * slab, w_l1, w_dssim, inv_n, grad + v * n);
+}
+
 size_t image_loss_scratch_bytes(int H, int W) {
     const size_t nblk = (size_t)((W + LT - 1) / LT) * ((H + LT - 1) / LT);
     return 256 + ((3 * (size_t)H * W * sizeof(float) + 255) & ~(size_t)255) + nblk * 2 * sizeof(float);
@@ -201,6 +244,41 @@ int launch_image_loss(cudaStream_t st, int H, int W, const float* image, const f
     ssim_stats_kernel<<<grid, block, 0, st>>>(H, W, image, target, win, grad_out ? maps : nullptr, partial);
     ssim_reduce_kernel<<<1, 1024, 0, st>>>(nblk, partial, inv_n, w_l1, w_dssim, loss_out);
     if (grad_out) ssim_grad_kernel<<<grid, block, 0, st>>>(H, W, image, target, win, maps, w_l1, w_dssim, inv_n, grad_out);
+    R2X_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+// N images: slab v of the scratch holds image v's maps [3][H][W] and then its per-CTA partials, laid out as the
+// single-image scratch (so every image goes through exactly the single-image arithmetic).
+static size_t image_loss_slab_bytes(int H, int W) {
+    const size_t nblk = (size_t)((W + LT - 1) / LT) * ((H + LT - 1) / LT);
+    return ((3 * (size_t)H * W * sizeof(float) + 255) & ~(size_t)255) + ((nblk * 2 * sizeof(float) + 255) & ~(size_t)255);
+}
+
+size_t image_loss_views_scratch_bytes(int N, int H, int W) {
+    if (N < 1 || H <= 0 || W <= 0) return 0;
+    return 256 + (size_t)N * image_loss_slab_bytes(H, W);
+}
+
+int launch_image_loss_views(cudaStream_t st, int N, int H, int W, const float* images, const float* targets, float w_l1,
+                            float w_dssim, float* loss_out, float* grad_out, void* scratch, size_t scratch_bytes) {
+    if (N < 1 || N > 65535) return fail_msg(R2X_ERR_INVALID, "r2x_image_loss_views: bad N (need 1 <= N <= 65535)");
+    if (H <= 0 || W <= 0) return fail_msg(R2X_ERR_INVALID, "r2x_image_loss_views: bad H/W");
+    if (!images || !targets || !loss_out || !scratch) return fail_msg(R2X_ERR_INVALID, "r2x_image_loss_views: null pointer");
+    if (scratch_bytes < image_loss_views_scratch_bytes(N, H, W))
+        return fail_msg(R2X_ERR_INVALID, "r2x_image_loss_views: scratch too small");
+    static const SsimWindow win = make_window();
+    const dim3 grid((W + LT - 1) / LT, (H + LT - 1) / LT, N), block(LT, LT);
+    const int nblk = (int)(grid.x * grid.y);
+    const size_t slab = image_loss_slab_bytes(H, W) / sizeof(float);
+    float* maps = (float*)(((size_t)scratch + 255) & ~(size_t)255);
+    float* partial = (float*)((char*)maps + ((3 * (size_t)H * W * sizeof(float) + 255) & ~(size_t)255));
+    const float inv_n = 1.0f / (float)((double)H * (double)W);
+    ssim_stats_views_kernel<<<grid, block, 0, st>>>(H, W, images, targets, win, grad_out ? maps : nullptr, partial, slab);
+    ssim_reduce_views_kernel<<<N, 1024, 0, st>>>(nblk, partial, slab, inv_n, w_l1, w_dssim, loss_out);
+    if (grad_out)
+        ssim_grad_views_kernel<<<grid, block, 0, st>>>(H, W, images, targets, win, maps, slab, w_l1, w_dssim, inv_n,
+                                                       grad_out);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -368,6 +446,43 @@ int launch_densify_stats(cudaStream_t st, int P, const int* radii, const float* 
                          float* denom, const uint32_t* guard0, const uint32_t* guard1) {
     if (P <= 0) return 0;
     densify_stats_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, radii, grad2d, max_radii, accum, denom, guard0, guard1);
+    R2X_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+// N views' statistics in one launch: radii[N,P], grad2d[N,P,3]; each Gaussian takes the views in order with the
+// single-view kernel's arithmetic on values held in registers (bit for bit N launches of densify_stats_kernel).
+__global__ void __launch_bounds__(256) densify_stats_views_kernel(int N, int P, const int* __restrict__ radii,
+                                                                  const float* __restrict__ grad2d,
+                                                                  float* __restrict__ max_radii, float* __restrict__ accum,
+                                                                  float* __restrict__ denom, const uint32_t* guard0,
+                                                                  const uint32_t* guard1) {
+    if ((guard0 && guard0[1]) || (guard1 && guard1[1])) return;
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= P) return;
+    float mr = 0.f, acc = 0.f, den = 0.f;
+    bool seen = false;
+    for (int v = 0; v < N; ++v) {
+        const size_t vg = (size_t)v * P + g;
+        const int r = radii[vg];
+        if (r <= 0) continue;
+        if (!seen) { mr = max_radii[g]; acc = accum[g]; den = denom[g]; seen = true; }
+        mr = fmaxf(mr, (float)r);
+        const float gx = grad2d[3 * vg], gy = grad2d[3 * vg + 1];
+        acc = __fadd_rn(acc, sqrtf(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy))));
+        den = __fadd_rn(den, 1.0f);
+    }
+    if (!seen) return;
+    max_radii[g] = mr;
+    accum[g] = acc;
+    denom[g] = den;
+}
+
+int launch_densify_stats_views(cudaStream_t st, int N, int P, const int* radii, const float* grad2d, float* max_radii,
+                               float* accum, float* denom, const uint32_t* guard0, const uint32_t* guard1) {
+    if (P <= 0) return 0;
+    densify_stats_views_kernel<<<(P + 255) / 256, 256, 0, st>>>(N, P, radii, grad2d, max_radii, accum, denom, guard0,
+                                                                guard1);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }

@@ -134,6 +134,17 @@ def read_scene(source_path: str, eval: bool = True) -> SceneInfo:
     raise ValueError(f"Could not recognize scene type: {source_path}.")
 
 
+def train_view_count(source_path: str) -> int:
+    """Number of train views of a scene (either format), without reading its projections."""
+    if os.path.exists(os.path.join(source_path, "meta_data.json")):
+        with open(os.path.join(source_path, "meta_data.json")) as f:
+            return len(json.load(f)["proj_train"])
+    if source_path.split(".")[-1] in ("pickle", "pkl"):
+        with open(source_path, "rb") as f:
+            return int(pickle.load(f)["numTrain"])
+    raise ValueError(f"Could not recognize scene type: {source_path}.")
+
+
 class Camera:
     """What render() needs from a view (`dataset/cameras.py:20-84`), on `device`."""
 

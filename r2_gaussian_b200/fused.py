@@ -108,6 +108,34 @@ class _RasterizeRawMatrices(torch.autograd.Function):
         return g3, g2, gd, gs, gr, gv, gp, None, None
 
 
+class _RasterizeViewsRaw(torch.autograd.Function):
+    """`_RasterizeRaw` for N views of one cloud in one native call: forward inputs (means3D, means2D[N,P,3], raw_density,
+    raw_scales, raw_rotations, viewmatrices[N,4,4], projmatrices[N,4,4], settings, act) -> (images[N,H,W], radii[N,P]);
+    the settings' own matrices are ignored.  The backward sums the raw gradients over the views in view order and hands
+    means2D the per-view screen-space gradients."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, raw_density, raw_scales, raw_rotations, viewmatrices, projmatrices, settings, act):
+        s = settings
+        with _C.speculative(any(ctx.needs_input_grad)):
+            R, images, radii, geom, binning, img = _C.rasterize_views_raw(
+                means3D, raw_density, raw_scales, raw_rotations, s.scale_modifier, viewmatrices, projmatrices, s.tanfovx,
+                s.tanfovy, s.image_height, s.image_width, s.mode, act)
+        ctx.settings, ctx.act, ctx.num_rendered = s, act, R
+        ctx.save_for_backward(means3D, raw_scales, raw_rotations, viewmatrices, projmatrices, radii, geom, binning, img)
+        ctx.mark_non_differentiable(radii)
+        return images, radii
+
+    @staticmethod
+    def backward(ctx, grad_images, _grad_radii):
+        s, act = ctx.settings, ctx.act
+        means3D, raw_scales, raw_rotations, viewmatrices, projmatrices, radii, geom, binning, img = ctx.saved_tensors
+        g2, gd, g3, _gcov, gs, gr = _C.rasterize_views_raw_backward(
+            means3D, radii, raw_scales, raw_rotations, s.scale_modifier, viewmatrices, projmatrices, s.tanfovx,
+            s.tanfovy, grad_images, geom, ctx.num_rendered, binning, img, s.mode, act)
+        return g3, g2, gd, gs, gr, None, None, None, None
+
+
 class _VoxelizeRaw(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, raw_density, raw_scales, raw_rotations, settings, act):
@@ -170,6 +198,17 @@ def rasterize_raw_matrices(means3D, means2D, raw, viewmatrix, projmatrix, settin
     """`rasterize_raw` whose image is also differentiable with respect to `viewmatrix` / `projmatrix`."""
     return _RasterizeRawMatrices.apply(means3D, means2D, raw["density"], raw["scaling"], raw["rotation"], viewmatrix,
                                        projmatrix, settings, _act(raw))
+
+
+def rasterize_views_raw(means3D, means2D, raw, viewmatrices, projmatrices, settings):
+    """`rasterize_raw` for N views in one call -> (images [N,H,W], radii [N,P]).  viewmatrices / projmatrices [N,4,4]
+    (not differentiated); `means2D` [N,P,3] receives the per-view screen-space gradients.  Image v and radii[v] are bit
+    for bit `rasterize_raw` of view v; each raw gradient is the single-view ones summed in view order (float32)."""
+    N = _C.check_views_args(means3D, viewmatrices, projmatrices)
+    if tuple(means2D.shape) != (N, means3D.shape[0], 3):
+        raise ValueError(f"means2D must have dimensions ({N}, {means3D.shape[0]}, 3), got {tuple(means2D.shape)}")
+    return _RasterizeViewsRaw.apply(means3D, means2D, raw["density"], raw["scaling"], raw["rotation"],
+                                    viewmatrices.detach(), projmatrices.detach(), settings, _act(raw))
 
 
 def voxelize_raw(means3D, raw, settings):

@@ -33,6 +33,14 @@ With `pose=(PoseCorrection, FusedAdam over [omega] and [nu], one group each)` th
 iteration).  Pose refinement with Gaussian sharding is refused at bind time: each rank would hold only a partial sum
 of the matrix gradients.  With `pose=None` the launch sequence is the one above.
 
+A LIST of B > 1 cameras (with a [B,H,W] target) makes one iteration of B views: the objective is
+sum_v [L1 + lambda_dssim (1 - SSIM)](view v) + B lambda_tv TV(crop), one Adam step, the statistics of every view in view
+order.  The raster and loss calls become their batched forms (r2x_raster_forward_views_async_raw, r2x_image_loss_views,
+r2x_raster_backward_views_raw, r2x_densify_stats_views), so each view's image and image gradient is bit for bit its
+single-view one and the launch count does not grow with B.  The buffers are bound per B; a repeated iteration repeats
+the same batch.  Batches take no pose refinement and no Gaussian sharding.  A list of one camera is the single-view
+iteration.
+
 The model's tensors are updated in place: `GaussianModel._xyz/_density/_scaling/_rotation`, the `FusedAdam` state of
 `gaussians.optimizer` (same `exp_avg`, `exp_avg_sq`, `step`, so checkpoints and the densification surgery are
 unchanged) and `max_radii2D / xyz_gradient_accum / denom`.  After densification (new tensors) the step re-binds itself.
@@ -70,41 +78,51 @@ class NativeTrainStep:
         self.repeats = 0            # iterations repeated after a capacity overflow
 
     # ------------------------------------------------------------------ buffers
-    def _signature(self, H, W):
+    def _signature(self, H, W, B):
         gm = self.gm
         sig = (sharded.enabled(), gm._xyz.data_ptr(), gm._density.data_ptr(), gm._scaling.data_ptr(), gm._rotation.data_ptr(),
-               int(gm._xyz.shape[0]), H, W, gm.max_radii2D.data_ptr(), gm.xyz_gradient_accum.data_ptr())
+               int(gm._xyz.shape[0]), H, W, B, gm.max_radii2D.data_ptr(), gm.xyz_gradient_accum.data_ptr())
         if self.pose is not None:
             sig += (self.pose.omega.data_ptr(), self.pose.nu.data_ptr())
         return sig
 
-    def _bind(self, H, W):
+    def _bind(self, H, W, B):
         gm, lib = self.gm, self.lib
         dev = gm._xyz.device
         P = int(gm._xyz.shape[0])
-        self.P, self.H, self.W, self.dev = P, H, W, dev
+        self.P, self.H, self.W, self.B, self.dev = P, H, W, B, dev
         f32 = dict(dtype=torch.float32, device=dev)
         u8 = dict(dtype=torch.uint8, device=dev)
         i32 = dict(dtype=torch.int32, device=dev)
+        self.sharded = sharded.enabled()
+        if B > 1 and (self.sharded or self.pose is not None):
+            raise RuntimeError("NativeTrainStep: a batch of views takes no Gaussian sharding and no pose refinement")
         with torch.cuda.device(dev):
             # raster.  Gaussian-sharded runs: the image travels through the exchange with one extra word, this rank's
             # overflow flag, so that after the sum EVERY rank knows whether ANY rank's forward overflowed (the summed
-            # image is then wrong everywhere) and all ranks skip / repeat the iteration together.
-            self.sharded = sharded.enabled()
-            self.image_ext = torch.zeros(H * W + 4, **f32)
-            self.image = self.image_ext[:H * W].view(1, H, W)
-            self.flag_r = self.image_ext[H * W:H * W + 1]
-            self.radii = torch.empty((P,), **i32)
-            self.geom, self.img = _C.RASTER.state(P, (W, H), dev)
+            # image is then wrong everywhere) and all ranks skip / repeat the iteration together.  B views: images,
+            # radii and dL/dmean2D per view, the stacked camera matrices, and the batched forward's state.
+            self.image_ext = torch.zeros(B * H * W + 4, **f32)
+            self.image = self.image_ext[:B * H * W].view(B, H, W)
+            self.flag_r = self.image_ext[B * H * W:B * H * W + 1]
+            self.radii = torch.empty((P,) if B == 1 else (B, P), **i32)
+            if B == 1:
+                self.geom, self.img = _C.RASTER.state(P, (W, H), dev)
+            else:
+                self.geom, self.img = _C.views_state(P, B, W, H, dev)
+                self.views = torch.empty((B, 4, 4), **f32); self.projs = torch.empty((B, 4, 4), **f32)
             self.status_r = torch.zeros(2, **i32)
-            self.key_r = _C.raster_key(dev, P, W, H)
-            self.g2 = torch.empty((P, 3), **f32); self.gd = torch.empty((P, 1), **f32); self.g3 = torch.empty((P, 3), **f32)
+            self.key_r = _C.raster_key(dev, P, W, H) if B == 1 else _C.views_key(dev, P, B, W, H)
+            self.g2 = torch.empty((P, 3) if B == 1 else (B, P, 3), **f32)
+            self.gd = torch.empty((P, 1), **f32); self.g3 = torch.empty((P, 3), **f32)
             self.gcov = torch.empty((P, 6), **f32); self.gs = torch.empty((P, 3), **f32); self.gr = torch.empty((P, 4), **f32)
             # image loss
-            self.loss_scratch_bytes = int(lib.r2x_image_loss_scratch_bytes(H, W))
+            self.loss_scratch_bytes = int(lib.r2x_image_loss_scratch_bytes(H, W) if B == 1 else
+                                          lib.r2x_image_loss_views_scratch_bytes(B, H, W))
             self.loss_scratch = torch.empty(self.loss_scratch_bytes, **u8)
-            self.loss_out = torch.zeros(3, **f32)            # L1, SSIM, lambda_l1 L1 + lambda_dssim (1 - SSIM)
-            self.dL_dimage = torch.empty((H, W), **f32)
+            # L1, SSIM, lambda_l1 L1 + lambda_dssim (1 - SSIM); one row per view
+            self.loss_out = torch.zeros(3 if B == 1 else (B, 3), **f32)
+            self.dL_dimage = torch.empty((H, W) if B == 1 else (B, H, W), **f32)
             # TV crop
             if self.use_tv:
                 nx, ny, nz = self.tv_n
@@ -153,7 +171,7 @@ class NativeTrainStep:
         self.act = fused._act(gm.raw_parameters())
         if self.pose is not None:
             self._bind_pose(P, dev)
-        self._bound = self._signature(H, W)
+        self._bound = self._signature(H, W, B)
 
     def _bind_pose(self, P, dev):
         """Buffers of the pose path: corrected matrices, their gradients, the pose gradients and the two Adam groups
@@ -195,7 +213,7 @@ class NativeTrainStep:
     def _provision(self):
         """Instance capacities for this iteration: both forwards are speculative.  The buffers only ever grow."""
         dev = self.dev
-        want_r = _C._Workspace.provision(self.key_r, self.P, _C.RASTER.seed, speculative=True)
+        want_r = _C._Workspace.provision(self.key_r, self.P * self.B, _C.RASTER.seed, speculative=True)
         if want_r > self.cap_r:
             self.cap_r = want_r
             self.binning_r, self.scratch_r = _C.binning_buffer(want_r, dev), _C.RASTER.bwd_scratch(want_r, dev)
@@ -208,15 +226,26 @@ class NativeTrainStep:
     # ------------------------------------------------------------------ one iteration
     def __call__(self, cam, gt, tv_centre=None, apply_update: bool = True, view: int | None = None,
                  pose_update: bool | None = None):
-        """Enqueue one iteration.  `cam`: camera (render_query.render's contract); `gt`: [1,H,W] or [H,W] CUDA float32
-        target; `tv_centre`: 3 floats (ignored without TV).  With `pose`: `view` is the camera's row of the
-        PoseCorrection and `pose_update` (default: `apply_update`) whether the pose Adam steps.  Returns {"render",
-        "radii", "loss" (device [3]: L1, SSIM, image total), "tv" (device [1] or None)} -- views of buffers that the
-        next call overwrites."""
+        """Enqueue one iteration.  `cam`: camera (render_query.render's contract), or a list of B cameras sharing image
+        size, field of view and mode; `gt`: [1,H,W] or [H,W] CUDA float32 target ([B,H,W] for B cameras); `tv_centre`:
+        3 floats (ignored without TV).  With `pose`: `view` is the camera's row of the PoseCorrection and `pose_update`
+        (default: `apply_update`) whether the pose Adam steps.  Returns {"render", "radii", "viewspace_grad", "loss"
+        (device [3]: L1, SSIM, image total; [B,3] for B cameras), "tv" (device [1] or None)} -- views of buffers that
+        the next call overwrites."""
         self.check()                                            # the previous iteration (one late; no stall)
-        H, W = int(cam.image_height), int(cam.image_width)
-        if self._bound != self._signature(H, W):
-            self._bind(H, W)
+        if isinstance(cam, (list, tuple)):
+            if not cam:
+                raise ValueError("NativeTrainStep: empty camera list")
+            cam = cam[0] if len(cam) == 1 else list(cam)
+        B = len(cam) if isinstance(cam, list) else 1
+        c0 = cam[0] if B > 1 else cam
+        H, W = int(c0.image_height), int(c0.image_width)
+        if B > 1:
+            key = lambda c: (int(c.image_height), int(c.image_width), int(c.mode), float(c.FoVx), float(c.FoVy))
+            if any(key(c) != key(c0) for c in cam[1:]):
+                raise ValueError("NativeTrainStep: the cameras of a batch must share image size, field of view and mode")
+        if self._bound != self._signature(H, W, B):
+            self._bind(H, W, B)
         if self.P == 0 and not self.sharded:
             raise RuntimeError("NativeTrainStep: empty model")
         # an EMPTY SHARD of a Gaussian-sharded run goes through the same sequence: the library calls are no-ops that
@@ -232,19 +261,25 @@ class NativeTrainStep:
         return self.result
 
     def _enqueue(self, cam, gt, tv_centre, apply_update, pose_args):
-        gm, lib, dev, P, H, W = self.gm, self.lib, self.dev, self.P, self.H, self.W
+        gm, lib, dev, P, H, W, B = self.gm, self.lib, self.dev, self.P, self.H, self.W, self.B
         self._provision()
-        mode = int(cam.mode)
+        c0 = cam[0] if B > 1 else cam
+        mode = int(c0.mode)
         if mode == 0:
             tfx = tfy = 1.0
         elif mode == 1:
-            tfx, tfy = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
+            tfx, tfy = math.tan(c0.FoVx * 0.5), math.tan(c0.FoVy * 0.5)
         else:
             raise ValueError("Unsupported mode!")
-        gt = gt.reshape(H, W)
+        gt = gt.reshape(H, W) if B == 1 else gt.reshape(B, H, W)
         if gt.dtype != torch.float32 or not gt.is_contiguous() or gt.device != dev:
             gt = gt.to(device=dev, dtype=torch.float32).contiguous()
-        view, proj, campos = cam.world_view_transform, cam.full_proj_transform, cam.camera_center
+        if B > 1:
+            torch.stack([c.world_view_transform for c in cam], out=self.views)
+            torch.stack([c.full_proj_transform for c in cam], out=self.projs)
+            view, proj, campos = self.views, self.projs, None
+        else:
+            view, proj, campos = cam.world_view_transform, cam.full_proj_transform, cam.camera_center
         act = C.byref(self.act)
         sm = self.scale_modifier
         xyz, dens, scal, rot = gm._xyz, gm._density, gm._scaling, gm._rotation
@@ -257,19 +292,32 @@ class NativeTrainStep:
                                          view.data_ptr(), proj.data_ptr(), cam.projection_matrix.data_ptr(),
                                          self.pose_view.data_ptr(), self.pose_full.data_ptr()), "r2x_pose_apply")
                 view, proj = self.pose_view, self.pose_full
-            check(lib.r2x_raster_forward_async_raw(
-                st, P, W, H, xyz.data_ptr(), dens.data_ptr(), scal.data_ptr(), sm, rot.data_ptr(), view.data_ptr(),
-                proj.data_ptr(), campos.data_ptr(), tfx, tfy, mode, self.image.data_ptr(), self.radii.data_ptr(),
-                self.geom.data_ptr(), self.img.data_ptr(), self.binning_r.data_ptr(), self.cap_r, self.status_r.data_ptr(),
-                act), "r2x_raster_forward_async_raw")
+            if B == 1:
+                check(lib.r2x_raster_forward_async_raw(
+                    st, P, W, H, xyz.data_ptr(), dens.data_ptr(), scal.data_ptr(), sm, rot.data_ptr(), view.data_ptr(),
+                    proj.data_ptr(), campos.data_ptr(), tfx, tfy, mode, self.image.data_ptr(), self.radii.data_ptr(),
+                    self.geom.data_ptr(), self.img.data_ptr(), self.binning_r.data_ptr(), self.cap_r,
+                    self.status_r.data_ptr(), act), "r2x_raster_forward_async_raw")
+            else:
+                check(lib.r2x_raster_forward_views_async_raw(
+                    st, P, B, W, H, xyz.data_ptr(), dens.data_ptr(), scal.data_ptr(), sm, rot.data_ptr(),
+                    view.data_ptr(), proj.data_ptr(), tfx, tfy, mode, self.image.data_ptr(), self.radii.data_ptr(),
+                    self.geom.data_ptr(), self.img.data_ptr(), self.binning_r.data_ptr(), self.cap_r,
+                    self.status_r.data_ptr(), act), "r2x_raster_forward_views_async_raw")
             image = self.image
             if self.sharded:
                 self.flag_r.copy_(self.status_r[1:2])          # my overflow flag rides with the image
                 sharded.sharded_sum_(self.image_ext)
                 self.status_r[1:2].copy_(self.flag_r)          # ... and comes back as "any rank overflowed"
-            check(lib.r2x_image_loss(st, H, W, image.data_ptr(), gt.data_ptr(), 1.0, self.lambda_dssim,
-                                     self.loss_out.data_ptr(), self.dL_dimage.data_ptr(), self.loss_scratch.data_ptr(),
-                                     self.loss_scratch_bytes), "r2x_image_loss")
+            if B == 1:
+                check(lib.r2x_image_loss(st, H, W, image.data_ptr(), gt.data_ptr(), 1.0, self.lambda_dssim,
+                                         self.loss_out.data_ptr(), self.dL_dimage.data_ptr(),
+                                         self.loss_scratch.data_ptr(), self.loss_scratch_bytes), "r2x_image_loss")
+            else:
+                check(lib.r2x_image_loss_views(st, B, H, W, image.data_ptr(), gt.data_ptr(), 1.0, self.lambda_dssim,
+                                               self.loss_out.data_ptr(), self.dL_dimage.data_ptr(),
+                                               self.loss_scratch.data_ptr(), self.loss_scratch_bytes),
+                      "r2x_image_loss_views")
             if self.use_tv:
                 nx, ny, nz = self.tv_n
                 grid = (nx, ny, nz, self.tv_s[0], self.tv_s[1], self.tv_s[2], tv_centre[0], tv_centre[1], tv_centre[2])
@@ -284,14 +332,22 @@ class NativeTrainStep:
                     self.status_v[1:2].copy_(self.flag_v)
                 check(lib.r2x_tv3d_loss(st, nx, ny, nz, vol.data_ptr(), 1, self.tv_out.data_ptr(), self.dL_dvol.data_ptr(),
                                         self.tv_scratch.data_ptr(), self.tv_scratch_bytes), "r2x_tv3d_loss")
-                self.dL_dvol.mul_(self.lambda_tv)
+                # B views: the TV term carries weight B lambda_tv (B times the batch mean of the single-view objective)
+                self.dL_dvol.mul_(self.lambda_tv if B == 1 else B * self.lambda_tv)
                 check(lib.r2x_voxel_backward_raw(
                     st, P, self.cap_v, *grid, xyz.data_ptr(), scal.data_ptr(), sm, rot.data_ptr(), self.rx.data_ptr(),
                     self.ry.data_ptr(), self.rz.data_ptr(), self.geom_v.data_ptr(), self.binning_v.data_ptr(),
                     self.img_v.data_ptr(), self.scratch_v.data_ptr(), self.dL_dvol.data_ptr(), self.gdv.data_ptr(),
                     self.g3v.data_ptr(), self.gcovv.data_ptr(), self.gsv.data_ptr(), self.grv.data_ptr(), act),
                     "r2x_voxel_backward_raw")
-            if pose_args is None:
+            if B > 1:
+                check(lib.r2x_raster_backward_views_raw(
+                    st, P, B, self.cap_r, W, H, xyz.data_ptr(), scal.data_ptr(), sm, rot.data_ptr(), view.data_ptr(),
+                    proj.data_ptr(), tfx, tfy, self.radii.data_ptr(), self.geom.data_ptr(), self.binning_r.data_ptr(),
+                    self.img.data_ptr(), self.scratch_r.data_ptr(), self.dL_dimage.data_ptr(), self.g2.data_ptr(),
+                    self.gd.data_ptr(), self.g3.data_ptr(), self.gcov.data_ptr(), self.gs.data_ptr(), self.gr.data_ptr(),
+                    mode, act), "r2x_raster_backward_views_raw")
+            elif pose_args is None:
                 check(lib.r2x_raster_backward_raw(
                     st, P, self.cap_r, W, H, xyz.data_ptr(), scal.data_ptr(), sm, rot.data_ptr(), view.data_ptr(),
                     proj.data_ptr(), campos.data_ptr(), tfx, tfy, self.radii.data_ptr(), self.geom.data_ptr(),
@@ -315,9 +371,15 @@ class NativeTrainStep:
                                         self.pose_gproj.data_ptr(), self.g_omega.data_ptr(), self.g_nu.data_ptr()),
                       "r2x_pose_grad")
             guard_v = self.status_v.data_ptr() if self.use_tv else None
-            check(lib.r2x_densify_stats(st, P, self.radii.data_ptr(), self.g2.data_ptr(), gm.max_radii2D.data_ptr(),
-                                        gm.xyz_gradient_accum.data_ptr(), gm.denom.data_ptr(), self.status_r.data_ptr(),
-                                        guard_v), "r2x_densify_stats")
+            if B == 1:
+                check(lib.r2x_densify_stats(st, P, self.radii.data_ptr(), self.g2.data_ptr(), gm.max_radii2D.data_ptr(),
+                                            gm.xyz_gradient_accum.data_ptr(), gm.denom.data_ptr(),
+                                            self.status_r.data_ptr(), guard_v), "r2x_densify_stats")
+            else:
+                check(lib.r2x_densify_stats_views(st, B, P, self.radii.data_ptr(), self.g2.data_ptr(),
+                                                  gm.max_radii2D.data_ptr(), gm.xyz_gradient_accum.data_ptr(),
+                                                  gm.denom.data_ptr(), self.status_r.data_ptr(), guard_v),
+                      "r2x_densify_stats_views")
             if apply_update:
                 steps = set()
                 for k, (group, p, stt, _g1, _g2) in enumerate(self.adam):
@@ -356,8 +418,9 @@ class NativeTrainStep:
                        "tv": self.tv_out if self.use_tv else None}
 
     def total_loss(self) -> float:
-        """Host value of the last iteration's loss (synchronises; logging only)."""
-        t = float(self.loss_out[2])
+        """Host value of the last iteration's loss (synchronises; logging only): for B views the batch mean of the image
+        losses plus lambda_tv TV, comparable with a single-view iteration's."""
+        t = float(self.loss_out[2]) if self.B == 1 else float(self.loss_out[:, 2].double().mean())
         return t + self.lambda_tv * float(self.tv_out[0]) if self.use_tv else t
 
     def check(self):

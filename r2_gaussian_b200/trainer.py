@@ -19,6 +19,15 @@ streams stay in lock-step (same seed, same draws), rank 0 writes one merged `poi
 `--iterations`), on both training paths; the poses step wherever the Gaussians would and at densification iterations.
 Train views are then evaluated with their corrected cameras, each save writes `train_poses.npz` and checkpoints carry
 the poses.  Without the switch nothing changes: same launches, settings files, checkpoints and printed keys.
+
+`--batch_size B` (default 1, at most the number of train views) takes B train views per optimizer step, rendered in one
+batched call (`fused.rasterize_views_raw`; `NativeTrainStep` with a list of cameras).  The views are popped from the
+camera stack with the draws B single-view iterations would make, so a run sees the B = 1 sequence of views grouped by
+B.  The objective is the SUM of the B views' image losses plus B lambda_tv TV of one crop (B times the batch mean; Adam
+is invariant to that scale up to its eps of 1e-15); the densification statistics count every view; the logged loss is
+the batch mean plus lambda_tv TV.  Iteration counts and the learning-rate and densification schedules stay in optimizer
+steps, so a run sees B times as many views.  B > 1 is refused with --pose_refine, Gaussian sharding and
+compute_cov3D_python.  With B = 1 nothing changes.
 """
 from __future__ import annotations
 
@@ -34,14 +43,15 @@ import torch
 
 from . import losses
 from ._C import CapacityOverflow
-from .dataset import Scene
+from .dataset import Scene, train_view_count
 from .gaussian_model import GaussianModel
 from .gaussian_utils import get_expon_lr_func
 from .metrics import metric_proj, metric_vol
 from .optim import FusedAdam
 from .pose import PoseCorrection
-from .render_query import query, render
-from . import sharded, train_step
+from .rasterization import GaussianRasterizationSettings
+from .render_query import _tan_fov, query, render
+from . import fused, sharded, train_step
 from .sharded import gather_point_cloud, shard_init_points, world_info
 
 
@@ -153,17 +163,68 @@ def evaluate(scene: Scene, gaussians: GaussianModel, pipe, with_ssim: bool = Tru
     return out
 
 
+def batch_refusal(batch_size: int, pose_refine: bool, world: int, compute_cov3D_python: bool) -> str | None:
+    """Why `--batch_size` cannot be used with these settings (None: it can).  Checked before any CUDA work."""
+    if batch_size < 1:
+        return f"--batch_size must be at least 1, got {batch_size}"
+    if batch_size == 1:
+        return None
+    if pose_refine:
+        return "--batch_size > 1 is not supported with --pose_refine (the batched rasterizer returns no matrix gradients)"
+    if world > 1:
+        return "--batch_size > 1 is not supported with Gaussian sharding (WORLD_SIZE > 1)"
+    if compute_cov3D_python:
+        return "--batch_size > 1 is not supported with compute_cov3D_python (the batched path folds the activations)"
+    return None
+
+
+def draw_train_views(stack, cameras, B: int):
+    """Pop B train views off the camera stack -> (views, stack): the draws of B single-view iterations, each a
+    `random.randint` on the stack, which is refilled from `cameras` when empty (`train.py:103-106`)."""
+    views = []
+    for _ in range(B):
+        if not stack:
+            stack = cameras.copy()
+        views.append(stack.pop(random.randint(0, len(stack) - 1)))
+    return views, stack
+
+
+def render_batch(cams, gaussians: GaussianModel) -> dict:
+    """The training render of B views of `gaussians` in one call on its raw parameters (`fused.rasterize_views_raw`) ->
+    {"render": [B,H,W], "viewspace_points": [B,P,3] (its .grad receives the per-view dL/dmean2D), "radii": [B,P]}.
+    Image v is bit for bit the single-view raw render of cams[v]."""
+    c0 = cams[0]
+    tanfovx, tanfovy = _tan_fov(c0)
+    views = torch.stack([c.world_view_transform for c in cams])
+    projs = torch.stack([c.full_proj_transform for c in cams])
+    xyz = gaussians.get_xyz
+    means2D = torch.zeros((len(cams),) + tuple(xyz.shape), dtype=xyz.dtype, device=xyz.device, requires_grad=True) + 0
+    means2D.retain_grad()
+    settings = GaussianRasterizationSettings(
+        image_height=int(c0.image_height), image_width=int(c0.image_width), tanfovx=tanfovx, tanfovy=tanfovy,
+        scale_modifier=1.0, viewmatrix=views[0], projmatrix=projs[0], campos=c0.camera_center, prefiltered=False,
+        mode=int(c0.mode), debug=False)
+    images, radii = fused.rasterize_views_raw(xyz, means2D, gaussians.raw_parameters(), views, projs, settings)
+    return {"render": images, "viewspace_points": means2D, "radii": radii}
+
+
 def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, testing_iterations=(),
              saving_iterations=(), checkpoint_iterations=(), checkpoint: str | None = None, init_points=None,
-             log=print, pose_params: PoseParams | None = None) -> dict:
+             log=print, pose_params: PoseParams | None = None, batch_size: int = 1) -> dict:
     first_iter = 0
     refine = pose_params is not None and pose_params.pose_refine
     if refine and world_info()[1] > 1:
         raise RuntimeError("--pose_refine is not supported with Gaussian sharding (WORLD_SIZE > 1): every rank would "
                            "hold only its shard's part of the camera-matrix gradients")
+    B = int(batch_size)
+    why = batch_refusal(B, refine, world_info()[1], bool(getattr(pipe, "compute_cov3D_python", False)))
+    if why is not None:
+        raise ValueError(why)
     scene = Scene(model.source_path, model.model_path, eval=model.eval, shuffle=False, device="cuda",
                   data_device=model.data_device)
     cfg = scene.scanner_cfg
+    if B > len(scene.getTrainCameras()):
+        raise ValueError(f"--batch_size {B} exceeds the scene's {len(scene.getTrainCameras())} train views")
     bbox_cpu = scene.bbox.float()
     bbox = bbox_cpu.cuda()
     ds = derived_settings(cfg, model, opt)
@@ -271,16 +332,57 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
         if corr is not None:
             for group, schedule in zip(pose_opt.param_groups, pose_lr):
                 group["lr"] = schedule(iteration)
-        if not stack:
-            stack = scene.getTrainCameras().copy()
-        cam = stack.pop(random.randint(0, len(stack) - 1))
+        cams, stack = draw_train_views(stack, scene.getTrainCameras(), B)
+        cam = cams[0]
 
         densify_due = iteration < opt.densify_until_iter and iteration > opt.densify_from_iter \
             and iteration % opt.densification_interval == 0
         centre = None
         if use_tv:
             centre = (bbox_cpu[0] + tv_s / 2) + (bbox_cpu[1] - tv_s - bbox_cpu[0]) * torch.rand(3)
-        if native is not None and (gaussians.get_xyz.shape[0] > 0 or world > 1):
+        logged = None
+        if B > 1 and native is not None and gaussians.get_xyz.shape[0] > 0:
+            # B views in one fixed launch sequence; at a densification iteration no Adam step, as below
+            native(cams, torch.stack([c.original_image for c in cams]).cuda(), centre,
+                   apply_update=(iteration < opt.iterations) and not densify_due)
+            total = None
+            with torch.no_grad():
+                if densify_due:
+                    native.flush()
+                    gaussians.densify_and_prune(opt.densify_grad_threshold, opt.density_min_threshold, opt.max_screen_size,
+                                                ds["max_scale"], opt.max_num_gaussians, ds["densify_scale_threshold"], bbox)
+        elif B > 1:
+            gts = [c.original_image.cuda() for c in cams]
+
+            def batch_objective():
+                """sum over the views of the image loss + B lambda_tv TV, and the logged batch mean + lambda_tv TV"""
+                pkg = render_batch(cams, gaussians)
+                image_sum = sum(losses.image_loss(pkg["render"][v], gts[v], lambda_dssim=opt.lambda_dssim)["total"]
+                                for v in range(B))
+                total, shown = image_sum, image_sum.detach() / B
+                if use_tv:
+                    tv = losses.tv_3d_loss(query(gaussians, centre, tv_n, tv_s, pipe)["vol"], reduction="mean")
+                    total = total + (B * opt.lambda_tv) * tv
+                    shown = shown + opt.lambda_tv * tv.detach()
+                return pkg, total, shown
+
+            pkg, total, logged = batch_objective()
+            try:
+                total.backward()
+            except CapacityOverflow:      # as below: the same views again with the raised capacity hint
+                gaussians.optimizer.zero_grad(set_to_none=True)
+                pkg, total, logged = batch_objective()
+                total.backward()
+            with torch.no_grad():
+                grads = pkg["viewspace_points"].grad
+                for v in range(B):        # the statistics of each view, in view order
+                    seen = pkg["radii"][v] > 0
+                    gaussians.update_max_radii(pkg["radii"][v], seen)
+                    gaussians.add_densification_stats(_ViewGrad(grads[v]), seen)
+                if densify_due:
+                    gaussians.densify_and_prune(opt.densify_grad_threshold, opt.density_min_threshold, opt.max_screen_size,
+                                                ds["max_scale"], opt.max_num_gaussians, ds["densify_scale_threshold"], bbox)
+        elif native is not None and (gaussians.get_xyz.shape[0] > 0 or world > 1):
             # fixed launch sequence, no autograd (train_step.py).  At a densification iteration the reference's
             # optimizer.step() comes AFTER the tensors were replaced and therefore applies nothing (their .grad is None,
             # train.py:158-176): the same here.
@@ -363,7 +465,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                     if world > 1:
                         torch.distributed.barrier()  # no rank runs ahead into the next exchange while others write
             if iteration % 100 == 0:
-                history["loss"].append((iteration, float(total) if total is not None else native.total_loss()))
+                shown = logged if logged is not None else total
+                history["loss"].append((iteration, float(shown) if shown is not None else native.total_loss()))
                 if world > 1:
                     sharded.check_peer_exchange()    # the loss read-out above synchronised anyway
             if iteration in testing_iterations:
@@ -400,6 +503,13 @@ def save_train_poses(scene: Scene, corr, iteration: int):
     np.savez(os.path.join(scene.model_path, f"point_cloud/iteration_{iteration}", "train_poses.npz"),
              omega=corr.omega.detach().cpu().numpy(), nu=corr.nu.detach().cpu().numpy(),
              world_view_transform=wvt.cpu().numpy(), angle=np.array([float(c.angle) for c in cams]))
+
+
+class _ViewGrad:
+    """One view's rows of a batched render's screen-space gradients, in the shape `add_densification_stats` reads."""
+
+    def __init__(self, grad):
+        self.grad = grad
 
 
 def rank_checkpoint_path(path: str, rank: int, world: int) -> str:
@@ -501,12 +611,25 @@ def parse_args(argv=None):
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--peer_exchange", action="store_true",
                     help="multi-GPU: sum partial images / volumes with the NVLink peer-memory kernel instead of NCCL")
+    ap.add_argument("--batch_size", type=int, default=1,
+                    help="train views per optimizer step (1 .. number of train views); schedules stay in steps")
     a = ap.parse_args(argv)
     pick = lambda cls: cls(**{k: getattr(a, k) for k in cls.__dataclass_fields__})
     model, pipe, opt, pose = pick(ModelParams), pick(PipelineParams), pick(OptimizationParams), pick(PoseParams)
-    if pose.pose_refine and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    if pose.pose_refine and world > 1:
         ap.error("--pose_refine is not supported with Gaussian sharding (WORLD_SIZE > 1): every rank would hold only "
                  "its shard's part of the camera-matrix gradients; train on one GPU")
+    why = batch_refusal(a.batch_size, pose.pose_refine, world, pipe.compute_cov3D_python)
+    if why is not None:
+        ap.error(why)
+    if a.batch_size > 1:
+        try:
+            n_train = train_view_count(a.source_path)
+        except (OSError, ValueError, KeyError) as e:
+            ap.error(f"--batch_size: cannot count the train views of {a.source_path}: {e}")
+        if a.batch_size > n_train:
+            ap.error(f"--batch_size {a.batch_size} exceeds the scene's {n_train} train views")
     return a, model, pipe, opt, pose
 
 
@@ -520,7 +643,8 @@ def main(argv=None):
         write_cfg_args(model.model_path, model, pipe, opt,
                        {"test_iterations": a.test_iterations, "save_iterations": a.save_iterations,
                         "checkpoint_iterations": a.checkpoint_iterations, "start_checkpoint": a.start_checkpoint,
-                        "quiet": False, "config": None, "detect_anomaly": False}, pose)
+                        "quiet": False, "config": None, "detect_anomaly": False,
+                        **({"batch_size": a.batch_size} if a.batch_size > 1 else {})}, pose)
     random.seed(a.seed), np.random.seed(a.seed), torch.manual_seed(a.seed)     # safe_state (`general_utils.py:61-63`)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if world > 1:                      # launched by torchrun: one process per GPU, Gaussians sharded by index
@@ -534,7 +658,7 @@ def main(argv=None):
             from .sharded import enable_peer_exchange
             enable_peer_exchange(True)
     hist = training(model, opt, pipe, set(a.test_iterations) | {opt.iterations}, set(a.save_iterations),
-                    set(a.checkpoint_iterations), a.start_checkpoint, pose_params=pose)
+                    set(a.checkpoint_iterations), a.start_checkpoint, pose_params=pose, batch_size=a.batch_size)
     final = hist["eval"].get(opt.iterations, {})
     if world > 1:
         import torch.distributed as dist
@@ -552,7 +676,8 @@ def main(argv=None):
                       "ms_per_iteration_with_save_and_eval": hist["seconds"] / n_it * 1e3,
                       "steady_ms_per_iteration": hist.get("steady_ms_per_iteration"),
                       "repeated_iterations": hist.get("repeated_iterations", 0),
-                      "gaussians": hist["gaussians"], **final}))
+                      "gaussians": hist["gaussians"], **({"batch_size": a.batch_size} if a.batch_size > 1 else {}),
+                      **final}))
 
 
 if __name__ == "__main__":
