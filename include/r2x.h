@@ -317,6 +317,26 @@ int r2x_pose_grad(void* stream, const float* omega, const float* nu, int n_views
                   const float* world_view_transform, const float* projection_matrix, const float* dL_dview,
                   const float* dL_dproj, float* dL_domega, float* dL_dnu);
 
+/* ---- horizontal detector offset on the device (detector.DetectorOffset, NativeTrainStep(detector=...)) ---------- */
+/* offset[1] (device): s, the shift of the detector along u in pixels; a view whose content lies s columns towards
+ * larger column index than the nominal geometry predicts has s > 0.  The shift moves every projected 2-D mean by s
+ * pixels and leaves rays, conics and mu alone, so only the full projection changes.
+ * r2x_detector_offset_apply writes, for each of n_views full projections (16 floats each, row-major as the torch
+ * tensors store them, i.e. the rasterizer's column-major matrix), the matrix whose x row (entries 0, 4, 8, 12) gains
+ * (2 s / W) times its w row (entries 3, 7, 11, 15); every other entry is copied.  Each entry is the float64 sum rounded
+ * to float32 once, and a zero increment counts as -0.0, so s = 0 returns the input bit for bit.  The view matrix does
+ * not change.  out_full_proj may not alias full_proj.
+ * r2x_detector_offset_grad writes dL_doffset[0] = (2 / W) sum over the n_views x P rows of dL_dmean2D[n_views, P, 3]
+ * of the x component (dL/dndc as every raster backward writes it), i.e. the sum of dL/dpix_x with cull, radii and tile
+ * rectangles held fixed.  Two launches: float64 partial sums of contiguous chunks into `scratch`
+ * (>= r2x_detector_offset_grad_scratch_bytes(P, n_views) bytes), then their sum in a fixed order: no atomics, bitwise
+ * reproducible; the result is written, not accumulated.  Arguments are checked before any CUDA work; asynchronous. */
+int r2x_detector_offset_apply(void* stream, const float* offset, int W, int n_views, const float* full_proj,
+                              float* out_full_proj);
+size_t r2x_detector_offset_grad_scratch_bytes(int P, int n_views);
+int r2x_detector_offset_grad(void* stream, int P, int n_views, int W, const float* dL_dmean2D, float* dL_doffset,
+                             void* scratch, size_t scratch_bytes);
+
 int r2x_voxel_forward_async_raw(void* stream, int P, int nx, int ny, int nz, float sx, float sy, float sz, float cx,
                                 float cy, float cz, const float* means3D, const float* raw_density,
                                 const float* raw_scales, float scale_modifier, const float* raw_rotations,

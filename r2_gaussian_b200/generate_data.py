@@ -45,6 +45,37 @@ def draw_test_angles(cfg: dict, n_test: int, rng: np.random.RandomState) -> np.n
     return np.sort(rng.rand(n_test) * 2.0 * np.pi) + cfg["startAngle"] / 180 * np.pi    # the full circle, always
 
 
+def shift_projections(case_path: str, columns: int, empty: float = 1e-6) -> None:
+    """Move every train and test projection of a generated case `columns` columns (> 0: towards larger column index,
+    < 0: towards smaller), filling with zeros -- what a horizontal detector offset of -columns pixels does to the data
+    (`detector.py` for the sign).  The columns that fall off must be empty: each view's are at most `empty` times its
+    maximum (the projector leaves float32 round-off of ~1e-9 outside the object), else ValueError and nothing written."""
+    import json
+
+    k = int(columns)
+    if k == 0:
+        return
+    with open(os.path.join(case_path, "meta_data.json")) as f:
+        meta = json.load(f)
+    paths = [os.path.join(case_path, fr["file_path"]) for split in ("proj_train", "proj_test") for fr in meta[split]]
+    out = []
+    for p in paths:
+        a = np.load(p)
+        if abs(k) >= a.shape[-1]:
+            raise ValueError(f"shift_projections: {k} columns is not less than the detector width {a.shape[-1]}")
+        lost = a[..., -k:] if k > 0 else a[..., :-k]
+        if float(np.abs(lost).max()) > empty * float(np.abs(a).max()):
+            raise ValueError(f"shift_projections: {p}: the {abs(k)} columns that would fall off are not empty")
+        b = np.zeros_like(a)
+        if k > 0:
+            b[..., k:] = a[..., :-k]
+        else:
+            b[..., :k] = a[..., -k:]
+        out.append((p, b))
+    for p, b in out:
+        np.save(p, b)
+
+
 def main(argv=None) -> str:
     ap = argparse.ArgumentParser(description="Data generator parameters")
     ap.add_argument("--vol", required=True, type=str, help="Path to volume.")

@@ -33,6 +33,15 @@ With `pose=(PoseCorrection, FusedAdam over [omega] and [nu], one group each)` th
 iteration).  Pose refinement with Gaussian sharding is refused at bind time: each rank would hold only a partial sum
 of the matrix gradients.  With `pose=None` the launch sequence is the one above.
 
+With `detector=(DetectorOffset, FusedAdam over [offset])` the step also learns the horizontal detector offset
+(`detector.py`), for one camera or a batch:
+
+    shifted full projections             r2x_detector_offset_apply            (the B views' matrices, one launch)
+    offset gradient                      r2x_detector_offset_grad             (from this step's dL/dmean2D)
+    Adam on the offset                   r2x_adam_step_sum                    (after the Gaussians', same guards)
+
+The offset's step count is kept like the pose's.  Not combined with pose refinement or Gaussian sharding.
+
 A LIST of B > 1 cameras (with a [B,H,W] target) makes one iteration of B views: the objective is
 sum_v [L1 + lambda_dssim (1 - SSIM)](view v) + B lambda_tv TV(crop), one Adam step, the statistics of every view in view
 order.  The raster and loss calls become their batched forms (r2x_raster_forward_views_async_raw, r2x_image_loss_views,
@@ -63,9 +72,12 @@ def enabled() -> bool:
 
 class NativeTrainStep:
     def __init__(self, gaussians, lambda_dssim: float, lambda_tv: float = 0.0, tv_vol_nVoxel=None, tv_vol_sVoxel=None,
-                 scaling_modifier: float = 1.0, pose=None, pose_anchor: int = 0):
+                 scaling_modifier: float = 1.0, pose=None, pose_anchor: int = 0, detector=None):
         self.gm = gaussians
         self.pose, self.pose_opt = (None, None) if pose is None else pose
+        self.det, self.det_opt = (None, None) if detector is None else detector
+        if self.pose is not None and self.det is not None:
+            raise ValueError("NativeTrainStep: pose refinement and the detector offset cannot be combined")
         self.pose_anchor = int(pose_anchor)
         self.lambda_dssim, self.lambda_tv = float(lambda_dssim), float(lambda_tv)
         self.tv_n = None if tv_vol_nVoxel is None else tuple(int(v) for v in tv_vol_nVoxel)
@@ -84,6 +96,8 @@ class NativeTrainStep:
                int(gm._xyz.shape[0]), H, W, B, gm.max_radii2D.data_ptr(), gm.xyz_gradient_accum.data_ptr())
         if self.pose is not None:
             sig += (self.pose.omega.data_ptr(), self.pose.nu.data_ptr())
+        if self.det is not None:
+            sig += (self.det.offset.data_ptr(),)
         return sig
 
     def _bind(self, H, W, B):
@@ -171,6 +185,8 @@ class NativeTrainStep:
         self.act = fused._act(gm.raw_parameters())
         if self.pose is not None:
             self._bind_pose(P, dev)
+        if self.det is not None:
+            self._bind_detector(P, B, dev)
         self._bound = self._signature(H, W, B)
 
     def _bind_pose(self, P, dev):
@@ -210,6 +226,36 @@ class NativeTrainStep:
             a.param, a.grad, a.exp_avg, a.exp_avg_sq = p.data_ptr(), g.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr()
             a.numel = p.numel()
 
+    def _bind_detector(self, P, B, dev):
+        """Buffers of the detector-offset path: the shifted full projections, the offset gradient and its scratch, and
+        one Adam group on the detector optimizer's own state tensors."""
+        if self.sharded:
+            raise RuntimeError("NativeTrainStep: the detector offset is not supported with Gaussian sharding (every rank "
+                               "would hold only its shard's part of the gradient sum)")
+        det, opt = self.det, self.det_opt
+        p = det.offset
+        if p.device != dev or p.dtype != torch.float32 or not p.is_contiguous() or tuple(p.shape) != (1,):
+            raise RuntimeError(f"NativeTrainStep: the detector offset must be a contiguous float32 [1] on {dev}")
+        groups = opt.param_groups
+        if len(groups) != 1 or groups[0]["params"] != [p]:
+            raise RuntimeError("NativeTrainStep: the detector optimizer must hold one group, [offset]")
+        f32 = dict(dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            self.det_full = torch.empty((4, 4) if B == 1 else (B, 4, 4), **f32)
+            self.det_grad = torch.empty(1, **f32)
+            self.det_scratch_bytes = int(self.lib.r2x_detector_offset_grad_scratch_bytes(P, B))
+            self.det_scratch = torch.empty(self.det_scratch_bytes, dtype=torch.uint8, device=dev)
+        st = opt.state[p]
+        if len(st) == 0:
+            st["step"] = torch.tensor(0.0, dtype=torch.float32)
+            st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+            st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+        self.det_adam = (groups[0], p, st)
+        self.det_groups = (AdamGroup * 1)()
+        a = self.det_groups[0]
+        a.param, a.grad, a.exp_avg, a.exp_avg_sq = p.data_ptr(), self.det_grad.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr()
+        a.numel = 1
+
     def _provision(self):
         """Instance capacities for this iteration: both forwards are speculative.  The buffers only ever grow."""
         dev = self.dev
@@ -225,11 +271,12 @@ class NativeTrainStep:
 
     # ------------------------------------------------------------------ one iteration
     def __call__(self, cam, gt, tv_centre=None, apply_update: bool = True, view: int | None = None,
-                 pose_update: bool | None = None):
+                 pose_update: bool | None = None, detector_update: bool | None = None):
         """Enqueue one iteration.  `cam`: camera (render_query.render's contract), or a list of B cameras sharing image
         size, field of view and mode; `gt`: [1,H,W] or [H,W] CUDA float32 target ([B,H,W] for B cameras); `tv_centre`:
         3 floats (ignored without TV).  With `pose`: `view` is the camera's row of the PoseCorrection and `pose_update`
-        (default: `apply_update`) whether the pose Adam steps.  Returns {"render", "radii", "viewspace_grad", "loss"
+        (default: `apply_update`) whether the pose Adam steps; with `detector`, `detector_update` (default: `apply_update`)
+        whether the offset's Adam steps.  Returns {"render", "radii", "viewspace_grad", "loss"
         (device [3]: L1, SSIM, image total; [B,3] for B cameras), "tv" (device [1] or None)} -- views of buffers that
         the next call overwrites."""
         self.check()                                            # the previous iteration (one late; no stall)
@@ -256,11 +303,15 @@ class NativeTrainStep:
             if view is None or not 0 <= int(view) < self.n_views:
                 raise ValueError(f"NativeTrainStep: pose refinement needs the view index (0..{self.n_views - 1}), got {view}")
             pose_args = (int(view), bool(apply_update if pose_update is None else pose_update))
-        args = (cam, gt, None if tv_centre is None else tuple(float(v) for v in tv_centre), bool(apply_update), pose_args)
+        det_update = None
+        if self.det is not None:
+            det_update = bool(apply_update if detector_update is None else detector_update)
+        args = (cam, gt, None if tv_centre is None else tuple(float(v) for v in tv_centre), bool(apply_update), pose_args,
+                det_update)
         self._enqueue(*args)
         return self.result
 
-    def _enqueue(self, cam, gt, tv_centre, apply_update, pose_args):
+    def _enqueue(self, cam, gt, tv_centre, apply_update, pose_args, det_update):
         gm, lib, dev, P, H, W, B = self.gm, self.lib, self.dev, self.P, self.H, self.W, self.B
         self._provision()
         c0 = cam[0] if B > 1 else cam
@@ -292,6 +343,11 @@ class NativeTrainStep:
                                          view.data_ptr(), proj.data_ptr(), cam.projection_matrix.data_ptr(),
                                          self.pose_view.data_ptr(), self.pose_full.data_ptr()), "r2x_pose_apply")
                 view, proj = self.pose_view, self.pose_full
+            if det_update is not None:
+                # the shifted full projections of the B views (the view matrices stay the cameras')
+                check(lib.r2x_detector_offset_apply(st, self.det.offset.data_ptr(), W, B, proj.data_ptr(),
+                                                    self.det_full.data_ptr()), "r2x_detector_offset_apply")
+                proj = self.det_full
             if B == 1:
                 check(lib.r2x_raster_forward_async_raw(
                     st, P, W, H, xyz.data_ptr(), dens.data_ptr(), scal.data_ptr(), sm, rot.data_ptr(), view.data_ptr(),
@@ -370,6 +426,10 @@ class NativeTrainStep:
                                         cam.projection_matrix.data_ptr(), self.pose_gview.data_ptr(),
                                         self.pose_gproj.data_ptr(), self.g_omega.data_ptr(), self.g_nu.data_ptr()),
                       "r2x_pose_grad")
+            if det_update is not None:
+                check(lib.r2x_detector_offset_grad(st, P, B, W, self.g2.data_ptr(), self.det_grad.data_ptr(),
+                                                   self.det_scratch.data_ptr(), self.det_scratch_bytes),
+                      "r2x_detector_offset_grad")
             guard_v = self.status_v.data_ptr() if self.use_tv else None
             if B == 1:
                 check(lib.r2x_densify_stats(st, P, self.radii.data_ptr(), self.g2.data_ptr(), gm.max_radii2D.data_ptr(),
@@ -409,11 +469,20 @@ class NativeTrainStep:
                 check(lib.r2x_adam_step_sum(st, 2, C.cast(self.pose_groups, C.c_void_p), None, float(b1), float(b2),
                                             float(pg["eps"]), steps.pop(), self.status_r.data_ptr(), guard_v),
                       "r2x_adam_step_sum")
+            if det_update:
+                # the offset's step, guarded by both forwards' status words like the Gaussians' own
+                group, _p, stt = self.det_adam
+                stt["step"] += 1
+                self.det_groups[0].lr = float(group["lr"])
+                b1, b2 = group["betas"]
+                check(lib.r2x_adam_step_sum(st, 1, C.cast(self.det_groups, C.c_void_p), None, float(b1), float(b2),
+                                            float(group["eps"]), int(stt["step"].item()), self.status_r.data_ptr(),
+                                            guard_v), "r2x_adam_step_sum")
             # the status words travel to pinned host memory behind an event; read one iteration late
             host = _C._Workspace.to_host(self.status_r), (_C._Workspace.to_host(self.status_v) if self.use_tv else None)
             ev = torch.cuda.Event()
             ev.record(torch.cuda.current_stream(dev))
-        self._pending = (host, ev, (cam, gt, tv_centre, apply_update, pose_args))
+        self._pending = (host, ev, (cam, gt, tv_centre, apply_update, pose_args, det_update))
         self.result = {"render": image, "radii": self.radii, "viewspace_grad": self.g2, "loss": self.loss_out,
                        "tv": self.tv_out if self.use_tv else None}
 
@@ -443,6 +512,8 @@ class NativeTrainStep:
             if args[4] is not None and args[4][1]:
                 for _group, _p, stt, _g in self.pose_adam:
                     stt["step"] -= 1
+            if args[5]:
+                self.det_adam[2]["step"] -= 1
             self._enqueue(*args)
             self.check()
 

@@ -28,6 +28,12 @@ is invariant to that scale up to its eps of 1e-15); the densification statistics
 the batch mean plus lambda_tv TV.  Iteration counts and the learning-rate and densification schedules stay in optimizer
 steps, so a run sees B times as many views.  B > 1 is refused with --pose_refine, Gaussian sharding and
 compute_cov3D_python.  With B = 1 nothing changes.
+
+`--detector_offset_refine` also learns the scan's horizontal detector offset (`detector.DetectorOffset`, one value in
+pixels; `DetectorParams` learning rates, log-linear over `--iterations`) with its own FusedAdam, on both training paths
+and at any --batch_size; it steps wherever the poses would.  Train and test views are evaluated with the offset (it is a
+property of the scanner), each save writes `detector_offset.yml` and checkpoints carry the offset and its Adam state.
+It is refused with --pose_refine and with Gaussian sharding.  Without the switch nothing changes.
 """
 from __future__ import annotations
 
@@ -48,6 +54,7 @@ from .gaussian_model import GaussianModel
 from .gaussian_utils import get_expon_lr_func
 from .metrics import metric_proj, metric_vol
 from .optim import FusedAdam
+from .detector import SIGN_CONVENTION, DetectorOffset
 from .pose import PoseCorrection
 from .rasterization import GaussianRasterizationSettings
 from .render_query import _tan_fov, query, render
@@ -116,6 +123,30 @@ class PoseParams:
 POSE_ANCHOR = 0     # the train view whose correction stays exactly zero
 
 
+@dataclass
+class DetectorParams:
+    """`--detector_offset_refine`: learn the horizontal detector offset (pixels, `detector.DetectorOffset`) together
+    with the scene.  The learning rate decays log-linearly from init to final over `--iterations`; the defaults were
+    chosen on a 48^3 generate_data scene (24 views of 96^2, cone beam) shifted by 3 columns, among 1e-1, 5e-2 and 2e-2
+    (final = init / 100; DESIGN section 8)."""
+    detector_offset_refine: bool = False
+    detector_offset_lr_init: float = 2e-2
+    detector_offset_lr_final: float = 2e-4
+
+
+def detector_refusal(detector_offset_refine: bool, pose_refine: bool, world: int) -> str | None:
+    """Why `--detector_offset_refine` cannot be used with these settings (None: it can).  Checked before any CUDA
+    work."""
+    if not detector_offset_refine:
+        return None
+    if pose_refine:
+        return "--detector_offset_refine is not supported with --pose_refine (composing the two maps is not implemented)"
+    if world > 1:
+        return ("--detector_offset_refine is not supported with Gaussian sharding (WORLD_SIZE > 1): every rank would "
+                "see only its shard's part of the offset gradient")
+    return None
+
+
 def default_init_path(source_path: str) -> str:
     """`<scene>/init_<scene>.npy` for directories, `<dir>/init_<stem>.npy` for NAF pickles (`initialize.py:29-41`)."""
     if os.path.exists(os.path.join(source_path, "meta_data.json")):
@@ -141,10 +172,11 @@ def derived_settings(scanner_cfg: dict, model: ModelParams, opt: OptimizationPar
 
 
 @torch.no_grad()
-def evaluate(scene: Scene, gaussians: GaussianModel, pipe, with_ssim: bool = True, pose=None) -> dict:
+def evaluate(scene: Scene, gaussians: GaussianModel, pipe, with_ssim: bool = True, pose=None, detector=None) -> dict:
     """3-D PSNR / SSIM of the queried volume and 2-D PSNR / SSIM of the rendered train and test views, with the
     reference's metric definitions (`train.py:262-330`, `utils/image_utils.py:90-183`).  `pose` (a PoseCorrection over
-    the train views): train views are rendered with their corrected cameras; test views keep their nominal poses."""
+    the train views): train views are rendered with their corrected cameras; test views keep their nominal poses.
+    `detector` (a DetectorOffset): train and test views are rendered with the offset applied."""
     cfg = scene.scanner_cfg
     vol = query(gaussians, cfg["offOrigin"], cfg["nVoxel"], cfg["sVoxel"], pipe)["vol"]
     out = {"psnr_3d": metric_vol(scene.vol_gt, vol, "psnr")[0]}
@@ -155,6 +187,8 @@ def evaluate(scene: Scene, gaussians: GaussianModel, pipe, with_ssim: bool = Tru
             continue
         if name == "train" and pose is not None:
             cams = [pose.device_camera(c, c.uid, POSE_ANCHOR) for c in cams]
+        if detector is not None:
+            cams = detector.cameras(cams)
         imgs = torch.concat([render(c, gaussians, pipe)["render"] for c in cams], 0).permute(1, 2, 0)
         gts = torch.concat([c.original_image.to(imgs.device) for c in cams], 0).permute(1, 2, 0)
         out[f"psnr_2d_{name}"] = metric_proj(gts, imgs, "psnr")[0]
@@ -210,12 +244,17 @@ def render_batch(cams, gaussians: GaussianModel) -> dict:
 
 def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, testing_iterations=(),
              saving_iterations=(), checkpoint_iterations=(), checkpoint: str | None = None, init_points=None,
-             log=print, pose_params: PoseParams | None = None, batch_size: int = 1) -> dict:
+             log=print, pose_params: PoseParams | None = None, batch_size: int = 1,
+             detector_params: DetectorParams | None = None) -> dict:
     first_iter = 0
     refine = pose_params is not None and pose_params.pose_refine
     if refine and world_info()[1] > 1:
         raise RuntimeError("--pose_refine is not supported with Gaussian sharding (WORLD_SIZE > 1): every rank would "
                            "hold only its shard's part of the camera-matrix gradients")
+    refine_det = detector_params is not None and detector_params.detector_offset_refine
+    why = detector_refusal(refine_det, refine, world_info()[1])
+    if why is not None:
+        raise ValueError(why)
     B = int(batch_size)
     why = batch_refusal(B, refine, world_info()[1], bool(getattr(pipe, "compute_cov3D_python", False)))
     if why is not None:
@@ -260,6 +299,12 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                                      max_steps=opt.iterations),
                    get_expon_lr_func(pose_params.pose_translation_lr_init, pose_params.pose_translation_lr_final,
                                      max_steps=opt.iterations))
+    det = det_opt = det_lr = None
+    if refine_det:
+        det = DetectorOffset("cuda")
+        det_opt = FusedAdam([{"params": [det.offset], "lr": 0.0, "name": "detector_offset"}], lr=0.0, eps=1e-15)
+        det_lr = get_expon_lr_func(detector_params.detector_offset_lr_init, detector_params.detector_offset_lr_final,
+                                   max_steps=opt.iterations)
     if checkpoint is not None:
         path = rank_checkpoint_path(checkpoint, rank, world)
         payload = torch.load(path, weights_only=False)
@@ -281,6 +326,14 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                 corr.omega.copy_(pose_state["omega"])
                 corr.nu.copy_(pose_state["nu"])
             pose_opt.load_state_dict(pose_state["optimizer"])
+        det_state = payload[4] if len(payload) > 4 else None
+        if refine_det != (det_state is not None):
+            raise RuntimeError(f"checkpoint {path} was written {'with' if det_state is not None else 'without'} "
+                               f"--detector_offset_refine; resume it with the same setting")
+        if refine_det:
+            with torch.no_grad():
+                det.offset.copy_(det_state["offset"])
+            det_opt.load_state_dict(det_state["optimizer"])
         log(f"Load checkpoint {os.path.basename(path)}.")
 
     use_tv = opt.lambda_tv > 0
@@ -295,7 +348,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
     if train_step.enabled() and not getattr(pipe, "debug", False) and not getattr(pipe, "compute_cov3D_python", False):
         native = train_step.NativeTrainStep(gaussians, opt.lambda_dssim, opt.lambda_tv if use_tv else 0.0, tv_n,
                                             [float(v) for v in tv_s],
-                                            **({} if corr is None else dict(pose=(corr, pose_opt), pose_anchor=POSE_ANCHOR)))
+                                            **({} if corr is None else dict(pose=(corr, pose_opt), pose_anchor=POSE_ANCHOR)),
+                                            **({} if det is None else dict(detector=(det, det_opt))))
     if world > 1:
         # one exchange of each shape before the clock starts: the NCCL communicator / the peer-memory reducers are
         # created on first use (seconds at 8 ranks), which is set-up, not a training step
@@ -332,6 +386,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
         if corr is not None:
             for group, schedule in zip(pose_opt.param_groups, pose_lr):
                 group["lr"] = schedule(iteration)
+        if det is not None:
+            det_opt.param_groups[0]["lr"] = det_lr(iteration)
         cams, stack = draw_train_views(stack, scene.getTrainCameras(), B)
         cam = cams[0]
 
@@ -344,7 +400,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
         if B > 1 and native is not None and gaussians.get_xyz.shape[0] > 0:
             # B views in one fixed launch sequence; at a densification iteration no Adam step, as below
             native(cams, torch.stack([c.original_image for c in cams]).cuda(), centre,
-                   apply_update=(iteration < opt.iterations) and not densify_due)
+                   apply_update=(iteration < opt.iterations) and not densify_due,
+                   **({} if det is None else dict(detector_update=iteration < opt.iterations)))
             total = None
             with torch.no_grad():
                 if densify_due:
@@ -356,7 +413,7 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
 
             def batch_objective():
                 """sum over the views of the image loss + B lambda_tv TV, and the logged batch mean + lambda_tv TV"""
-                pkg = render_batch(cams, gaussians)
+                pkg = render_batch(cams if det is None else det.cameras(cams), gaussians)
                 image_sum = sum(losses.image_loss(pkg["render"][v], gts[v], lambda_dssim=opt.lambda_dssim)["total"]
                                 for v in range(B))
                 total, shown = image_sum, image_sum.detach() / B
@@ -375,6 +432,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                 total.backward()
             with torch.no_grad():
                 grads = pkg["viewspace_points"].grad
+                if det is not None:
+                    det.grad_from(grads, int(cam.image_width))
                 for v in range(B):        # the statistics of each view, in view order
                     seen = pkg["radii"][v] > 0
                     gaussians.update_max_radii(pkg["radii"][v], seen)
@@ -389,6 +448,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
             # The pose gradient is valid at a densification iteration too, so the poses step there (both paths).
             gt = cam.original_image.cuda()
             pose_kw = {} if corr is None else dict(view=cam.uid, pose_update=iteration < opt.iterations)
+            if det is not None:
+                pose_kw = dict(detector_update=iteration < opt.iterations)
             native(cam, gt, centre, apply_update=(iteration < opt.iterations) and not densify_due, **pose_kw)
             total = None
             with torch.no_grad():
@@ -398,6 +459,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                                                 ds["max_scale"], opt.max_num_gaussians, ds["densify_scale_threshold"], bbox)
         else:
             view_cam = (lambda: cam) if corr is None else (lambda: corr.device_camera(cam, cam.uid, POSE_ANCHOR))
+            if det is not None:
+                view_cam = lambda: det.camera(cam)
             pkg = render(view_cam(), gaussians, pipe)
             gt = cam.original_image.cuda()
             loss = losses.image_loss(pkg["render"], gt, lambda_dssim=opt.lambda_dssim)
@@ -420,6 +483,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                                                                       reduction="mean")
                 total.backward()
             with torch.no_grad():
+                if det is not None:
+                    det.grad_from(pkg["viewspace_points"].grad, int(cam.image_width))
                 gaussians.update_max_radii(pkg["radii"], pkg["visibility_filter"])
                 gaussians.add_densification_stats(pkg["viewspace_points"], pkg["visibility_filter"])
                 if densify_due:
@@ -439,6 +504,9 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                 if pose_opt is not None:
                     pose_opt.step()
                     pose_opt.zero_grad(set_to_none=True)
+                if det_opt is not None:
+                    det_opt.step()
+                    det_opt.zero_grad(set_to_none=True)
             if native is not None and (iteration in saving_iterations or iteration in checkpoint_iterations or
                                        iteration in testing_iterations or iteration == opt.iterations):
                 native.flush()       # the last enqueued iteration is checked (and repeated if it had overflowed)
@@ -449,6 +517,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                         scene.save(iteration, queryfunc)
                         if corr is not None:
                             save_train_poses(scene, corr, iteration)
+                        if det is not None:
+                            save_detector_offset(scene, det, iteration)
                     else:
                         save_sharded(scene, gaussians, iteration, queryfunc, rank)
             if scene.model_path and iteration in checkpoint_iterations:
@@ -461,6 +531,10 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                         payload = (payload[0], iteration, {"rank": rank, "world": world},
                                    {"omega": corr.omega.detach().cpu(), "nu": corr.nu.detach().cpu(),
                                     "optimizer": pose_opt.state_dict()})
+                    if det is not None:     # (model, iteration, tag, poses or None, offset): only with the switch
+                        payload = (payload[0], iteration, {"rank": rank, "world": world},
+                                   payload[3] if len(payload) > 3 else None,
+                                   {"offset": det.offset.detach().cpu(), "optimizer": det_opt.state_dict()})
                     torch.save(payload, os.path.join(ckpt_dir, name))
                     if world > 1:
                         torch.distributed.barrier()  # no rank runs ahead into the next exchange while others write
@@ -471,7 +545,7 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                     sharded.check_peer_exchange()    # the loss read-out above synchronised anyway
             if iteration in testing_iterations:
                 with _aside():
-                    history["eval"][iteration] = evaluate(scene, gaussians, pipe, pose=corr)
+                    history["eval"][iteration] = evaluate(scene, gaussians, pipe, pose=corr, detector=det)
                 log(f"[ITER {iteration}] {history['eval'][iteration]}  points {gaussians.get_xyz.shape[0]}")
                 if world > 1:
                     sharded.check_peer_exchange()
@@ -491,6 +565,9 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
     history["scene"], history["model"] = scene, gaussians
     if corr is not None:
         history["pose"] = corr
+    if det is not None:
+        history["detector"] = det
+        history["detector_offset_px"] = float(det.offset.detach()[0])
     return history
 
 
@@ -503,6 +580,17 @@ def save_train_poses(scene: Scene, corr, iteration: int):
     np.savez(os.path.join(scene.model_path, f"point_cloud/iteration_{iteration}", "train_poses.npz"),
              omega=corr.omega.detach().cpu().numpy(), nu=corr.nu.detach().cpu().numpy(),
              world_view_transform=wvt.cpu().numpy(), angle=np.array([float(c.angle) for c in cams]))
+
+
+@torch.no_grad()
+def save_detector_offset(scene: Scene, det, iteration: int):
+    """`point_cloud/iteration_<N>/detector_offset.yml`: the learned offset in pixels and in scene units at the detector,
+    and the sign convention in words."""
+    import yaml
+    doc = {"offset_px": float(det.offset.detach()[0]), "offset_scene": det.scene_units(scene.scanner_cfg),
+           "sign_convention": SIGN_CONVENTION}
+    with open(os.path.join(scene.model_path, f"point_cloud/iteration_{iteration}", "detector_offset.yml"), "w") as f:
+        yaml.dump(doc, f, default_flow_style=False, sort_keys=False)
 
 
 class _ViewGrad:
@@ -547,18 +635,23 @@ def write_eval_yaml(model_path: str, iteration: int, ev: dict):
                 yaml.dump(d2, f, default_flow_style=False, sort_keys=False)
 
 
-def write_cfg_args(model_path: str, model, pipe, opt, extra: dict, pose: PoseParams | None = None):
+def write_cfg_args(model_path: str, model, pipe, opt, extra: dict, pose: PoseParams | None = None,
+                   detector: DetectorParams | None = None):
     """`<model_path>/cfg_args`: the Namespace repr the reference's test.py evaluates (`arguments/__init__.py:74-95`,
     written by `utils/log_utils.py:28-29`), with the reference's field names, next to a JSON copy.  The pose settings
-    are added (flat, and as "pose" in the JSON) only when `pose.pose_refine` is on."""
+    are added (flat, and as "pose" in the JSON) only when `pose.pose_refine` is on, the detector settings (as "detector")
+    only when `detector.detector_offset_refine` is on."""
     from argparse import Namespace
     pose_fields = asdict(pose) if pose is not None and pose.pose_refine else {}
-    flat = {**asdict(model), **asdict(pipe), **asdict(opt), **pose_fields, **extra}
+    det_fields = asdict(detector) if detector is not None and detector.detector_offset_refine else {}
+    flat = {**asdict(model), **asdict(pipe), **asdict(opt), **pose_fields, **det_fields, **extra}
     with open(os.path.join(model_path, "cfg_args"), "w") as f:
         f.write(str(Namespace(**flat)))
     doc = {"model": asdict(model), "pipe": asdict(pipe), "opt": asdict(opt)}
     if pose_fields:
         doc["pose"] = pose_fields
+    if det_fields:
+        doc["detector"] = det_fields
     with open(os.path.join(model_path, "cfg_args.json"), "w") as f:
         json.dump(doc, f, indent=1)
 
@@ -596,7 +689,8 @@ def _add_dataclass_args(parser, cls, skip=()):
 
 
 def parse_args(argv=None):
-    """-> (argparse namespace, ModelParams, PipelineParams, OptimizationParams, PoseParams) of the command line."""
+    """-> (argparse namespace, ModelParams, PipelineParams, OptimizationParams, PoseParams) of the command line; the
+    namespace's `detector_params` holds the DetectorParams."""
     ap = argparse.ArgumentParser(description="Train R2-Gaussian on one scene (H100-native pipeline)")
     ap.add_argument("-s", "--source_path", required=True)
     ap.add_argument("-m", "--model_path", default="")
@@ -604,6 +698,7 @@ def parse_args(argv=None):
     _add_dataclass_args(ap, PipelineParams)
     _add_dataclass_args(ap, OptimizationParams)
     _add_dataclass_args(ap, PoseParams)
+    _add_dataclass_args(ap, DetectorParams)
     ap.add_argument("--test_iterations", nargs="+", type=int, default=[5000, 10000, 20000, 30000])
     ap.add_argument("--save_iterations", nargs="+", type=int, default=[])
     ap.add_argument("--checkpoint_iterations", nargs="+", type=int, default=[])
@@ -621,6 +716,10 @@ def parse_args(argv=None):
         ap.error("--pose_refine is not supported with Gaussian sharding (WORLD_SIZE > 1): every rank would hold only "
                  "its shard's part of the camera-matrix gradients; train on one GPU")
     why = batch_refusal(a.batch_size, pose.pose_refine, world, pipe.compute_cov3D_python)
+    if why is not None:
+        ap.error(why)
+    a.detector_params = pick(DetectorParams)
+    why = detector_refusal(a.detector_params.detector_offset_refine, pose.pose_refine, world)
     if why is not None:
         ap.error(why)
     if a.batch_size > 1:
@@ -644,7 +743,7 @@ def main(argv=None):
                        {"test_iterations": a.test_iterations, "save_iterations": a.save_iterations,
                         "checkpoint_iterations": a.checkpoint_iterations, "start_checkpoint": a.start_checkpoint,
                         "quiet": False, "config": None, "detect_anomaly": False,
-                        **({"batch_size": a.batch_size} if a.batch_size > 1 else {})}, pose)
+                        **({"batch_size": a.batch_size} if a.batch_size > 1 else {})}, pose, a.detector_params)
     random.seed(a.seed), np.random.seed(a.seed), torch.manual_seed(a.seed)     # safe_state (`general_utils.py:61-63`)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if world > 1:                      # launched by torchrun: one process per GPU, Gaussians sharded by index
@@ -658,7 +757,8 @@ def main(argv=None):
             from .sharded import enable_peer_exchange
             enable_peer_exchange(True)
     hist = training(model, opt, pipe, set(a.test_iterations) | {opt.iterations}, set(a.save_iterations),
-                    set(a.checkpoint_iterations), a.start_checkpoint, pose_params=pose, batch_size=a.batch_size)
+                    set(a.checkpoint_iterations), a.start_checkpoint, pose_params=pose, batch_size=a.batch_size,
+                    detector_params=a.detector_params)
     final = hist["eval"].get(opt.iterations, {})
     if world > 1:
         import torch.distributed as dist
@@ -677,6 +777,7 @@ def main(argv=None):
                       "steady_ms_per_iteration": hist.get("steady_ms_per_iteration"),
                       "repeated_iterations": hist.get("repeated_iterations", 0),
                       "gaussians": hist["gaussians"], **({"batch_size": a.batch_size} if a.batch_size > 1 else {}),
+                      **({"detector_offset_px": hist["detector_offset_px"]} if "detector_offset_px" in hist else {}),
                       **final}))
 
 
