@@ -433,6 +433,26 @@ int r2x_volume_backproject(void* stream, int n_views, int H, int W, const float*
                            float sx, float sy, float sz, float cx, float cy, float cz, float step, float* out_volume,
                            float* out_weight, void* scratch, size_t scratch_bytes);
 
+/* ---- isotropic total variation on a volume (FISTA-TV, r2_gaussian_b200/recon.py and tv.py) --------------------- */
+/* Volumes are float32 [nx,ny,nz] (z fastest).  grad x = forward differences along x, y, z, 0 across the last index;
+ *   TV(x) = sum over voxels of sqrt(dx^2 + dy^2 + dz^2)      (isotropic; not the anisotropic r2x_tv3d_loss)
+ * r2x_tv_prox writes out = argmin over x in C of 1/2 |x - v|^2 + weight TV(x), C = {x >= 0} when nonneg, else all,
+ * by `niter` iterations of Beck-Teboulle's fast gradient projection (FGP) on the dual field p[3,nx,ny,nz]: cold start
+ * p = 0, step 1 / (12 weight), projection onto |p_voxel| <= 1, out = P_C(v - weight div p) (the recurrence is stated in
+ * csrc/r2x_tv.cu).  niter + 1 launches; the three dual fields it rotates live in `scratch` (>=
+ * r2x_tv_prox_scratch_bytes(nx, ny, nz) = 36 bytes per voxel).  weight 0 writes P_C(v) bit for bit (u < 0 ? 0 : u, or
+ * v itself).  out may not alias v.
+ * r2x_tv_value writes out[0] (device, float64) = TV(x) with each term in float64: float64 partial sums of contiguous
+ * chunks into `scratch` (>= r2x_tv_value_scratch_bytes), then their sum in a fixed order.
+ * Both: no atomics, bitwise reproducible; arguments are checked before any CUDA work; asynchronous on `stream`.
+ * Limits: nx <= 262140, ny <= 524280. */
+size_t r2x_tv_prox_scratch_bytes(int nx, int ny, int nz);
+int r2x_tv_prox(void* stream, int nx, int ny, int nz, const float* v, float weight, int niter, int nonneg, float* out,
+                void* scratch, size_t scratch_bytes);
+size_t r2x_tv_value_scratch_bytes(int nx, int ny, int nz);
+int r2x_tv_value(void* stream, int nx, int ny, int nz, const float* x, double* out, void* scratch,
+                 size_t scratch_bytes);
+
 /* ---- multi-GPU exchange step: one-shot sum over NVLink peer memory ------------------------------ */
 /* The Gaussian-sharded projector (one process per GPU, every rank renders its index shard) needs ONE exchange per
  * projection: the sum of the per-rank partial detector images (BASELINE north_star; the reference itself is

@@ -95,6 +95,10 @@ PROTOTYPES = {
     "r2x_volume_backproject_scratch_bytes": (_sz, [_i, _i, _i]),
     "r2x_volume_backproject": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _i, _i, _i, _f, _f, _f, _f, _f, _f, _f,
                                     _vp, _vp, _vp, _sz]),
+    "r2x_tv_prox_scratch_bytes": (_sz, [_i, _i, _i]),
+    "r2x_tv_prox": (_i, [_vp, _i, _i, _i, _vp, _f, _i, _i, _vp, _vp, _sz]),
+    "r2x_tv_value_scratch_bytes": (_sz, [_i, _i, _i]),
+    "r2x_tv_value": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _sz]),
     "r2x_peer_alloc": (_i, [_sz, C.POINTER(_vp)]),
     "r2x_peer_free": (_i, [_vp]),
     "r2x_ipc_export": (_i, [_vp, _vp]),

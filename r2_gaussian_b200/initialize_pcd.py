@@ -1,7 +1,7 @@
 """Initial point cloud for a scene -- the reference's `initialize_pcd.py:26-172`.
 
     python -m r2_gaussian_b200.initialize_pcd --data <scene dir | NAF pickle> [--output init.npy]
-        [--recon_method random|fdk|cgls|volume] [--recon recon.npy] [--n_points 50000] [--density_thresh 0.05]
+        [--recon_method random|fdk|cgls|fista_tv|volume] [--recon recon.npy] [--n_points 50000] [--density_thresh 0.05]
         [--density_rescale 0.15] [--random_density_max 1.0] [--evaluate]
 
 `random` draws positions uniformly in the volume and densities in [0, random_density_max) with numpy's global
@@ -9,7 +9,8 @@ generator seeded with 0, exactly like the reference.  `fdk` reconstructs the vol
 GPU FDK of `r2_gaussian_b200.fdk` (the reference calls TIGRE's `algs.fdk`), then samples `n_points` voxels above
 `density_thresh` and scales their densities by `density_rescale`, the reference's way; it needs a CUDA device and at
 least MIN_FDK_VIEWS train views.  `cgls` does the same with 60 CGLS iterations over the GPU projector pair
-(`r2_gaussian_b200.recon`, the reference's `algs.cgls`); it also needs a CUDA device.  `volume` samples a reconstruction made elsewhere (`--recon`, an .npy in the scene's
+(`r2_gaussian_b200.recon`, the reference's `algs.cgls`); it also needs a CUDA device.  `fista_tv` does the same with
+the TV-regularised FISTA-TV of `r2_gaussian_b200.recon` at its default settings (CUDA as well).  `volume` samples a reconstruction made elsewhere (`--recon`, an .npy in the scene's
 voxel grid) the same way.  Writes [n_points, 4] = (x, y, z, density) in the scene's normalised [-1,1]^3 coordinates to
 `<scene>/init_<name>.npy` unless `--output` is given.  `--evaluate` builds the Gaussians from the written cloud, queries
 them on the scene grid and prints their 3D PSNR against the ground-truth volume (`initialize_pcd.py:135-156`).
@@ -81,7 +82,7 @@ def main(argv=None) -> str:
     ap = argparse.ArgumentParser(description="Generate initialization parameters")
     ap.add_argument("--data", required=True, help="Path to data.")
     ap.add_argument("--output", default=None, help="Path to output.")
-    ap.add_argument("--recon_method", default="random", choices=["random", "volume", "fdk", "cgls"])
+    ap.add_argument("--recon_method", default="random", choices=["random", "volume", "fdk", "cgls", "fista_tv"])
     ap.add_argument("--recon", default=None, help="reconstruction volume (.npy) for --recon_method volume")
     ap.add_argument("--n_points", type=int, default=50000)
     ap.add_argument("--density_thresh", type=float, default=0.05)
@@ -90,7 +91,7 @@ def main(argv=None) -> str:
     ap.add_argument("--evaluate", default=False, action="store_true",
                     help="Add this flag to evaluate quality (given GT volume, for debug only)")
     a = ap.parse_args(argv)
-    if a.recon_method in ("fdk", "cgls"):
+    if a.recon_method in ("fdk", "cgls", "fista_tv"):
         _require_cuda_for(a.recon_method)
     np.random.seed(0)                                    # initialize_pcd.py:23
     info = read_scene(os.path.abspath(a.data), eval=False)
@@ -106,7 +107,7 @@ def main(argv=None) -> str:
     if os.path.exists(out):
         raise SystemExit(f"Initialization file {out} exists! Delete it first.")
     os.makedirs(os.path.dirname(out) or ".", exist_ok=True)
-    if a.recon_method in ("fdk", "cgls"):
+    if a.recon_method in ("fdk", "cgls", "fista_tv"):
         recon = recon_train_views(info, a.recon_method)  # no draws from numpy's generator before np.random.choice
     pts = init_point_cloud(info.scanner_cfg, a.n_points, recon=recon, density_thresh=a.density_thresh,
                            density_rescale=a.density_rescale, random_density_max=a.random_density_max)

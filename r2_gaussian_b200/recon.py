@@ -1,9 +1,11 @@
 """Traditional CT reconstructions on the GPU -- FDK, SART / OS-SART and CGLS, what the reference obtains from TIGRE's
-`algs` (`r2_gaussian/utils/ct_utils.py::recon_volume` / `run_ct_recon_algs`, `scripts/run_traditional_methods.py`).
+`algs` (`r2_gaussian/utils/ct_utils.py::recon_volume` / `run_ct_recon_algs`, `scripts/run_traditional_methods.py`),
+and the TV-regularised FISTA-TV.
 
     x, l2 = cgls(projs, angles, scanner_cfg, niter=60)
     x = sart(projs, angles, scanner_cfg, niter=20, lmbda=1.0, lmbda_red=0.999, blocksize=1, nonneg=True)
-    x = recon_volume(projs, angles, scanner_cfg, method)           # fdk | cgls | sart | ossart
+    x, history = fista_tv(projs, angles, scanner_cfg, niter=FISTA_NITER, lmbda=FISTA_LAMBDA, tviter=20, nonneg=True)
+    x = recon_volume(projs, angles, scanner_cfg, method)           # fdk | cgls | sart | ossart | fista_tv
 
 `projs` is a CUDA [N, H, W] tensor in the dataset layout (scene units, as the readers return it) and `scanner_cfg` the
 scaled dict of `dataset.read_scene`; volumes are [nx, ny, nz] in the voxelizer's layout.  A is `projector.project`
@@ -26,7 +28,24 @@ SART (blocksize 1) / OS-SART (blocksize > 1), from x = 0:
         x += lmbda * num / den where den > 0;  x = max(x, 0) if nonneg;
     after each sweep lmbda *= lmbda_red.
 
-Parity with TIGRE's binaries is not pinned (as for FDK and the projector).  ASD-POCS / OS-ASD-POCS are not built.
+FISTA-TV solves the TV-regularised least-squares problem
+    minimise  F(x) = 1/2 |A x - b|^2 + lmbda TV(x)   subject to x >= 0   (nonneg=False drops the constraint)
+    TV(x) = sum over voxels of sqrt(dx^2 + dy^2 + dz^2)   (isotropic; forward differences, 0 across the last index)
+in the scene-scaled units of `dataset.read_scene`.  This TV is not the training loss `r2x_tv3d_loss`, which is the
+anisotropic sum of absolute differences of the reference's `loss_utils`.  FISTA (Beck-Teboulle), from x_0 = y_1 = 0,
+t_1 = 1; per iteration k:
+    v = y_k - (1/L) A^T (A y_k - b)                             (one A and one A^T over all views)
+    x_k = prox_{(lmbda/L) TV + indicator(x >= 0)}(v)            (`tviter` FGP iterations, `tv.tv_denoise`)
+    t_{k+1} = (1 + sqrt(1 + 4 t_k^2)) / 2,   y_{k+1} = x_k + ((t_k - 1) / t_{k+1}) (x_k - x_{k-1}).
+The prox is Beck-Teboulle's fast gradient projection for constrained TV denoising (csrc/r2x_tv.cu): the dual field
+p[3, nx, ny, nz] cold-started at 0, step 1 / (12 lmbda / L), projection onto |p_voxel| <= 1 and onto x >= 0.  L >= |A|^2
+defaults to the Schur bound max(A 1) max(A^T 1) (A is non-negative; two operator calls), or is passed as `L=`.
+history[k] = {"data": 1/2 |A x_k - b|^2, "tv": TV(x_k), "F": data + lmbda tv} (one more A per iteration).  It is a
+recognised convex baseline (TIGRE's algorithm collection has a FISTA with a TV proximal step); ASD-POCS, whose adaptive
+step and stop rules are defined by TIGRE's implementation, is not what it computes.
+
+Parity with TIGRE's binaries is not pinned (as for FDK and the projector).  ASD-POCS / OS-ASD-POCS are not built;
+`fista_tv` is the TV-regularised method this project offers.
 
     python -m r2_gaussian_b200.recon -s <scene> -m <output> [--methods fdk,sart,cgls]
 
@@ -39,6 +58,7 @@ keyed by method.  PNG slices and projections are not written (matplotlib is not 
 from __future__ import annotations
 
 import argparse
+import math
 import os
 import sys
 import time
@@ -46,12 +66,16 @@ import time
 import numpy as np
 import torch
 
-METHODS = ("fdk", "sart", "ossart", "cgls")
+METHODS = ("fdk", "sart", "ossart", "cgls", "fista_tv")
 NOT_BUILT = ("asd_pocs", "os_asd_pocs")
 # iteration counts and parameters of ct_utils.recon_volume / run_ct_recon_algs
 CGLS_NITER = 60
 SART_NITER = 20
 OSSART_BLOCKSIZE = 10
+# FISTA-TV defaults, chosen on one noisy fixture (DESIGN §8)
+FISTA_NITER = 50
+FISTA_LAMBDA = 1e-3
+FISTA_TVITER = 20
 
 
 def _dot(a: torch.Tensor, b: torch.Tensor) -> float:
@@ -102,6 +126,56 @@ def sart_solve(b: torch.Tensor, A, At, shape, niter: int, lmbda: float = 1.0, lm
     return x
 
 
+def _check_fista(niter, lmbda, tviter, L):
+    if int(niter) != niter or niter < 1:
+        raise ValueError(f"fista_tv: niter must be an integer >= 1, got {niter}")
+    if not (float(lmbda) >= 0.0 and math.isfinite(float(lmbda))):
+        raise ValueError(f"fista_tv: lmbda must be finite and >= 0, got {lmbda}")
+    if int(tviter) != tviter or tviter < 1:
+        raise ValueError(f"fista_tv: tviter must be an integer >= 1, got {tviter}")
+    if L is not None and not (float(L) > 0.0 and math.isfinite(float(L))):
+        raise ValueError(f"fista_tv: L must be finite and > 0, got {L}")
+
+
+def schur_lipschitz(b: torch.Tensor, A, At, shape) -> float:
+    """max(A 1) max(A^T 1), an upper bound of |A|^2 for a non-negative A (|A|_2^2 <= |A|_1 |A|_inf)."""
+    everything = slice(None)
+    a1 = A(torch.ones(tuple(shape), dtype=b.dtype, device=b.device), everything)
+    at1 = At(torch.ones_like(b), everything, False)
+    return float(a1.max()) * float(at1.max())
+
+
+def fista_tv_solve(b: torch.Tensor, A, At, shape, niter: int, lmbda: float, tviter: int = FISTA_TVITER, L=None,
+                   nonneg: bool = True, prox=None, tv=None):
+    """FISTA-TV from x = 0 over the callables A(x, views) / At(y, views, weights); `shape` is the volume's.  `prox(v,
+    weight, tviter, nonneg)` and `tv(x)` default to the GPU `tv.tv_denoise` / `tv.tv_value`.  Returns (x, history)."""
+    _check_fista(niter, lmbda, tviter, L)
+    if prox is None:
+        from .tv import tv_denoise as prox
+    if tv is None:
+        from .tv import tv_value as tv
+    everything = slice(None)
+    if L is None:
+        L = schur_lipschitz(b, A, At, shape)
+        if not L > 0.0:
+            raise ValueError("fista_tv: A 1 or A^T 1 is zero: no ray meets the volume")
+    L = float(L)
+    x_prev = torch.zeros(tuple(shape), dtype=b.dtype, device=b.device)
+    y = x_prev
+    t = 1.0
+    history = []
+    for _ in range(niter):
+        grad = At(A(y, everything).sub_(b), everything, False)
+        x = prox(y.sub(grad, alpha=1.0 / L), float(lmbda) / L, tviter, nonneg)
+        t_next = 0.5 * (1.0 + math.sqrt(1.0 + 4.0 * t * t))
+        y = x.add(x - x_prev, alpha=(t - 1.0) / t_next)
+        r = A(x, everything).sub_(b)
+        data, tvx = 0.5 * _dot(r, r), float(tv(x))
+        history.append({"data": data, "tv": tvx, "F": data + float(lmbda) * tvx})
+        x_prev, t = x, t_next
+    return x_prev, history
+
+
 def _operator(projs, angles, scanner_cfg):
     from .projector import CTOperator
 
@@ -128,6 +202,14 @@ def sart(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = SART_NITER
     return sart_solve(b, op.A, op.At, op.nvox, niter, lmbda, lmbda_red, blocksize, nonneg)
 
 
+def fista_tv(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = FISTA_NITER, lmbda: float = FISTA_LAMBDA,
+             tviter: int = FISTA_TVITER, nonneg: bool = True, L=None):
+    """FISTA-TV on the GPU projector pair and the GPU TV prox; returns (volume, history)."""
+    _check_fista(niter, lmbda, tviter, L)
+    op, b = _operator(projs, angles, scanner_cfg)
+    return fista_tv_solve(b, op.A, op.At, op.nvox, niter, lmbda, tviter, L, nonneg)
+
+
 def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str) -> torch.Tensor:
     """The reconstructions of ct_utils.recon_volume / run_ct_recon_algs with their iteration counts."""
     if method == "fdk":
@@ -140,6 +222,8 @@ def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str) ->
         return sart(projs, angles, scanner_cfg, SART_NITER)
     if method == "ossart":
         return sart(projs, angles, scanner_cfg, SART_NITER, blocksize=OSSART_BLOCKSIZE)
+    if method == "fista_tv":
+        return fista_tv(projs, angles, scanner_cfg)[0]
     raise ValueError(f"recon_volume: unknown method {method!r} (supported: {', '.join(METHODS)})")
 
 
@@ -147,8 +231,8 @@ def _parse_methods(text: str) -> list[str]:
     methods = [m.strip() for m in text.split(",") if m.strip()]
     for m in methods:
         if m in NOT_BUILT:
-            raise SystemExit(f"method {m} is not built (TV-regularised ASD-POCS is not part of this project); "
-                             f"supported: {', '.join(METHODS)}")
+            raise SystemExit(f"method {m} is not built (ASD-POCS is not part of this project; fista_tv is its "
+                             f"TV-regularised alternative); supported: {', '.join(METHODS)}")
         if m not in METHODS:
             raise SystemExit(f"unknown method {m!r}; supported: {', '.join(METHODS)}")
     if not methods:
@@ -157,7 +241,7 @@ def _parse_methods(text: str) -> list[str]:
 
 
 def main(argv=None) -> dict:
-    ap = argparse.ArgumentParser(description="Traditional CT reconstructions (FDK, SART, OS-SART, CGLS) of a scene")
+    ap = argparse.ArgumentParser(description="Traditional CT reconstructions (FDK, SART, OS-SART, CGLS, FISTA-TV) of a scene")
     ap.add_argument("-s", "--source_path", required=True, help="scene directory or NAF pickle")
     ap.add_argument("-m", "--model_path", required=True, help="output directory")
     ap.add_argument("--methods", default="fdk,sart,cgls", help=f"comma-separated subset of {','.join(METHODS)}")
