@@ -379,8 +379,8 @@ int r2x_gather_rows(void* stream, int ntensors, const r2x_gather_desc* descs, co
  *   3. voxel-driven backprojection: voxel centres center - s/2 + (i + 1/2) s/n, projected through projmatrix and the
  *      rasterizer's ndc -> pixel mapping, bilinear sample (0 outside the detector), weight U^2 with U = DSO / z_view
  *      (cone; 0 for z_view <= 0) or 1 (parallel); out_volume[nx,ny,nz] = (pi / N) * sum over views in index order.
- * No Parker weights: a cone-beam short scan is reconstructed as if it were a full one (as TIGRE's default fdk).
- * Deterministic (no atomics).  `scratch` holds r2x_fdk_scratch_bytes(N, H, W) (the filtered views).  Asynchronous on
+ * r2x_fdk has no Parker weights: it reconstructs a cone-beam short scan as if it were a full one (as TIGRE's default
+ * fdk); r2x_fdk_short_scan below weights a short scan.  Deterministic (no atomics).  `scratch` holds r2x_fdk_scratch_bytes(N, H, W) (the filtered views).  Asynchronous on
  * `stream`.  Limits: W <= 16384, N * H < 2^31, nx <= 262140, nz <= 524280. */
 size_t r2x_fdk_scratch_bytes(int n_views, int H, int W);
 int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
@@ -393,6 +393,20 @@ int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, 
 int r2x_fdk_backproject(void* stream, int n_views, int H, int W, const float* filtered, const float* viewmatrices,
                         const float* projmatrices, int mode, float dso, int nx, int ny, int nz, float sx, float sy,
                         float sz, float cx, float cy, float cz, float* out_volume);
+/* FDK of a short scan (Parker 1982, in Silver 2000's overscan form; the statement is tests/fdk_short_scan_oracle.py): an arc B
+ * with pi + 2 gamma_max <= B < 2 pi (gamma_max = atan(tan_fovx) for cone beam, 0 for parallel beam) measures some rays
+ * once and some twice.  Step 1 becomes P' = w(beta'_v, gamma_j) * dbeta_v * (cone: cosine weight) * P, with
+ *   gamma_j = -atan(ndc_x(j) tan_fovx) (cone; the detector's u axis runs along the rotation) or 0 (parallel),
+ *   delta = (B - pi) / 2 and the Parker weight w = sin^2(pi/4 beta' / (delta - gamma)) for beta' < 2 (delta - gamma),
+ *   1 up to pi - 2 gamma, sin^2(pi/4 (B - beta') / (delta + gamma)) up to B, 0 beyond;
+ * step 2 is unchanged and step 3 sums with scale 1 instead of pi / N.  view_weights[N,2] (device) holds each view's
+ * (beta'_v, dbeta_v): its arc position from the start of the scan and its angular interval, as fdk.short_scan_views
+ * computes them in float64 (they are not read on the host, so their finiteness is the caller's).  Same arguments,
+ * scratch and limits as r2x_fdk otherwise; also checks N >= 2 and pi + 2 gamma_max <= B < 2 pi. */
+int r2x_fdk_short_scan(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                       const float* projmatrices, const float* view_weights, float arc, float tan_fovx, float tan_fovy,
+                       int mode, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
+                       float cz, float* out_volume, void* scratch, size_t scratch_bytes);
 
 /* ---- forward projection of a voxel volume (synthetic projection data) --------------------------- */
 /* Replaces TIGRE's `Ax` (data_generator/synthetic_dataset/generate_data.py).  Lengths in the scene-scaled units of the

@@ -17,8 +17,12 @@
 //                           weighted by U^2, U = DSO / z_view (cone; 1 for parallel beam).  The views are summed in
 //                           index order in registers and each voxel is stored once: no atomics, so the volume is
 //                           bitwise reproducible.
+//   fdk_parker_filter_kernel  the filter of a short scan (r2x_fdk_short_scan): fdk_filter_kernel with each pixel also
+//                           weighted by its Parker redundancy weight and its view's angular interval; the backprojection
+//                           that follows is fdk_backproject_kernel with scale 1 instead of pi / N.
 //
-// The float64 NumPy statement of the same definition is oracle/fdk_oracle.py.
+// The float64 NumPy statements of the same definitions are oracle/fdk_oracle.py (plain) and
+// tests/fdk_short_scan_oracle.py (short scan, Parker weights).
 #include <cmath>
 #include <cstdint>
 
@@ -155,13 +159,88 @@ __global__ void __launch_bounds__(FDK_BX * FDK_BY) fdk_backproject_kernel(
         if (z0 + k < nz) out[z0 + k] = acc[k] * scale;
 }
 
+// Parker redundancy weight of the ray at arc position beta (radians from the start of the scan) and fan angle gam
+// (signed so that its conjugate ray is (beta + pi + 2 gam, -gam)) on a short scan of arc B = pi + 2 delta.  A region
+// whose bounds cross (delta - gam <= 0 or delta + gam <= 0) is empty, so no branch divides by a non-positive value.
+__device__ __forceinline__ float fdk_parker_weight(float beta, float gam, float arc, float delta) {
+    const float rise = delta - gam;
+    if (beta < 2.0f * rise) {
+        const float s = sinpif(0.25f * beta / rise);
+        return s * s;
+    }
+    if (beta < 3.14159265358979f - 2.0f * gam) return 1.0f;
+    if (beta < arc) {
+        const float s = sinpif(0.25f * (arc - beta) / (delta + gam));
+        return s * s;
+    }
+    return 0.0f;
+}
+
+// fdk_filter_kernel for a short scan: each pixel is also weighted by its Parker weight and its view's angular interval
+// while the row is staged (view weights vw[v] = (beta'_v, dbeta_v)); the Ram-Lak convolution is the same.  The weight is
+// computed per pixel (one atanf and one sinpif), which costs little next to the W/2-tap convolution of each pixel.
+__global__ void __launch_bounds__(256) fdk_parker_filter_kernel(int H, int W, const float* __restrict__ projs,
+                                                                float tanx, float tany, int cone, float inv_delta,
+                                                                const float2* __restrict__ vw, float arc, float delta,
+                                                                float* __restrict__ q) {
+    extern __shared__ float sm[];
+    float* row = sm;              // [3W]: zeros | weighted row | zeros
+    float* g = sm + 3 * W;        // [(W+1)/2]: g[m] = 1 / (pi^2 (2m+1)^2)
+    const size_t r = blockIdx.x;  // view * H + detector row
+    const float* src = projs + r * W;
+    const float2 bv = vw[r / H];
+    const float step = 2.0f / (float)W, first = 1.0f / (float)W - 1.0f;
+    const float b = cone ? fmaf((float)(r % H), 2.0f / (float)H, 1.0f / (float)H - 1.0f) * tany : 0.0f;
+    for (int j = threadIdx.x; j < W; j += blockDim.x) {
+        float p = src[j];
+        float gam = 0.0f;
+        if (cone) {
+            const float a = fmaf((float)j, step, first) * tanx;
+            p *= rsqrtf(fmaf(a, a, fmaf(b, b, 1.0f)));
+            gam = -atanf(a);  // column u runs along the rotation, so a ray at +u leans back: gamma = -atan(u / DSD)
+        }
+        row[j] = 0.0f;
+        row[W + j] = p * (fdk_parker_weight(bv.x, gam, arc, delta) * bv.y);
+        row[2 * W + j] = 0.0f;
+    }
+    for (int m = threadIdx.x; m < (W + 1) / 2; m += blockDim.x) {
+        const float k = (float)(2 * m + 1);
+        g[m] = 1.0f / (9.869604401089358f * k * k);
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < W; j += blockDim.x) {
+        const float* c = row + W + j;
+        float acc = 0.0f;
+        for (int m = 0, k = 1; k < W; ++m, k += 2) acc = fmaf(g[m], c[-k] + c[k], acc);
+        q[r * W + j] = fmaf(0.25f, c[0], -acc) * inv_delta;
+    }
+}
+
+// isocentre pitch: cone dDetector_u * DSO / DSD = 2 tan_fovx DSO / W; parallel 2 / W (ndc [-1,1] = scene [-1,1])
+static double fdk_pitch(int W, float tanx, int mode, float dso) {
+    return mode == 1 ? 2.0 * (double)tanx * (double)dso / W : 2.0 / W;
+}
+
+static int fdk_parker_filter(cudaStream_t st, int N, int H, int W, const float* projs, float tanx, float tany, int mode,
+                             float dso, const float* view_weights, float arc, float* q) {
+    const size_t smem = fdk_filter_smem(W);
+    if (smem > 48 * 1024)
+        R2X_CUDA_OK(cudaFuncSetAttribute(fdk_parker_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem));
+    const float delta = (float)(0.5 * ((double)arc - 3.141592653589793));
+    fdk_parker_filter_kernel<<<(unsigned)((long long)N * H), 256, smem, st>>>(
+        H, W, projs, tanx, tany, mode, (float)(1.0 / fdk_pitch(W, tanx, mode, dso)), (const float2*)view_weights, arc,
+        delta, q);
+    R2X_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
 static int fdk_filter(cudaStream_t st, int N, int H, int W, const float* projs, float tanx, float tany, int mode,
                       float dso, float* q) {
     const size_t smem = fdk_filter_smem(W);
     if (smem > 48 * 1024)
         R2X_CUDA_OK(cudaFuncSetAttribute(fdk_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    // isocentre pitch: cone dDetector_u * DSO / DSD = 2 tan_fovx DSO / W; parallel 2 / W (ndc [-1,1] = scene [-1,1])
-    const double delta = mode == 1 ? 2.0 * (double)tanx * (double)dso / W : 2.0 / W;
+    const double delta = fdk_pitch(W, tanx, mode, dso);
     fdk_filter_kernel<<<(unsigned)((long long)N * H), 256, smem, st>>>(H, W, projs, tanx, tany, mode, (float)(1.0 / delta),
                                                                        q);
     R2X_CUDA_OK(cudaGetLastError());
@@ -170,12 +249,11 @@ static int fdk_filter(cudaStream_t st, int N, int H, int W, const float* projs, 
 
 static int fdk_backproject(cudaStream_t st, int N, int H, int W, const float* q, const float* viewm, const float* projm,
                            int mode, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
-                           float cz, float* vol) {
+                           float cz, float scale, float* vol) {
     const float dx = sx / nx, dy = sy / ny, dz = sz / nz;
     const float ox = cx - 0.5f * sx + 0.5f * dx, oy = cy - 0.5f * sy + 0.5f * dy, oz = cz - 0.5f * sz + 0.5f * dz;
     const dim3 grid((ny + FDK_BX - 1) / FDK_BX, (nx + FDK_BY - 1) / FDK_BY, (nz + FDK_ZR - 1) / FDK_ZR);
     const dim3 block(FDK_BX, FDK_BY);
-    const float scale = (float)(3.141592653589793 / N);
     if (mode == 1)
         fdk_backproject_kernel<true><<<grid, block, 0, st>>>(N, H, W, q, viewm, projm, dso, nx, ny, nz, ox, oy, oz, dx, dy,
                                                             dz, scale, vol);
@@ -223,7 +301,29 @@ int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const f
     float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
     if (int rc = r2x::fdk_filter(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, q)) return rc;
     return r2x::fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx,
-                                cy, cz, out_volume);
+                                cy, cz, (float)(3.141592653589793 / n_views), out_volume);
+}
+
+int r2x_fdk_short_scan(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                       const float* projmatrices, const float* view_weights, float arc, float tan_fovx, float tan_fovy,
+                       int mode, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
+                       float cz, float* out_volume, void* scratch, size_t scratch_bytes) {
+    if (int rc = r2x::fdk_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode,
+                                   dso, nx, ny, nz, sx, sy, sz, out_volume, scratch, scratch_bytes))
+        return rc;
+    if (n_views < 2) return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan: bad N (a short scan needs >= 2 views)");
+    if (!view_weights) return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan: bad pointer (view_weights NULL)");
+    // the arc must hold pi plus the full fan (within float rounding of the arc) and stay short of a full circle
+    const double pi = 3.141592653589793;
+    const double need = pi + (mode == 1 ? 2.0 * std::atan((double)tan_fovx) : 0.0);
+    if (!(std::isfinite(arc) && (double)arc >= need - 1e-6 && (double)arc < 2.0 * pi))
+        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan: bad arc (needs pi + 2 atan(tan_fovx) <= arc < 2 pi)");
+    const cudaStream_t st = (cudaStream_t)stream;
+    float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
+    if (int rc = r2x::fdk_parker_filter(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, view_weights, arc, q))
+        return rc;
+    return r2x::fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx,
+                                cy, cz, 1.0f, out_volume);
 }
 
 int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, float tan_fovx, float tan_fovy,
@@ -244,7 +344,7 @@ int r2x_fdk_backproject(void* stream, int n_views, int H, int W, const float* fi
                                    mode, dso, nx, ny, nz, sx, sy, sz, out_volume, filtered, (size_t)-1))
         return rc;
     return r2x::fdk_backproject((cudaStream_t)stream, n_views, H, W, filtered, viewmatrices, projmatrices, mode, dso, nx,
-                                ny, nz, sx, sy, sz, cx, cy, cz, out_volume);
+                                ny, nz, sx, sy, sz, cx, cy, cz, (float)(3.141592653589793 / n_views), out_volume);
 }
 
 }  // extern "C"

@@ -1,27 +1,69 @@
 """FDK reconstruction on the GPU over the C ABI (r2x_fdk) -- what the reference obtains from TIGRE's `algs.fdk`
 (`r2_gaussian/utils/ct_utils.py::recon_volume`) to initialise its point cloud.
 
-    vol = fdk(projections, angles, scanner_cfg)        # [nx, ny, nz], the voxelizer's layout
+    vol = fdk(projections, angles, scanner_cfg)                    # [nx, ny, nz], the voxelizer's layout
+    vol = fdk(projections, angles, scanner_cfg, short_scan=True)   # Parker-weighted, for an arc short of 360 degrees
 
 `projections` is a CUDA float32 [N, H, W] tensor in the dataset layout (rows = v, columns = u, already multiplied by
 scene_scale); `scanner_cfg` is the scaled dict of `dataset.read_scene` / `Scene.scanner_cfg`.  The per-view geometry is
 the rasterizer's (`scene.make_view`), so the reconstruction agrees with render() on detector orientation, axis order and
-angle convention by construction.  Band-limited Ram-Lak filter only (`filter: null` or "ram_lak"), no Parker weights
-(a cone-beam short scan is reconstructed as a full scan, as TIGRE's default fdk does).  Runs on the current stream;
-no CPU fallback.
+angle convention by construction.  Band-limited Ram-Lak filter only (`filter: null` or "ram_lak").  Runs on the current
+stream; no CPU fallback.
+
+The plain path weights every view by pi / N, which assumes each ray is measured twice: right for a full 360-degree scan
+and a 180-degree parallel scan, not for a cone-beam short scan (180 degrees plus the fan angle), which it reconstructs
+as a full one with low-frequency shading, as TIGRE's default fdk does.  `short_scan=True` runs r2x_fdk_short_scan
+instead: Parker redundancy weights (Parker 1982, in Silver 2000's overscan form) and each view's own angular interval,
+from `short_scan_views`.  It refuses fewer than 2 views, an arc shorter than 180 degrees plus the fan angle and a full
+circle.  The definition is stated in float64 in tests/fdk_short_scan_oracle.py (the plain FDK's in
+oracle/fdk_oracle.py).
 """
 from __future__ import annotations
+
+import math
 
 import numpy as np
 import torch
 
 from ._lib import check, load
-from .scene import make_view
+from .scene import MODE_CONE, make_view
 
 SUPPORTED_FILTERS = (None, "ram_lak")
+# slack on the arc refusals: a scan sampled at linspace(0, pi, n + 1)[:-1] covers pi only up to rounding
+ARC_TOLERANCE = 1e-9
 
 
-def fdk(projections: torch.Tensor, angles, scanner_cfg: dict) -> torch.Tensor:
+def short_scan_views(angles, mode: int, tan_fovx: float):
+    """(view_weights [N, 2] float64 of (beta'_v, dbeta_v), arc B) of a short scan with the views at `angles` (radians,
+    any order), after the refusals.  The largest circular gap between the angles marks the start of the scan; view v
+    sits at beta_v = (theta_v - theta_start) mod 2 pi and stands for an interval of the mean step D = beta_max / (N - 1)
+    around it, so beta'_v = beta_v + D / 2 and B = beta_max + D (`linspace(0, R, n + 1)[:-1]` gives B = R).  dbeta_v
+    runs between the midpoints of the sorted beta' (0 and B at the ends); views at the same angle share theirs."""
+    theta = np.mod(np.asarray(angles, np.float64).reshape(-1), 2.0 * math.pi)
+    N = len(theta)
+    if N < 2:
+        raise ValueError(f"fdk short scan: needs at least 2 views, got {N}")
+    s = np.sort(theta)
+    gaps = np.append(np.diff(s), s[0] + 2.0 * math.pi - s[-1])
+    start = s[(int(np.argmax(gaps)) + 1) % N]
+    beta = np.mod(theta - start, 2.0 * math.pi)
+    step = beta.max() / (N - 1)
+    bp, arc = beta + 0.5 * step, beta.max() + step
+    gamma_max = math.atan(tan_fovx) if mode == MODE_CONE else 0.0
+    need = math.pi + 2.0 * gamma_max
+    if arc < need - ARC_TOLERANCE:
+        raise ValueError(f"fdk short scan: the views cover an arc of {math.degrees(arc):.2f} degrees, a short scan needs "
+                         f"at least {math.degrees(need):.2f} (180 plus the fan angle {math.degrees(2 * gamma_max):.2f})")
+    if arc >= 2.0 * math.pi - ARC_TOLERANCE:
+        raise ValueError(f"fdk short scan: the views cover an arc of {math.degrees(arc):.2f} degrees, a full circle, "
+                         "which needs no redundancy weights: use fdk without short_scan")
+    u, inv, count = np.unique(bp, return_inverse=True, return_counts=True)
+    edges = np.concatenate([[0.0], 0.5 * (u[1:] + u[:-1]), [arc]])
+    dbeta = (np.diff(edges) / count)[inv]
+    return np.stack([bp, dbeta], 1), arc
+
+
+def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool = False) -> torch.Tensor:
     if not isinstance(projections, torch.Tensor) or projections.device.type != "cuda":
         raise RuntimeError("fdk: projections must be a CUDA tensor (this build has no CPU fallback; "
                            f"got {getattr(projections, 'device', type(projections))})")
@@ -40,6 +82,8 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict) -> torch.Tensor:
         raise ValueError("fdk: no projections")
     views = [make_view(scanner_cfg, float(a)) for a in angles]
     mode = views[0].mode
+    if short_scan:
+        view_weights, arc = short_scan_views(angles, mode, float(views[0].tanfovx))
     nx, ny, nz = (int(v) for v in scanner_cfg["nVoxel"])
     sx, sy, sz = (float(v) for v in scanner_cfg["sVoxel"])
     cx, cy, cz = (float(v) for v in scanner_cfg["offOrigin"])
@@ -52,9 +96,16 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict) -> torch.Tensor:
         vol = torch.empty((nx, ny, nz), dtype=torch.float32, device=dev)
         nbytes = int(lib.r2x_fdk_scratch_bytes(N, H, W))
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        rc = lib.r2x_fdk(torch.cuda.current_stream(dev).cuda_stream, N, H, W, projs.data_ptr(), vm.data_ptr(),
-                         pm.data_ptr(), float(views[0].tanfovx), float(views[0].tanfovy), int(mode),
-                         float(scanner_cfg["DSO"]), nx, ny, nz, sx, sy, sz, cx, cy, cz, vol.data_ptr(),
-                         scratch.data_ptr(), nbytes)
-    check(rc, "r2x_fdk")
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        tail = (float(views[0].tanfovx), float(views[0].tanfovy), int(mode), float(scanner_cfg["DSO"]), nx, ny, nz, sx,
+                sy, sz, cx, cy, cz, vol.data_ptr(), scratch.data_ptr(), nbytes)
+        if short_scan:
+            vw = torch.from_numpy(view_weights.astype(np.float32)).to(dev, non_blocking=False)
+            name = "r2x_fdk_short_scan"
+            rc = lib.r2x_fdk_short_scan(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), vw.data_ptr(),
+                                        float(arc), *tail)
+        else:
+            name = "r2x_fdk"
+            rc = lib.r2x_fdk(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), *tail)
+    check(rc, name)
     return vol

@@ -47,13 +47,16 @@ step and stop rules are defined by TIGRE's implementation, is not what it comput
 Parity with TIGRE's binaries is not pinned (as for FDK and the projector).  ASD-POCS / OS-ASD-POCS are not built;
 `fista_tv` is the TV-regularised method this project offers.
 
-    python -m r2_gaussian_b200.recon -s <scene> -m <output> [--methods fdk,sart,cgls]
+    python -m r2_gaussian_b200.recon -s <scene> -m <output> [--methods fdk,sart,cgls] [--short_scan]
 
 mirrors `scripts/run_traditional_methods.py`: it reconstructs the scene's train views with each method, scores the
 volume against `vol_gt` with `metrics.metric_vol` and writes, per method, `<output>/<method>/ct_gt.npy`, `ct_pred.npy`,
-`eval_3d.yml` (method, psnr_3d, ssim_3d, ssim_3d_x/y/z, duration (sec), duration (min)) and the test views
+`eval_3d.yml` (method, psnr_3d, ssim_3d, ssim_3d_x/y/z, duration (sec), duration (min); fdk under `--short_scan`
+also `short_scan: true`) and the test views
 `projs/{i:05d}_render.npy` (projections of the reconstruction) and `projs/{i:05d}_gt.npy`, plus `<output>/eval_3d.yml`
 keyed by method.  PNG slices and projections are not written (matplotlib is not a dependency of this project).
+`--short_scan` reconstructs fdk with Parker redundancy weights (`fdk.fdk(short_scan=True)`), for scenes whose train
+views cover less than a full circle; it is refused when --methods has no fdk.
 """
 from __future__ import annotations
 
@@ -210,12 +213,16 @@ def fista_tv(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = FISTA_
     return fista_tv_solve(b, op.A, op.At, op.nvox, niter, lmbda, tviter, L, nonneg)
 
 
-def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str) -> torch.Tensor:
-    """The reconstructions of ct_utils.recon_volume / run_ct_recon_algs with their iteration counts."""
+def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, short_scan: bool = False) -> torch.Tensor:
+    """The reconstructions of ct_utils.recon_volume / run_ct_recon_algs with their iteration counts.  `short_scan`
+    selects the Parker-weighted FDK and applies to method fdk only."""
+    if short_scan and method != "fdk":
+        raise ValueError(f"recon_volume: short_scan applies to fdk only, not {method!r} (the iterative methods need no "
+                         "redundancy weights)")
     if method == "fdk":
         from .fdk import fdk
 
-        return fdk(projs, angles, scanner_cfg)
+        return fdk(projs, angles, scanner_cfg, short_scan=short_scan)
     if method == "cgls":
         return cgls(projs, angles, scanner_cfg, CGLS_NITER)[0]
     if method == "sart":
@@ -245,8 +252,13 @@ def main(argv=None) -> dict:
     ap.add_argument("-s", "--source_path", required=True, help="scene directory or NAF pickle")
     ap.add_argument("-m", "--model_path", required=True, help="output directory")
     ap.add_argument("--methods", default="fdk,sart,cgls", help=f"comma-separated subset of {','.join(METHODS)}")
+    ap.add_argument("--short_scan", default=False, action="store_true",
+                    help="reconstruct fdk with Parker redundancy weights (a scan over less than 360 degrees)")
     a = ap.parse_args(argv)
     methods = _parse_methods(a.methods)
+    if a.short_scan and "fdk" not in methods:
+        raise SystemExit("--short_scan applies to the fdk method, which --methods does not include (the iterative "
+                         "methods need no redundancy weights)")
     if not torch.cuda.is_available():
         raise SystemExit("the reconstructions need a CUDA device: they run on the GPU and have no CPU fallback")
     import yaml
@@ -270,7 +282,8 @@ def main(argv=None) -> dict:
         os.makedirs(os.path.join(save, "projs"), exist_ok=True)
         torch.cuda.synchronize()
         t0 = time.time()
-        pred = recon_volume(projs_train, train_angles, cfg, method)
+        short_scan = a.short_scan and method == "fdk"
+        pred = recon_volume(projs_train, train_angles, cfg, method, short_scan=short_scan)
         torch.cuda.synchronize()
         duration = time.time() - t0
         ct_pred = pred.cpu().numpy()
@@ -281,6 +294,8 @@ def main(argv=None) -> dict:
         report = {"method": method, "psnr_3d": float(psnr_3d), "ssim_3d": float(ssim_3d),
                   "ssim_3d_x": float(ssim_axis[0]), "ssim_3d_y": float(ssim_axis[1]), "ssim_3d_z": float(ssim_axis[2]),
                   "duration (sec)": duration, "duration (min)": duration / 60}
+        if short_scan:
+            report["short_scan"] = True
         with open(os.path.join(save, "eval_3d.yml"), "w") as f:
             yaml.dump(report, f, default_flow_style=False, sort_keys=False)
         if test_angles:
