@@ -407,6 +407,27 @@ int r2x_fdk_short_scan(void* stream, int n_views, int H, int W, const float* pro
                        const float* projmatrices, const float* view_weights, float arc, float tan_fovx, float tan_fovy,
                        int mode, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
                        float cz, float* out_volume, void* scratch, size_t scratch_bytes);
+/* FDK with the detector offset by (shift_u, shift_v) pixels: t_u = offDetector[0] / dDetector_u, t_v = offDetector[1] /
+ * dDetector_v of the scanner file, replacing TIGRE's `geo.offDetector` (r2_gaussian/utils/ct_utils.py::get_geometry_tigre;
+ * scene.detector_shift states the convention).  Image pixel (row i, column j) holds the ray of the centred detector's
+ * fractional pixel (i - t_v, j + t_u), so step 1 takes its cosine weight at ndc ((2j+1)/W - 1 + 2 t_u/W,
+ * (2i+1)/H - 1 - 2 t_v/H); step 2 is unchanged; step 3 is r2x_fdk's, through the caller's projmatrices, which must be
+ * the offset ones (scene.make_view(..., use_offDetector=True)).  half_fan = 1 (a full circle with the axis off centre,
+ * 0 < |t_u| < W/2; the caller checks the circle) also weights each pixel in step 1 by Wang's (2002) redundancy weight of
+ * its fan coordinate a_j = ndc_x(j) * (cone: tan_fovx; parallel: 1): with delta = (1 - 2|t_u|/W) * (tan_fovx or 1) and
+ * sigma = sign(t_u), w = 2 sin^2(pi/4 (1 + sigma a / delta)) for |a| <= delta, 2 for sigma a > delta; the scale stays
+ * pi / N.  The statement is tests/offset_detector_oracle.py.  Same arguments, scratch and limits as r2x_fdk otherwise. */
+int r2x_fdk_shifted(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                    const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
+                    int half_fan, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
+                    float cz, float* out_volume, void* scratch, size_t scratch_bytes);
+/* r2x_fdk_short_scan with the detector offset vertically by shift_v pixels (as r2x_fdk_shifted); shift_u must be 0:
+ * Parker weights assume each ray's conjugate is on the detector.  projmatrices must be the offset ones. */
+int r2x_fdk_short_scan_shifted(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                               const float* projmatrices, const float* view_weights, float arc, float tan_fovx,
+                               float tan_fovy, int mode, float shift_u, float shift_v, float dso, int nx, int ny, int nz,
+                               float sx, float sy, float sz, float cx, float cy, float cz, float* out_volume,
+                               void* scratch, size_t scratch_bytes);
 
 /* ---- forward projection of a voxel volume (synthetic projection data) --------------------------- */
 /* Replaces TIGRE's `Ax` (data_generator/synthetic_dataset/generate_data.py).  Lengths in the scene-scaled units of the
@@ -427,6 +448,13 @@ int r2x_fdk_short_scan(void* stream, int n_views, int H, int W, const float* pro
 int r2x_volume_project(void* stream, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
                        float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
                        float tan_fovx, float tan_fovy, int mode, float step, float* out_projs);
+/* r2x_volume_project with the detector offset by (shift_u, shift_v) pixels (TIGRE's `geo.offDetector`, as
+ * r2x_fdk_shifted): pixel (i, j) takes the ray of ndc ((2j+1)/W - 1 + 2 shift_u/W, (2i+1)/H - 1 - 2 shift_v/H), computed
+ * in the same float64 setup; everything else as r2x_volume_project.  Zero shifts give the same rays. */
+int r2x_volume_project_shifted(void* stream, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
+                               float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
+                               float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v, float step,
+                               float* out_projs);
 
 /* ---- matched backprojection: the transpose of r2x_volume_project (iterative reconstruction) ------------------- */
 /* Replaces TIGRE's `Atb` inside `algs.cgls` / `algs.sart` / `algs.ossart` (r2_gaussian/utils/ct_utils.py).  Same
@@ -446,6 +474,14 @@ int r2x_volume_backproject(void* stream, int n_views, int H, int W, const float*
                            const float* projmatrices, float tan_fovx, float tan_fovy, int mode, int nx, int ny, int nz,
                            float sx, float sy, float sz, float cx, float cy, float cz, float step, float* out_volume,
                            float* out_weight, void* scratch, size_t scratch_bytes);
+/* The exact transpose of r2x_volume_project_shifted (TIGRE's `Atb` with `geo.offDetector`): the samples are that
+ * projector's; projmatrices must be the offset ones (scene.make_view(..., use_offDetector=True)) so that each voxel's
+ * footprint covers the offset rays.  Otherwise as r2x_volume_backproject. */
+int r2x_volume_backproject_shifted(void* stream, int n_views, int H, int W, const float* projs,
+                                   const float* viewmatrices, const float* projmatrices, float tan_fovx, float tan_fovy,
+                                   int mode, float shift_u, float shift_v, int nx, int ny, int nz, float sx, float sy,
+                                   float sz, float cx, float cy, float cz, float step, float* out_volume,
+                                   float* out_weight, void* scratch, size_t scratch_bytes);
 
 /* ---- isotropic total variation on a volume (FISTA-TV, r2_gaussian_b200/recon.py and tv.py) --------------------- */
 /* Volumes are float32 [nx,ny,nz] (z fastest).  grad x = forward differences along x, y, z, 0 across the last index;

@@ -20,9 +20,14 @@
 //   fdk_parker_filter_kernel  the filter of a short scan (r2x_fdk_short_scan): fdk_filter_kernel with each pixel also
 //                           weighted by its Parker redundancy weight and its view's angular interval; the backprojection
 //                           that follows is fdk_backproject_kernel with scale 1 instead of pi / N.
+//   fdk_filter_shift_kernel  the filter of a detector offset by (t_u, t_v) pixels (r2x_fdk_shifted,
+//                           r2x_fdk_short_scan_shifted): each pixel's cosine weight (and fan angle) at its offset ndc,
+//                           plus optional half-fan (Wang 2002) or Parker weights.  The backprojection is
+//                           fdk_backproject_kernel, unchanged, fed the offset projmatrices by the caller.
 //
-// The float64 NumPy statements of the same definitions are oracle/fdk_oracle.py (plain) and
-// tests/fdk_short_scan_oracle.py (short scan, Parker weights).
+// The float64 NumPy statements of the same definitions are oracle/fdk_oracle.py (plain),
+// tests/fdk_short_scan_oracle.py (short scan, Parker weights) and tests/offset_detector_oracle.py (offset detector,
+// half-fan weights).
 #include <cmath>
 #include <cstdint>
 
@@ -216,6 +221,67 @@ __global__ void __launch_bounds__(256) fdk_parker_filter_kernel(int H, int W, co
     }
 }
 
+// Half-fan redundancy weight (Wang 2002) of the ray at fan coordinate a (tan of the fan angle; ndc for parallel beam)
+// on a full circle with the axis off the detector's centre: 2 sin^2(pi/4 (1 + sigma a / delta)) on the overlap
+// |a| <= delta, 2 beyond it on the wide side (sigma a > delta), 0 beyond it on the narrow side (no pixel lies there).
+// w(a) + w(-a) = 2 on the overlap, so a ray measured twice keeps the plain FDK's total weight.
+__device__ __forceinline__ float fdk_half_fan_weight(float a, float inv_delta, float sigma) {
+    const float x = sigma * a * inv_delta;
+    if (x >= 1.0f) return 2.0f;
+    if (x <= -1.0f) return 0.0f;
+    const float s = sinpif(0.25f * (1.0f + x));
+    return 2.0f * (s * s);
+}
+
+enum FdkWeighting { FDK_PLAIN = 0, FDK_PARKER = 1, FDK_HALF_FAN = 2 };
+
+// The filter of a detector offset by (t_u, t_v) pixels (r2x_fdk_shifted, r2x_fdk_short_scan_shifted): fdk_filter_kernel
+// (or fdk_parker_filter_kernel) with each pixel's ndc moved by (su, sv) = (2 t_u / W, -2 t_v / H) in the cosine weight
+// and the fan angle; HALF_FAN also weights each pixel by fdk_half_fan_weight of its fan coordinate a = ndc_x * fan
+// (fan = tan_fovx for cone beam, 1 for parallel beam).  The Ram-Lak convolution is shift-invariant and the same.
+template <int WEIGHT>
+__global__ void __launch_bounds__(256) fdk_filter_shift_kernel(int H, int W, const float* __restrict__ projs,
+                                                               float tanx, float tany, int cone, float inv_delta,
+                                                               float su, float sv, const float2* __restrict__ vw,
+                                                               float arc, float delta, float fan, float hf_inv_delta,
+                                                               float hf_sigma, float* __restrict__ q) {
+    extern __shared__ float sm[];
+    float* row = sm;              // [3W]: zeros | weighted row | zeros
+    float* g = sm + 3 * W;        // [(W+1)/2]: g[m] = 1 / (pi^2 (2m+1)^2)
+    const size_t r = blockIdx.x;  // view * H + detector row
+    const float* src = projs + r * W;
+    const float step = 2.0f / (float)W, first = 1.0f / (float)W - 1.0f;
+    const float b = cone ? (fmaf((float)(r % H), 2.0f / (float)H, 1.0f / (float)H - 1.0f) + sv) * tany : 0.0f;
+    float2 bv = make_float2(0.0f, 0.0f);
+    if (WEIGHT == FDK_PARKER) bv = vw[r / H];
+    for (int j = threadIdx.x; j < W; j += blockDim.x) {
+        float p = src[j];
+        const float nd = fmaf((float)j, step, first) + su;
+        float gam = 0.0f;
+        if (cone) {
+            const float a = nd * tanx;
+            p *= rsqrtf(fmaf(a, a, fmaf(b, b, 1.0f)));
+            if (WEIGHT == FDK_PARKER) gam = -atanf(a);
+        }
+        if (WEIGHT == FDK_PARKER) p *= fdk_parker_weight(bv.x, gam, arc, delta) * bv.y;
+        if (WEIGHT == FDK_HALF_FAN) p *= fdk_half_fan_weight(nd * fan, hf_inv_delta, hf_sigma);
+        row[j] = 0.0f;
+        row[W + j] = p;
+        row[2 * W + j] = 0.0f;
+    }
+    for (int m = threadIdx.x; m < (W + 1) / 2; m += blockDim.x) {
+        const float k = (float)(2 * m + 1);
+        g[m] = 1.0f / (9.869604401089358f * k * k);
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < W; j += blockDim.x) {
+        const float* c = row + W + j;
+        float acc = 0.0f;
+        for (int m = 0, k = 1; k < W; ++m, k += 2) acc = fmaf(g[m], c[-k] + c[k], acc);
+        q[r * W + j] = fmaf(0.25f, c[0], -acc) * inv_delta;
+    }
+}
+
 // isocentre pitch: cone dDetector_u * DSO / DSD = 2 tan_fovx DSO / W; parallel 2 / W (ndc [-1,1] = scene [-1,1])
 static double fdk_pitch(int W, float tanx, int mode, float dso) {
     return mode == 1 ? 2.0 * (double)tanx * (double)dso / W : 2.0 / W;
@@ -243,6 +309,21 @@ static int fdk_filter(cudaStream_t st, int N, int H, int W, const float* projs, 
     const double delta = fdk_pitch(W, tanx, mode, dso);
     fdk_filter_kernel<<<(unsigned)((long long)N * H), 256, smem, st>>>(H, W, projs, tanx, tany, mode, (float)(1.0 / delta),
                                                                        q);
+    R2X_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+template <int WEIGHT>
+static int fdk_filter_shift_launch(cudaStream_t st, int N, int H, int W, const float* projs, float tanx, float tany,
+                                   int mode, float dso, float su, float sv, const float* view_weights, float arc,
+                                   float delta, float fan, float hf_inv_delta, float hf_sigma, float* q) {
+    const size_t smem = fdk_filter_smem(W);
+    if (smem > 48 * 1024)
+        R2X_CUDA_OK(cudaFuncSetAttribute(fdk_filter_shift_kernel<WEIGHT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem));
+    fdk_filter_shift_kernel<WEIGHT><<<(unsigned)((long long)N * H), 256, smem, st>>>(
+        H, W, projs, tanx, tany, mode, (float)(1.0 / fdk_pitch(W, tanx, mode, dso)), su, sv,
+        (const float2*)view_weights, arc, delta, fan, hf_inv_delta, hf_sigma, q);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -321,6 +402,71 @@ int r2x_fdk_short_scan(void* stream, int n_views, int H, int W, const float* pro
     const cudaStream_t st = (cudaStream_t)stream;
     float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
     if (int rc = r2x::fdk_parker_filter(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, view_weights, arc, q))
+        return rc;
+    return r2x::fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx,
+                                cy, cz, 1.0f, out_volume);
+}
+
+int r2x_fdk_shifted(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                    const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
+                    int half_fan, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
+                    float cz, float* out_volume, void* scratch, size_t scratch_bytes) {
+    if (int rc = r2x::fdk_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode,
+                                   dso, nx, ny, nz, sx, sy, sz, out_volume, scratch, scratch_bytes))
+        return rc;
+    if (!(std::isfinite(shift_u) && std::isfinite(shift_v)))
+        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_shifted: bad shift (must be finite)");
+    if (half_fan != 0 && half_fan != 1) return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_shifted: bad half_fan (0 or 1)");
+    // half fan: the rotation axis strictly inside the detector and off its centre, 0 < |t_u| < W / 2
+    if (half_fan && !(shift_u != 0.0f && 2.0 * std::fabs((double)shift_u) < (double)W))
+        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_shifted: bad shift_u for half_fan (needs 0 < |shift_u| < W / 2)");
+    const cudaStream_t st = (cudaStream_t)stream;
+    float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
+    const float su = (float)(2.0 * (double)shift_u / W), sv = (float)(-2.0 * (double)shift_v / H);
+    int rc;
+    if (half_fan) {
+        const double fan = mode == 1 ? (double)tan_fovx : 1.0;
+        const double hf_delta = (1.0 - 2.0 * std::fabs((double)shift_u) / W) * fan;
+        rc = r2x::fdk_filter_shift_launch<r2x::FDK_HALF_FAN>(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, su,
+                                                              sv, nullptr, 0.0f, 0.0f, (float)fan, (float)(1.0 / hf_delta),
+                                                              shift_u > 0.0f ? 1.0f : -1.0f, q);
+    } else {
+        rc = r2x::fdk_filter_shift_launch<r2x::FDK_PLAIN>(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, su, sv,
+                                                           nullptr, 0.0f, 0.0f, 1.0f, 1.0f, 1.0f, q);
+    }
+    if (rc) return rc;
+    return r2x::fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx,
+                                cy, cz, (float)(3.141592653589793 / n_views), out_volume);
+}
+
+int r2x_fdk_short_scan_shifted(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                               const float* projmatrices, const float* view_weights, float arc, float tan_fovx,
+                               float tan_fovy, int mode, float shift_u, float shift_v, float dso, int nx, int ny, int nz,
+                               float sx, float sy, float sz, float cx, float cy, float cz, float* out_volume,
+                               void* scratch, size_t scratch_bytes) {
+    if (int rc = r2x::fdk_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode,
+                                   dso, nx, ny, nz, sx, sy, sz, out_volume, scratch, scratch_bytes))
+        return rc;
+    if (n_views < 2)
+        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan_shifted: bad N (a short scan needs >= 2 views)");
+    if (!view_weights)
+        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan_shifted: bad pointer (view_weights NULL)");
+    if (!std::isfinite(shift_v))
+        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan_shifted: bad shift_v (must be finite)");
+    // Parker weights assume each ray's conjugate is on the detector, which a horizontal offset breaks
+    if (shift_u != 0.0f)
+        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan_shifted: bad shift_u (a short scan needs shift_u = 0)");
+    const double pi = 3.141592653589793;
+    const double need = pi + (mode == 1 ? 2.0 * std::atan((double)tan_fovx) : 0.0);
+    if (!(std::isfinite(arc) && (double)arc >= need - 1e-6 && (double)arc < 2.0 * pi))
+        return r2x::fail_msg(R2X_ERR_INVALID,
+                             "r2x_fdk_short_scan_shifted: bad arc (needs pi + 2 atan(tan_fovx) <= arc < 2 pi)");
+    const cudaStream_t st = (cudaStream_t)stream;
+    float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
+    const float delta = (float)(0.5 * ((double)arc - pi));
+    if (int rc = r2x::fdk_filter_shift_launch<r2x::FDK_PARKER>(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso,
+                                                                0.0f, (float)(-2.0 * (double)shift_v / H), view_weights,
+                                                                arc, delta, 1.0f, 1.0f, 1.0f, q))
         return rc;
     return r2x::fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx,
                                 cy, cz, 1.0f, out_volume);

@@ -26,7 +26,7 @@ from dataclasses import dataclass, field
 import numpy as np
 import torch
 
-from .scene import angle2pose, projection_matrix
+from .scene import angle2pose, detector_shift, projection_matrix, shifted_projection_matrix
 
 MODE_ID = {"parallel": 0, "cone": 1}
 _LENGTH_KEYS = ("dVoxel", "sVoxel", "sDetector", "dDetector", "offOrigin", "offDetector", "DSD", "DSO")
@@ -146,9 +146,12 @@ def train_view_count(source_path: str) -> int:
 
 
 class Camera:
-    """What render() needs from a view (`dataset/cameras.py:20-84`), on `device`."""
+    """What render() needs from a view (`dataset/cameras.py:20-84`), on `device`.  `use_offDetector` puts the scanner's
+    offDetector into `projection_matrix` (`scene.detector_shift`), so full_proj_transform, pose corrections, batched
+    views and the native training step all see it; off, or with a zero offset, the camera is today's bit for bit."""
 
-    def __init__(self, info: CameraInfo, uid: int | None = None, device="cuda", data_device=None):
+    def __init__(self, info: CameraInfo, uid: int | None = None, device="cuda", data_device=None,
+                 use_offDetector: bool = False):
         self.uid = info.uid if uid is None else uid
         self.colmap_id = info.uid
         self.R, self.T, self.angle = info.R, info.T, info.angle
@@ -162,7 +165,10 @@ class Camera:
         Rt[3, 3] = 1.0
         w2c = np.float32(np.linalg.inv(np.linalg.inv(Rt)))               # getWorld2View2 with zero translate
         self.world_view_transform = torch.tensor(w2c).transpose(0, 1).contiguous().to(device)
-        proj = torch.tensor(projection_matrix(info.FovX, info.FovY, info.mode), dtype=torch.float32)
+        P = projection_matrix(info.FovX, info.FovY, info.mode)
+        if use_offDetector:
+            P = shifted_projection_matrix(P, *detector_shift(info.scanner_cfg), self.image_width, self.image_height)
+        proj = torch.tensor(P, dtype=torch.float32)
         self.projection_matrix = proj.transpose(0, 1).contiguous().to(device)
         self.full_proj_transform = (self.world_view_transform.unsqueeze(0).bmm(self.projection_matrix.unsqueeze(0))
                                     ).squeeze(0).contiguous()
@@ -171,14 +177,15 @@ class Camera:
 
 class Scene:
     def __init__(self, source_path: str, model_path: str = "", eval: bool = True, shuffle: bool = True, device="cuda",
-                 data_device=None):
+                 data_device=None, use_offDetector: bool = False):
         self.model_path = model_path
         info = read_scene(source_path, eval)
         if shuffle:
             random.shuffle(info.train_cameras)
             random.shuffle(info.test_cameras)
-        self.train_cameras = [Camera(c, i, device, data_device) for i, c in enumerate(info.train_cameras)]
-        self.test_cameras = [Camera(c, i, device, data_device) for i, c in enumerate(info.test_cameras)]
+        self.use_offDetector = bool(use_offDetector)
+        self.train_cameras = [Camera(c, i, device, data_device, use_offDetector) for i, c in enumerate(info.train_cameras)]
+        self.test_cameras = [Camera(c, i, device, data_device, use_offDetector) for i, c in enumerate(info.test_cameras)]
         self.vol_gt = torch.from_numpy(info.vol).float().to(device)
         self.scanner_cfg, self.scene_scale = info.scanner_cfg, info.scene_scale
         off, size = torch.tensor(self.scanner_cfg["offOrigin"]), torch.tensor(self.scanner_cfg["sVoxel"])

@@ -13,8 +13,10 @@ scanner yml comments index 0 "u direction"; its ct_utils hands TIGRE geo.offDete
 [v, u] order).  TIGRE places detector column j at u = dDetector_u * (j - nDetector_u / 2 + 0.5) + offDetector_u, and
 image columns run along u (the reference flips only v), so a detector mounted with a horizontal offset d shows its
 content d / dDetector_u columns towards SMALLER index: the learned offset corresponds to the scanner file's
-offDetector[0] (u; TIGRE's geo.offDetector[1]) = -s * dDetector[1] = -s * sDetector[1] / nDetector[1].  The projector
-and FDK still refuse a non-zero offDetector; the learned offset is reported, not written back into the scene.
+offDetector[0] (u; TIGRE's geo.offDetector[1]) = -s * dDetector[1] = -s * sDetector[1] / nDetector[1]
+(`scene.detector_shift`'s t_u = -s).  The learned offset is reported, not written back into the scene: put it into the
+scanner file and run the projector, FDK and training with `use_offDetector` (`--use_offDetector`).  With
+`trainer --use_offDetector` the learned s acts on top of the file's offset.
 
 The map.  The shift moves the detector, not the source: every ray, conic and mu stays the same, and only each
 Gaussian's 2-D mean moves by s pixels along u.  Since the rasterizer maps ndc to pixels by ((x / w + 1) W - 1) / 2,

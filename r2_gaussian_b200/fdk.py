@@ -3,6 +3,7 @@
 
     vol = fdk(projections, angles, scanner_cfg)                    # [nx, ny, nz], the voxelizer's layout
     vol = fdk(projections, angles, scanner_cfg, short_scan=True)   # Parker-weighted, for an arc short of 360 degrees
+    vol = fdk(projections, angles, scanner_cfg, use_offDetector=True, half_fan=True)   # offset detector, 360 degrees
 
 `projections` is a CUDA float32 [N, H, W] tensor in the dataset layout (rows = v, columns = u, already multiplied by
 scene_scale); `scanner_cfg` is the scaled dict of `dataset.read_scene` / `Scene.scanner_cfg`.  The per-view geometry is
@@ -17,20 +18,66 @@ instead: Parker redundancy weights (Parker 1982, in Silver 2000's overscan form)
 from `short_scan_views`.  It refuses fewer than 2 views, an arc shorter than 180 degrees plus the fan angle and a full
 circle.  The definition is stated in float64 in tests/fdk_short_scan_oracle.py (the plain FDK's in
 oracle/fdk_oracle.py).
+
+Without `use_offDetector` the scanner's `offDetector` is ignored (with a warning when it is not zero): the volume is
+reconstructed as if the detector were centred.  `use_offDetector=True` reconstructs through the offset detector
+(r2x_fdk_shifted / r2x_fdk_short_scan_shifted, TIGRE's `geo.offDetector`; the convention is `scene.detector_shift`'s):
+the cosine weight is taken at each pixel's offset position and the backprojection goes through the offset matrices.
+A short scan allows a vertical offset only.  `half_fan=True` (with `use_offDetector`) is for a full-circle scan whose
+detector is shifted sideways to widen the field of view: rays near the axis are measured twice and the outer rays once,
+and Wang's (2002) redundancy weights (`half_fan_weight`) give each its share, where the plain FDK would reconstruct the
+outer part at about half its density.  It refuses a centred axis, an axis not strictly inside the detector, views that
+do not cover a full circle and a short scan.  The float64 statement is tests/offset_detector_oracle.py.
 """
 from __future__ import annotations
 
 import math
+import warnings
 
 import numpy as np
 import torch
 
 from ._lib import check, load
-from .scene import MODE_CONE, make_view
+from .scene import MODE_CONE, detector_shift, make_view
 
 SUPPORTED_FILTERS = (None, "ram_lak")
 # slack on the arc refusals: a scan sampled at linspace(0, pi, n + 1)[:-1] covers pi only up to rounding
 ARC_TOLERANCE = 1e-9
+
+
+def scan_arc(angles) -> float:
+    """The arc (radians) that views at `angles` cover: the circle less its largest gap between the angles, plus the
+    mean step between the views (the arc of `short_scan_views`; linspace(0, R, n + 1)[:-1] gives R)."""
+    theta = np.mod(np.asarray(angles, np.float64).reshape(-1), 2.0 * math.pi)
+    N = len(theta)
+    if N < 2:
+        return 0.0
+    s = np.sort(theta)
+    gaps = np.append(np.diff(s), s[0] + 2.0 * math.pi - s[-1])
+    start = s[(int(np.argmax(gaps)) + 1) % N]
+    beta = np.mod(theta - start, 2.0 * math.pi)
+    return float(beta.max() + beta.max() / (N - 1))
+
+
+def half_fan_weight(a, t_u: float, W: int, fan: float):
+    """Wang's (2002) redundancy weight of the ray at fan coordinate `a` (tan of its fan angle for cone beam, ndc for
+    parallel beam) on a full circle whose detector is offset by t_u pixels: delta = (1 - 2 |t_u| / W) fan is the
+    half-width of the part of the detector symmetric about the axis, sigma = sign(t_u), and
+    w(a) = 2 sin^2(pi/4 (1 + sigma a / delta)) for |a| <= delta, 2 beyond delta on the wide side (0 beyond it on the
+    narrow side, where no pixel lies).  w(a) + w(-a) = 2, so a ray measured twice keeps the plain FDK's weight."""
+    check_half_fan_shift(t_u, W)
+    delta = (1.0 - 2.0 * abs(t_u) / W) * fan
+    x = np.clip(math.copysign(1.0, t_u) * np.asarray(a, np.float64) / delta, -1.0, 1.0)
+    return 2.0 * np.sin(0.25 * math.pi * (1.0 + x)) ** 2
+
+
+def check_half_fan_shift(t_u: float, W: int):
+    if t_u == 0.0:
+        raise ValueError("fdk half fan: the detector is centred (offDetector[0] = 0): every ray is measured twice, so "
+                         "use fdk without half_fan")
+    if not abs(t_u) < 0.5 * W:
+        raise ValueError(f"fdk half fan: the rotation axis is not strictly inside the detector (offset of {t_u:g} "
+                         f"pixels on a detector {W} pixels wide needs |offset| < {0.5 * W:g})")
 
 
 def short_scan_views(angles, mode: int, tan_fovx: float):
@@ -63,7 +110,28 @@ def short_scan_views(angles, mode: int, tan_fovx: float):
     return np.stack([bp, dbeta], 1), arc
 
 
-def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool = False) -> torch.Tensor:
+def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool = False, use_offDetector: bool = False,
+        half_fan: bool = False) -> torch.Tensor:
+    if half_fan and not use_offDetector:
+        raise ValueError("fdk: half_fan needs use_offDetector=True (the half-fan weights follow the detector offset)")
+    if half_fan and short_scan:
+        raise ValueError("fdk: half_fan and short_scan cannot be combined (half-fan weights need a full circle, a short "
+                         "scan's Parker weights a centred detector)")
+    t_u, t_v = detector_shift(scanner_cfg) if use_offDetector else (0.0, 0.0)
+    if not use_offDetector and np.any(np.asarray(scanner_cfg.get("offDetector", [0.0, 0.0]), np.float64) != 0.0):
+        warnings.warn("fdk: the scanner's offDetector is not zero and is ignored (the volume is reconstructed as if the "
+                      "detector were centred); pass use_offDetector=True to use it", stacklevel=2)
+    if not (math.isfinite(t_u) and math.isfinite(t_v)):
+        raise ValueError(f"fdk: offDetector must be finite, got {scanner_cfg.get('offDetector')}")
+    if short_scan and t_u != 0.0:
+        raise ValueError(f"fdk short scan: the detector has a horizontal offset of {t_u:g} pixels; Parker weights assume "
+                         "that each ray's conjugate is on the detector, so a short scan allows a vertical offset only")
+    if half_fan:
+        check_half_fan_shift(t_u, int(scanner_cfg["nDetector"][1]))
+        arc = scan_arc(angles)
+        if arc < 2.0 * math.pi - ARC_TOLERANCE:
+            raise ValueError(f"fdk half fan: the views cover an arc of {math.degrees(arc):.2f} degrees; half-fan "
+                             "weights need a full circle")
     if not isinstance(projections, torch.Tensor) or projections.device.type != "cuda":
         raise RuntimeError("fdk: projections must be a CUDA tensor (this build has no CPU fallback; "
                            f"got {getattr(projections, 'device', type(projections))})")
@@ -80,7 +148,7 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool =
         raise ValueError(f"fdk: projections are {H}x{W}, scanner nDetector is {list(scanner_cfg['nDetector'])}")
     if N == 0:
         raise ValueError("fdk: no projections")
-    views = [make_view(scanner_cfg, float(a)) for a in angles]
+    views = [make_view(scanner_cfg, float(a), use_offDetector) for a in angles]
     mode = views[0].mode
     if short_scan:
         view_weights, arc = short_scan_views(angles, mode, float(views[0].tanfovx))
@@ -99,11 +167,17 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool =
         stream = torch.cuda.current_stream(dev).cuda_stream
         tail = (float(views[0].tanfovx), float(views[0].tanfovy), int(mode), float(scanner_cfg["DSO"]), nx, ny, nz, sx,
                 sy, sz, cx, cy, cz, vol.data_ptr(), scratch.data_ptr(), nbytes)
+        if use_offDetector:
+            tail = tail[:3] + (t_u, t_v) + tail[3:]
         if short_scan:
             vw = torch.from_numpy(view_weights.astype(np.float32)).to(dev, non_blocking=False)
-            name = "r2x_fdk_short_scan"
-            rc = lib.r2x_fdk_short_scan(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), vw.data_ptr(),
-                                        float(arc), *tail)
+            name = "r2x_fdk_short_scan_shifted" if use_offDetector else "r2x_fdk_short_scan"
+            rc = getattr(lib, name)(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), vw.data_ptr(),
+                                    float(arc), *tail)
+        elif use_offDetector:
+            name = "r2x_fdk_shifted"
+            rc = lib.r2x_fdk_shifted(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), *tail[:5],
+                                     int(half_fan), *tail[5:])
         else:
             name = "r2x_fdk"
             rc = lib.r2x_fdk(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), *tail)

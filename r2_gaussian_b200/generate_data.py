@@ -1,7 +1,7 @@
 """Synthetic CT scene from a volume -- the reference's `data_generator/synthetic_dataset/generate_data.py`.
 
     python -m r2_gaussian_b200.generate_data --vol X.npy --scanner cone_beam.yml --output DIR
-        [--n_train 50] [--n_test 100] [--seed 0]
+        [--n_train 50] [--n_test 100] [--seed 0] [--use_offDetector]
 
 Reads the scanner configuration (the reference's yml format), projects the volume on the GPU with
 `projector.project` (the reference uses TIGRE's `Ax`) at the train angles linspace(0, totalAngle, n_train + 1)[:-1]
@@ -11,7 +11,12 @@ the configuration asks for it, and writes `<output>/<volume name>_<mode>/` (`met
 
 Differences from the reference: the noise and the test angles come from one `numpy.random.RandomState(--seed)`, drawn
 in the reference's order (train noise first, then test angles), where the reference uses numpy's unseeded global
-generator; the projector is defined by render()'s geometry, not bit-identical to TIGRE's; `offDetector` must be zero.
+generator; the projector is defined by render()'s geometry, not bit-identical to TIGRE's.  A scanner whose
+`offDetector` is not zero is refused unless `--use_offDetector` is given, which projects through the offset detector
+(`projector.project(..., use_offDetector=True)`, TIGRE's `geo.offDetector`; the convention is
+`scene.detector_shift`'s).  The reference's real-data generator takes the same offset on its command line; here it is
+the scanner file's `offDetector` ([u, v], in the file's units), written unchanged into `meta_data.json`, so the scene
+is then reconstructed and trained with the same switch.
 """
 from __future__ import annotations
 
@@ -84,6 +89,8 @@ def main(argv=None) -> str:
     ap.add_argument("--n_train", default=50, type=int, help="Number of projections for training.")
     ap.add_argument("--n_test", default=100, type=int, help="Number of projections for evaluation.")
     ap.add_argument("--seed", default=0, type=int, help="Seed of the noise and of the test angles.")
+    ap.add_argument("--use_offDetector", default=False, action="store_true",
+                    help="Project through the scanner's offDetector (else a non-zero offDetector is refused).")
     a = ap.parse_args(argv)
 
     import torch
@@ -92,12 +99,16 @@ def main(argv=None) -> str:
     from .dataset import scale_scanner, write_blender
     from .projector import project
 
+    with open(a.scanner) as f:
+        cfg = yaml.safe_load(f)
+    off = [float(v) for v in cfg.get("offDetector", [0.0, 0.0])]
+    if any(v != 0.0 for v in off) and not a.use_offDetector:
+        raise SystemExit(f"the scanner's offDetector is {off}: pass --use_offDetector to project through the offset "
+                         "detector (and use it again to reconstruct and train on the scene)")
     if not torch.cuda.is_available():
         raise SystemExit("generate_data needs a CUDA device: the projector runs on the GPU and has no CPU fallback")
     if a.n_train < 1 or a.n_test < 1:
         raise SystemExit("--n_train and --n_test must be at least 1")
-    with open(a.scanner) as f:
-        cfg = yaml.safe_load(f)
     vol_name = os.path.basename(a.vol)[:-4]
     case_name = f"{vol_name}_{cfg['mode']}"
     print(f"Generate data for case {case_name}")
@@ -110,11 +121,11 @@ def main(argv=None) -> str:
 
     dvol = torch.from_numpy(vol).cuda()
     angles_train = train_angles(cfg, a.n_train)
-    projs_train = (project(dvol, angles_train, scaled) / scene_scale).cpu().numpy()
+    projs_train = (project(dvol, angles_train, scaled, a.use_offDetector) / scene_scale).cpu().numpy()
     if cfg.get("noise", False):
         projs_train = add_noise(projs_train, cfg["possion_noise"], cfg["gaussian_noise"], rng)
     angles_test = draw_test_angles(cfg, a.n_test, rng)
-    projs_test = (project(dvol, angles_test, scaled) / scene_scale).cpu().numpy()
+    projs_test = (project(dvol, angles_test, scaled, a.use_offDetector) / scene_scale).cpu().numpy()
 
     case_path = os.path.join(a.output, case_name)
     write_blender(case_path, cfg, list(zip(angles_train, projs_train)), list(zip(angles_test, projs_test)), vol)

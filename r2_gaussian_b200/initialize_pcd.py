@@ -2,7 +2,7 @@
 
     python -m r2_gaussian_b200.initialize_pcd --data <scene dir | NAF pickle> [--output init.npy]
         [--recon_method random|fdk|cgls|fista_tv|volume] [--recon recon.npy] [--n_points 50000] [--density_thresh 0.05]
-        [--density_rescale 0.15] [--random_density_max 1.0] [--evaluate] [--short_scan]
+        [--density_rescale 0.15] [--random_density_max 1.0] [--evaluate] [--short_scan] [--use_offDetector [--half_fan]]
 
 `random` draws positions uniformly in the volume and densities in [0, random_density_max) with numpy's global
 generator seeded with 0, exactly like the reference.  `fdk` reconstructs the volume from the train views with the
@@ -10,7 +10,10 @@ GPU FDK of `r2_gaussian_b200.fdk` (the reference calls TIGRE's `algs.fdk`), then
 `density_thresh` and scales their densities by `density_rescale`, the reference's way; it needs a CUDA device and at
 least MIN_FDK_VIEWS train views.  `--short_scan` makes that FDK Parker-weighted (`fdk.fdk(short_scan=True)`), for a
 scan over less than 360 degrees: the plain FDK shades such a volume, which moves the `density_thresh` cut across it;
-the flag is refused with any other method.  `cgls` does the same with 60 CGLS iterations over the GPU projector pair
+the flag is refused with any other method.  `--use_offDetector` reconstructs through the scanner's offDetector
+(fdk, cgls and fista_tv; without it the projector pair refuses a non-zero offset and fdk ignores it), and `--half_fan`
+adds half-fan redundancy weights to that FDK for a full circle whose detector is shifted sideways (`fdk.fdk(...,
+half_fan=True)`; fdk only, not with --short_scan).  `cgls` does the same with 60 CGLS iterations over the GPU projector pair
 (`r2_gaussian_b200.recon`, the reference's `algs.cgls`); it also needs a CUDA device.  `fista_tv` does the same with
 the TV-regularised FISTA-TV of `r2_gaussian_b200.recon` at its default settings (CUDA as well).  `volume` samples a reconstruction made elsewhere (`--recon`, an .npy in the scene's
 voxel grid) the same way.  Writes [n_points, 4] = (x, y, z, density) in the scene's normalised [-1,1]^3 coordinates to
@@ -42,15 +45,17 @@ def _require_cuda_for(method: str):
                          "CPU fallback (use --recon_method random, or --recon_method volume --recon <vol.npy>)")
 
 
-def recon_train_views(info, method: str, short_scan: bool = False) -> np.ndarray:
-    """`recon.recon_volume(..., method, short_scan)` of the train views of a `read_scene` result, as a host float32
-    [nx, ny, nz] array."""
+def recon_train_views(info, method: str, short_scan: bool = False, use_offDetector: bool = False,
+                      half_fan: bool = False) -> np.ndarray:
+    """`recon.recon_volume(..., method, short_scan, use_offDetector, half_fan)` of the train views of a `read_scene`
+    result, as a host float32 [nx, ny, nz] array."""
     import torch
 
     from .recon import recon_volume
 
     projs = torch.from_numpy(np.stack([np.asarray(c.image, np.float32) for c in info.train_cameras])).cuda()
-    vol = recon_volume(projs, [c.angle for c in info.train_cameras], info.scanner_cfg, method, short_scan=short_scan)
+    vol = recon_volume(projs, [c.angle for c in info.train_cameras], info.scanner_cfg, method, short_scan=short_scan,
+                       use_offDetector=use_offDetector, half_fan=half_fan)
     return vol.cpu().numpy()
 
 
@@ -94,10 +99,25 @@ def main(argv=None) -> str:
                     help="Add this flag to evaluate quality (given GT volume, for debug only)")
     ap.add_argument("--short_scan", default=False, action="store_true",
                     help="with --recon_method fdk: Parker redundancy weights for a scan over less than 360 degrees")
+    ap.add_argument("--use_offDetector", default=False, action="store_true",
+                    help="with --recon_method fdk, cgls or fista_tv: reconstruct through the scanner's offDetector")
+    ap.add_argument("--half_fan", default=False, action="store_true",
+                    help="with --recon_method fdk and --use_offDetector: half-fan redundancy weights for a full circle "
+                         "with the detector shifted sideways")
     a = ap.parse_args(argv)
     if a.short_scan and a.recon_method != "fdk":
         raise SystemExit(f"--short_scan applies to --recon_method fdk only, not {a.recon_method}: the iterative methods "
                          "need no redundancy weights")
+    if a.half_fan and a.recon_method != "fdk":
+        raise SystemExit(f"--half_fan applies to --recon_method fdk only, not {a.recon_method}: the iterative methods "
+                         "need no redundancy weights")
+    if a.half_fan and not a.use_offDetector:
+        raise SystemExit("--half_fan needs --use_offDetector: the half-fan weights follow the detector offset")
+    if a.half_fan and a.short_scan:
+        raise SystemExit("--half_fan and --short_scan cannot be combined (half-fan weights need a full circle)")
+    if a.use_offDetector and a.recon_method not in ("fdk", "cgls", "fista_tv"):
+        raise SystemExit(f"--use_offDetector applies to --recon_method fdk, cgls or fista_tv, not {a.recon_method}: "
+                         "no projections are reconstructed")
     if a.recon_method in ("fdk", "cgls", "fista_tv"):
         _require_cuda_for(a.recon_method)
     np.random.seed(0)                                    # initialize_pcd.py:23
@@ -115,7 +135,8 @@ def main(argv=None) -> str:
         raise SystemExit(f"Initialization file {out} exists! Delete it first.")
     os.makedirs(os.path.dirname(out) or ".", exist_ok=True)
     if a.recon_method in ("fdk", "cgls", "fista_tv"):
-        recon = recon_train_views(info, a.recon_method, a.short_scan)  # no draws from numpy's generator before np.random.choice
+        # no draws from numpy's generator before np.random.choice
+        recon = recon_train_views(info, a.recon_method, a.short_scan, a.use_offDetector, a.half_fan)
     pts = init_point_cloud(info.scanner_cfg, a.n_points, recon=recon, density_thresh=a.density_thresh,
                            density_rescale=a.density_rescale, random_density_max=a.random_density_max)
     np.save(out, pts)

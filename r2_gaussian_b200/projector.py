@@ -4,6 +4,7 @@ transpose (r2x_volume_backproject), TIGRE's `Atb` inside the iterative reconstru
 
     projs = project(volume, angles, scanner_cfg)                 # [N, H, W], rows = v, columns = u
     vol = backproject(projs, angles, scanner_cfg)                # [nx, ny, nz] = A^T projs
+    projs = project(volume, angles, scanner_cfg, use_offDetector=True)   # through the scanner's offDetector
     vol, weight = backproject(projs, angles, scanner_cfg, weights=True)   # weight = A^T 1, from the same launch
 
 `volume` is a CUDA float32 [nx, ny, nz] tensor in the voxelizer's layout; `scanner_cfg` is the scaled dict of
@@ -11,7 +12,11 @@ transpose (r2x_volume_backproject), TIGRE's `Atb` inside the iterative reconstru
 training).  The per-view geometry is the rasterizer's (`scene.make_view`), so the projections agree with render() by
 construction.  Each pixel is the line integral of the volume's trilinear field, sampled every
 `accuracy * min(dVoxel)` along the ray (`accuracy` defaults to 0.5, as in the reference's scanner files); the exact
-definition is in include/r2x.h.  `backproject` sums every (ray, sample, voxel) triple `project` uses, with the same
+definition is in include/r2x.h.  A scanner whose `offDetector` is not zero is refused unless `use_offDetector=True`,
+which projects through the offset detector (r2x_volume_project_shifted / r2x_volume_backproject_shifted, TIGRE's
+`geo.offDetector`; the convention is `scene.detector_shift`'s) and matches a render() whose cameras carry the same
+offset (`dataset.Scene(use_offDetector=True)`, `scene.make_view(..., use_offDetector=True)`).
+`backproject` sums every (ray, sample, voxel) triple `project` uses, with the same
 weight, so <project(x), y> = <x, backproject(y)> up to float32 rounding.  Both run on the current stream; no CPU
 fallback.  `CTOperator` binds the pair to one set of angles for repeated use (the iterative solvers).
 """
@@ -21,19 +26,23 @@ import numpy as np
 import torch
 
 from ._lib import check, load
-from .scene import make_view
+from .scene import detector_shift, make_view
 
 DEFAULT_ACCURACY = 0.5
 
 
-def _check_geometry(what: str, scanner_cfg: dict) -> float:
+def _check_geometry(what: str, scanner_cfg: dict, use_offDetector: bool = False) -> float:
     """The scanner settings the projector pair supports; returns `accuracy`."""
     accuracy = float(scanner_cfg.get("accuracy", DEFAULT_ACCURACY))
     if not accuracy > 0.0:
         raise ValueError(f"{what}: accuracy must be > 0, got {accuracy}")
-    if np.any(np.asarray(scanner_cfg.get("offDetector", [0.0, 0.0]), np.float64) != 0.0):
-        raise ValueError(f"{what}: offDetector must be [0, 0]: render() has no detector offset, so such projections "
-                         "would not match training")
+    off = np.asarray(scanner_cfg.get("offDetector", [0.0, 0.0]), np.float64)
+    if use_offDetector:
+        if not np.all(np.isfinite(off)):
+            raise ValueError(f"{what}: offDetector must be finite, got {off.tolist()}")
+    elif np.any(off != 0.0):
+        raise ValueError(f"{what}: offDetector must be [0, 0] without use_offDetector=True: the centred projector would "
+                         "not match the scan, nor a render() of cameras without the offset")
     if scanner_cfg["mode"] != "cone" and not np.allclose(np.asarray(scanner_cfg["sDetector"], np.float64), 2.0,
                                                          rtol=1e-6, atol=0.0):
         raise ValueError(f"{what}: a parallel-beam detector must span the scene's [-1, 1] (scaled sDetector [2, 2]), "
@@ -41,19 +50,19 @@ def _check_geometry(what: str, scanner_cfg: dict) -> float:
     return accuracy
 
 
-def project(volume: torch.Tensor, angles, scanner_cfg: dict) -> torch.Tensor:
+def project(volume: torch.Tensor, angles, scanner_cfg: dict, use_offDetector: bool = False) -> torch.Tensor:
     nvox = tuple(int(v) for v in scanner_cfg["nVoxel"])
     if tuple(getattr(volume, "shape", ())) != nvox:
         raise ValueError(f"project: volume shape {tuple(getattr(volume, 'shape', ()))} is not the scanner's nVoxel "
                          f"{list(nvox)}")
-    accuracy = _check_geometry("project", scanner_cfg)
+    accuracy = _check_geometry("project", scanner_cfg, use_offDetector)
     if not isinstance(volume, torch.Tensor) or volume.device.type != "cuda":
         raise RuntimeError("project: volume must be a CUDA tensor (this build has no CPU fallback; "
                            f"got {getattr(volume, 'device', type(volume))})")
     angles =np.asarray(angles, dtype=np.float64).reshape(-1)
     if len(angles) == 0:
         raise ValueError("project: no angles")
-    views = [make_view(scanner_cfg, float(a)) for a in angles]
+    views = [make_view(scanner_cfg, float(a)) for a in angles]   # the viewmatrices: the offset is in the kernel's rays
     N, H, W = len(views), views[0].image_height, views[0].image_width
     sx, sy, sz = (float(v) for v in scanner_cfg["sVoxel"])
     cx, cy, cz = (float(v) for v in scanner_cfg["offOrigin"])
@@ -64,10 +73,16 @@ def project(volume: torch.Tensor, angles, scanner_cfg: dict) -> torch.Tensor:
         vol = volume.detach().to(torch.float32).contiguous()
         vm = torch.from_numpy(np.stack([v.viewmatrix.reshape(16) for v in views])).to(dev)
         out = torch.empty((N, H, W), dtype=torch.float32, device=dev)
-        rc = lib.r2x_volume_project(torch.cuda.current_stream(dev).cuda_stream, *nvox, vol.data_ptr(), sx, sy, sz,
-                                    cx, cy, cz, N, H, W, vm.data_ptr(), float(views[0].tanfovx),
-                                    float(views[0].tanfovy), int(views[0].mode), step, out.data_ptr())
-    check(rc, "r2x_volume_project")
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        head = (*nvox, vol.data_ptr(), sx, sy, sz, cx, cy, cz, N, H, W, vm.data_ptr(), float(views[0].tanfovx),
+                float(views[0].tanfovy), int(views[0].mode))
+        if use_offDetector:
+            name = "r2x_volume_project_shifted"
+            rc = lib.r2x_volume_project_shifted(stream, *head, *detector_shift(scanner_cfg), step, out.data_ptr())
+        else:
+            name = "r2x_volume_project"
+            rc = lib.r2x_volume_project(stream, *head, step, out.data_ptr())
+    check(rc, name)
     return out
 
 
@@ -75,14 +90,17 @@ class CTOperator:
     """A = r2x_volume_project and A^T = r2x_volume_backproject for fixed angles and scanner on one CUDA device, with the
     per-view matrices uploaded once.  `A(x, views)` projects a [nx, ny, nz] volume into the views `views` (a slice of
     the angle list) and `At(y, views, weights)` backprojects their [n, H, W] projections, returning (A_views^T y,
-    A_views^T 1) when `weights` is true.  Inputs are used as float32 contiguous tensors on the operator's device."""
+    A_views^T 1) when `weights` is true.  Inputs are used as float32 contiguous tensors on the operator's device.
+    `use_offDetector` binds the offset-detector pair (both directions, and the offset projmatrices the backprojector's
+    footprints need)."""
 
-    def __init__(self, angles, scanner_cfg: dict, device):
-        accuracy = _check_geometry("backproject", scanner_cfg)
+    def __init__(self, angles, scanner_cfg: dict, device, use_offDetector: bool = False):
+        accuracy = _check_geometry("backproject", scanner_cfg, use_offDetector)
         angles = np.asarray(angles, dtype=np.float64).reshape(-1)
         if len(angles) == 0:
             raise ValueError("backproject: no angles")
-        views = [make_view(scanner_cfg, float(a)) for a in angles]
+        views = [make_view(scanner_cfg, float(a), use_offDetector) for a in angles]
+        self.shift = detector_shift(scanner_cfg) if use_offDetector else None
         self.device = torch.device(device)
         self.nvox = tuple(int(v) for v in scanner_cfg["nVoxel"])
         self.N, self.H, self.W = len(views), views[0].image_height, views[0].image_width
@@ -107,11 +125,16 @@ class CTOperator:
             if tuple(vol.shape) != self.nvox:
                 raise ValueError(f"project: volume shape {tuple(vol.shape)} is not the scanner's nVoxel {list(self.nvox)}")
             out = torch.empty((n, self.H, self.W), dtype=torch.float32, device=self.device)
-            rc = self.lib.r2x_volume_project(torch.cuda.current_stream(self.device).cuda_stream, *self.nvox,
-                                             vol.data_ptr(), *self.size, *self.centre, n, self.H, self.W,
-                                             self.vm[v0].data_ptr(), self.tanx, self.tany, self.mode, self.step,
-                                             out.data_ptr())
-        check(rc, "r2x_volume_project")
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            head = (*self.nvox, vol.data_ptr(), *self.size, *self.centre, n, self.H, self.W, self.vm[v0].data_ptr(),
+                    self.tanx, self.tany, self.mode)
+            if self.shift is not None:
+                name = "r2x_volume_project_shifted"
+                rc = self.lib.r2x_volume_project_shifted(stream, *head, *self.shift, self.step, out.data_ptr())
+            else:
+                name = "r2x_volume_project"
+                rc = self.lib.r2x_volume_project(stream, *head, self.step, out.data_ptr())
+        check(rc, name)
         return out
 
     def At(self, y: torch.Tensor, views: slice = slice(None), weights: bool = False):
@@ -125,18 +148,25 @@ class CTOperator:
             wgt = torch.empty(self.nvox, dtype=torch.float32, device=self.device) if weights else None
             nbytes = int(self.lib.r2x_volume_backproject_scratch_bytes(n, self.H, self.W))
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            rc = self.lib.r2x_volume_backproject(torch.cuda.current_stream(self.device).cuda_stream, n, self.H, self.W,
-                                                 projs.data_ptr(), self.vm[v0].data_ptr(), self.pm[v0].data_ptr(),
-                                                 self.tanx, self.tany, self.mode, *self.nvox, *self.size, *self.centre,
-                                                 self.step, vol.data_ptr(), wgt.data_ptr() if weights else None,
-                                                 scratch.data_ptr(), nbytes)
-        check(rc, "r2x_volume_backproject")
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            head = (n, self.H, self.W, projs.data_ptr(), self.vm[v0].data_ptr(), self.pm[v0].data_ptr(), self.tanx,
+                    self.tany, self.mode)
+            tail = (*self.nvox, *self.size, *self.centre, self.step, vol.data_ptr(),
+                    wgt.data_ptr() if weights else None, scratch.data_ptr(), nbytes)
+            if self.shift is not None:
+                name = "r2x_volume_backproject_shifted"
+                rc = self.lib.r2x_volume_backproject_shifted(stream, *head, *self.shift, *tail)
+            else:
+                name = "r2x_volume_backproject"
+                rc = self.lib.r2x_volume_backproject(stream, *head, *tail)
+        check(rc, name)
         return (vol, wgt) if weights else vol
 
 
-def backproject(projections: torch.Tensor, angles, scanner_cfg: dict, weights: bool = False):
-    """A^T projections for the projector of `project(., angles, scanner_cfg)`: [nx, ny, nz], or (volume, A^T 1) when
-    `weights` is true."""
+def backproject(projections: torch.Tensor, angles, scanner_cfg: dict, weights: bool = False,
+                use_offDetector: bool = False):
+    """A^T projections for the projector of `project(., angles, scanner_cfg, use_offDetector)`: [nx, ny, nz], or
+    (volume, A^T 1) when `weights` is true."""
     shape = tuple(getattr(projections, "shape", ()))
     if len(shape) != 3:
         raise ValueError(f"backproject: expected projections of shape [N, H, W], got {shape}")
@@ -146,8 +176,8 @@ def backproject(projections: torch.Tensor, angles, scanner_cfg: dict, weights: b
     det = (int(scanner_cfg["nDetector"][0]), int(scanner_cfg["nDetector"][1]))
     if shape[1:] != det:
         raise ValueError(f"backproject: projections are {shape[1]}x{shape[2]}, scanner nDetector is {list(det)}")
-    _check_geometry("backproject", scanner_cfg)
+    _check_geometry("backproject", scanner_cfg, use_offDetector)
     if not isinstance(projections, torch.Tensor) or projections.device.type != "cuda":
         raise RuntimeError("backproject: projections must be a CUDA tensor (this build has no CPU fallback; "
                            f"got {getattr(projections, 'device', type(projections))})")
-    return CTOperator(angles, scanner_cfg, projections.device).At(projections, slice(None), weights)
+    return CTOperator(angles, scanner_cfg, projections.device, use_offDetector).At(projections, slice(None), weights)

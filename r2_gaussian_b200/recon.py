@@ -48,6 +48,7 @@ Parity with TIGRE's binaries is not pinned (as for FDK and the projector).  ASD-
 `fista_tv` is the TV-regularised method this project offers.
 
     python -m r2_gaussian_b200.recon -s <scene> -m <output> [--methods fdk,sart,cgls] [--short_scan]
+        [--use_offDetector [--half_fan]]
 
 mirrors `scripts/run_traditional_methods.py`: it reconstructs the scene's train views with each method, scores the
 volume against `vol_gt` with `metrics.metric_vol` and writes, per method, `<output>/<method>/ct_gt.npy`, `ct_pred.npy`,
@@ -56,7 +57,11 @@ also `short_scan: true`) and the test views
 `projs/{i:05d}_render.npy` (projections of the reconstruction) and `projs/{i:05d}_gt.npy`, plus `<output>/eval_3d.yml`
 keyed by method.  PNG slices and projections are not written (matplotlib is not a dependency of this project).
 `--short_scan` reconstructs fdk with Parker redundancy weights (`fdk.fdk(short_scan=True)`), for scenes whose train
-views cover less than a full circle; it is refused when --methods has no fdk.
+views cover less than a full circle; it is refused when --methods has no fdk.  `--use_offDetector` reconstructs and
+reprojects every method through the scanner's offDetector (without it a non-zero offset is refused by the projector
+pair and ignored by fdk); `--half_fan` (with it, fdk only, not with --short_scan) adds half-fan redundancy weights for
+a full circle whose detector is shifted sideways.  The reports add `half_fan: true` / `use_offDetector: true` only when
+those flags are on.
 """
 from __future__ import annotations
 
@@ -179,58 +184,63 @@ def fista_tv_solve(b: torch.Tensor, A, At, shape, niter: int, lmbda: float, tvit
     return x_prev, history
 
 
-def _operator(projs, angles, scanner_cfg):
+def _operator(projs, angles, scanner_cfg, use_offDetector: bool = False):
     from .projector import CTOperator
 
     if not isinstance(projs, torch.Tensor) or projs.device.type != "cuda":
         raise RuntimeError("recon: projections must be a CUDA tensor (this build has no CPU fallback; "
                            f"got {getattr(projs, 'device', type(projs))})")
-    op = CTOperator(angles, scanner_cfg, projs.device)
+    op = CTOperator(angles, scanner_cfg, projs.device, use_offDetector)
     b = projs.detach().to(torch.float32).contiguous()
     if tuple(b.shape) != (op.N, op.H, op.W):
         raise ValueError(f"recon: projections {list(b.shape)} do not match {op.N} angles of {op.H}x{op.W} pixels")
     return op, b
 
 
-def cgls(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = CGLS_NITER):
+def cgls(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = CGLS_NITER, use_offDetector: bool = False):
     """CGLS on the GPU projector pair; returns (volume, l2 per iteration)."""
-    op, b = _operator(projs, angles, scanner_cfg)
+    op, b = _operator(projs, angles, scanner_cfg, use_offDetector)
     return cgls_solve(b, op.A, op.At, niter)
 
 
 def sart(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = SART_NITER, lmbda: float = 1.0,
-         lmbda_red: float = 0.999, blocksize: int = 1, nonneg: bool = True) -> torch.Tensor:
+         lmbda_red: float = 0.999, blocksize: int = 1, nonneg: bool = True,
+         use_offDetector: bool = False) -> torch.Tensor:
     """SART (blocksize 1) or OS-SART on the GPU projector pair."""
-    op, b = _operator(projs, angles, scanner_cfg)
+    op, b = _operator(projs, angles, scanner_cfg, use_offDetector)
     return sart_solve(b, op.A, op.At, op.nvox, niter, lmbda, lmbda_red, blocksize, nonneg)
 
 
 def fista_tv(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = FISTA_NITER, lmbda: float = FISTA_LAMBDA,
-             tviter: int = FISTA_TVITER, nonneg: bool = True, L=None):
+             tviter: int = FISTA_TVITER, nonneg: bool = True, L=None, use_offDetector: bool = False):
     """FISTA-TV on the GPU projector pair and the GPU TV prox; returns (volume, history)."""
     _check_fista(niter, lmbda, tviter, L)
-    op, b = _operator(projs, angles, scanner_cfg)
+    op, b = _operator(projs, angles, scanner_cfg, use_offDetector)
     return fista_tv_solve(b, op.A, op.At, op.nvox, niter, lmbda, tviter, L, nonneg)
 
 
-def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, short_scan: bool = False) -> torch.Tensor:
+def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, short_scan: bool = False,
+                 use_offDetector: bool = False, half_fan: bool = False) -> torch.Tensor:
     """The reconstructions of ct_utils.recon_volume / run_ct_recon_algs with their iteration counts.  `short_scan`
-    selects the Parker-weighted FDK and applies to method fdk only."""
-    if short_scan and method != "fdk":
-        raise ValueError(f"recon_volume: short_scan applies to fdk only, not {method!r} (the iterative methods need no "
-                         "redundancy weights)")
+    selects the Parker-weighted FDK and `half_fan` the half-fan-weighted one; both apply to method fdk only.
+    `use_offDetector` reconstructs through the scanner's offDetector (every method)."""
+    for flag, on in (("short_scan", short_scan), ("half_fan", half_fan)):
+        if on and method != "fdk":
+            raise ValueError(f"recon_volume: {flag} applies to fdk only, not {method!r} (the iterative methods need no "
+                             "redundancy weights)")
+    off = use_offDetector
     if method == "fdk":
         from .fdk import fdk
 
-        return fdk(projs, angles, scanner_cfg, short_scan=short_scan)
+        return fdk(projs, angles, scanner_cfg, short_scan=short_scan, use_offDetector=off, half_fan=half_fan)
     if method == "cgls":
-        return cgls(projs, angles, scanner_cfg, CGLS_NITER)[0]
+        return cgls(projs, angles, scanner_cfg, CGLS_NITER, use_offDetector=off)[0]
     if method == "sart":
-        return sart(projs, angles, scanner_cfg, SART_NITER)
+        return sart(projs, angles, scanner_cfg, SART_NITER, use_offDetector=off)
     if method == "ossart":
-        return sart(projs, angles, scanner_cfg, SART_NITER, blocksize=OSSART_BLOCKSIZE)
+        return sart(projs, angles, scanner_cfg, SART_NITER, blocksize=OSSART_BLOCKSIZE, use_offDetector=off)
     if method == "fista_tv":
-        return fista_tv(projs, angles, scanner_cfg)[0]
+        return fista_tv(projs, angles, scanner_cfg, use_offDetector=off)[0]
     raise ValueError(f"recon_volume: unknown method {method!r} (supported: {', '.join(METHODS)})")
 
 
@@ -254,11 +264,23 @@ def main(argv=None) -> dict:
     ap.add_argument("--methods", default="fdk,sart,cgls", help=f"comma-separated subset of {','.join(METHODS)}")
     ap.add_argument("--short_scan", default=False, action="store_true",
                     help="reconstruct fdk with Parker redundancy weights (a scan over less than 360 degrees)")
+    ap.add_argument("--use_offDetector", default=False, action="store_true",
+                    help="reconstruct and reproject through the scanner's offDetector (every method)")
+    ap.add_argument("--half_fan", default=False, action="store_true",
+                    help="with --use_offDetector: reconstruct fdk with half-fan redundancy weights (a full circle with "
+                         "the detector shifted sideways)")
     a = ap.parse_args(argv)
     methods = _parse_methods(a.methods)
     if a.short_scan and "fdk" not in methods:
         raise SystemExit("--short_scan applies to the fdk method, which --methods does not include (the iterative "
                          "methods need no redundancy weights)")
+    if a.half_fan and "fdk" not in methods:
+        raise SystemExit("--half_fan applies to the fdk method, which --methods does not include (the iterative "
+                         "methods need no redundancy weights)")
+    if a.half_fan and not a.use_offDetector:
+        raise SystemExit("--half_fan needs --use_offDetector: the half-fan weights follow the detector offset")
+    if a.half_fan and a.short_scan:
+        raise SystemExit("--half_fan and --short_scan cannot be combined (half-fan weights need a full circle)")
     if not torch.cuda.is_available():
         raise SystemExit("the reconstructions need a CUDA device: they run on the GPU and have no CPU fallback")
     import yaml
@@ -283,7 +305,9 @@ def main(argv=None) -> dict:
         torch.cuda.synchronize()
         t0 = time.time()
         short_scan = a.short_scan and method == "fdk"
-        pred = recon_volume(projs_train, train_angles, cfg, method, short_scan=short_scan)
+        half_fan = a.half_fan and method == "fdk"
+        pred = recon_volume(projs_train, train_angles, cfg, method, short_scan=short_scan,
+                            use_offDetector=a.use_offDetector, half_fan=half_fan)
         torch.cuda.synchronize()
         duration = time.time() - t0
         ct_pred = pred.cpu().numpy()
@@ -296,10 +320,14 @@ def main(argv=None) -> dict:
                   "duration (sec)": duration, "duration (min)": duration / 60}
         if short_scan:
             report["short_scan"] = True
+        if half_fan:
+            report["half_fan"] = True
+        if a.use_offDetector:
+            report["use_offDetector"] = True
         with open(os.path.join(save, "eval_3d.yml"), "w") as f:
             yaml.dump(report, f, default_flow_style=False, sort_keys=False)
         if test_angles:
-            render = project(pred, test_angles, cfg).cpu().numpy()
+            render = project(pred, test_angles, cfg, use_offDetector=a.use_offDetector).cpu().numpy()
             for i, cam in enumerate(info.test_cameras):
                 np.save(os.path.join(save, "projs", f"{i:05d}_render.npy"), render[i])
                 np.save(os.path.join(save, "projs", f"{i:05d}_gt.npy"), np.asarray(cam.image, np.float32))

@@ -68,6 +68,43 @@ def projection_matrix(fovx: float, fovy: float, mode: int) -> np.ndarray:
     return P
 
 
+def detector_shift(scanner_cfg: dict) -> tuple[float, float]:
+    """(t_u, t_v): the scanner's `offDetector` in detector pixels, t_u = offDetector[0] / dDetector_u and
+    t_v = offDetector[1] / dDetector_v with dDetector_u = sDetector[1] / nDetector[1], dDetector_v = sDetector[0] /
+    nDetector[0] (scanner files store nDetector / sDetector as [v, u] but offDetector as [u, v]; only ratios are used,
+    so any consistent units do).  A missing offDetector is (0, 0).
+
+    Convention: image pixel (row r, column c) sees the ray that the centred detector has at fractional pixel
+    (r - t_v, c + t_u).  In ndc the pixel centre (2c + 1) / W - 1 gains 2 t_u / W and the row's (2r + 1) / H - 1 loses
+    2 t_v / H; in the camera intrinsics the x row of the projection matrix (math sense) gains -(2 t_u / W) times its w
+    row and the y row +(2 t_v / H) times it (`shifted_projection_matrix`).
+
+    Derivation.  TIGRE (which the reference hands `geo.offDetector = [offDetector[1], offDetector[0]]`,
+    r2_gaussian/utils/ct_utils.py::get_geometry_tigre) places detector column iu at
+    u = dDetector_u (iu - n_u / 2 + 0.5) + offDetector_u, and image columns run along u: column c holds the ray of the
+    centred detector's column c + t_u.  This is the horizontal convention of `detector.py`, with
+    `DetectorOffset` s = -t_u (offDetector[0] = -s dDetector_u).  Row iv sits at v = dDetector_v (iv - n_v / 2 + 0.5) +
+    offDetector_v, and the reference hands TIGRE `projs[:, ::-1, :]`, so image row r is iv = n_v - 1 - r: row r holds
+    the ray of the centred detector's row r - t_v.  The vertical sign rests on that flip and has not been checked
+    against TIGRE itself."""
+    off = scanner_cfg.get("offDetector", [0.0, 0.0])
+    du = float(scanner_cfg["sDetector"][1]) / float(scanner_cfg["nDetector"][1])
+    dv = float(scanner_cfg["sDetector"][0]) / float(scanner_cfg["nDetector"][0])
+    return float(off[0]) / du, float(off[1]) / dv
+
+
+def shifted_projection_matrix(P: np.ndarray, t_u: float, t_v: float, W: int, H: int) -> np.ndarray:
+    """P' (math sense, float32) of a detector offset by (t_u, t_v) pixels: the x row gains -(2 t_u / W) times the w row
+    and the y row +(2 t_v / H) times it, in float64 rounded once.  Cone beam changes P[0,2] and P[1,2] (w row
+    (0, 0, 1, 0)), parallel beam P[0,3] and P[1,3] (P = I).  Zero shifts return P unchanged."""
+    if t_u == 0.0 and t_v == 0.0:
+        return P
+    Q = np.asarray(P, np.float64).copy()
+    Q[0] -= (2.0 * t_u / W) * Q[3]
+    Q[1] += (2.0 * t_v / H) * Q[3]
+    return Q.astype(np.float32)
+
+
 @dataclass
 class View:
     """One projection geometry in the layout the rasterizer expects."""
@@ -84,7 +121,10 @@ class View:
     FoVy: float = 0.0
 
 
-def make_view(scanner: dict, angle: float) -> View:
+def make_view(scanner: dict, angle: float, use_offDetector: bool = False) -> View:
+    """The view at `angle`.  `use_offDetector` puts the scanner's offDetector into the projection matrix
+    (`detector_shift`, `shifted_projection_matrix`); off, or with a zero offset, the view is bit for bit the centred
+    one."""
     mode = MODE_CONE if scanner["mode"] == "cone" else MODE_PARALLEL
     c2w = angle2pose(scanner["DSO"], angle)
     w2c = np.linalg.inv(c2w)
@@ -98,7 +138,11 @@ def make_view(scanner: dict, angle: float) -> View:
     fovx = math.atan2(scanner["sDetector"][1] / 2, scanner["DSD"]) * 2
     fovy = math.atan2(scanner["sDetector"][0] / 2, scanner["DSD"]) * 2
     view_t = np.ascontiguousarray(Rt.T.astype(np.float32))
-    proj_t = np.ascontiguousarray(projection_matrix(fovx, fovy, mode).T.astype(np.float32))
+    P = projection_matrix(fovx, fovy, mode)
+    if use_offDetector:
+        P = shifted_projection_matrix(P, *detector_shift(scanner), int(scanner["nDetector"][1]),
+                                      int(scanner["nDetector"][0]))
+    proj_t = np.ascontiguousarray(P.T.astype(np.float32))
     full = (view_t.astype(np.float32) @ proj_t.astype(np.float32)).astype(np.float32)
     campos = np.linalg.inv(view_t.astype(np.float64))[3, :3].astype(np.float32)
     if mode == MODE_PARALLEL:

@@ -34,6 +34,14 @@ pixels; `DetectorParams` learning rates, log-linear over `--iterations`) with it
 and at any --batch_size; it steps wherever the poses would.  Train and test views are evaluated with the offset (it is a
 property of the scanner), each save writes `detector_offset.yml` and checkpoints carry the offset and its Adam state.
 It is refused with --pose_refine and with Gaussian sharding.  Without the switch nothing changes.
+
+`--use_offDetector` trains through the scanner's offDetector: every train and test camera carries it in its
+projection_matrix (`dataset.Scene(use_offDetector=True)`, `scene.detector_shift`), so pose corrections, batched views
+and the native step see it too.  With `--detector_offset_refine` the learned offset acts on top of the file's, and
+`detector_offset.yml` also reports the total `offDetector_u` = offDetector[0] - offset_px * dDetector_u in the scanner
+file's units.  The rasterizer clamps each Gaussian's EWA Jacobian at 1.3 tan_fov about the axis, as the reference does,
+so with an offset of more than 0.15 W a Gaussian whose centre projects beyond that clamp gets a clamped footprint.
+Without the switch the offset is ignored (the reference's render() has none) and nothing changes.
 """
 from __future__ import annotations
 
@@ -245,7 +253,7 @@ def render_batch(cams, gaussians: GaussianModel) -> dict:
 def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, testing_iterations=(),
              saving_iterations=(), checkpoint_iterations=(), checkpoint: str | None = None, init_points=None,
              log=print, pose_params: PoseParams | None = None, batch_size: int = 1,
-             detector_params: DetectorParams | None = None) -> dict:
+             detector_params: DetectorParams | None = None, use_offDetector: bool = False) -> dict:
     first_iter = 0
     refine = pose_params is not None and pose_params.pose_refine
     if refine and world_info()[1] > 1:
@@ -260,7 +268,7 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
     if why is not None:
         raise ValueError(why)
     scene = Scene(model.source_path, model.model_path, eval=model.eval, shuffle=False, device="cuda",
-                  data_device=model.data_device)
+                  data_device=model.data_device, use_offDetector=use_offDetector)
     cfg = scene.scanner_cfg
     if B > len(scene.getTrainCameras()):
         raise ValueError(f"--batch_size {B} exceeds the scene's {len(scene.getTrainCameras())} train views")
@@ -589,6 +597,10 @@ def save_detector_offset(scene: Scene, det, iteration: int):
     import yaml
     doc = {"offset_px": float(det.offset.detach()[0]), "offset_scene": det.scene_units(scene.scanner_cfg),
            "sign_convention": SIGN_CONVENTION}
+    if getattr(scene, "use_offDetector", False):
+        # the learned offset acts on top of the scanner file's: the total, back in the file's units
+        cfg = scene.scanner_cfg
+        doc["offDetector_u"] = (float(cfg.get("offDetector", [0.0, 0.0])[0]) - det.scene_units(cfg)) / scene.scene_scale
     with open(os.path.join(scene.model_path, f"point_cloud/iteration_{iteration}", "detector_offset.yml"), "w") as f:
         yaml.dump(doc, f, default_flow_style=False, sort_keys=False)
 
@@ -708,6 +720,8 @@ def parse_args(argv=None):
                     help="multi-GPU: sum partial images / volumes with the NVLink peer-memory kernel instead of NCCL")
     ap.add_argument("--batch_size", type=int, default=1,
                     help="train views per optimizer step (1 .. number of train views); schedules stay in steps")
+    ap.add_argument("--use_offDetector", action="store_true",
+                    help="train through the scanner's offDetector (every camera's projection matrix carries it)")
     a = ap.parse_args(argv)
     pick = lambda cls: cls(**{k: getattr(a, k) for k in cls.__dataclass_fields__})
     model, pipe, opt, pose = pick(ModelParams), pick(PipelineParams), pick(OptimizationParams), pick(PoseParams)
@@ -743,7 +757,8 @@ def main(argv=None):
                        {"test_iterations": a.test_iterations, "save_iterations": a.save_iterations,
                         "checkpoint_iterations": a.checkpoint_iterations, "start_checkpoint": a.start_checkpoint,
                         "quiet": False, "config": None, "detect_anomaly": False,
-                        **({"batch_size": a.batch_size} if a.batch_size > 1 else {})}, pose, a.detector_params)
+                        **({"batch_size": a.batch_size} if a.batch_size > 1 else {}),
+                        **({"use_offDetector": True} if a.use_offDetector else {})}, pose, a.detector_params)
     random.seed(a.seed), np.random.seed(a.seed), torch.manual_seed(a.seed)     # safe_state (`general_utils.py:61-63`)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if world > 1:                      # launched by torchrun: one process per GPU, Gaussians sharded by index
@@ -758,7 +773,7 @@ def main(argv=None):
             enable_peer_exchange(True)
     hist = training(model, opt, pipe, set(a.test_iterations) | {opt.iterations}, set(a.save_iterations),
                     set(a.checkpoint_iterations), a.start_checkpoint, pose_params=pose, batch_size=a.batch_size,
-                    detector_params=a.detector_params)
+                    detector_params=a.detector_params, use_offDetector=a.use_offDetector)
     final = hist["eval"].get(opt.iterations, {})
     if world > 1:
         import torch.distributed as dist
