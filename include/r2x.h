@@ -379,62 +379,57 @@ int r2x_gather_rows(void* stream, int ntensors, const r2x_gather_desc* descs, co
  *   3. voxel-driven backprojection: voxel centres center - s/2 + (i + 1/2) s/n, projected through projmatrix and the
  *      rasterizer's ndc -> pixel mapping, bilinear sample (0 outside the detector), weight U^2 with U = DSO / z_view
  *      (cone; 0 for z_view <= 0) or 1 (parallel); out_volume[nx,ny,nz] = (pi / N) * sum over views in index order.
- * r2x_fdk has no Parker weights: it reconstructs a cone-beam short scan as if it were a full one (as TIGRE's default
- * fdk); r2x_fdk_short_scan below weights a short scan.  Deterministic (no atomics).  `scratch` holds r2x_fdk_scratch_bytes(N, H, W) (the filtered views).  Asynchronous on
- * `stream`.  Limits: W <= 16384, N * H < 2^31, nx <= 262140, nz <= 524280. */
+ * Detector offset: shift_u, shift_v are TIGRE's `geo.offDetector` in pixels, t_u = offDetector[0] / dDetector_u and
+ * t_v = offDetector[1] / dDetector_v of the scanner file (r2_gaussian/utils/ct_utils.py::get_geometry_tigre;
+ * scene.detector_shift states the convention); 0, 0 for a centred detector.  Image pixel (row i, column j) holds the
+ * ray of the centred detector's fractional pixel (i - t_v, j + t_u), so step 1 takes its cosine weight at ndc
+ * ((2j+1)/W - 1 + 2 t_u/W, (2i+1)/H - 1 - 2 t_v/H); step 3 goes through the caller's projmatrices, which must be the
+ * offset ones (scene.make_view(..., use_offDetector=True)).  A zero offset gives the centred result bit for bit.
+ * weighting (the redundancy weight step 1 also applies; the plain FDK's is oracle/fdk_oracle.py):
+ *   R2X_FDK_PLAIN     none.  It reconstructs a cone-beam short scan as if it were a full one (as TIGRE's default fdk).
+ *   R2X_FDK_PARKER    a short scan (Parker 1982, in Silver 2000's overscan form; tests/fdk_short_scan_oracle.py): an arc
+ *                     B = arc with pi + 2 gamma_max <= B < 2 pi (gamma_max = atan(tan_fovx) for cone beam, 0 for
+ *                     parallel beam) measures some rays once and some twice.  P' = w(beta'_v, gamma_j) * dbeta_v * P,
+ *                     with gamma_j = -atan(ndc_x(j) tan_fovx) (cone; the detector's u axis runs along the rotation) or 0
+ *                     (parallel), delta = (B - pi) / 2 and the Parker weight w = sin^2(pi/4 beta' / (delta - gamma))
+ *                     for beta' < 2 (delta - gamma), 1 up to pi - 2 gamma, sin^2(pi/4 (B - beta') / (delta + gamma)) up
+ *                     to B, 0 beyond; step 3 sums with scale 1 instead of pi / N.  view_weights[N,2] (device) holds each
+ *                     view's (beta'_v, dbeta_v): its arc position from the start of the scan and its angular interval,
+ *                     as fdk.short_scan_views computes them in float64 (they are not read on the host, so their
+ *                     finiteness is the caller's).  Refuses N < 2, a NULL view_weights, B outside [pi + 2 gamma_max,
+ *                     2 pi) and shift_u != 0 (Parker weights assume each ray's conjugate is on the detector).
+ *   R2X_FDK_HALF_FAN  a full circle with the axis off the detector's centre (Wang 2002; tests/offset_detector_oracle.py;
+ *                     the caller checks the circle): P' = w(a_j) * P for the fan coordinate a_j = ndc_x(j) * (cone:
+ *                     tan_fovx; parallel: 1), with delta = (1 - 2|t_u|/W) * (tan_fovx or 1), sigma = sign(t_u) and
+ *                     w = 2 sin^2(pi/4 (1 + sigma a / delta)) for |a| <= delta, 2 for sigma a > delta; the scale stays
+ *                     pi / N.  Refuses unless 0 < |shift_u| < W/2.
+ * view_weights and arc are read for R2X_FDK_PARKER only.  Deterministic (no atomics).  `scratch` holds
+ * r2x_fdk_scratch_bytes(N, H, W) (the filtered views).  Asynchronous on `stream`.  Limits: W <= 16384, N * H < 2^31,
+ * nx <= 262140, nz <= 524280. */
+#define R2X_FDK_PLAIN 0
+#define R2X_FDK_PARKER 1
+#define R2X_FDK_HALF_FAN 2
 size_t r2x_fdk_scratch_bytes(int n_views, int H, int W);
 int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
-            const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float dso, int nx, int ny, int nz,
-            float sx, float sy, float sz, float cx, float cy, float cz, float* out_volume, void* scratch,
-            size_t scratch_bytes);
-/* The two stages of r2x_fdk on their own (measurement): filtered[N,H,W] = steps 1-2; out_volume = step 3 of it. */
+            const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
+            int weighting, const float* view_weights, float arc, float dso, int nx, int ny, int nz, float sx, float sy,
+            float sz, float cx, float cy, float cz, float* out_volume, void* scratch, size_t scratch_bytes);
+/* The two stages of r2x_fdk on their own (measurement; centred, R2X_FDK_PLAIN): filtered[N,H,W] = steps 1-2;
+ * out_volume = step 3 of it. */
 int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, float tan_fovx, float tan_fovy,
                    int mode, float dso, float* filtered);
 int r2x_fdk_backproject(void* stream, int n_views, int H, int W, const float* filtered, const float* viewmatrices,
                         const float* projmatrices, int mode, float dso, int nx, int ny, int nz, float sx, float sy,
                         float sz, float cx, float cy, float cz, float* out_volume);
-/* FDK of a short scan (Parker 1982, in Silver 2000's overscan form; the statement is tests/fdk_short_scan_oracle.py): an arc B
- * with pi + 2 gamma_max <= B < 2 pi (gamma_max = atan(tan_fovx) for cone beam, 0 for parallel beam) measures some rays
- * once and some twice.  Step 1 becomes P' = w(beta'_v, gamma_j) * dbeta_v * (cone: cosine weight) * P, with
- *   gamma_j = -atan(ndc_x(j) tan_fovx) (cone; the detector's u axis runs along the rotation) or 0 (parallel),
- *   delta = (B - pi) / 2 and the Parker weight w = sin^2(pi/4 beta' / (delta - gamma)) for beta' < 2 (delta - gamma),
- *   1 up to pi - 2 gamma, sin^2(pi/4 (B - beta') / (delta + gamma)) up to B, 0 beyond;
- * step 2 is unchanged and step 3 sums with scale 1 instead of pi / N.  view_weights[N,2] (device) holds each view's
- * (beta'_v, dbeta_v): its arc position from the start of the scan and its angular interval, as fdk.short_scan_views
- * computes them in float64 (they are not read on the host, so their finiteness is the caller's).  Same arguments,
- * scratch and limits as r2x_fdk otherwise; also checks N >= 2 and pi + 2 gamma_max <= B < 2 pi. */
-int r2x_fdk_short_scan(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
-                       const float* projmatrices, const float* view_weights, float arc, float tan_fovx, float tan_fovy,
-                       int mode, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
-                       float cz, float* out_volume, void* scratch, size_t scratch_bytes);
-/* FDK with the detector offset by (shift_u, shift_v) pixels: t_u = offDetector[0] / dDetector_u, t_v = offDetector[1] /
- * dDetector_v of the scanner file, replacing TIGRE's `geo.offDetector` (r2_gaussian/utils/ct_utils.py::get_geometry_tigre;
- * scene.detector_shift states the convention).  Image pixel (row i, column j) holds the ray of the centred detector's
- * fractional pixel (i - t_v, j + t_u), so step 1 takes its cosine weight at ndc ((2j+1)/W - 1 + 2 t_u/W,
- * (2i+1)/H - 1 - 2 t_v/H); step 2 is unchanged; step 3 is r2x_fdk's, through the caller's projmatrices, which must be
- * the offset ones (scene.make_view(..., use_offDetector=True)).  half_fan = 1 (a full circle with the axis off centre,
- * 0 < |t_u| < W/2; the caller checks the circle) also weights each pixel in step 1 by Wang's (2002) redundancy weight of
- * its fan coordinate a_j = ndc_x(j) * (cone: tan_fovx; parallel: 1): with delta = (1 - 2|t_u|/W) * (tan_fovx or 1) and
- * sigma = sign(t_u), w = 2 sin^2(pi/4 (1 + sigma a / delta)) for |a| <= delta, 2 for sigma a > delta; the scale stays
- * pi / N.  The statement is tests/offset_detector_oracle.py.  Same arguments, scratch and limits as r2x_fdk otherwise. */
-int r2x_fdk_shifted(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
-                    const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
-                    int half_fan, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
-                    float cz, float* out_volume, void* scratch, size_t scratch_bytes);
-/* r2x_fdk_short_scan with the detector offset vertically by shift_v pixels (as r2x_fdk_shifted); shift_u must be 0:
- * Parker weights assume each ray's conjugate is on the detector.  projmatrices must be the offset ones. */
-int r2x_fdk_short_scan_shifted(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
-                               const float* projmatrices, const float* view_weights, float arc, float tan_fovx,
-                               float tan_fovy, int mode, float shift_u, float shift_v, float dso, int nx, int ny, int nz,
-                               float sx, float sy, float sz, float cx, float cy, float cz, float* out_volume,
-                               void* scratch, size_t scratch_bytes);
 
 /* ---- forward projection of a voxel volume (synthetic projection data) --------------------------- */
 /* Replaces TIGRE's `Ax` (data_generator/synthetic_dataset/generate_data.py).  Lengths in the scene-scaled units of the
  * dataset readers.  volume[nx,ny,nz] (index x*ny*nz + y*nz + z) with size (sx,sy,sz) centred at (cx,cy,cz);
  * viewmatrices[N,16] are the rasterizer's per-view matrices, tan_fovx / tan_fovy the values render() passes (parallel
  * beam: 1); out_projs[N,H,W] (rows = v, columns = u).  For every detector pixel (row i, column j):
- *   ray    ndc = ((2j+1)/W - 1, (2i+1)/H - 1); cone beam: from the camera centre along camera-frame
+ *   ray    ndc = ((2j+1)/W - 1 + 2 shift_u/W, (2i+1)/H - 1 - 2 shift_v/H) in float64, where (shift_u, shift_v) is the
+ *          detector offset in pixels as for r2x_fdk (0, 0 when centred; zero shifts give the centred rays bit for bit;
+ *          finite); cone beam: from the camera centre along camera-frame
  *          (ndc_x tan_fovx, ndc_y tan_fovy, 1); parallel beam: from camera-frame (ndc_x, ndc_y, 0) along (0, 0, 1); both
  *          taken to world space by the rigid inverse of the viewmatrix; unit direction d, so t is a length.
  *   field  f = trilinear interpolation between the voxel centres c - s/2 + (i + 1/2) s/n, every lattice point outside
@@ -447,19 +442,15 @@ int r2x_fdk_short_scan_shifted(void* stream, int n_views, int H, int W, const fl
  * Limits: H <= 2097120 (grid.y), W and N up to INT_MAX (views are launched 65535 at a time), N*H*W indexed in 64 bits. */
 int r2x_volume_project(void* stream, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
                        float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
-                       float tan_fovx, float tan_fovy, int mode, float step, float* out_projs);
-/* r2x_volume_project with the detector offset by (shift_u, shift_v) pixels (TIGRE's `geo.offDetector`, as
- * r2x_fdk_shifted): pixel (i, j) takes the ray of ndc ((2j+1)/W - 1 + 2 shift_u/W, (2i+1)/H - 1 - 2 shift_v/H), computed
- * in the same float64 setup; everything else as r2x_volume_project.  Zero shifts give the same rays. */
-int r2x_volume_project_shifted(void* stream, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
-                               float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
-                               float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v, float step,
-                               float* out_projs);
+                       float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v, float step,
+                       float* out_projs);
 
 /* ---- matched backprojection: the transpose of r2x_volume_project (iterative reconstruction) ------------------- */
 /* Replaces TIGRE's `Atb` inside `algs.cgls` / `algs.sart` / `algs.ossart` (r2_gaussian/utils/ct_utils.py).  Same
  * geometry arguments and units as r2x_volume_project, plus the per-view projmatrices (the rasterizer's, as for r2x_fdk)
- * for each voxel's detector footprint.  projs[N,H,W] (rows = v, columns = u); out_volume / out_weight [nx,ny,nz]:
+ * for each voxel's detector footprint (with a detector offset the offset ones, scene.make_view(...,
+ * use_offDetector=True), so that the footprint covers the offset rays).  projs[N,H,W] (rows = v, columns = u);
+ * out_volume / out_weight [nx,ny,nz]:
  *   out_volume[x] = step * sum over views (index order) of sum over pixels of projs[v,i,j] * sum_{k in K} h_x(p_k)
  *   out_weight[x] = the same with projs = 1 (optional: NULL skips it)
  * where p_k = fmaf(k, s, g) is r2x_volume_project's own float32 index-space sample of pixel (i, j), K its own k range
@@ -471,17 +462,10 @@ int r2x_volume_project_shifted(void* stream, int nx, int ny, int nz, const float
  * Asynchronous on `stream`.  Limits: nx <= 65535, ny <= 262140, fewer than 2^24 samples per half ray. */
 size_t r2x_volume_backproject_scratch_bytes(int n_views, int H, int W);
 int r2x_volume_backproject(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
-                           const float* projmatrices, float tan_fovx, float tan_fovy, int mode, int nx, int ny, int nz,
-                           float sx, float sy, float sz, float cx, float cy, float cz, float step, float* out_volume,
-                           float* out_weight, void* scratch, size_t scratch_bytes);
-/* The exact transpose of r2x_volume_project_shifted (TIGRE's `Atb` with `geo.offDetector`): the samples are that
- * projector's; projmatrices must be the offset ones (scene.make_view(..., use_offDetector=True)) so that each voxel's
- * footprint covers the offset rays.  Otherwise as r2x_volume_backproject. */
-int r2x_volume_backproject_shifted(void* stream, int n_views, int H, int W, const float* projs,
-                                   const float* viewmatrices, const float* projmatrices, float tan_fovx, float tan_fovy,
-                                   int mode, float shift_u, float shift_v, int nx, int ny, int nz, float sx, float sy,
-                                   float sz, float cx, float cy, float cz, float step, float* out_volume,
-                                   float* out_weight, void* scratch, size_t scratch_bytes);
+                           const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u,
+                           float shift_v, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
+                           float cz, float step, float* out_volume, float* out_weight, void* scratch,
+                           size_t scratch_bytes);
 
 /* ---- isotropic total variation on a volume (FISTA-TV, r2_gaussian_b200/recon.py and tv.py) --------------------- */
 /* Volumes are float32 [nx,ny,nz] (z fastest).  grad x = forward differences along x, y, z, 0 across the last index;

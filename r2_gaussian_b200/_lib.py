@@ -88,23 +88,15 @@ PROTOTYPES = {
     "r2x_mask_select": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _sz]),
     "r2x_gather_rows": (_i, [_vp, _i, _vp, _vp, _ll]),
     "r2x_fdk_scratch_bytes": (_sz, [_i, _i, _i]),
-    "r2x_fdk": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _f, _i, _i, _i, _f, _f, _f, _f, _f, _f, _vp, _vp, _sz]),
+    "r2x_fdk": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _f, _f, _i, _vp, _f, _f, _i, _i, _i, _f, _f, _f, _f, _f,
+                     _f, _vp, _vp, _sz]),
     "r2x_fdk_filter": (_i, [_vp, _i, _i, _i, _vp, _f, _f, _i, _f, _vp]),
     "r2x_fdk_backproject": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _i, _f, _i, _i, _i, _f, _f, _f, _f, _f, _f, _vp]),
-    "r2x_fdk_short_scan": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _f, _f, _i, _f, _i, _i, _i, _f, _f, _f, _f, _f,
-                                _f, _vp, _vp, _sz]),
-    "r2x_fdk_shifted": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _f, _f, _i, _f, _i, _i, _i, _f, _f, _f, _f, _f,
-                             _f, _vp, _vp, _sz]),
-    "r2x_fdk_short_scan_shifted": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _f, _f, _i, _f, _f, _f, _i, _i, _i, _f,
-                                        _f, _f, _f, _f, _f, _vp, _vp, _sz]),
-    "r2x_volume_project": (_i, [_vp, _i, _i, _i, _vp, _f, _f, _f, _f, _f, _f, _i, _i, _i, _vp, _f, _f, _i, _f, _vp]),
-    "r2x_volume_project_shifted": (_i, [_vp, _i, _i, _i, _vp, _f, _f, _f, _f, _f, _f, _i, _i, _i, _vp, _f, _f, _i, _f,
-                                        _f, _f, _vp]),
+    "r2x_volume_project": (_i, [_vp, _i, _i, _i, _vp, _f, _f, _f, _f, _f, _f, _i, _i, _i, _vp, _f, _f, _i, _f, _f, _f,
+                                _vp]),
     "r2x_volume_backproject_scratch_bytes": (_sz, [_i, _i, _i]),
-    "r2x_volume_backproject": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _i, _i, _i, _f, _f, _f, _f, _f, _f, _f,
-                                    _vp, _vp, _vp, _sz]),
-    "r2x_volume_backproject_shifted": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _f, _f, _i, _i, _i, _f, _f, _f,
-                                            _f, _f, _f, _f, _vp, _vp, _vp, _sz]),
+    "r2x_volume_backproject": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _f, _f, _i, _i, _i, _f, _f, _f, _f, _f,
+                                    _f, _f, _vp, _vp, _vp, _sz]),
     "r2x_tv_prox_scratch_bytes": (_sz, [_i, _i, _i]),
     "r2x_tv_prox": (_i, [_vp, _i, _i, _i, _vp, _f, _i, _i, _vp, _vp, _sz]),
     "r2x_tv_value_scratch_bytes": (_sz, [_i, _i, _i]),

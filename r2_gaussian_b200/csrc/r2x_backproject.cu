@@ -7,10 +7,9 @@
 //   backproject_rays_kernel    one thread per detector pixel of a chunk of views: the projector's per-ray setup
 //                              (project_ray_setup, r2x_project.cuh, the same inlined code) written as two float4,
 //                              (g_x, g_y, g_z, k0) and (s_x, s_y, s_z, k1), so the gather sees the projector's float32
-//                              sample positions p_k = fma(k, s, g) and k range by construction.
-//   backproject_rays_shift_kernel  the same table for a detector offset by (t_u, t_v) pixels (project_ray_setup<CONE,
-//                              true>); the gather below is unchanged and finds each voxel's footprint through the
-//                              caller's offset projmatrices, so it stays the transpose of r2x_volume_project_shifted.
+//                              sample positions p_k = fma(k, s, g) and k range by construction, for a detector offset
+//                              by (t_u, t_v) pixels as well; the gather below finds each voxel's footprint through the
+//                              caller's offset projmatrices, so it stays the transpose of the offset projector.
 //   volume_backproject_kernel  a thread owns one voxel x; a CTA is 32 voxels along z (the lanes) x 4 along y.  Per view
 //                              (index order; projmatrix / viewmatrix rows staged in shared memory per chunk) the 8
 //                              corners of x's open support box (x-1, x+1)^3 go through projmatrix and the rasterizer's
@@ -45,18 +44,17 @@ size_t backproject_scratch_bytes(int N, int H, int W) {
     return bp_al256((size_t)(N < BP_CHUNK ? N : BP_CHUNK) * H * W * 2 * sizeof(float4)) + 256;
 }
 
-// The ray-table kernel's body; SHIFT selects the offset-detector rays (project_ray_setup), tu / tv unused without it.
-template <bool CONE, bool SHIFT>
-__device__ __forceinline__ void backproject_rays_body(
+template <bool CONE>
+__global__ void __launch_bounds__(BP_RAYS_THREADS) backproject_rays_kernel(
     int H, int W, const float* __restrict__ viewm, int nx, int ny, int nz, float sx, float sy, float sz, float cx,
-    float cy, float cz, float tanx, float tany, float step, float tu, float tv, float4* __restrict__ rays) {
+    float cy, float cz, float tanx, float tany, float step, ProjShift shift, float4* __restrict__ rays) {
     const long long p = (long long)blockIdx.x * BP_RAYS_THREADS + threadIdx.x;
     const long long HW = (long long)H * W;
     if (p >= HW) return;
     const int view = blockIdx.y;
     const int v = (int)(p / W), u = (int)(p % W);
-    const ProjRay r = project_ray_setup<CONE, SHIFT>(viewm, view, u, v, H, W, nx, ny, nz, sx, sy, sz, cx, cy, cz, tanx,
-                                                     tany, step, tu, tv);
+    const ProjRay r = project_ray_setup<CONE>(viewm, view, u, v, H, W, nx, ny, nz, sx, sy, sz, cx, cy, cz, tanx, tany,
+                                              step, shift);
     long long k0 = r.k0, k1 = r.k1;
     if (k0 > k1) {
         k0 = 1; k1 = 0;                                                   // the ray misses the box
@@ -67,22 +65,6 @@ __device__ __forceinline__ void backproject_rays_body(
     float4* o = rays + 2 * ((size_t)view * HW + p);
     o[0] = make_float4(r.gx, r.gy, r.gz, __int_as_float((int)k0));
     o[1] = make_float4(r.sx, r.sy, r.sz, __int_as_float((int)k1));
-}
-
-template <bool CONE>
-__global__ void __launch_bounds__(BP_RAYS_THREADS) backproject_rays_kernel(
-    int H, int W, const float* __restrict__ viewm, int nx, int ny, int nz, float sx, float sy, float sz, float cx,
-    float cy, float cz, float tanx, float tany, float step, float4* __restrict__ rays) {
-    backproject_rays_body<CONE, false>(H, W, viewm, nx, ny, nz, sx, sy, sz, cx, cy, cz, tanx, tany, step, 0.0f, 0.0f,
-                                       rays);
-}
-
-// The ray table of a detector offset by (tu, tv) pixels (r2x_volume_backproject_shifted).
-template <bool CONE>
-__global__ void __launch_bounds__(BP_RAYS_THREADS) backproject_rays_shift_kernel(
-    int H, int W, const float* __restrict__ viewm, int nx, int ny, int nz, float sx, float sy, float sz, float cx,
-    float cy, float cz, float tanx, float tany, float step, float tu, float tv, float4* __restrict__ rays) {
-    backproject_rays_body<CONE, true>(H, W, viewm, nx, ny, nz, sx, sy, sz, cx, cy, cz, tanx, tany, step, tu, tv, rays);
 }
 
 // Cut [lo, hi] to the k whose sample fma(k, s, g) on this axis can lie in (c - 1, c + 1); false if none can.  The
@@ -222,10 +204,10 @@ static int backproject_validate(int N, int H, int W, const float* projs, const f
     return 0;
 }
 
-template <bool CONE, bool SHIFT>
+template <bool CONE>
 static int backproject_launch(cudaStream_t st, int N, int H, int W, const float* projs, const float* viewm,
                               const float* projm, float tanx, float tany, int nx, int ny, int nz, float sx, float sy,
-                              float sz, float cx, float cy, float cz, float step, float tu, float tv, float* out,
+                              float sz, float cx, float cy, float cz, float step, ProjShift shift, float* out,
                               float* wgt, float4* rays) {
     const float dx = sx / nx, dy = sy / ny, dz = sz / nz;
     const float ox = cx - 0.5f * sx + 0.5f * dx, oy = cy - 0.5f * sy + 0.5f * dy, oz = cz - 0.5f * sz + 0.5f * dz;
@@ -235,12 +217,8 @@ static int backproject_launch(cudaStream_t st, int N, int H, int W, const float*
         const int nc = min(BP_CHUNK, N - v0);
         const float* vm = viewm + (size_t)v0 * 16;
         const dim3 rgrid((unsigned)((HW + BP_RAYS_THREADS - 1) / BP_RAYS_THREADS), nc);
-        if (SHIFT)
-            backproject_rays_shift_kernel<CONE><<<rgrid, BP_RAYS_THREADS, 0, st>>>(H, W, vm, nx, ny, nz, sx, sy, sz, cx,
-                                                                                   cy, cz, tanx, tany, step, tu, tv, rays);
-        else
-            backproject_rays_kernel<CONE><<<rgrid, BP_RAYS_THREADS, 0, st>>>(H, W, vm, nx, ny, nz, sx, sy, sz, cx, cy,
-                                                                             cz, tanx, tany, step, rays);
+        backproject_rays_kernel<CONE><<<rgrid, BP_RAYS_THREADS, 0, st>>>(H, W, vm, nx, ny, nz, sx, sy, sz, cx, cy, cz,
+                                                                         tanx, tany, step, shift, rays);
         R2X_CUDA_OK(cudaGetLastError());
         const int first = v0 == 0;
         const float scale = v0 + nc == N ? step : 1.0f;   // partial sums stay unscaled between chunks
@@ -267,44 +245,24 @@ size_t r2x_volume_backproject_scratch_bytes(int n_views, int H, int W) {
 }
 
 int r2x_volume_backproject(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
-                           const float* projmatrices, float tan_fovx, float tan_fovy, int mode, int nx, int ny, int nz,
-                           float sx, float sy, float sz, float cx, float cy, float cz, float step, float* out_volume,
-                           float* out_weight, void* scratch, size_t scratch_bytes) {
-    using namespace r2x;
-    if (int rc = backproject_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode, nx,
-                                      ny, nz, sx, sy, sz, cx, cy, cz, step, out_volume, scratch, scratch_bytes))
-        return rc;
-    const cudaStream_t st = (cudaStream_t)stream;
-    float4* rays = (float4*)(((size_t)scratch + 255) & ~(size_t)255);
-    if (mode == 1)
-        return backproject_launch<true, false>(st, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy,
-                                               nx, ny, nz, sx, sy, sz, cx, cy, cz, step, 0.0f, 0.0f, out_volume,
-                                               out_weight, rays);
-    return backproject_launch<false, false>(st, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, nx,
-                                            ny, nz, sx, sy, sz, cx, cy, cz, step, 0.0f, 0.0f, out_volume, out_weight,
-                                            rays);
-}
-
-int r2x_volume_backproject_shifted(void* stream, int n_views, int H, int W, const float* projs,
-                                   const float* viewmatrices, const float* projmatrices, float tan_fovx, float tan_fovy,
-                                   int mode, float shift_u, float shift_v, int nx, int ny, int nz, float sx, float sy,
-                                   float sz, float cx, float cy, float cz, float step, float* out_volume,
-                                   float* out_weight, void* scratch, size_t scratch_bytes) {
+                           const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u,
+                           float shift_v, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
+                           float cz, float step, float* out_volume, float* out_weight, void* scratch,
+                           size_t scratch_bytes) {
     using namespace r2x;
     if (int rc = backproject_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode, nx,
                                       ny, nz, sx, sy, sz, cx, cy, cz, step, out_volume, scratch, scratch_bytes))
         return rc;
     if (!(std::isfinite(shift_u) && std::isfinite(shift_v)))
-        return fail_msg(R2X_ERR_INVALID, "r2x_volume_backproject_shifted: bad shift (must be finite)");
+        return fail_msg(R2X_ERR_INVALID, "r2x_volume_backproject: bad shift (must be finite)");
+    const ProjShift shift = proj_shift(shift_u, shift_v, H, W);
     const cudaStream_t st = (cudaStream_t)stream;
     float4* rays = (float4*)(((size_t)scratch + 255) & ~(size_t)255);
     if (mode == 1)
-        return backproject_launch<true, true>(st, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy,
-                                              nx, ny, nz, sx, sy, sz, cx, cy, cz, step, shift_u, shift_v, out_volume,
-                                              out_weight, rays);
-    return backproject_launch<false, true>(st, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, nx,
-                                           ny, nz, sx, sy, sz, cx, cy, cz, step, shift_u, shift_v, out_volume, out_weight,
-                                           rays);
+        return backproject_launch<true>(st, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, nx, ny,
+                                        nz, sx, sy, sz, cx, cy, cz, step, shift, out_volume, out_weight, rays);
+    return backproject_launch<false>(st, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, nx, ny,
+                                     nz, sx, sy, sz, cx, cy, cz, step, shift, out_volume, out_weight, rays);
 }
 
 }  // extern "C"

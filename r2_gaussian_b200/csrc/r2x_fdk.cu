@@ -4,9 +4,12 @@
 // by initialize_pcd.py).  FDK is a weighted ramp filter along the detector rows followed by one voxel-driven
 // backprojection; both are small data-parallel kernels, and the geometry they need is the rasterizer's own:
 //
-//   fdk_filter_kernel       one CTA per detector row: cosine weight (cone beam), stage the row in shared memory between
-//                           two rows of zeros, then the band-limited Ram-Lak filter as a linear convolution over the
-//                           whole row, using the symmetric odd-only taps:
+//   fdk_filter_kernel       one CTA per detector row: cosine weight (cone beam) at each pixel's ndc, moved by the
+//                           detector offset (t_u, t_v) pixels when there is one, times the redundancy weight of the
+//                           weighting (R2X_FDK_PLAIN none, R2X_FDK_PARKER Parker's for a short scan, R2X_FDK_HALF_FAN
+//                           Wang's for an offset detector on a full circle); stage the row in shared memory between two
+//                           rows of zeros, then the band-limited Ram-Lak filter as a linear convolution over the whole
+//                           row, using the symmetric odd-only taps:
 //                             Q_j = (r_j / 4 - sum_{k odd} (r_{j-k} + r_{j+k}) / (pi^2 k^2)) / D
 //                           (D = isocentre pitch), summed for k = 1, 3, 5, ... in that order.
 //   fdk_backproject_kernel  a thread owns one (x, y) voxel column and a run of FDK_ZR voxels along z.  Every view's
@@ -16,14 +19,9 @@
 //                           filtered view is sampled bilinearly through L1/L2 (__ldg; 0 outside the detector) and
 //                           weighted by U^2, U = DSO / z_view (cone; 1 for parallel beam).  The views are summed in
 //                           index order in registers and each voxel is stored once: no atomics, so the volume is
-//                           bitwise reproducible.
-//   fdk_parker_filter_kernel  the filter of a short scan (r2x_fdk_short_scan): fdk_filter_kernel with each pixel also
-//                           weighted by its Parker redundancy weight and its view's angular interval; the backprojection
-//                           that follows is fdk_backproject_kernel with scale 1 instead of pi / N.
-//   fdk_filter_shift_kernel  the filter of a detector offset by (t_u, t_v) pixels (r2x_fdk_shifted,
-//                           r2x_fdk_short_scan_shifted): each pixel's cosine weight (and fan angle) at its offset ndc,
-//                           plus optional half-fan (Wang 2002) or Parker weights.  The backprojection is
-//                           fdk_backproject_kernel, unchanged, fed the offset projmatrices by the caller.
+//                           bitwise reproducible.  An offset detector needs nothing here: the caller passes the offset
+//                           projmatrices.  The scale is pi / N, or 1 for Parker weights (they hold each view's
+//                           interval).
 //
 // The float64 NumPy statements of the same definitions are oracle/fdk_oracle.py (plain),
 // tests/fdk_short_scan_oracle.py (short scan, Parker weights) and tests/offset_detector_oracle.py (offset detector,
@@ -49,38 +47,6 @@ size_t fdk_scratch_bytes(int N, int H, int W) {
 }
 
 static size_t fdk_filter_smem(int W) { return (size_t)(3 * W + (W + 1) / 2) * sizeof(float); }
-
-__global__ void __launch_bounds__(256) fdk_filter_kernel(int H, int W, const float* __restrict__ projs, float tanx,
-                                                         float tany, int cone, float inv_delta, float* __restrict__ q) {
-    extern __shared__ float sm[];
-    float* row = sm;              // [3W]: zeros | weighted row | zeros
-    float* g = sm + 3 * W;        // [(W+1)/2]: g[m] = 1 / (pi^2 (2m+1)^2)
-    const size_t r = blockIdx.x;  // view * H + detector row
-    const float* src = projs + r * W;
-    const float step = 2.0f / (float)W, first = 1.0f / (float)W - 1.0f;
-    const float b = cone ? fmaf((float)(r % H), 2.0f / (float)H, 1.0f / (float)H - 1.0f) * tany : 0.0f;
-    for (int j = threadIdx.x; j < W; j += blockDim.x) {
-        float p = src[j];
-        if (cone) {
-            const float a = fmaf((float)j, step, first) * tanx;
-            p *= rsqrtf(fmaf(a, a, fmaf(b, b, 1.0f)));
-        }
-        row[j] = 0.0f;
-        row[W + j] = p;
-        row[2 * W + j] = 0.0f;
-    }
-    for (int m = threadIdx.x; m < (W + 1) / 2; m += blockDim.x) {
-        const float k = (float)(2 * m + 1);
-        g[m] = 1.0f / (9.869604401089358f * k * k);
-    }
-    __syncthreads();
-    for (int j = threadIdx.x; j < W; j += blockDim.x) {
-        const float* c = row + W + j;
-        float acc = 0.0f;
-        for (int m = 0, k = 1; k < W; ++m, k += 2) acc = fmaf(g[m], c[-k] + c[k], acc);
-        q[r * W + j] = fmaf(0.25f, c[0], -acc) * inv_delta;
-    }
-}
 
 template <bool CONE>
 __global__ void __launch_bounds__(FDK_BX * FDK_BY) fdk_backproject_kernel(
@@ -181,46 +147,6 @@ __device__ __forceinline__ float fdk_parker_weight(float beta, float gam, float 
     return 0.0f;
 }
 
-// fdk_filter_kernel for a short scan: each pixel is also weighted by its Parker weight and its view's angular interval
-// while the row is staged (view weights vw[v] = (beta'_v, dbeta_v)); the Ram-Lak convolution is the same.  The weight is
-// computed per pixel (one atanf and one sinpif), which costs little next to the W/2-tap convolution of each pixel.
-__global__ void __launch_bounds__(256) fdk_parker_filter_kernel(int H, int W, const float* __restrict__ projs,
-                                                                float tanx, float tany, int cone, float inv_delta,
-                                                                const float2* __restrict__ vw, float arc, float delta,
-                                                                float* __restrict__ q) {
-    extern __shared__ float sm[];
-    float* row = sm;              // [3W]: zeros | weighted row | zeros
-    float* g = sm + 3 * W;        // [(W+1)/2]: g[m] = 1 / (pi^2 (2m+1)^2)
-    const size_t r = blockIdx.x;  // view * H + detector row
-    const float* src = projs + r * W;
-    const float2 bv = vw[r / H];
-    const float step = 2.0f / (float)W, first = 1.0f / (float)W - 1.0f;
-    const float b = cone ? fmaf((float)(r % H), 2.0f / (float)H, 1.0f / (float)H - 1.0f) * tany : 0.0f;
-    for (int j = threadIdx.x; j < W; j += blockDim.x) {
-        float p = src[j];
-        float gam = 0.0f;
-        if (cone) {
-            const float a = fmaf((float)j, step, first) * tanx;
-            p *= rsqrtf(fmaf(a, a, fmaf(b, b, 1.0f)));
-            gam = -atanf(a);  // column u runs along the rotation, so a ray at +u leans back: gamma = -atan(u / DSD)
-        }
-        row[j] = 0.0f;
-        row[W + j] = p * (fdk_parker_weight(bv.x, gam, arc, delta) * bv.y);
-        row[2 * W + j] = 0.0f;
-    }
-    for (int m = threadIdx.x; m < (W + 1) / 2; m += blockDim.x) {
-        const float k = (float)(2 * m + 1);
-        g[m] = 1.0f / (9.869604401089358f * k * k);
-    }
-    __syncthreads();
-    for (int j = threadIdx.x; j < W; j += blockDim.x) {
-        const float* c = row + W + j;
-        float acc = 0.0f;
-        for (int m = 0, k = 1; k < W; ++m, k += 2) acc = fmaf(g[m], c[-k] + c[k], acc);
-        q[r * W + j] = fmaf(0.25f, c[0], -acc) * inv_delta;
-    }
-}
-
 // Half-fan redundancy weight (Wang 2002) of the ray at fan coordinate a (tan of the fan angle; ndc for parallel beam)
 // on a full circle with the axis off the detector's centre: 2 sin^2(pi/4 (1 + sigma a / delta)) on the overlap
 // |a| <= delta, 2 beyond it on the wide side (sigma a > delta), 0 beyond it on the narrow side (no pixel lies there).
@@ -233,18 +159,23 @@ __device__ __forceinline__ float fdk_half_fan_weight(float a, float inv_delta, f
     return 2.0f * (s * s);
 }
 
-enum FdkWeighting { FDK_PLAIN = 0, FDK_PARKER = 1, FDK_HALF_FAN = 2 };
+// The arguments only one weighting reads.
+struct FdkWeights {
+    const float2* vw = nullptr;          // PARKER: each view's (beta'_v, dbeta_v)
+    float arc = 0.0f, delta = 0.0f;      // PARKER: the arc B and delta = (B - pi) / 2
+    float fan = 1.0f, hf_inv_delta = 1.0f, hf_sigma = 1.0f;   // HALF_FAN: a = ndc_x * fan, 1 / delta, sign(t_u)
+};
 
-// The filter of a detector offset by (t_u, t_v) pixels (r2x_fdk_shifted, r2x_fdk_short_scan_shifted): fdk_filter_kernel
-// (or fdk_parker_filter_kernel) with each pixel's ndc moved by (su, sv) = (2 t_u / W, -2 t_v / H) in the cosine weight
-// and the fan angle; HALF_FAN also weights each pixel by fdk_half_fan_weight of its fan coordinate a = ndc_x * fan
-// (fan = tan_fovx for cone beam, 1 for parallel beam).  The Ram-Lak convolution is shift-invariant and the same.
+// Steps 1-2 of FDK, one CTA per detector row of a detector offset by (t_u, t_v) pixels (zero when centred): each pixel's
+// cosine weight (cone beam) at its ndc moved by (su, sv) = (2 t_u / W, -2 t_v / H), then WEIGHT's redundancy weight:
+// PARKER its Parker weight at fan angle -atan(a) (cone; 0 for parallel beam) times its view's angular interval, HALF_FAN
+// fdk_half_fan_weight of its fan coordinate a = ndc_x * fan.  The weight is computed per pixel, which costs little next
+// to the W/2-tap convolution of each pixel.  The row is staged in shared memory between two rows of zeros and filtered
+// with the band-limited Ram-Lak taps (shift-invariant, so the same for any offset).
 template <int WEIGHT>
-__global__ void __launch_bounds__(256) fdk_filter_shift_kernel(int H, int W, const float* __restrict__ projs,
-                                                               float tanx, float tany, int cone, float inv_delta,
-                                                               float su, float sv, const float2* __restrict__ vw,
-                                                               float arc, float delta, float fan, float hf_inv_delta,
-                                                               float hf_sigma, float* __restrict__ q) {
+__global__ void __launch_bounds__(256) fdk_filter_kernel(int H, int W, const float* __restrict__ projs, float tanx,
+                                                         float tany, int cone, float inv_delta, float su, float sv,
+                                                         FdkWeights fw, float* __restrict__ q) {
     extern __shared__ float sm[];
     float* row = sm;              // [3W]: zeros | weighted row | zeros
     float* g = sm + 3 * W;        // [(W+1)/2]: g[m] = 1 / (pi^2 (2m+1)^2)
@@ -253,7 +184,7 @@ __global__ void __launch_bounds__(256) fdk_filter_shift_kernel(int H, int W, con
     const float step = 2.0f / (float)W, first = 1.0f / (float)W - 1.0f;
     const float b = cone ? (fmaf((float)(r % H), 2.0f / (float)H, 1.0f / (float)H - 1.0f) + sv) * tany : 0.0f;
     float2 bv = make_float2(0.0f, 0.0f);
-    if (WEIGHT == FDK_PARKER) bv = vw[r / H];
+    if (WEIGHT == R2X_FDK_PARKER) bv = fw.vw[r / H];
     for (int j = threadIdx.x; j < W; j += blockDim.x) {
         float p = src[j];
         const float nd = fmaf((float)j, step, first) + su;
@@ -261,10 +192,11 @@ __global__ void __launch_bounds__(256) fdk_filter_shift_kernel(int H, int W, con
         if (cone) {
             const float a = nd * tanx;
             p *= rsqrtf(fmaf(a, a, fmaf(b, b, 1.0f)));
-            if (WEIGHT == FDK_PARKER) gam = -atanf(a);
+            // column u runs along the rotation, so a ray at +u leans back: gamma = -atan(u / DSD)
+            if (WEIGHT == R2X_FDK_PARKER) gam = -atanf(a);
         }
-        if (WEIGHT == FDK_PARKER) p *= fdk_parker_weight(bv.x, gam, arc, delta) * bv.y;
-        if (WEIGHT == FDK_HALF_FAN) p *= fdk_half_fan_weight(nd * fan, hf_inv_delta, hf_sigma);
+        if (WEIGHT == R2X_FDK_PARKER) p *= fdk_parker_weight(bv.x, gam, fw.arc, fw.delta) * bv.y;
+        if (WEIGHT == R2X_FDK_HALF_FAN) p *= fdk_half_fan_weight(nd * fw.fan, fw.hf_inv_delta, fw.hf_sigma);
         row[j] = 0.0f;
         row[W + j] = p;
         row[2 * W + j] = 0.0f;
@@ -287,43 +219,16 @@ static double fdk_pitch(int W, float tanx, int mode, float dso) {
     return mode == 1 ? 2.0 * (double)tanx * (double)dso / W : 2.0 / W;
 }
 
-static int fdk_parker_filter(cudaStream_t st, int N, int H, int W, const float* projs, float tanx, float tany, int mode,
-                             float dso, const float* view_weights, float arc, float* q) {
+static int fdk_filter(cudaStream_t st, int weighting, int N, int H, int W, const float* projs, float tanx, float tany,
+                      int mode, float dso, float su, float sv, const FdkWeights& fw, float* q) {
+    auto kernel = weighting == R2X_FDK_PARKER     ? fdk_filter_kernel<R2X_FDK_PARKER>
+                  : weighting == R2X_FDK_HALF_FAN ? fdk_filter_kernel<R2X_FDK_HALF_FAN>
+                                                  : fdk_filter_kernel<R2X_FDK_PLAIN>;
     const size_t smem = fdk_filter_smem(W);
     if (smem > 48 * 1024)
-        R2X_CUDA_OK(cudaFuncSetAttribute(fdk_parker_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem));
-    const float delta = (float)(0.5 * ((double)arc - 3.141592653589793));
-    fdk_parker_filter_kernel<<<(unsigned)((long long)N * H), 256, smem, st>>>(
-        H, W, projs, tanx, tany, mode, (float)(1.0 / fdk_pitch(W, tanx, mode, dso)), (const float2*)view_weights, arc,
-        delta, q);
-    R2X_CUDA_OK(cudaGetLastError());
-    return 0;
-}
-
-static int fdk_filter(cudaStream_t st, int N, int H, int W, const float* projs, float tanx, float tany, int mode,
-                      float dso, float* q) {
-    const size_t smem = fdk_filter_smem(W);
-    if (smem > 48 * 1024)
-        R2X_CUDA_OK(cudaFuncSetAttribute(fdk_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const double delta = fdk_pitch(W, tanx, mode, dso);
-    fdk_filter_kernel<<<(unsigned)((long long)N * H), 256, smem, st>>>(H, W, projs, tanx, tany, mode, (float)(1.0 / delta),
-                                                                       q);
-    R2X_CUDA_OK(cudaGetLastError());
-    return 0;
-}
-
-template <int WEIGHT>
-static int fdk_filter_shift_launch(cudaStream_t st, int N, int H, int W, const float* projs, float tanx, float tany,
-                                   int mode, float dso, float su, float sv, const float* view_weights, float arc,
-                                   float delta, float fan, float hf_inv_delta, float hf_sigma, float* q) {
-    const size_t smem = fdk_filter_smem(W);
-    if (smem > 48 * 1024)
-        R2X_CUDA_OK(cudaFuncSetAttribute(fdk_filter_shift_kernel<WEIGHT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem));
-    fdk_filter_shift_kernel<WEIGHT><<<(unsigned)((long long)N * H), 256, smem, st>>>(
-        H, W, projs, tanx, tany, mode, (float)(1.0 / fdk_pitch(W, tanx, mode, dso)), su, sv,
-        (const float2*)view_weights, arc, delta, fan, hf_inv_delta, hf_sigma, q);
+        R2X_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<(unsigned)((long long)N * H), 256, smem, st>>>(H, W, projs, tanx, tany, mode,
+                                                            (float)(1.0 / fdk_pitch(W, tanx, mode, dso)), su, sv, fw, q);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -372,104 +277,50 @@ extern "C" {
 size_t r2x_fdk_scratch_bytes(int n_views, int H, int W) { return r2x::fdk_scratch_bytes(n_views, H, W); }
 
 int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
-            const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float dso, int nx, int ny, int nz,
-            float sx, float sy, float sz, float cx, float cy, float cz, float* out_volume, void* scratch,
-            size_t scratch_bytes) {
-    if (int rc = r2x::fdk_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode,
-                                   dso, nx, ny, nz, sx, sy, sz, out_volume, scratch, scratch_bytes))
-        return rc;
-    const cudaStream_t st = (cudaStream_t)stream;
-    float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
-    if (int rc = r2x::fdk_filter(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, q)) return rc;
-    return r2x::fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx,
-                                cy, cz, (float)(3.141592653589793 / n_views), out_volume);
-}
-
-int r2x_fdk_short_scan(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
-                       const float* projmatrices, const float* view_weights, float arc, float tan_fovx, float tan_fovy,
-                       int mode, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
-                       float cz, float* out_volume, void* scratch, size_t scratch_bytes) {
-    if (int rc = r2x::fdk_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode,
-                                   dso, nx, ny, nz, sx, sy, sz, out_volume, scratch, scratch_bytes))
-        return rc;
-    if (n_views < 2) return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan: bad N (a short scan needs >= 2 views)");
-    if (!view_weights) return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan: bad pointer (view_weights NULL)");
-    // the arc must hold pi plus the full fan (within float rounding of the arc) and stay short of a full circle
-    const double pi = 3.141592653589793;
-    const double need = pi + (mode == 1 ? 2.0 * std::atan((double)tan_fovx) : 0.0);
-    if (!(std::isfinite(arc) && (double)arc >= need - 1e-6 && (double)arc < 2.0 * pi))
-        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan: bad arc (needs pi + 2 atan(tan_fovx) <= arc < 2 pi)");
-    const cudaStream_t st = (cudaStream_t)stream;
-    float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
-    if (int rc = r2x::fdk_parker_filter(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, view_weights, arc, q))
-        return rc;
-    return r2x::fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx,
-                                cy, cz, 1.0f, out_volume);
-}
-
-int r2x_fdk_shifted(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
-                    const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
-                    int half_fan, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
-                    float cz, float* out_volume, void* scratch, size_t scratch_bytes) {
-    if (int rc = r2x::fdk_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode,
-                                   dso, nx, ny, nz, sx, sy, sz, out_volume, scratch, scratch_bytes))
+            const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
+            int weighting, const float* view_weights, float arc, float dso, int nx, int ny, int nz, float sx, float sy,
+            float sz, float cx, float cy, float cz, float* out_volume, void* scratch, size_t scratch_bytes) {
+    using namespace r2x;
+    if (int rc = fdk_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode, dso, nx, ny,
+                              nz, sx, sy, sz, out_volume, scratch, scratch_bytes))
         return rc;
     if (!(std::isfinite(shift_u) && std::isfinite(shift_v)))
-        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_shifted: bad shift (must be finite)");
-    if (half_fan != 0 && half_fan != 1) return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_shifted: bad half_fan (0 or 1)");
-    // half fan: the rotation axis strictly inside the detector and off its centre, 0 < |t_u| < W / 2
-    if (half_fan && !(shift_u != 0.0f && 2.0 * std::fabs((double)shift_u) < (double)W))
-        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_shifted: bad shift_u for half_fan (needs 0 < |shift_u| < W / 2)");
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad shift (must be finite)");
+    if (weighting != R2X_FDK_PLAIN && weighting != R2X_FDK_PARKER && weighting != R2X_FDK_HALF_FAN)
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad weighting (0 = plain, 1 = Parker, 2 = half fan)");
+    const double pi = 3.141592653589793;
+    FdkWeights fw;
+    if (weighting == R2X_FDK_PARKER) {
+        if (n_views < 2) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad N (a short scan needs >= 2 views)");
+        if (!view_weights) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad pointer (view_weights NULL)");
+        // Parker weights assume each ray's conjugate is on the detector, which a horizontal offset breaks
+        if (shift_u != 0.0f)
+            return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad shift_u (a short scan needs shift_u = 0)");
+        // the arc must hold pi plus the full fan (within float rounding of the arc) and stay short of a full circle
+        const double need = pi + (mode == 1 ? 2.0 * std::atan((double)tan_fovx) : 0.0);
+        if (!(std::isfinite(arc) && (double)arc >= need - 1e-6 && (double)arc < 2.0 * pi))
+            return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad arc (needs pi + 2 atan(tan_fovx) <= arc < 2 pi)");
+        fw.vw = (const float2*)view_weights;
+        fw.arc = arc;
+        fw.delta = (float)(0.5 * ((double)arc - pi));
+    }
+    if (weighting == R2X_FDK_HALF_FAN) {
+        // the rotation axis strictly inside the detector and off its centre, 0 < |t_u| < W / 2
+        if (!(shift_u != 0.0f && 2.0 * std::fabs((double)shift_u) < (double)W))
+            return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad shift_u for half fan (needs 0 < |shift_u| < W / 2)");
+        const double fan = mode == 1 ? (double)tan_fovx : 1.0;
+        fw.fan = (float)fan;
+        fw.hf_inv_delta = (float)(1.0 / ((1.0 - 2.0 * std::fabs((double)shift_u) / W) * fan));
+        fw.hf_sigma = shift_u > 0.0f ? 1.0f : -1.0f;
+    }
     const cudaStream_t st = (cudaStream_t)stream;
     float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
     const float su = (float)(2.0 * (double)shift_u / W), sv = (float)(-2.0 * (double)shift_v / H);
-    int rc;
-    if (half_fan) {
-        const double fan = mode == 1 ? (double)tan_fovx : 1.0;
-        const double hf_delta = (1.0 - 2.0 * std::fabs((double)shift_u) / W) * fan;
-        rc = r2x::fdk_filter_shift_launch<r2x::FDK_HALF_FAN>(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, su,
-                                                              sv, nullptr, 0.0f, 0.0f, (float)fan, (float)(1.0 / hf_delta),
-                                                              shift_u > 0.0f ? 1.0f : -1.0f, q);
-    } else {
-        rc = r2x::fdk_filter_shift_launch<r2x::FDK_PLAIN>(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, su, sv,
-                                                           nullptr, 0.0f, 0.0f, 1.0f, 1.0f, 1.0f, q);
-    }
-    if (rc) return rc;
-    return r2x::fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx,
-                                cy, cz, (float)(3.141592653589793 / n_views), out_volume);
-}
-
-int r2x_fdk_short_scan_shifted(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
-                               const float* projmatrices, const float* view_weights, float arc, float tan_fovx,
-                               float tan_fovy, int mode, float shift_u, float shift_v, float dso, int nx, int ny, int nz,
-                               float sx, float sy, float sz, float cx, float cy, float cz, float* out_volume,
-                               void* scratch, size_t scratch_bytes) {
-    if (int rc = r2x::fdk_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode,
-                                   dso, nx, ny, nz, sx, sy, sz, out_volume, scratch, scratch_bytes))
-        return rc;
-    if (n_views < 2)
-        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan_shifted: bad N (a short scan needs >= 2 views)");
-    if (!view_weights)
-        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan_shifted: bad pointer (view_weights NULL)");
-    if (!std::isfinite(shift_v))
-        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan_shifted: bad shift_v (must be finite)");
-    // Parker weights assume each ray's conjugate is on the detector, which a horizontal offset breaks
-    if (shift_u != 0.0f)
-        return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_short_scan_shifted: bad shift_u (a short scan needs shift_u = 0)");
-    const double pi = 3.141592653589793;
-    const double need = pi + (mode == 1 ? 2.0 * std::atan((double)tan_fovx) : 0.0);
-    if (!(std::isfinite(arc) && (double)arc >= need - 1e-6 && (double)arc < 2.0 * pi))
-        return r2x::fail_msg(R2X_ERR_INVALID,
-                             "r2x_fdk_short_scan_shifted: bad arc (needs pi + 2 atan(tan_fovx) <= arc < 2 pi)");
-    const cudaStream_t st = (cudaStream_t)stream;
-    float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
-    const float delta = (float)(0.5 * ((double)arc - pi));
-    if (int rc = r2x::fdk_filter_shift_launch<r2x::FDK_PARKER>(st, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso,
-                                                                0.0f, (float)(-2.0 * (double)shift_v / H), view_weights,
-                                                                arc, delta, 1.0f, 1.0f, 1.0f, q))
-        return rc;
-    return r2x::fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx,
-                                cy, cz, 1.0f, out_volume);
+    if (int rc = fdk_filter(st, weighting, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, su, sv, fw, q)) return rc;
+    // Parker's dbeta_v already holds each view's share of the arc
+    const float scale = weighting == R2X_FDK_PARKER ? 1.0f : (float)(pi / n_views);
+    return fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx, cy,
+                           cz, scale, out_volume);
 }
 
 int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, float tan_fovx, float tan_fovy,
@@ -480,7 +331,8 @@ int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, 
     if (mode == 1 && !(dso > 0.0f && tan_fovx > 0.0f && tan_fovy > 0.0f))
         return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_filter: bad DSO / tan_fov");
     if (!projs || !filtered) return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_filter: bad pointer (NULL)");
-    return r2x::fdk_filter((cudaStream_t)stream, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, filtered);
+    return r2x::fdk_filter((cudaStream_t)stream, R2X_FDK_PLAIN, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso,
+                           0.0f, 0.0f, r2x::FdkWeights(), filtered);
 }
 
 int r2x_fdk_backproject(void* stream, int n_views, int H, int W, const float* filtered, const float* viewmatrices,

@@ -13,9 +13,8 @@
 //                          t_c, index-space position g_c and step, k range from a slab test); samples
 //                          g_k = fma(k, step, g_c) in float32, floor, 8 predicated __ldg loads, float32 sum in k order.
 //                          The 32 x 8 tile is staged in shared memory so the [N,H,W] rows are stored in whole sectors.
-//                          No atomics: the projections are bitwise reproducible.
-//   volume_project_shift_kernel  the same body for a detector offset by (t_u, t_v) pixels (TIGRE's geo.offDetector):
-//                          only the pixel's ndc in the float64 setup moves (project_ray_setup<CONE, true>).
+//                          No atomics: the projections are bitwise reproducible.  A detector offset by (t_u, t_v)
+//                          pixels (TIGRE's geo.offDetector) only moves the pixel's ndc in the float64 setup.
 //
 // The float64 NumPy statement of the same definition is oracle/projector_oracle.py.
 #include <cmath>
@@ -30,11 +29,10 @@ namespace r2x {
 constexpr int PRJ_BV = 32, PRJ_BU = 8;   // CTA: 32 detector rows (lanes) x 8 detector columns
 constexpr int PRJ_MAX_VIEWS = 65535;     // views per launch (grid.z); more are launched in chunks
 
-// The kernel's body; SHIFT selects the offset-detector rays (project_ray_setup), tu / tv are unused without it.
-template <bool CONE, bool SHIFT>
-__device__ __forceinline__ void volume_project_body(
+template <bool CONE>
+__global__ void __launch_bounds__(PRJ_BV * PRJ_BU) volume_project_kernel(
     const float* __restrict__ vol, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy, float cz,
-    int H, int W, const float* __restrict__ viewm, float tanx, float tany, float step, float tu, float tv,
+    int H, int W, const float* __restrict__ viewm, float tanx, float tany, float step, ProjShift shift,
     float* __restrict__ out) {
     __shared__ float tile[PRJ_BV][PRJ_BU + 1];
     const int v = blockIdx.y * PRJ_BV + threadIdx.x;   // detector row
@@ -42,8 +40,8 @@ __device__ __forceinline__ void volume_project_body(
     const int view = blockIdx.z;
     float acc = 0.0f;
     if (v < H && u < W) {
-        const ProjRay ray = project_ray_setup<CONE, SHIFT>(viewm, view, u, v, H, W, nx, ny, nz, sx, sy, sz, cx, cy, cz,
-                                                           tanx, tany, step, tu, tv);
+        const ProjRay ray = project_ray_setup<CONE>(viewm, view, u, v, H, W, nx, ny, nz, sx, sy, sz, cx, cy, cz, tanx,
+                                                    tany, step, shift);
         const long long sy_ = nz, sx_ = (long long)ny * nz;
         for (long long k = ray.k0; k <= ray.k1; ++k) {
             const float fk = (float)k;
@@ -77,23 +75,6 @@ __device__ __forceinline__ void volume_project_body(
     if (ro < H && co < W) out[((size_t)view * H + ro) * W + co] = tile[t / PRJ_BU][t % PRJ_BU];
 }
 
-template <bool CONE>
-__global__ void __launch_bounds__(PRJ_BV * PRJ_BU) volume_project_kernel(
-    const float* __restrict__ vol, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy, float cz,
-    int H, int W, const float* __restrict__ viewm, float tanx, float tany, float step, float* __restrict__ out) {
-    volume_project_body<CONE, false>(vol, nx, ny, nz, sx, sy, sz, cx, cy, cz, H, W, viewm, tanx, tany, step, 0.0f, 0.0f,
-                                     out);
-}
-
-// The projector of a detector offset by (tu, tv) pixels (r2x_volume_project_shifted).
-template <bool CONE>
-__global__ void __launch_bounds__(PRJ_BV * PRJ_BU) volume_project_shift_kernel(
-    const float* __restrict__ vol, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy, float cz,
-    int H, int W, const float* __restrict__ viewm, float tanx, float tany, float step, float tu, float tv,
-    float* __restrict__ out) {
-    volume_project_body<CONE, true>(vol, nx, ny, nz, sx, sy, sz, cx, cy, cz, H, W, viewm, tanx, tany, step, tu, tv, out);
-}
-
 static int project_validate(int nx, int ny, int nz, const float* volume, float sx, float sy, float sz, float cx,
                             float cy, float cz, int N, int H, int W, const float* viewm, float tanx, float tany,
                             int mode, float step, const float* out) {
@@ -121,11 +102,15 @@ extern "C" {
 
 int r2x_volume_project(void* stream, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
                        float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
-                       float tan_fovx, float tan_fovy, int mode, float step, float* out_projs) {
+                       float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v, float step,
+                       float* out_projs) {
     using namespace r2x;
     if (int rc = project_validate(nx, ny, nz, volume, sx, sy, sz, cx, cy, cz, n_views, H, W, viewmatrices, tan_fovx,
                                   tan_fovy, mode, step, out_projs))
         return rc;
+    if (!(std::isfinite(shift_u) && std::isfinite(shift_v)))
+        return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad shift (must be finite)");
+    const ProjShift shift = proj_shift(shift_u, shift_v, H, W);
     const cudaStream_t st = (cudaStream_t)stream;
     const dim3 block(PRJ_BV, PRJ_BU);
     for (int v0 = 0; v0 < n_views; v0 += PRJ_MAX_VIEWS) {
@@ -135,38 +120,10 @@ int r2x_volume_project(void* stream, int nx, int ny, int nz, const float* volume
         float* o = out_projs + (size_t)v0 * H * W;
         if (mode == 1)
             volume_project_kernel<true><<<grid, block, 0, st>>>(volume, nx, ny, nz, sx, sy, sz, cx, cy, cz, H, W, vm,
-                                                                tan_fovx, tan_fovy, step, o);
+                                                                tan_fovx, tan_fovy, step, shift, o);
         else
             volume_project_kernel<false><<<grid, block, 0, st>>>(volume, nx, ny, nz, sx, sy, sz, cx, cy, cz, H, W, vm,
-                                                                 tan_fovx, tan_fovy, step, o);
-        R2X_CUDA_OK(cudaGetLastError());
-    }
-    return 0;
-}
-
-int r2x_volume_project_shifted(void* stream, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
-                               float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
-                               float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v, float step,
-                               float* out_projs) {
-    using namespace r2x;
-    if (int rc = project_validate(nx, ny, nz, volume, sx, sy, sz, cx, cy, cz, n_views, H, W, viewmatrices, tan_fovx,
-                                  tan_fovy, mode, step, out_projs))
-        return rc;
-    if (!(std::isfinite(shift_u) && std::isfinite(shift_v)))
-        return fail_msg(R2X_ERR_INVALID, "r2x_volume_project_shifted: bad shift (must be finite)");
-    const cudaStream_t st = (cudaStream_t)stream;
-    const dim3 block(PRJ_BV, PRJ_BU);
-    for (int v0 = 0; v0 < n_views; v0 += PRJ_MAX_VIEWS) {
-        const int nv = min(PRJ_MAX_VIEWS, n_views - v0);
-        const dim3 grid((W + PRJ_BU - 1) / PRJ_BU, (H + PRJ_BV - 1) / PRJ_BV, nv);
-        const float* vm = viewmatrices + (size_t)v0 * 16;
-        float* o = out_projs + (size_t)v0 * H * W;
-        if (mode == 1)
-            volume_project_shift_kernel<true><<<grid, block, 0, st>>>(volume, nx, ny, nz, sx, sy, sz, cx, cy, cz, H, W,
-                                                                      vm, tan_fovx, tan_fovy, step, shift_u, shift_v, o);
-        else
-            volume_project_shift_kernel<false><<<grid, block, 0, st>>>(volume, nx, ny, nz, sx, sy, sz, cx, cy, cz, H, W,
-                                                                       vm, tan_fovx, tan_fovy, step, shift_u, shift_v, o);
+                                                                 tan_fovx, tan_fovy, step, shift, o);
         R2X_CUDA_OK(cudaGetLastError());
     }
     return 0;

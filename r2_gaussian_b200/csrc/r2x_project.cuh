@@ -15,14 +15,23 @@ struct ProjRay {
     long long k0, k1;
 };
 
-// SHIFT: the detector is offset by (tu, tv) pixels (TIGRE's geo.offDetector over its pixel pitch), so pixel (v, u) sees
-// the ray of the centred detector's fractional pixel (v - tv, u + tu): ndc_x gains 2 tu / W and ndc_y loses 2 tv / H.
-// SHIFT = false ignores tu, tv and is the centred projector's code.
-template <bool CONE, bool SHIFT = false>
+// The detector is offset by (tu, tv) pixels (TIGRE's geo.offDetector over its pixel pitch; 0, 0 when centred), so pixel
+// (v, u) sees the ray of the centred detector's fractional pixel (v - tv, u + tu): ndc_x gains su = 2 tu / W and ndc_y
+// loses sv = 2 tv / H (ProjShift, divided once on the host: IEEE division gives the same bits there).  Zero shifts add
+// exact zeros, so a centred detector's rays are unchanged bit for bit.
+struct ProjShift {
+    double su, sv;
+};
+
+static inline ProjShift proj_shift(float tu, float tv, int H, int W) {
+    return {2.0 * (double)tu / W, 2.0 * (double)tv / H};
+}
+
+template <bool CONE>
 __device__ __forceinline__ ProjRay project_ray_setup(const float* __restrict__ viewm, int view, int u, int v, int H,
                                                      int W, int nx, int ny, int nz, float sx, float sy, float sz,
                                                      float cx, float cy, float cz, float tanx, float tany,
-                                                     float step, float tu = 0.0f, float tv = 0.0f) {
+                                                     float step, ProjShift shift) {
     // world -> camera: rotation Rw[r][c] = m[4c + r], translation T[r] = m[12 + r] (column-major flat)
     const float* m = viewm + (size_t)view * 16;
     double Rw[3][3], T[3];
@@ -34,10 +43,8 @@ __device__ __forceinline__ ProjRay project_ray_setup(const float* __restrict__ v
     }
     // camera-frame ray of the pixel centre: cone from the source, parallel from (ndc_x, ndc_y, 0), both along +z
     double ndx = (2.0 * u + 1.0) / W - 1.0, ndy = (2.0 * v + 1.0) / H - 1.0;
-    if (SHIFT) {
-        ndx += 2.0 * (double)tu / W;
-        ndy -= 2.0 * (double)tv / H;
-    }
+    ndx += shift.su;
+    ndy -= shift.sv;
     const double oc[3] = {CONE ? 0.0 : ndx, CONE ? 0.0 : ndy, 0.0};
     const double dc[3] = {CONE ? ndx * (double)tanx : 0.0, CONE ? ndy * (double)tany : 0.0, 1.0};
     // to world through the rigid inverse (Rw^T, -Rw^T T), relative to the volume centre

@@ -13,15 +13,15 @@ stream; no CPU fallback.
 
 The plain path weights every view by pi / N, which assumes each ray is measured twice: right for a full 360-degree scan
 and a 180-degree parallel scan, not for a cone-beam short scan (180 degrees plus the fan angle), which it reconstructs
-as a full one with low-frequency shading, as TIGRE's default fdk does.  `short_scan=True` runs r2x_fdk_short_scan
-instead: Parker redundancy weights (Parker 1982, in Silver 2000's overscan form) and each view's own angular interval,
-from `short_scan_views`.  It refuses fewer than 2 views, an arc shorter than 180 degrees plus the fan angle and a full
-circle.  The definition is stated in float64 in tests/fdk_short_scan_oracle.py (the plain FDK's in
+as a full one with low-frequency shading, as TIGRE's default fdk does.  `short_scan=True` runs r2x_fdk with
+R2X_FDK_PARKER instead: Parker redundancy weights (Parker 1982, in Silver 2000's overscan form) and each view's own
+angular interval, from `short_scan_views`.  It refuses fewer than 2 views, an arc shorter than 180 degrees plus the fan
+angle and a full circle.  The definition is stated in float64 in tests/fdk_short_scan_oracle.py (the plain FDK's in
 oracle/fdk_oracle.py).
 
 Without `use_offDetector` the scanner's `offDetector` is ignored (with a warning when it is not zero): the volume is
 reconstructed as if the detector were centred.  `use_offDetector=True` reconstructs through the offset detector
-(r2x_fdk_shifted / r2x_fdk_short_scan_shifted, TIGRE's `geo.offDetector`; the convention is `scene.detector_shift`'s):
+(r2x_fdk's shift_u / shift_v, TIGRE's `geo.offDetector`; the convention is `scene.detector_shift`'s):
 the cosine weight is taken at each pixel's offset position and the backprojection goes through the offset matrices.
 A short scan allows a vertical offset only.  `half_fan=True` (with `use_offDetector`) is for a full-circle scan whose
 detector is shifted sideways to widen the field of view: rays near the axis are measured twice and the outer rays once,
@@ -41,22 +41,29 @@ from ._lib import check, load
 from .scene import MODE_CONE, detector_shift, make_view
 
 SUPPORTED_FILTERS = (None, "ram_lak")
+R2X_FDK_PLAIN, R2X_FDK_PARKER, R2X_FDK_HALF_FAN = 0, 1, 2   # r2x_fdk's weighting (include/r2x.h)
 # slack on the arc refusals: a scan sampled at linspace(0, pi, n + 1)[:-1] covers pi only up to rounding
 ARC_TOLERANCE = 1e-9
+
+
+def _arc_positions(angles):
+    """(beta, arc): each view's position (radians) from the start of the scan, which the largest circular gap between
+    the angles marks, and the arc beta_max + D the views cover with the mean step D = beta_max / (N - 1).  N >= 2."""
+    theta = np.mod(np.asarray(angles, np.float64).reshape(-1), 2.0 * math.pi)
+    N = len(theta)
+    s = np.sort(theta)
+    gaps = np.append(np.diff(s), s[0] + 2.0 * math.pi - s[-1])
+    start = s[(int(np.argmax(gaps)) + 1) % N]
+    beta = np.mod(theta - start, 2.0 * math.pi)
+    return beta, beta.max() + beta.max() / (N - 1)
 
 
 def scan_arc(angles) -> float:
     """The arc (radians) that views at `angles` cover: the circle less its largest gap between the angles, plus the
     mean step between the views (the arc of `short_scan_views`; linspace(0, R, n + 1)[:-1] gives R)."""
-    theta = np.mod(np.asarray(angles, np.float64).reshape(-1), 2.0 * math.pi)
-    N = len(theta)
-    if N < 2:
+    if np.asarray(angles).size < 2:
         return 0.0
-    s = np.sort(theta)
-    gaps = np.append(np.diff(s), s[0] + 2.0 * math.pi - s[-1])
-    start = s[(int(np.argmax(gaps)) + 1) % N]
-    beta = np.mod(theta - start, 2.0 * math.pi)
-    return float(beta.max() + beta.max() / (N - 1))
+    return float(_arc_positions(angles)[1])
 
 
 def half_fan_weight(a, t_u: float, W: int, fan: float):
@@ -86,16 +93,11 @@ def short_scan_views(angles, mode: int, tan_fovx: float):
     sits at beta_v = (theta_v - theta_start) mod 2 pi and stands for an interval of the mean step D = beta_max / (N - 1)
     around it, so beta'_v = beta_v + D / 2 and B = beta_max + D (`linspace(0, R, n + 1)[:-1]` gives B = R).  dbeta_v
     runs between the midpoints of the sorted beta' (0 and B at the ends); views at the same angle share theirs."""
-    theta = np.mod(np.asarray(angles, np.float64).reshape(-1), 2.0 * math.pi)
-    N = len(theta)
+    N = np.asarray(angles).size
     if N < 2:
         raise ValueError(f"fdk short scan: needs at least 2 views, got {N}")
-    s = np.sort(theta)
-    gaps = np.append(np.diff(s), s[0] + 2.0 * math.pi - s[-1])
-    start = s[(int(np.argmax(gaps)) + 1) % N]
-    beta = np.mod(theta - start, 2.0 * math.pi)
-    step = beta.max() / (N - 1)
-    bp, arc = beta + 0.5 * step, beta.max() + step
+    beta, arc = _arc_positions(angles)
+    bp = beta + 0.5 * (beta.max() / (N - 1))
     gamma_max = math.atan(tan_fovx) if mode == MODE_CONE else 0.0
     need = math.pi + 2.0 * gamma_max
     if arc < need - ARC_TOLERANCE:
@@ -150,7 +152,9 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool =
         raise ValueError("fdk: no projections")
     views = [make_view(scanner_cfg, float(a), use_offDetector) for a in angles]
     mode = views[0].mode
+    weighting, view_weights, arc = (R2X_FDK_HALF_FAN if half_fan else R2X_FDK_PLAIN), None, 0.0
     if short_scan:
+        weighting = R2X_FDK_PARKER
         view_weights, arc = short_scan_views(angles, mode, float(views[0].tanfovx))
     nx, ny, nz = (int(v) for v in scanner_cfg["nVoxel"])
     sx, sy, sz = (float(v) for v in scanner_cfg["sVoxel"])
@@ -165,21 +169,10 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool =
         nbytes = int(lib.r2x_fdk_scratch_bytes(N, H, W))
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        tail = (float(views[0].tanfovx), float(views[0].tanfovy), int(mode), float(scanner_cfg["DSO"]), nx, ny, nz, sx,
-                sy, sz, cx, cy, cz, vol.data_ptr(), scratch.data_ptr(), nbytes)
-        if use_offDetector:
-            tail = tail[:3] + (t_u, t_v) + tail[3:]
-        if short_scan:
-            vw = torch.from_numpy(view_weights.astype(np.float32)).to(dev, non_blocking=False)
-            name = "r2x_fdk_short_scan_shifted" if use_offDetector else "r2x_fdk_short_scan"
-            rc = getattr(lib, name)(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), vw.data_ptr(),
-                                    float(arc), *tail)
-        elif use_offDetector:
-            name = "r2x_fdk_shifted"
-            rc = lib.r2x_fdk_shifted(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), *tail[:5],
-                                     int(half_fan), *tail[5:])
-        else:
-            name = "r2x_fdk"
-            rc = lib.r2x_fdk(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), *tail)
-    check(rc, name)
+        vw = None if view_weights is None else torch.from_numpy(view_weights.astype(np.float32)).to(dev)
+        rc = lib.r2x_fdk(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), float(views[0].tanfovx),
+                         float(views[0].tanfovy), int(mode), t_u, t_v, weighting,
+                         None if vw is None else vw.data_ptr(), float(arc), float(scanner_cfg["DSO"]), nx, ny, nz, sx,
+                         sy, sz, cx, cy, cz, vol.data_ptr(), scratch.data_ptr(), nbytes)
+    check(rc, "r2x_fdk")
     return vol

@@ -30,6 +30,7 @@ import os
 import numpy as np
 
 from .dataset import init_point_cloud, read_scene
+from .recon import check_fdk_flags
 from .trainer import default_init_path
 
 # A filtered backprojection from a handful of views is dominated by streaks, and thresholding it gives no useful
@@ -105,16 +106,8 @@ def main(argv=None) -> str:
                     help="with --recon_method fdk and --use_offDetector: half-fan redundancy weights for a full circle "
                          "with the detector shifted sideways")
     a = ap.parse_args(argv)
-    if a.short_scan and a.recon_method != "fdk":
-        raise SystemExit(f"--short_scan applies to --recon_method fdk only, not {a.recon_method}: the iterative methods "
-                         "need no redundancy weights")
-    if a.half_fan and a.recon_method != "fdk":
-        raise SystemExit(f"--half_fan applies to --recon_method fdk only, not {a.recon_method}: the iterative methods "
-                         "need no redundancy weights")
-    if a.half_fan and not a.use_offDetector:
-        raise SystemExit("--half_fan needs --use_offDetector: the half-fan weights follow the detector offset")
-    if a.half_fan and a.short_scan:
-        raise SystemExit("--half_fan and --short_scan cannot be combined (half-fan weights need a full circle)")
+    check_fdk_flags(a, a.recon_method == "fdk", f"{{flag}} applies to --recon_method fdk only, not {a.recon_method}: "
+                    "the iterative methods need no redundancy weights")
     if a.use_offDetector and a.recon_method not in ("fdk", "cgls", "fista_tv"):
         raise SystemExit(f"--use_offDetector applies to --recon_method fdk, cgls or fista_tv, not {a.recon_method}: "
                          "no projections are reconstructed")

@@ -13,9 +13,9 @@ training).  The per-view geometry is the rasterizer's (`scene.make_view`), so th
 construction.  Each pixel is the line integral of the volume's trilinear field, sampled every
 `accuracy * min(dVoxel)` along the ray (`accuracy` defaults to 0.5, as in the reference's scanner files); the exact
 definition is in include/r2x.h.  A scanner whose `offDetector` is not zero is refused unless `use_offDetector=True`,
-which projects through the offset detector (r2x_volume_project_shifted / r2x_volume_backproject_shifted, TIGRE's
-`geo.offDetector`; the convention is `scene.detector_shift`'s) and matches a render() whose cameras carry the same
-offset (`dataset.Scene(use_offDetector=True)`, `scene.make_view(..., use_offDetector=True)`).
+which projects through the offset detector (the shift_u / shift_v of r2x_volume_project / r2x_volume_backproject,
+TIGRE's `geo.offDetector`; the convention is `scene.detector_shift`'s) and matches a render() whose cameras carry the
+same offset (`dataset.Scene(use_offDetector=True)`, `scene.make_view(..., use_offDetector=True)`).
 `backproject` sums every (ray, sample, voxel) triple `project` uses, with the same
 weight, so <project(x), y> = <x, backproject(y)> up to float32 rounding.  Both run on the current stream; no CPU
 fallback.  `CTOperator` binds the pair to one set of angles for repeated use (the iterative solvers).
@@ -55,35 +55,13 @@ def project(volume: torch.Tensor, angles, scanner_cfg: dict, use_offDetector: bo
     if tuple(getattr(volume, "shape", ())) != nvox:
         raise ValueError(f"project: volume shape {tuple(getattr(volume, 'shape', ()))} is not the scanner's nVoxel "
                          f"{list(nvox)}")
-    accuracy = _check_geometry("project", scanner_cfg, use_offDetector)
+    _check_geometry("project", scanner_cfg, use_offDetector)
     if not isinstance(volume, torch.Tensor) or volume.device.type != "cuda":
         raise RuntimeError("project: volume must be a CUDA tensor (this build has no CPU fallback; "
                            f"got {getattr(volume, 'device', type(volume))})")
-    angles =np.asarray(angles, dtype=np.float64).reshape(-1)
-    if len(angles) == 0:
+    if np.asarray(angles, dtype=np.float64).size == 0:
         raise ValueError("project: no angles")
-    views = [make_view(scanner_cfg, float(a)) for a in angles]   # the viewmatrices: the offset is in the kernel's rays
-    N, H, W = len(views), views[0].image_height, views[0].image_width
-    sx, sy, sz = (float(v) for v in scanner_cfg["sVoxel"])
-    cx, cy, cz = (float(v) for v in scanner_cfg["offOrigin"])
-    step = accuracy * min(sx / nvox[0], sy / nvox[1], sz / nvox[2])
-    dev = volume.device
-    lib = load()
-    with torch.cuda.device(dev):
-        vol = volume.detach().to(torch.float32).contiguous()
-        vm = torch.from_numpy(np.stack([v.viewmatrix.reshape(16) for v in views])).to(dev)
-        out = torch.empty((N, H, W), dtype=torch.float32, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        head = (*nvox, vol.data_ptr(), sx, sy, sz, cx, cy, cz, N, H, W, vm.data_ptr(), float(views[0].tanfovx),
-                float(views[0].tanfovy), int(views[0].mode))
-        if use_offDetector:
-            name = "r2x_volume_project_shifted"
-            rc = lib.r2x_volume_project_shifted(stream, *head, *detector_shift(scanner_cfg), step, out.data_ptr())
-        else:
-            name = "r2x_volume_project"
-            rc = lib.r2x_volume_project(stream, *head, step, out.data_ptr())
-    check(rc, name)
-    return out
+    return CTOperator(angles, scanner_cfg, volume.device, use_offDetector).A(volume)
 
 
 class CTOperator:
@@ -100,7 +78,7 @@ class CTOperator:
         if len(angles) == 0:
             raise ValueError("backproject: no angles")
         views = [make_view(scanner_cfg, float(a), use_offDetector) for a in angles]
-        self.shift = detector_shift(scanner_cfg) if use_offDetector else None
+        self.shift = detector_shift(scanner_cfg) if use_offDetector else (0.0, 0.0)
         self.device = torch.device(device)
         self.nvox = tuple(int(v) for v in scanner_cfg["nVoxel"])
         self.N, self.H, self.W = len(views), views[0].image_height, views[0].image_width
@@ -126,15 +104,10 @@ class CTOperator:
                 raise ValueError(f"project: volume shape {tuple(vol.shape)} is not the scanner's nVoxel {list(self.nvox)}")
             out = torch.empty((n, self.H, self.W), dtype=torch.float32, device=self.device)
             stream = torch.cuda.current_stream(self.device).cuda_stream
-            head = (*self.nvox, vol.data_ptr(), *self.size, *self.centre, n, self.H, self.W, self.vm[v0].data_ptr(),
-                    self.tanx, self.tany, self.mode)
-            if self.shift is not None:
-                name = "r2x_volume_project_shifted"
-                rc = self.lib.r2x_volume_project_shifted(stream, *head, *self.shift, self.step, out.data_ptr())
-            else:
-                name = "r2x_volume_project"
-                rc = self.lib.r2x_volume_project(stream, *head, self.step, out.data_ptr())
-        check(rc, name)
+            rc = self.lib.r2x_volume_project(stream, *self.nvox, vol.data_ptr(), *self.size, *self.centre, n, self.H,
+                                             self.W, self.vm[v0].data_ptr(), self.tanx, self.tany, self.mode,
+                                             *self.shift, self.step, out.data_ptr())
+        check(rc, "r2x_volume_project")
         return out
 
     def At(self, y: torch.Tensor, views: slice = slice(None), weights: bool = False):
@@ -149,17 +122,11 @@ class CTOperator:
             nbytes = int(self.lib.r2x_volume_backproject_scratch_bytes(n, self.H, self.W))
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
             stream = torch.cuda.current_stream(self.device).cuda_stream
-            head = (n, self.H, self.W, projs.data_ptr(), self.vm[v0].data_ptr(), self.pm[v0].data_ptr(), self.tanx,
-                    self.tany, self.mode)
-            tail = (*self.nvox, *self.size, *self.centre, self.step, vol.data_ptr(),
-                    wgt.data_ptr() if weights else None, scratch.data_ptr(), nbytes)
-            if self.shift is not None:
-                name = "r2x_volume_backproject_shifted"
-                rc = self.lib.r2x_volume_backproject_shifted(stream, *head, *self.shift, *tail)
-            else:
-                name = "r2x_volume_backproject"
-                rc = self.lib.r2x_volume_backproject(stream, *head, *tail)
-        check(rc, name)
+            rc = self.lib.r2x_volume_backproject(stream, n, self.H, self.W, projs.data_ptr(), self.vm[v0].data_ptr(),
+                                                 self.pm[v0].data_ptr(), self.tanx, self.tany, self.mode, *self.shift,
+                                                 *self.nvox, *self.size, *self.centre, self.step, vol.data_ptr(),
+                                                 wgt.data_ptr() if weights else None, scratch.data_ptr(), nbytes)
+        check(rc, "r2x_volume_backproject")
         return (vol, wgt) if weights else vol
 
 

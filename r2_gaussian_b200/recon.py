@@ -244,6 +244,18 @@ def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, sh
     raise ValueError(f"recon_volume: unknown method {method!r} (supported: {', '.join(METHODS)})")
 
 
+def check_fdk_flags(args, fdk_selected: bool, not_fdk: str):
+    """The refusals of the FDK flags (--short_scan, --half_fan) that the recon and initialize_pcd CLIs share; `not_fdk`
+    is the CLI's message for a flag given without the fdk method, with `{flag}` standing for the flag."""
+    for flag, on in (("--short_scan", args.short_scan), ("--half_fan", args.half_fan)):
+        if on and not fdk_selected:
+            raise SystemExit(not_fdk.format(flag=flag))
+    if args.half_fan and not args.use_offDetector:
+        raise SystemExit("--half_fan needs --use_offDetector: the half-fan weights follow the detector offset")
+    if args.half_fan and args.short_scan:
+        raise SystemExit("--half_fan and --short_scan cannot be combined (half-fan weights need a full circle)")
+
+
 def _parse_methods(text: str) -> list[str]:
     methods = [m.strip() for m in text.split(",") if m.strip()]
     for m in methods:
@@ -271,16 +283,8 @@ def main(argv=None) -> dict:
                          "the detector shifted sideways)")
     a = ap.parse_args(argv)
     methods = _parse_methods(a.methods)
-    if a.short_scan and "fdk" not in methods:
-        raise SystemExit("--short_scan applies to the fdk method, which --methods does not include (the iterative "
-                         "methods need no redundancy weights)")
-    if a.half_fan and "fdk" not in methods:
-        raise SystemExit("--half_fan applies to the fdk method, which --methods does not include (the iterative "
-                         "methods need no redundancy weights)")
-    if a.half_fan and not a.use_offDetector:
-        raise SystemExit("--half_fan needs --use_offDetector: the half-fan weights follow the detector offset")
-    if a.half_fan and a.short_scan:
-        raise SystemExit("--half_fan and --short_scan cannot be combined (half-fan weights need a full circle)")
+    check_fdk_flags(a, "fdk" in methods, "{flag} applies to the fdk method, which --methods does not include (the "
+                    "iterative methods need no redundancy weights)")
     if not torch.cuda.is_available():
         raise SystemExit("the reconstructions need a CUDA device: they run on the GPU and have no CPU fallback")
     import yaml

@@ -1,11 +1,11 @@
-"""Cost and quality of the short-scan FDK (r2x_fdk_short_scan) against the plain one (r2x_fdk):
+"""Cost and quality of the short-scan FDK (r2x_fdk with R2X_FDK_PARKER) against the plain one (R2X_FDK_PLAIN):
 
     python scripts/gpu/fdk_short_scan_bench.py [--reps 20] [--out DIR]
 
 Time: the fdk row of scripts/secondary.py (50 seeded cone-beam views of 512^2 into 256^3), the plain call on the full
 circle and the short-scan call on 220 degrees, alternated, each timed with CUDA events (median of --reps).  The filter
-kernels (fdk_filter_kernel, fdk_parker_filter_kernel) and the backprojection are timed in a separate torch.profiler
-run.  Quality: recon_baselines.py's seeded 256^3 phantom and noisy cone-beam scanner, 50 train views at 220 degrees
+kernels (fdk_filter_kernel<R2X_FDK_PLAIN>, fdk_filter_kernel<R2X_FDK_PARKER>) and the backprojection are timed in a
+separate torch.profiler run.  Quality: recon_baselines.py's seeded 256^3 phantom and noisy cone-beam scanner, 50 train views at 220 degrees
 reconstructed by plain and short-scan FDK, and 82 train views on the full circle (the same view density) by plain FDK;
 3D PSNR / SSIM against the phantom.  Prints one JSON line with the card name and power limit."""
 from __future__ import annotations
@@ -31,7 +31,7 @@ def timing(dev, reps: int) -> dict:
     import torch
 
     from r2_gaussian_b200 import _lib, scene
-    from r2_gaussian_b200.fdk import short_scan_views
+    from r2_gaussian_b200.fdk import R2X_FDK_PARKER, R2X_FDK_PLAIN, short_scan_views
 
     lib = _lib.load()
     sc = scene.cone_beam_scanner(512, 256)
@@ -54,15 +54,15 @@ def timing(dev, reps: int) -> dict:
     vw = torch.tensor(vw_host.astype(np.float32), device=dev)
     tx, ty, dso = float(v0.tanfovx), float(v0.tanfovy), float(sc["DSO"])
     stream = lambda: torch.cuda.current_stream(dev).cuda_stream
-    tail = (tx, ty, 1, dso, *grid, vol.data_ptr(), scratch.data_ptr(), nbytes)
+    tail = (dso, *grid, vol.data_ptr(), scratch.data_ptr(), nbytes)
 
     def plain():
-        _lib.check(lib.r2x_fdk(stream(), N, H, W, projs.data_ptr(), vm_full.data_ptr(), pm_full.data_ptr(), *tail),
-                   "r2x_fdk")
+        _lib.check(lib.r2x_fdk(stream(), N, H, W, projs.data_ptr(), vm_full.data_ptr(), pm_full.data_ptr(), tx, ty, 1,
+                               0.0, 0.0, R2X_FDK_PLAIN, None, 0.0, *tail), "r2x_fdk")
 
     def short():
-        _lib.check(lib.r2x_fdk_short_scan(stream(), N, H, W, projs.data_ptr(), vm_short.data_ptr(), pm_short.data_ptr(),
-                                          vw.data_ptr(), float(arc), *tail), "r2x_fdk_short_scan")
+        _lib.check(lib.r2x_fdk(stream(), N, H, W, projs.data_ptr(), vm_short.data_ptr(), pm_short.data_ptr(), tx, ty, 1,
+                               0.0, 0.0, R2X_FDK_PARKER, vw.data_ptr(), float(arc), *tail), "r2x_fdk")
 
     for f in (plain, short, plain, short):                  # warm-up of both shapes
         f()
@@ -88,7 +88,7 @@ def timing(dev, reps: int) -> dict:
         torch.cuda.synchronize(dev)
     kernels = {}
     for ev in prof.key_averages():
-        for key in ("fdk_parker_filter_kernel", "fdk_filter_kernel", "fdk_backproject_kernel"):
+        for key in ("fdk_filter_kernel<1>", "fdk_filter_kernel<0>", "fdk_backproject_kernel"):
             if key in ev.key:
                 t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0.0)
                 k = kernels.setdefault(key, [0.0, 0])
@@ -97,8 +97,8 @@ def timing(dev, reps: int) -> dict:
                 break
     for key, (t_us, count) in kernels.items():
         row[key + "_ms"] = t_us / count / 1e3
-    if "fdk_filter_kernel_ms" in row and "fdk_parker_filter_kernel_ms" in row:
-        row["filter_ratio"] = row["fdk_parker_filter_kernel_ms"] / row["fdk_filter_kernel_ms"]
+    if "fdk_filter_kernel<0>_ms" in row and "fdk_filter_kernel<1>_ms" in row:
+        row["filter_ratio"] = row["fdk_filter_kernel<1>_ms"] / row["fdk_filter_kernel<0>_ms"]
     row["call_ratio"] = row["short_call_ms"] / row["plain_call_ms"]
     return row
 
@@ -150,8 +150,8 @@ def main() -> None:
     dev = torch.device("cuda")
     out = a.out or tempfile.mkdtemp(prefix="fdk_short_scan_")
     os.makedirs(out, exist_ok=True)
-    row = {"workload": f"FDK, {N_VIEWS} cone-beam views of 512x512 (DSD 7, DSO 5) -> 256^3: r2x_fdk on 360 degrees "
-                       f"against r2x_fdk_short_scan on {ARC_DEG:g} degrees", **timing(dev, a.reps)}
+    row = {"workload": f"FDK, {N_VIEWS} cone-beam views of 512x512 (DSD 7, DSO 5) -> 256^3: r2x_fdk(R2X_FDK_PLAIN) on 360 "
+                       f"degrees against r2x_fdk(R2X_FDK_PARKER) on {ARC_DEG:g} degrees", **timing(dev, a.reps)}
     row["quality"] = quality(out)
     print(json.dumps({**row, **secondary.card(dev)}))
 

@@ -346,7 +346,7 @@ def measure_project(dev, timed) -> dict:
 
     def run(_i):
         _lib.check(lib.r2x_volume_project(torch.cuda.current_stream(dev).cuda_stream, n, n, n, vol.data_ptr(), 2.0, 2.0,
-                                          2.0, 0.0, 0.0, 0.0, N, H, W, vm.data_ptr(), tx, ty, 1, step,
+                                          2.0, 0.0, 0.0, 0.0, N, H, W, vm.data_ptr(), tx, ty, 1, 0.0, 0.0, step,
                                           projs.data_ptr()), "r2x_volume_project")
 
     row = {"workload": "forward projection, seeded 256^3 volume -> 150 cone-beam views (50 train + 100 test) of "
@@ -366,6 +366,7 @@ def measure_fdk(dev, timed) -> dict:
     import torch
 
     from r2_gaussian_b200 import _lib, scene
+    from r2_gaussian_b200.fdk import R2X_FDK_PLAIN
 
     lib = _lib.load()
     sc = scene.cone_beam_scanner(512, 256)
@@ -390,8 +391,9 @@ def measure_fdk(dev, timed) -> dict:
                                            vol.data_ptr()), "r2x_fdk_backproject")
 
     def total(_i):
-        _lib.check(lib.r2x_fdk(stream(), N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), tx, ty, 1, dso, *grid,
-                               vol.data_ptr(), scratch.data_ptr(), nbytes), "r2x_fdk")
+        _lib.check(lib.r2x_fdk(stream(), N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), tx, ty, 1, 0.0, 0.0,
+                               R2X_FDK_PLAIN, None, 0.0, dso, *grid, vol.data_ptr(), scratch.data_ptr(), nbytes),
+                   "r2x_fdk")
 
     row = {"workload": "FDK, 50 cone-beam views of 512x512 (DSD 7, DSO 5) -> 256^3 volume, Ram-Lak filter + voxel-driven "
                        "backprojection (r2x_fdk)",

@@ -1,6 +1,7 @@
 """The FDK definition (oracle/fdk_oracle.py) on the CPU: amplitude pinned by an analytic ball, geometry pinned by a round
 trip through the rasterizer and voxelizer oracles; argument checks of the C ABI and of fdk() that need no GPU."""
 import ctypes
+import math
 
 import numpy as np
 import pytest
@@ -68,18 +69,20 @@ def test_abi_rejects_bad_arguments_before_any_cuda_call():
     lib = _lib.load()
     assert lib.r2x_fdk_scratch_bytes(50, 512, 512) >= 50 * 512 * 512 * 4
     dummy = ctypes.c_void_p(16)
-    base = dict(N=2, H=8, W=8, mode=1, dso=5.0, n=4, s=2.0)
+    base = dict(N=2, H=8, W=8, mode=1, su=0.0, sv=0.0, weighting=0, w=None, arc=0.0, dso=5.0, n=4, s=2.0, nbytes=1 << 20)
 
     def call(**kw):
         a = dict(base, **kw)
-        return lib.r2x_fdk(None, a["N"], a["H"], a["W"], dummy, dummy, dummy, 0.3, 0.3, a["mode"], a["dso"], a["n"],
-                           a["n"], a["n"], a["s"], a["s"], a["s"], 0.0, 0.0, 0.0, dummy, dummy, 1 << 20)
+        return lib.r2x_fdk(None, a["N"], a["H"], a["W"], dummy, dummy, dummy, 0.3, 0.3, a["mode"], a["su"], a["sv"],
+                           a["weighting"], a["w"], a["arc"], a["dso"], a["n"], a["n"], a["n"], a["s"], a["s"], a["s"], 0.0,
+                           0.0, 0.0, dummy, dummy, a["nbytes"])
 
-    for kw in (dict(N=0), dict(H=0), dict(W=0), dict(n=0), dict(mode=2), dict(dso=0.0), dict(s=0.0)):
+    for kw in (dict(N=0), dict(H=0), dict(W=0), dict(n=0), dict(mode=2), dict(dso=0.0), dict(s=0.0),
+               dict(su=math.nan), dict(sv=math.inf), dict(weighting=3), dict(weighting=-1),
+               dict(weighting=2, su=0.0), dict(weighting=2, su=4.0), dict(weighting=2, su=-4.0)):
         assert call(**kw) != 0, kw
         assert b"bad" in lib.r2x_last_error(), kw
-    assert lib.r2x_fdk(None, 2, 8, 8, dummy, dummy, dummy, 0.3, 0.3, 1, 5.0, 4, 4, 4, 2.0, 2.0, 2.0, 0.0, 0.0, 0.0,
-                       dummy, dummy, 16) != 0                  # scratch too small
+    assert call(nbytes=16) != 0                                 # scratch too small
     assert b"scratch" in lib.r2x_last_error()
 
 

@@ -195,19 +195,19 @@ def test_abi_rejects_bad_arguments_before_any_cuda_call():
     lib = _lib.load()
     dummy = ctypes.c_void_p(16)
     tx = 0.3
-    base = dict(N=2, H=8, W=8, mode=1, dso=5.0, n=4, s=2.0, w=dummy, arc=math.radians(220.0))
+    base = dict(N=2, H=8, W=8, mode=1, su=0.0, dso=5.0, n=4, s=2.0, w=dummy, arc=math.radians(220.0), nbytes=1 << 20)
 
     def call(**kw):
         a = dict(base, **kw)
-        return lib.r2x_fdk_short_scan(None, a["N"], a["H"], a["W"], dummy, dummy, dummy, a["w"], a["arc"], tx, tx,
-                                      a["mode"], a["dso"], a["n"], a["n"], a["n"], a["s"], a["s"], a["s"], 0.0, 0.0,
-                                      0.0, dummy, dummy, 1 << 20)
+        return lib.r2x_fdk(None, a["N"], a["H"], a["W"], dummy, dummy, dummy, tx, tx, a["mode"], a["su"], 0.0, 1, a["w"],
+                           a["arc"], a["dso"], a["n"], a["n"], a["n"], a["s"], a["s"], a["s"], 0.0, 0.0, 0.0, dummy, dummy,
+                           a["nbytes"])
 
     for kw in (dict(N=0), dict(N=1), dict(H=0), dict(W=0), dict(n=0), dict(mode=2), dict(dso=0.0), dict(s=0.0),
                dict(w=None), dict(arc=0.0), dict(arc=2.0 * math.pi), dict(arc=float("nan")),
-               dict(arc=math.pi + 2.0 * math.atan(tx) - 1e-3), dict(mode=0, arc=math.pi - 1e-3)):
+               dict(arc=math.pi + 2.0 * math.atan(tx) - 1e-3), dict(mode=0, arc=math.pi - 1e-3), dict(su=0.5),
+               dict(su=-1.0)):
         assert call(**kw) != 0, kw
         assert b"bad" in lib.r2x_last_error(), kw
-    assert lib.r2x_fdk_short_scan(None, 2, 8, 8, dummy, dummy, dummy, dummy, math.radians(220.0), tx, tx, 1, 5.0, 4, 4,
-                                  4, 2.0, 2.0, 2.0, 0.0, 0.0, 0.0, dummy, dummy, 16) != 0      # scratch too small
+    assert call(nbytes=16) != 0                                 # scratch too small
     assert b"scratch" in lib.r2x_last_error()

@@ -1,5 +1,5 @@
-"""Short-scan FDK on the GPU (fdk(short_scan=True) over r2x_fdk_short_scan) against the float64 oracle, bitwise
-reproducibility, the 180-degree parallel case, the render -> fdk -> query round trip at 220 degrees, and
+"""Short-scan FDK on the GPU (fdk(short_scan=True) over r2x_fdk with R2X_FDK_PARKER) against the float64 oracle,
+bitwise reproducibility, the 180-degree parallel case, the render -> fdk -> query round trip at 220 degrees, and
 `initialize_pcd --recon_method fdk --short_scan --evaluate` on a generate_data scene."""
 import json
 import math

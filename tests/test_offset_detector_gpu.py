@@ -98,6 +98,30 @@ def test_offset_fdk_matches_oracle(mode, half_fan):
     assert err <= 1e-4 * np.abs(want).max(), (err, np.abs(want).max())
 
 
+@pytest.mark.parametrize("op", ["project", "backproject", "fdk", "fdk_short_scan"])
+@pytest.mark.parametrize("mode", ["cone", "parallel"])
+def test_zero_offset_is_the_centred_result_bit_for_bit(mode, op):
+    """offDetector = [0, 0] with use_offDetector=True adds exact zeros to every ray and cosine weight: each output is
+    the centred one bit for bit (the backprojector's weights included)."""
+    torch = _torch()
+    from r2_gaussian_b200.fdk import fdk
+    from r2_gaussian_b200.projector import backproject, project
+
+    det, vox = (24, 40), (20, 28, 12)
+    sc = dict(_scanner(mode, det, vox, (1.6, 1.8, 1.2), (0.1, -0.2, 0.15), 0.5), offDetector=[0.0, 0.0])
+    rng = np.random.RandomState(7)
+    angles = np.linspace(0.0, math.radians(240.0), 21)[:-1] if op == "fdk_short_scan" else fc.full_scan(12) + 0.2
+    x = torch.tensor(rng.uniform(0.0, 1.0, vox).astype(np.float32), device="cuda")
+    y = torch.tensor(rng.uniform(0.0, 1.0, (len(angles), *det)).astype(np.float32), device="cuda")
+    run = {"project": lambda off: (project(x, angles, sc, use_offDetector=off),),
+           "backproject": lambda off: backproject(y, angles, sc, weights=True, use_offDetector=off),
+           "fdk": lambda off: (fdk(y, angles, sc, use_offDetector=off),),
+           "fdk_short_scan": lambda off: (fdk(y, angles, sc, short_scan=True, use_offDetector=off),)}[op]
+    for centred, offset in zip(run(False), run(True)):
+        assert float(centred.abs().max()) > 0.0
+        assert torch.equal(centred.view(torch.int32), offset.view(torch.int32))
+
+
 def test_offset_short_scan_fdk_takes_a_vertical_offset():
     """Parker-weighted FDK with a vertical offset against the centred short scan of the row-moved projections."""
     torch = _torch()

@@ -56,18 +56,20 @@ def test_abi_rejects_bad_arguments_before_any_cuda_call():
 
     lib = _lib.load()
     dummy = ctypes.c_void_p(16)
-    base = dict(n=4, vol=dummy, s=2.0, c=0.0, N=2, H=8, W=8, vm=dummy, tan=0.3, mode=1, step=0.25, out=dummy)
+    base = dict(n=4, vol=dummy, s=2.0, c=0.0, N=2, H=8, W=8, vm=dummy, tan=0.3, mode=1, su=0.0, sv=0.0, step=0.25,
+                out=dummy)
 
     def call(**kw):
         a = dict(base, **kw)
         return lib.r2x_volume_project(None, a["n"], a["n"], a["n"], a["vol"], a["s"], a["s"], a["s"], a["c"], a["c"],
-                                      a["c"], a["N"], a["H"], a["W"], a["vm"], a["tan"], a["tan"], a["mode"],
-                                      a["step"], a["out"])
+                                      a["c"], a["N"], a["H"], a["W"], a["vm"], a["tan"], a["tan"], a["mode"], a["su"],
+                                      a["sv"], a["step"], a["out"])
 
     bad = (dict(n=0), dict(N=0), dict(H=0), dict(W=0), dict(H=65535 * 32 + 1), dict(mode=2), dict(mode=-1),
            dict(s=0.0), dict(s=-1.0), dict(s=math.inf), dict(s=math.nan), dict(c=math.nan), dict(tan=0.0),
            dict(tan=math.inf), dict(step=0.0), dict(step=-0.1), dict(step=math.nan), dict(step=math.inf),
-           dict(vol=None), dict(vm=None), dict(out=None))
+           dict(vol=None), dict(vm=None), dict(out=None), dict(su=math.nan), dict(su=-math.inf), dict(sv=math.nan),
+           dict(sv=math.inf))
     for kw in bad:
         assert call(**kw) != 0, kw
         assert b"r2x_volume_project: bad" in lib.r2x_last_error(), kw

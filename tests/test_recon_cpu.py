@@ -41,20 +41,22 @@ def test_abi_rejects_bad_arguments_before_any_cuda_call():
     dummy = ctypes.c_void_p(16)
     need = int(lib.r2x_volume_backproject_scratch_bytes(2, 8, 8))
     assert need >= 2 * 8 * 8 * 32
-    base = dict(N=2, H=8, W=8, projs=dummy, vm=dummy, pm=dummy, tan=0.3, mode=1, n=4, nx=4, s=2.0, c=0.0, step=0.25,
-                out=dummy, wgt=None, scratch=dummy, nbytes=need)
+    base = dict(N=2, H=8, W=8, projs=dummy, vm=dummy, pm=dummy, tan=0.3, mode=1, su=0.0, sv=0.0, n=4, nx=4, s=2.0,
+                c=0.0, step=0.25, out=dummy, wgt=None, scratch=dummy, nbytes=need)
 
     def call(**kw):
         a = dict(base, **kw)
         return lib.r2x_volume_backproject(None, a["N"], a["H"], a["W"], a["projs"], a["vm"], a["pm"], a["tan"],
-                                          a["tan"], a["mode"], a["nx"], a["n"], a["n"], a["s"], a["s"], a["s"], a["c"],
-                                          a["c"], a["c"], a["step"], a["out"], a["wgt"], a["scratch"], a["nbytes"])
+                                          a["tan"], a["mode"], a["su"], a["sv"], a["nx"], a["n"], a["n"], a["s"], a["s"],
+                                          a["s"], a["c"], a["c"], a["c"], a["step"], a["out"], a["wgt"], a["scratch"],
+                                          a["nbytes"])
 
     bad = (dict(n=0), dict(nx=0), dict(nx=65536), dict(n=4 * 65535 + 1), dict(N=0), dict(H=0), dict(W=0),
            dict(mode=2), dict(mode=-1), dict(s=0.0), dict(s=-1.0), dict(s=math.inf), dict(s=math.nan),
            dict(c=math.nan), dict(tan=0.0), dict(tan=math.inf), dict(step=0.0), dict(step=-0.1), dict(step=math.nan),
            dict(step=math.inf), dict(step=1e-8), dict(projs=None), dict(vm=None), dict(pm=None), dict(out=None),
-           dict(scratch=None), dict(nbytes=need - 1))
+           dict(scratch=None), dict(nbytes=need - 1), dict(su=math.nan), dict(su=math.inf), dict(sv=-math.inf),
+           dict(sv=math.nan))
     for kw in bad:
         assert call(**kw) != 0, kw
         assert b"r2x_volume_backproject: bad" in lib.r2x_last_error(), kw
