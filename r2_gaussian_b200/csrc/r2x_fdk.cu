@@ -11,7 +11,7 @@
 //                           rows of zeros, then the band-limited Ram-Lak filter as a linear convolution over the whole
 //                           row, using the symmetric odd-only taps:
 //                             Q_j = (r_j / 4 - sum_{k odd} (r_{j-k} + r_{j+k}) / (pi^2 k^2)) / D
-//                           (D = isocentre pitch), summed for k = 1, 3, 5, ... in that order.
+//                           (D = isocentre pitch), summed from the largest odd k < W down to k = 1.
 //   fdk_backproject_kernel  a thread owns one (x, y) voxel column and a run of FDK_ZR voxels along z.  Every view's
 //                           homogeneous coordinates are affine in z, so the per-view setup (4 matrix rows, staged per
 //                           chunk of views in shared memory) is paid once per run.  Each voxel centre goes through the
@@ -208,8 +208,10 @@ __global__ void __launch_bounds__(256) fdk_filter_kernel(int H, int W, const flo
     __syncthreads();
     for (int j = threadIdx.x; j < W; j += blockDim.x) {
         const float* c = row + W + j;
+        // smallest taps first: summed from k = 1 up, the accumulator is near r_j / 4 after a few taps and every tap
+        // below half its ulp (k beyond ~3700) is lost, which truncated the filter on wide rows
         float acc = 0.0f;
-        for (int m = 0, k = 1; k < W; ++m, k += 2) acc = fmaf(g[m], c[-k] + c[k], acc);
+        for (int m = W / 2 - 1; m >= 0; --m) acc = fmaf(g[m], c[-(2 * m + 1)] + c[2 * m + 1], acc);
         q[r * W + j] = fmaf(0.25f, c[0], -acc) * inv_delta;
     }
 }
