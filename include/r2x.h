@@ -487,6 +487,25 @@ size_t r2x_tv_value_scratch_bytes(int nx, int ny, int nz);
 int r2x_tv_value(void* stream, int nx, int ny, int nz, const float* x, double* out, void* scratch,
                  size_t scratch_bytes);
 
+/* ---- real-scan projection preparation (r2_gaussian_b200/generate_real_data.py) ---------------------------------- */
+/* Replaces the reference's per-view numpy + cv2 chain (data_generator/real_dataset/generate_data.py:91-109).
+ * img[n_views, H0, W0] (device, float64: the processed scan's `img` arrays) -> out[n_views, H, W] (device, float32):
+ *   1. p = float32(img / proj_rescale * object_scale), both operations in float64, one rounding;
+ *   2. p < 0 -> 0 (-0 and NaN are kept);
+ *   3. the image moves up 5 rows, zero fill (row r takes row r + 5);
+ *   4. subsample != 1: resize to int(H0 / subsample) x int(W0 / subsample) as cv2.resize's float32 INTER_LINEAR does
+ *      on the x86-64 OpenCV builds (their IPP path; tests/real_data_oracle.py states it): per axis the source position
+ *      (d + 0.5) (src / dst) - 0.5 in float64, float32 fraction t, fma(t, b - a, a) along the columns, then along
+ *      the rows, the last source sample repeated at the far edge; then the longer axis is centre-cropped by
+ *      int(diff / 2) on each side (a difference of 1 crops nothing).  subsample 1 neither resizes nor crops.
+ * r2x_projection_prepare_shape writes (H, W) to out_hw[2] without touching the GPU.  Arguments are checked before any
+ * CUDA work (n_views >= 1, H0, W0, subsample >= 1, a resized size >= 1, H * W < 2^31, proj_rescale finite and
+ * non-zero, object_scale finite).  Deterministic (no atomics; each output depends only on its view, so any split of the
+ * views into calls gives the same bits).  Asynchronous on `stream`.  n_views * H0 * W0 is indexed in 64 bits. */
+int r2x_projection_prepare_shape(int H0, int W0, int subsample, int* out_hw);
+int r2x_projection_prepare(void* stream, int n_views, int H0, int W0, int subsample, const double* img,
+                           double proj_rescale, double object_scale, float* out);
+
 /* ---- multi-GPU exchange step: one-shot sum over NVLink peer memory ------------------------------ */
 /* The Gaussian-sharded projector (one process per GPU, every rank renders its index shard) needs ONE exchange per
  * projection: the sum of the per-rank partial detector images (BASELINE north_star; the reference itself is

@@ -101,6 +101,8 @@ PROTOTYPES = {
     "r2x_tv_prox": (_i, [_vp, _i, _i, _i, _vp, _f, _i, _i, _vp, _vp, _sz]),
     "r2x_tv_value_scratch_bytes": (_sz, [_i, _i, _i]),
     "r2x_tv_value": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _sz]),
+    "r2x_projection_prepare_shape": (_i, [_i, _i, _i, C.POINTER(_i)]),
+    "r2x_projection_prepare": (_i, [_vp, _i, _i, _i, _i, _vp, C.c_double, C.c_double, _vp]),
     "r2x_peer_alloc": (_i, [_sz, C.POINTER(_vp)]),
     "r2x_peer_free": (_i, [_vp]),
     "r2x_ipc_export": (_i, [_vp, _vp]),
