@@ -374,8 +374,18 @@ int r2x_gather_rows(void* stream, int ntensors, const r2x_gather_desc* descs, co
  * the scene-scaled units of the dataset readers.  projs[N,H,W] (rows = v, columns = u); viewmatrices / projmatrices
  * [N,16] are the rasterizer's per-view matrices, tan_fovx / tan_fovy the values render() passes (parallel beam: 1).
  *   1. cone beam: cosine weight P * DSD / sqrt(DSD^2 + u^2 + v^2) at the pixel centres;
- *   2. band-limited Ram-Lak filter along each row, linear convolution, at the isocentre pitch D (cone:
- *      dDetector_u * DSO / DSD = 2 tan_fovx DSO / W; parallel: 2 / W, the rasterizer's detector spans ndc [-1,1]);
+ *   2. ramp filter along each row, linear convolution over the whole row (0 beyond it), at the isocentre pitch D (cone:
+ *      dDetector_u * DSO / DSD = 2 tan_fovx DSO / W; parallel: 2 / W, the rasterizer's detector spans ndc [-1,1]):
+ *      Q_j = (1 / D) sum_k h[k] P'_{j-k} with the taps h[k] = (1 / 2 pi^2) int_0^pi w Wn(w) cos(w k) dw of the filter
+ *      field of `weighting` (TIGRE's `geo.filter` windows at frequency scale 1; tests/fdk_window_oracle.py):
+ *        R2X_FDK_RAM_LAK      Wn = 1, the band-limited Ram-Lak filter: h[0] = 1/4, h[k odd] = -1 / (pi^2 k^2), 0 at
+ *                             even k != 0 (oracle/fdk_oracle.py);
+ *        R2X_FDK_SHEPP_LOGAN  Wn = sin(w/2) / (w/2): h[k] = -2 / (pi^2 (4k^2 - 1));
+ *        R2X_FDK_COSINE       Wn = cos(w/2): h[k] = -(-1)^k / (pi (4k^2 - 1)) - (1/(2k+1)^2 + 1/(2k-1)^2) / pi^2;
+ *        R2X_FDK_HAMMING      Wn = 0.54 + 0.46 cos w: h[k] = 0.54 h_RL[k] + 0.23 (h_RL[k-1] + h_RL[k+1]);
+ *        R2X_FDK_HANN         Wn = (1 + cos w) / 2: h[k] = 0.5 h_RL[k] + 0.25 (h_RL[k-1] + h_RL[k+1]);
+ *      (h_RL = the Ram-Lak taps).  The filter changes the taps only: steps 1 and 3, the pitch, the redundancy weights
+ *      and the scale are the same for every filter;
  *   3. voxel-driven backprojection: voxel centres center - s/2 + (i + 1/2) s/n, projected through projmatrix and the
  *      rasterizer's ndc -> pixel mapping, bilinear sample (0 outside the detector), weight U^2 with U = DSO / z_view
  *      (cone; 0 for z_view <= 0) or 1 (parallel); out_volume[nx,ny,nz] = (pi / N) * sum over views in index order.
@@ -385,7 +395,9 @@ int r2x_gather_rows(void* stream, int ntensors, const r2x_gather_desc* descs, co
  * ray of the centred detector's fractional pixel (i - t_v, j + t_u), so step 1 takes its cosine weight at ndc
  * ((2j+1)/W - 1 + 2 t_u/W, (2i+1)/H - 1 - 2 t_v/H); step 3 goes through the caller's projmatrices, which must be the
  * offset ones (scene.make_view(..., use_offDetector=True)).  A zero offset gives the centred result bit for bit.
- * weighting (the redundancy weight step 1 also applies; the plain FDK's is oracle/fdk_oracle.py):
+ * weighting = one redundancy weight below OR-ed with one filter of step 2 (R2X_FDK_RAM_LAK is 0, so a bare weight is
+ * Ram-Lak); any other bit or value is refused.  The redundancy weight step 1 also applies (the plain FDK's is
+ * oracle/fdk_oracle.py):
  *   R2X_FDK_PLAIN     none.  It reconstructs a cone-beam short scan as if it were a full one (as TIGRE's default fdk).
  *   R2X_FDK_PARKER    a short scan (Parker 1982, in Silver 2000's overscan form; tests/fdk_short_scan_oracle.py): an arc
  *                     B = arc with pi + 2 gamma_max <= B < 2 pi (gamma_max = atan(tan_fovx) for cone beam, 0 for
@@ -409,12 +421,17 @@ int r2x_gather_rows(void* stream, int ntensors, const r2x_gather_desc* descs, co
 #define R2X_FDK_PLAIN 0
 #define R2X_FDK_PARKER 1
 #define R2X_FDK_HALF_FAN 2
+#define R2X_FDK_RAM_LAK 0x000
+#define R2X_FDK_SHEPP_LOGAN 0x100
+#define R2X_FDK_COSINE 0x200
+#define R2X_FDK_HAMMING 0x300
+#define R2X_FDK_HANN 0x400
 size_t r2x_fdk_scratch_bytes(int n_views, int H, int W);
 int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
             const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
             int weighting, const float* view_weights, float arc, float dso, int nx, int ny, int nz, float sx, float sy,
             float sz, float cx, float cy, float cz, float* out_volume, void* scratch, size_t scratch_bytes);
-/* The two stages of r2x_fdk on their own (measurement; centred, R2X_FDK_PLAIN): filtered[N,H,W] = steps 1-2;
+/* The two stages of r2x_fdk on their own (measurement; centred, R2X_FDK_PLAIN, Ram-Lak): filtered[N,H,W] = steps 1-2;
  * out_volume = step 3 of it. */
 int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, float tan_fovx, float tan_fovy,
                    int mode, float dso, float* filtered);

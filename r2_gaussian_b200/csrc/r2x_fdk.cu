@@ -12,6 +12,12 @@
 //                           row, using the symmetric odd-only taps:
 //                             Q_j = (r_j / 4 - sum_{k odd} (r_{j-k} + r_{j+k}) / (pi^2 k^2)) / D
 //                           (D = isocentre pitch), summed from the largest odd k < W down to k = 1.
+//   fdk_window_kernel       the same weights, then a windowed ramp filter (Shepp-Logan, cosine, Hamming, Hann): taps
+//                           h[k] = (1 / 2 pi^2) int_0^pi w Wn(w) cos(w k) dw, closed forms in fdk_window_tap, non-zero at
+//                           every k.  Shared memory holds the row and the W taps h[0 .. W-1] (2 W floats, 128 KB at
+//                           W = 16384) and no zero pads: a pixel j sums the one-sided taps beyond its nearer edge first,
+//                           then the two-sided ones, each from the largest k down to k = 1:
+//                             Q_j = (h[0] r_j + sum_{k=1}^{W-1} h[k] (r_{j-k} + r_{j+k})) / D   (r = 0 outside the row)
 //   fdk_backproject_kernel  a thread owns one (x, y) voxel column and a run of FDK_ZR voxels along z.  Every view's
 //                           homogeneous coordinates are affine in z, so the per-view setup (4 matrix rows, staged per
 //                           chunk of views in shared memory) is paid once per run.  Each voxel centre goes through the
@@ -34,7 +40,8 @@
 
 namespace r2x {
 
-constexpr int FDK_MAX_W = 16384;     // filter row staging: (3 W + W / 2) floats of shared memory (<= 227 KB)
+constexpr int FDK_MAX_W = 16384;     // filter row staging: (3 W + W / 2) floats of shared memory (<= 227 KB);
+                                     // windowed filters 2 W floats
 constexpr int FDK_BX = 32, FDK_BY = 4; // backprojection CTA: 32 y-columns x 4 x-columns
 constexpr int FDK_ZR = 8;            // voxels per thread along z
 constexpr int FDK_VCHUNK = 32;       // views staged in shared memory at a time
@@ -47,6 +54,7 @@ size_t fdk_scratch_bytes(int N, int H, int W) {
 }
 
 static size_t fdk_filter_smem(int W) { return (size_t)(3 * W + (W + 1) / 2) * sizeof(float); }
+static size_t fdk_window_smem(int W) { return (size_t)(2 * W) * sizeof(float); }
 
 template <bool CONE>
 __global__ void __launch_bounds__(FDK_BX * FDK_BY) fdk_backproject_kernel(
@@ -166,20 +174,15 @@ struct FdkWeights {
     float fan = 1.0f, hf_inv_delta = 1.0f, hf_sigma = 1.0f;   // HALF_FAN: a = ndc_x * fan, 1 / delta, sign(t_u)
 };
 
-// Steps 1-2 of FDK, one CTA per detector row of a detector offset by (t_u, t_v) pixels (zero when centred): each pixel's
-// cosine weight (cone beam) at its ndc moved by (su, sv) = (2 t_u / W, -2 t_v / H), then WEIGHT's redundancy weight:
-// PARKER its Parker weight at fan angle -atan(a) (cone; 0 for parallel beam) times its view's angular interval, HALF_FAN
-// fdk_half_fan_weight of its fan coordinate a = ndc_x * fan.  The weight is computed per pixel, which costs little next
-// to the W/2-tap convolution of each pixel.  The row is staged in shared memory between two rows of zeros and filtered
-// with the band-limited Ram-Lak taps (shift-invariant, so the same for any offset).
-template <int WEIGHT>
-__global__ void __launch_bounds__(256) fdk_filter_kernel(int H, int W, const float* __restrict__ projs, float tanx,
-                                                         float tany, int cone, float inv_delta, float su, float sv,
-                                                         FdkWeights fw, float* __restrict__ q) {
-    extern __shared__ float sm[];
-    float* row = sm;              // [3W]: zeros | weighted row | zeros
-    float* g = sm + 3 * W;        // [(W+1)/2]: g[m] = 1 / (pi^2 (2m+1)^2)
-    const size_t r = blockIdx.x;  // view * H + detector row
+// Step 1 of FDK on detector row r (view * H + row) of a detector offset by (t_u, t_v) pixels (zero when centred): each
+// pixel's cosine weight (cone beam) at its ndc moved by (su, sv) = (2 t_u / W, -2 t_v / H), then WEIGHT's redundancy
+// weight: PARKER its Parker weight at fan angle -atan(a) (cone; 0 for parallel beam) times its view's angular interval,
+// HALF_FAN fdk_half_fan_weight of its fan coordinate a = ndc_x * fan.  The weight is computed per pixel, which costs
+// little next to the convolution of each pixel.  put(j, p) receives weighted pixel j; the CTA's threads stride the row.
+template <int WEIGHT, class Put>
+__device__ __forceinline__ void fdk_weight_row(size_t r, int H, int W, const float* __restrict__ projs, float tanx,
+                                               float tany, int cone, float su, float sv, const FdkWeights& fw,
+                                               Put put) {
     const float* src = projs + r * W;
     const float step = 2.0f / (float)W, first = 1.0f / (float)W - 1.0f;
     const float b = cone ? (fmaf((float)(r % H), 2.0f / (float)H, 1.0f / (float)H - 1.0f) + sv) * tany : 0.0f;
@@ -197,10 +200,26 @@ __global__ void __launch_bounds__(256) fdk_filter_kernel(int H, int W, const flo
         }
         if (WEIGHT == R2X_FDK_PARKER) p *= fdk_parker_weight(bv.x, gam, fw.arc, fw.delta) * bv.y;
         if (WEIGHT == R2X_FDK_HALF_FAN) p *= fdk_half_fan_weight(nd * fw.fan, fw.hf_inv_delta, fw.hf_sigma);
+        put(j, p);
+    }
+}
+
+// Steps 1-2 of FDK with the band-limited Ram-Lak filter, one CTA per detector row: fdk_weight_row, the row staged in
+// shared memory between two rows of zeros and filtered with the Ram-Lak taps (shift-invariant, so the same for any
+// offset).
+template <int WEIGHT>
+__global__ void __launch_bounds__(256) fdk_filter_kernel(int H, int W, const float* __restrict__ projs, float tanx,
+                                                         float tany, int cone, float inv_delta, float su, float sv,
+                                                         FdkWeights fw, float* __restrict__ q) {
+    extern __shared__ float sm[];
+    float* row = sm;              // [3W]: zeros | weighted row | zeros
+    float* g = sm + 3 * W;        // [(W+1)/2]: g[m] = 1 / (pi^2 (2m+1)^2)
+    const size_t r = blockIdx.x;  // view * H + detector row
+    fdk_weight_row<WEIGHT>(r, H, W, projs, tanx, tany, cone, su, sv, fw, [&](int j, float p) {
         row[j] = 0.0f;
         row[W + j] = p;
         row[2 * W + j] = 0.0f;
-    }
+    });
     for (int m = threadIdx.x; m < (W + 1) / 2; m += blockDim.x) {
         const float k = (float)(2 * m + 1);
         g[m] = 1.0f / (9.869604401089358f * k * k);
@@ -216,17 +235,81 @@ __global__ void __launch_bounds__(256) fdk_filter_kernel(int H, int W, const flo
     }
 }
 
+// Band-limited Ram-Lak tap h_RL[k] in units of 1 / D: 1/4 at 0, -1 / (pi^2 k^2) at odd k, 0 at even k != 0.
+__device__ __forceinline__ double fdk_ram_lak_tap(int k) {
+    k = abs(k);
+    return k == 0 ? 0.25 : (k & 1) ? -1.0 / (9.869604401089358 * k * k) : 0.0;
+}
+
+// Tap h[k] (k >= 0, units of 1 / D) of the ramp times WINDOW's Wn (TIGRE's windows at frequency scale 1), in float64:
+//   SHEPP_LOGAN  Wn = sin(w/2) / (w/2)   h[k] = -2 / (pi^2 (4k^2 - 1))
+//   COSINE       Wn = cos(w/2)           h[k] = -(-1)^k / (pi (4k^2 - 1)) - (1/(2k+1)^2 + 1/(2k-1)^2) / pi^2
+//   HAMMING      Wn = 0.54 + 0.46 cos w  h[k] = 0.54 h_RL[k] + 0.23 (h_RL[k-1] + h_RL[k+1])
+//   HANN         Wn = (1 + cos w) / 2    h[k] = 0.5 h_RL[k] + 0.25 (h_RL[k-1] + h_RL[k+1])
+template <int WINDOW>
+__device__ __forceinline__ double fdk_window_tap(int k) {
+    const double pi = 3.141592653589793, pi2 = 9.869604401089358, kk = (double)k, d = 4.0 * kk * kk - 1.0;
+    if (WINDOW == R2X_FDK_SHEPP_LOGAN) return -2.0 / (pi2 * d);
+    if (WINDOW == R2X_FDK_COSINE) {
+        const double a = 2.0 * kk + 1.0, b = 2.0 * kk - 1.0;
+        return -((k & 1) ? -1.0 : 1.0) / (pi * d) - (1.0 / (a * a) + 1.0 / (b * b)) / pi2;
+    }
+    const double c0 = WINDOW == R2X_FDK_HAMMING ? 0.54 : 0.5, c1 = WINDOW == R2X_FDK_HAMMING ? 0.23 : 0.25;
+    return c0 * fdk_ram_lak_tap(k) + c1 * (fdk_ram_lak_tap(k - 1) + fdk_ram_lak_tap(k + 1));
+}
+
+// Steps 1-2 of FDK with WINDOW's ramp filter, one CTA per detector row: fdk_weight_row into shared memory, the taps
+// h[0 .. W-1] rounded once from float64 next to it, then the linear convolution over the whole row.  Pixel j's partner
+// pixels j - k and j + k both lie in the row for k <= near = min(j, W-1-j), one of them up to far = max(j, W-1-j);
+// the sum runs from k = far down to 1, smallest taps first (as fdk_filter_kernel's), with no bounds checks in either
+// loop.
+template <int WEIGHT, int WINDOW>
+__global__ void __launch_bounds__(256) fdk_window_kernel(int H, int W, const float* __restrict__ projs, float tanx,
+                                                         float tany, int cone, float inv_delta, float su, float sv,
+                                                         FdkWeights fw, float* __restrict__ q) {
+    extern __shared__ float sm[];
+    float* row = sm;              // [W]: weighted row
+    float* h = sm + W;            // [W]: h[k]
+    const size_t r = blockIdx.x;  // view * H + detector row
+    fdk_weight_row<WEIGHT>(r, H, W, projs, tanx, tany, cone, su, sv, fw, [&](int j, float p) { row[j] = p; });
+    for (int k = threadIdx.x; k < W; k += blockDim.x) h[k] = (float)fdk_window_tap<WINDOW>(k);
+    __syncthreads();
+    for (int j = threadIdx.x; j < W; j += blockDim.x) {
+        const float* c = row + j;
+        const int near = min(j, W - 1 - j), far = max(j, W - 1 - j);
+        const int side = j < W - 1 - j ? 1 : -1;   // the partner that stays in the row beyond `near`
+        float acc = 0.0f;
+        for (int k = far; k > near; --k) acc = fmaf(h[k], c[side * k], acc);
+        for (int k = near; k > 0; --k) acc = fmaf(h[k], c[-k] + c[k], acc);
+        q[r * W + j] = fmaf(h[0], c[0], acc) * inv_delta;
+    }
+}
+
 // isocentre pitch: cone dDetector_u * DSO / DSD = 2 tan_fovx DSO / W; parallel 2 / W (ndc [-1,1] = scene [-1,1])
 static double fdk_pitch(int W, float tanx, int mode, float dso) {
     return mode == 1 ? 2.0 * (double)tanx * (double)dso / W : 2.0 / W;
 }
 
-static int fdk_filter(cudaStream_t st, int weighting, int N, int H, int W, const float* projs, float tanx, float tany,
-                      int mode, float dso, float su, float sv, const FdkWeights& fw, float* q) {
-    auto kernel = weighting == R2X_FDK_PARKER     ? fdk_filter_kernel<R2X_FDK_PARKER>
-                  : weighting == R2X_FDK_HALF_FAN ? fdk_filter_kernel<R2X_FDK_HALF_FAN>
-                                                  : fdk_filter_kernel<R2X_FDK_PLAIN>;
-    const size_t smem = fdk_filter_smem(W);
+using FdkFilterKernel = void (*)(int, int, const float*, float, float, int, float, float, float, FdkWeights, float*);
+
+template <int WEIGHT>
+static FdkFilterKernel fdk_filter_for(int window) {
+    switch (window) {
+        case R2X_FDK_SHEPP_LOGAN: return fdk_window_kernel<WEIGHT, R2X_FDK_SHEPP_LOGAN>;
+        case R2X_FDK_COSINE: return fdk_window_kernel<WEIGHT, R2X_FDK_COSINE>;
+        case R2X_FDK_HAMMING: return fdk_window_kernel<WEIGHT, R2X_FDK_HAMMING>;
+        case R2X_FDK_HANN: return fdk_window_kernel<WEIGHT, R2X_FDK_HANN>;
+        default: return fdk_filter_kernel<WEIGHT>;
+    }
+}
+
+// window: R2X_FDK_RAM_LAK or one of the windowed filters (r2x_fdk's filter field)
+static int fdk_filter(cudaStream_t st, int weighting, int window, int N, int H, int W, const float* projs, float tanx,
+                      float tany, int mode, float dso, float su, float sv, const FdkWeights& fw, float* q) {
+    auto kernel = weighting == R2X_FDK_PARKER     ? fdk_filter_for<R2X_FDK_PARKER>(window)
+                  : weighting == R2X_FDK_HALF_FAN ? fdk_filter_for<R2X_FDK_HALF_FAN>(window)
+                                                  : fdk_filter_for<R2X_FDK_PLAIN>(window);
+    const size_t smem = window == R2X_FDK_RAM_LAK ? fdk_filter_smem(W) : fdk_window_smem(W);
     if (smem > 48 * 1024)
         R2X_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<(unsigned)((long long)N * H), 256, smem, st>>>(H, W, projs, tanx, tany, mode,
@@ -288,6 +371,12 @@ int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const f
         return rc;
     if (!(std::isfinite(shift_u) && std::isfinite(shift_v)))
         return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad shift (must be finite)");
+    // the low byte is the redundancy weighting, bits 8 and up the filter
+    const int window = weighting & ~0xff;
+    if (weighting < 0 || window > R2X_FDK_HANN)
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad weighting (filter field 0x000 = Ram-Lak, 0x100 = Shepp-Logan, "
+                                         "0x200 = cosine, 0x300 = Hamming, 0x400 = Hann; no other bits)");
+    weighting &= 0xff;
     if (weighting != R2X_FDK_PLAIN && weighting != R2X_FDK_PARKER && weighting != R2X_FDK_HALF_FAN)
         return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad weighting (0 = plain, 1 = Parker, 2 = half fan)");
     const double pi = 3.141592653589793;
@@ -318,7 +407,8 @@ int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const f
     const cudaStream_t st = (cudaStream_t)stream;
     float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
     const float su = (float)(2.0 * (double)shift_u / W), sv = (float)(-2.0 * (double)shift_v / H);
-    if (int rc = fdk_filter(st, weighting, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, su, sv, fw, q)) return rc;
+    if (int rc = fdk_filter(st, weighting, window, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, su, sv, fw, q))
+        return rc;
     // Parker's dbeta_v already holds each view's share of the arc
     const float scale = weighting == R2X_FDK_PARKER ? 1.0f : (float)(pi / n_views);
     return fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx, cy,
@@ -333,7 +423,7 @@ int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, 
     if (mode == 1 && !(dso > 0.0f && tan_fovx > 0.0f && tan_fovy > 0.0f))
         return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_filter: bad DSO / tan_fov");
     if (!projs || !filtered) return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_filter: bad pointer (NULL)");
-    return r2x::fdk_filter((cudaStream_t)stream, R2X_FDK_PLAIN, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso,
+    return r2x::fdk_filter((cudaStream_t)stream, R2X_FDK_PLAIN, R2X_FDK_RAM_LAK, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso,
                            0.0f, 0.0f, r2x::FdkWeights(), filtered);
 }
 

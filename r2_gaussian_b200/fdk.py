@@ -4,12 +4,20 @@
     vol = fdk(projections, angles, scanner_cfg)                    # [nx, ny, nz], the voxelizer's layout
     vol = fdk(projections, angles, scanner_cfg, short_scan=True)   # Parker-weighted, for an arc short of 360 degrees
     vol = fdk(projections, angles, scanner_cfg, use_offDetector=True, half_fan=True)   # offset detector, 360 degrees
+    vol = fdk(projections, angles, scanner_cfg, filter="hann")     # Hann-windowed ramp filter
 
 `projections` is a CUDA float32 [N, H, W] tensor in the dataset layout (rows = v, columns = u, already multiplied by
 scene_scale); `scanner_cfg` is the scaled dict of `dataset.read_scene` / `Scene.scanner_cfg`.  The per-view geometry is
 the rasterizer's (`scene.make_view`), so the reconstruction agrees with render() on detector orientation, axis order and
-angle convention by construction.  Band-limited Ram-Lak filter only (`filter: null` or "ram_lak").  Runs on the current
-stream; no CPU fallback.
+angle convention by construction.  Runs on the current stream; no CPU fallback.
+
+The ramp filter is the band-limited Ram-Lak filter unless `filter=` names one of TIGRE's windowed filters
+(`FILTERS`: "ram_lak", "shepp_logan", "cosine", "hamming", "hann", the names of TIGRE's `geo.filter`).  A window damps
+the ramp towards Nyquist, which passes less detector noise into the volume at some cost in resolution; it changes the
+filter taps only (r2x_fdk's filter field), so it combines with every weighting below and any offset.  The keyword
+overrides the scanner's `filter`.  Without it the scanner's `filter` must be null or "ram_lak", and a window named
+there is refused rather than silently replaced by Ram-Lak: reconstructing with it is opt-in, as for `use_offDetector`.
+The definition is stated in float64 in tests/fdk_window_oracle.py.
 
 The plain path weights every view by pi / N, which assumes each ray is measured twice: right for a full 360-degree scan
 and a 180-degree parallel scan, not for a cone-beam short scan (180 degrees plus the fan angle), which it reconstructs
@@ -40,7 +48,10 @@ import torch
 from ._lib import check, load
 from .scene import MODE_CONE, detector_shift, make_view
 
+# the scanner filters fdk reconstructs without its `filter` keyword
 SUPPORTED_FILTERS = (None, "ram_lak")
+# the filters of the `filter` keyword (TIGRE's names); r2x_fdk's filter field is the index << 8 (include/r2x.h)
+FILTERS = ("ram_lak", "shepp_logan", "cosine", "hamming", "hann")
 R2X_FDK_PLAIN, R2X_FDK_PARKER, R2X_FDK_HALF_FAN = 0, 1, 2   # r2x_fdk's weighting (include/r2x.h)
 # slack on the arc refusals: a scan sampled at linspace(0, pi, n + 1)[:-1] covers pi only up to rounding
 ARC_TOLERANCE = 1e-9
@@ -112,8 +123,26 @@ def short_scan_views(angles, mode: int, tan_fovx: float):
     return np.stack([bp, dbeta], 1), arc
 
 
+def check_filter(filter, scanner_cfg: dict) -> str:
+    """The filter fdk reconstructs with: `filter` (one of FILTERS) when given, else the scanner's, which must then be
+    null or "ram_lak"."""
+    if filter is not None:
+        if filter not in FILTERS:
+            raise ValueError(f"fdk: unknown filter {filter!r} (supported: {', '.join(FILTERS)})")
+        return filter
+    filt = scanner_cfg.get("filter")
+    if filt in SUPPORTED_FILTERS:
+        return "ram_lak"
+    if filt in FILTERS:
+        raise ValueError(f"fdk: the scanner's filter {filt!r} is used only on request: pass filter={filt!r} "
+                         f"(--fdk_filter {filt} on the command lines); without it fdk reconstructs with the Ram-Lak "
+                         "filter only (null or 'ram_lak')")
+    raise ValueError(f"fdk: the scanner's filter {filt!r} is not supported (supported: null, {', '.join(FILTERS)})")
+
+
 def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool = False, use_offDetector: bool = False,
-        half_fan: bool = False) -> torch.Tensor:
+        half_fan: bool = False, filter: str | None = None) -> torch.Tensor:
+    filt = check_filter(filter, scanner_cfg)
     if half_fan and not use_offDetector:
         raise ValueError("fdk: half_fan needs use_offDetector=True (the half-fan weights follow the detector offset)")
     if half_fan and short_scan:
@@ -139,9 +168,6 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool =
                            f"got {getattr(projections, 'device', type(projections))})")
     if projections.dim() != 3:
         raise ValueError(f"fdk: expected projections of shape [N, H, W], got {tuple(projections.shape)}")
-    filt = scanner_cfg.get("filter")
-    if filt not in SUPPORTED_FILTERS:
-        raise ValueError(f"fdk: filter {filt!r} is not supported (only the Ram-Lak filter: null or 'ram_lak')")
     angles = np.asarray(angles, dtype=np.float64).reshape(-1)
     N, H, W = (int(s) for s in projections.shape)
     if len(angles) != N:
@@ -171,7 +197,7 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool =
         stream = torch.cuda.current_stream(dev).cuda_stream
         vw = None if view_weights is None else torch.from_numpy(view_weights.astype(np.float32)).to(dev)
         rc = lib.r2x_fdk(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), float(views[0].tanfovx),
-                         float(views[0].tanfovy), int(mode), t_u, t_v, weighting,
+                         float(views[0].tanfovy), int(mode), t_u, t_v, weighting | (FILTERS.index(filt) << 8),
                          None if vw is None else vw.data_ptr(), float(arc), float(scanner_cfg["DSO"]), nx, ny, nz, sx,
                          sy, sz, cx, cy, cz, vol.data_ptr(), scratch.data_ptr(), nbytes)
     check(rc, "r2x_fdk")

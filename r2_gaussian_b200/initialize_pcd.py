@@ -3,6 +3,7 @@
     python -m r2_gaussian_b200.initialize_pcd --data <scene dir | NAF pickle> [--output init.npy]
         [--recon_method random|fdk|cgls|fista_tv|volume] [--recon recon.npy] [--n_points 50000] [--density_thresh 0.05]
         [--density_rescale 0.15] [--random_density_max 1.0] [--evaluate] [--short_scan] [--use_offDetector [--half_fan]]
+        [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
 
 `random` draws positions uniformly in the volume and densities in [0, random_density_max) with numpy's global
 generator seeded with 0, exactly like the reference.  `fdk` reconstructs the volume from the train views with the
@@ -13,7 +14,9 @@ scan over less than 360 degrees: the plain FDK shades such a volume, which moves
 the flag is refused with any other method.  `--use_offDetector` reconstructs through the scanner's offDetector
 (fdk, cgls and fista_tv; without it the projector pair refuses a non-zero offset and fdk ignores it), and `--half_fan`
 adds half-fan redundancy weights to that FDK for a full circle whose detector is shifted sideways (`fdk.fdk(...,
-half_fan=True)`; fdk only, not with --short_scan).  `cgls` does the same with 60 CGLS iterations over the GPU projector pair
+half_fan=True)`; fdk only, not with --short_scan).  `--fdk_filter NAME` gives that FDK one of TIGRE's windowed ramp
+filters (`fdk.fdk(filter=NAME)`): the reference's FDK takes its window from the scanner's `filter`, this one only on
+request, and without the flag a scanner whose `filter` names a window is refused (fdk only).  `cgls` does the same with 60 CGLS iterations over the GPU projector pair
 (`r2_gaussian_b200.recon`, the reference's `algs.cgls`); it also needs a CUDA device.  `fista_tv` does the same with
 the TV-regularised FISTA-TV of `r2_gaussian_b200.recon` at its default settings (CUDA as well).  `volume` samples a reconstruction made elsewhere (`--recon`, an .npy in the scene's
 voxel grid) the same way.  Writes [n_points, 4] = (x, y, z, density) in the scene's normalised [-1,1]^3 coordinates to
@@ -30,7 +33,7 @@ import os
 import numpy as np
 
 from .dataset import init_point_cloud, read_scene
-from .recon import check_fdk_flags
+from .recon import add_fdk_filter_flag, check_fdk_flags
 from .trainer import default_init_path
 
 # A filtered backprojection from a handful of views is dominated by streaks, and thresholding it gives no useful
@@ -47,16 +50,16 @@ def _require_cuda_for(method: str):
 
 
 def recon_train_views(info, method: str, short_scan: bool = False, use_offDetector: bool = False,
-                      half_fan: bool = False) -> np.ndarray:
-    """`recon.recon_volume(..., method, short_scan, use_offDetector, half_fan)` of the train views of a `read_scene`
-    result, as a host float32 [nx, ny, nz] array."""
+                      half_fan: bool = False, fdk_filter: str | None = None) -> np.ndarray:
+    """`recon.recon_volume(..., method, short_scan, use_offDetector, half_fan, fdk_filter)` of the train views of a
+    `read_scene` result, as a host float32 [nx, ny, nz] array."""
     import torch
 
     from .recon import recon_volume
 
     projs = torch.from_numpy(np.stack([np.asarray(c.image, np.float32) for c in info.train_cameras])).cuda()
     vol = recon_volume(projs, [c.angle for c in info.train_cameras], info.scanner_cfg, method, short_scan=short_scan,
-                       use_offDetector=use_offDetector, half_fan=half_fan)
+                       use_offDetector=use_offDetector, half_fan=half_fan, fdk_filter=fdk_filter)
     return vol.cpu().numpy()
 
 
@@ -105,6 +108,7 @@ def main(argv=None) -> str:
     ap.add_argument("--half_fan", default=False, action="store_true",
                     help="with --recon_method fdk and --use_offDetector: half-fan redundancy weights for a full circle "
                          "with the detector shifted sideways")
+    add_fdk_filter_flag(ap, "with --recon_method fdk: the ramp filter")
     a = ap.parse_args(argv)
     check_fdk_flags(a, a.recon_method == "fdk", f"{{flag}} applies to --recon_method fdk only, not {a.recon_method}: "
                     "the iterative methods need no redundancy weights")
@@ -129,7 +133,7 @@ def main(argv=None) -> str:
     os.makedirs(os.path.dirname(out) or ".", exist_ok=True)
     if a.recon_method in ("fdk", "cgls", "fista_tv"):
         # no draws from numpy's generator before np.random.choice
-        recon = recon_train_views(info, a.recon_method, a.short_scan, a.use_offDetector, a.half_fan)
+        recon = recon_train_views(info, a.recon_method, a.short_scan, a.use_offDetector, a.half_fan, a.fdk_filter)
     pts = init_point_cloud(info.scanner_cfg, a.n_points, recon=recon, density_thresh=a.density_thresh,
                            density_rescale=a.density_rescale, random_density_max=a.random_density_max)
     np.save(out, pts)

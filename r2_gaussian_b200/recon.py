@@ -48,12 +48,12 @@ Parity with TIGRE's binaries is not pinned (as for FDK and the projector).  ASD-
 `fista_tv` is the TV-regularised method this project offers.
 
     python -m r2_gaussian_b200.recon -s <scene> -m <output> [--methods fdk,sart,cgls] [--short_scan]
-        [--use_offDetector [--half_fan]]
+        [--use_offDetector [--half_fan]] [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
 
 mirrors `scripts/run_traditional_methods.py`: it reconstructs the scene's train views with each method, scores the
 volume against `vol_gt` with `metrics.metric_vol` and writes, per method, `<output>/<method>/ct_gt.npy`, `ct_pred.npy`,
 `eval_3d.yml` (method, psnr_3d, ssim_3d, ssim_3d_x/y/z, duration (sec), duration (min); fdk under `--short_scan`
-also `short_scan: true`) and the test views
+also `short_scan: true`, and `filter: <name>` under a `--fdk_filter` other than ram_lak) and the test views
 `projs/{i:05d}_render.npy` (projections of the reconstruction) and `projs/{i:05d}_gt.npy`, plus `<output>/eval_3d.yml`
 keyed by method.  PNG slices and projections are not written (matplotlib is not a dependency of this project).
 `--short_scan` reconstructs fdk with Parker redundancy weights (`fdk.fdk(short_scan=True)`), for scenes whose train
@@ -61,7 +61,9 @@ views cover less than a full circle; it is refused when --methods has no fdk.  `
 reprojects every method through the scanner's offDetector (without it a non-zero offset is refused by the projector
 pair and ignored by fdk); `--half_fan` (with it, fdk only, not with --short_scan) adds half-fan redundancy weights for
 a full circle whose detector is shifted sideways.  The reports add `half_fan: true` / `use_offDetector: true` only when
-those flags are on.
+those flags are on.  `--fdk_filter NAME` reconstructs fdk with one of TIGRE's windowed ramp filters
+(`fdk.fdk(filter=NAME)`, overriding the scanner's `filter`); it is refused when --methods has no fdk.  Without it fdk
+refuses a scanner whose `filter` names a window.
 """
 from __future__ import annotations
 
@@ -220,19 +222,24 @@ def fista_tv(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = FISTA_
 
 
 def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, short_scan: bool = False,
-                 use_offDetector: bool = False, half_fan: bool = False) -> torch.Tensor:
+                 use_offDetector: bool = False, half_fan: bool = False, fdk_filter: str | None = None) -> torch.Tensor:
     """The reconstructions of ct_utils.recon_volume / run_ct_recon_algs with their iteration counts.  `short_scan`
-    selects the Parker-weighted FDK and `half_fan` the half-fan-weighted one; both apply to method fdk only.
-    `use_offDetector` reconstructs through the scanner's offDetector (every method)."""
+    selects the Parker-weighted FDK, `half_fan` the half-fan-weighted one and `fdk_filter` FDK's ramp filter
+    (`fdk.fdk(filter=...)`); all three apply to method fdk only.  `use_offDetector` reconstructs through the scanner's
+    offDetector (every method)."""
     for flag, on in (("short_scan", short_scan), ("half_fan", half_fan)):
         if on and method != "fdk":
             raise ValueError(f"recon_volume: {flag} applies to fdk only, not {method!r} (the iterative methods need no "
                              "redundancy weights)")
+    if fdk_filter is not None and method != "fdk":
+        raise ValueError(f"recon_volume: fdk_filter applies to fdk only, not {method!r} (the iterative methods have no "
+                         "ramp filter)")
     off = use_offDetector
     if method == "fdk":
         from .fdk import fdk
 
-        return fdk(projs, angles, scanner_cfg, short_scan=short_scan, use_offDetector=off, half_fan=half_fan)
+        return fdk(projs, angles, scanner_cfg, short_scan=short_scan, use_offDetector=off, half_fan=half_fan,
+                   filter=fdk_filter)
     if method == "cgls":
         return cgls(projs, angles, scanner_cfg, CGLS_NITER, use_offDetector=off)[0]
     if method == "sart":
@@ -245,15 +252,25 @@ def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, sh
 
 
 def check_fdk_flags(args, fdk_selected: bool, not_fdk: str):
-    """The refusals of the FDK flags (--short_scan, --half_fan) that the recon and initialize_pcd CLIs share; `not_fdk`
-    is the CLI's message for a flag given without the fdk method, with `{flag}` standing for the flag."""
-    for flag, on in (("--short_scan", args.short_scan), ("--half_fan", args.half_fan)):
+    """The refusals of the FDK flags (--short_scan, --half_fan, --fdk_filter) that the recon and initialize_pcd CLIs
+    share; `not_fdk` is the CLI's message for a flag given without the fdk method, with `{flag}` standing for the flag."""
+    for flag, on in (("--short_scan", args.short_scan), ("--half_fan", args.half_fan),
+                     ("--fdk_filter", args.fdk_filter is not None)):
         if on and not fdk_selected:
             raise SystemExit(not_fdk.format(flag=flag))
     if args.half_fan and not args.use_offDetector:
         raise SystemExit("--half_fan needs --use_offDetector: the half-fan weights follow the detector offset")
     if args.half_fan and args.short_scan:
         raise SystemExit("--half_fan and --short_scan cannot be combined (half-fan weights need a full circle)")
+
+
+def add_fdk_filter_flag(ap, help_text: str):
+    """--fdk_filter NAME (one of fdk.FILTERS) on a CLI's parser."""
+    from .fdk import FILTERS
+
+    ap.add_argument("--fdk_filter", default=None, choices=FILTERS, metavar="NAME",
+                    help=f"{help_text}: {', '.join(FILTERS)} (TIGRE's names; default: the scanner's filter, which must "
+                         "then be null or ram_lak)")
 
 
 def _parse_methods(text: str) -> list[str]:
@@ -281,6 +298,7 @@ def main(argv=None) -> dict:
     ap.add_argument("--half_fan", default=False, action="store_true",
                     help="with --use_offDetector: reconstruct fdk with half-fan redundancy weights (a full circle with "
                          "the detector shifted sideways)")
+    add_fdk_filter_flag(ap, "reconstruct fdk with this ramp filter")
     a = ap.parse_args(argv)
     methods = _parse_methods(a.methods)
     check_fdk_flags(a, "fdk" in methods, "{flag} applies to the fdk method, which --methods does not include (the "
@@ -310,8 +328,9 @@ def main(argv=None) -> dict:
         t0 = time.time()
         short_scan = a.short_scan and method == "fdk"
         half_fan = a.half_fan and method == "fdk"
+        fdk_filter = a.fdk_filter if method == "fdk" else None
         pred = recon_volume(projs_train, train_angles, cfg, method, short_scan=short_scan,
-                            use_offDetector=a.use_offDetector, half_fan=half_fan)
+                            use_offDetector=a.use_offDetector, half_fan=half_fan, fdk_filter=fdk_filter)
         torch.cuda.synchronize()
         duration = time.time() - t0
         ct_pred = pred.cpu().numpy()
@@ -326,6 +345,8 @@ def main(argv=None) -> dict:
             report["short_scan"] = True
         if half_fan:
             report["half_fan"] = True
+        if fdk_filter not in (None, "ram_lak"):
+            report["filter"] = fdk_filter
         if a.use_offDetector:
             report["use_offDetector"] = True
         with open(os.path.join(save, "eval_3d.yml"), "w") as f:
