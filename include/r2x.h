@@ -190,18 +190,21 @@ int r2x_knn3_mean_dist2(void* stream, int P, const float* points, float* mean_di
  * image: the reference's `l1_loss` + `ssim` (r2_gaussian/utils/loss_utils.py:37-104: 11-tap Gaussian window,
  * sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2) as combined in train.py:118-127.
  * loss_out[3] (device) = {mean|x-y|, mean SSIM, loss}; grad_out[H*W] (device, may be NULL) = d loss / d image.
- * Deterministic.  scratch: r2x_image_loss_scratch_bytes(H, W). */
+ * Deterministic.  scratch: r2x_image_loss_scratch_bytes(H, W).  H <= 1048560 (65535 rows of 16-pixel tiles): a taller
+ * image is refused before any launch. */
 size_t r2x_image_loss_scratch_bytes(int H, int W);
 int r2x_image_loss(void* stream, int H, int W, const float* image, const float* target, float w_l1,
                    float w_dssim, float* loss_out, float* grad_out, void* scratch, size_t scratch_bytes);
 /* The same for N images (1 <= N <= 65535) in the same three launches: images / targets / grad_out [N,H,W],
- * loss_out[N,3]; row v is bit for bit r2x_image_loss of image v.  scratch: r2x_image_loss_views_scratch_bytes. */
+ * loss_out[N,3]; row v is bit for bit r2x_image_loss of image v.  The same H limit.  scratch:
+ * r2x_image_loss_views_scratch_bytes. */
 size_t r2x_image_loss_views_scratch_bytes(int N, int H, int W);
 int r2x_image_loss_views(void* stream, int N, int H, int W, const float* images, const float* targets, float w_l1,
                          float w_dssim, float* loss_out, float* grad_out, void* scratch, size_t scratch_bytes);
 
 /* 3-D total variation of vol[nx][ny][nz] (`tv_3d_loss`, loss_utils.py:19-34): sum of absolute forward
- * differences along the three axes, divided by their number when reduction_mean != 0.  loss_out[1] (device),
+ * differences along the three axes, divided by their number when reduction_mean != 0 (a 1x1x1 volume has none: its
+ * mean is NaN, 0 / 0, and its gradient 0, as autograd gives the reference's).  loss_out[1] (device),
  * grad_out[nx*ny*nz] (device, may be NULL).  scratch: r2x_tv3d_scratch_bytes(nx, ny, nz). */
 size_t r2x_tv3d_scratch_bytes(int nx, int ny, int nz);
 int r2x_tv3d_loss(void* stream, int nx, int ny, int nz, const float* vol, int reduction_mean, float* loss_out,

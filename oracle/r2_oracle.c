@@ -895,25 +895,34 @@ void orc_mark_visible(int P, const float* means, const float* view, const float*
  * published result -- for every point the mean of the three smallest squared distances to OTHER points, kept
  * in ascending order from FLT_MAX placeholders (updateKBest<3>) -- by brute force.  PARITY UNPINNED against
  * the upstream binary (absent); pinned against an independent float64 k-d tree in tests/test_oracle_cpu.py. */
+static float knn3_one(int P, const float* pts, int i) {
+    float b0 = FLT_MAX, b1 = FLT_MAX, b2 = FLT_MAX;
+    const float x = pts[3 * (size_t)i], y = pts[3 * (size_t)i + 1], z = pts[3 * (size_t)i + 2];
+    for (int j = 0; j < P; ++j) {
+        if (j == i) continue;
+        const float dx = x - pts[3 * (size_t)j], dy = y - pts[3 * (size_t)j + 1], dz = z - pts[3 * (size_t)j + 2];
+        const float d = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
+        if (d < b2) {
+            if (d < b1) {
+                b2 = b1;
+                if (d < b0) { b1 = b0; b0 = d; }
+                else b1 = d;
+            } else b2 = d;
+        }
+    }
+    return ((b0 + b1) + b2) / 3.0f;
+}
+
+/* orc_knn3_mean_dist2's result for the n_query points idx[0 .. n_query-1] only (out[k] belongs to point idx[k]): the
+ * same loop over all P points, so a cloud of millions can be checked at chosen points in O(n_query * P). */
+void orc_knn3_mean_dist2_at(int P, const float* pts, int n_query, const int* idx, float* out) {
+#pragma omp parallel for schedule(dynamic, 16)
+    for (int k = 0; k < n_query; ++k) out[k] = knn3_one(P, pts, idx[k]);
+}
+
 void orc_knn3_mean_dist2(int P, const float* pts, float* out) {
 #pragma omp parallel for schedule(static)
-    for (int i = 0; i < P; ++i) {
-        float b0 = FLT_MAX, b1 = FLT_MAX, b2 = FLT_MAX;
-        const float x = pts[3 * (size_t)i], y = pts[3 * (size_t)i + 1], z = pts[3 * (size_t)i + 2];
-        for (int j = 0; j < P; ++j) {
-            if (j == i) continue;
-            const float dx = x - pts[3 * (size_t)j], dy = y - pts[3 * (size_t)j + 1], dz = z - pts[3 * (size_t)j + 2];
-            const float d = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-            if (d < b2) {
-                if (d < b1) {
-                    b2 = b1;
-                    if (d < b0) { b1 = b0; b0 = d; }
-                    else b1 = d;
-                } else b2 = d;
-            }
-        }
-        out[i] = ((b0 + b1) + b2) / 3.0f;
-    }
+    for (int i = 0; i < P; ++i) out[i] = knn3_one(P, pts, i);
 }
 
 int orc_num_threads(void) {

@@ -218,3 +218,16 @@ def knn3_mean_dist2(points):
     with np.errstate(over="ignore"):
         lib().orc_knn3_mean_dist2(C.c_int(pts.shape[0]), _p(pts, _fp), _p(out, _fp))
     return out
+
+
+def knn3_mean_dist2_at(points, idx):
+    """knn3_mean_dist2(points)[idx], computed for the points `idx` only (see orc_knn3_mean_dist2_at)."""
+    pts = _c(points, _f).reshape(-1, 3)
+    q = _c(idx, np.int32).reshape(-1)
+    if q.size and (q.min() < 0 or q.max() >= pts.shape[0]):
+        raise IndexError("knn3_mean_dist2_at: query index out of range")
+    out = np.zeros(q.shape[0], _f)
+    with np.errstate(over="ignore"):
+        lib().orc_knn3_mean_dist2_at(C.c_int(pts.shape[0]), _p(pts, _fp), C.c_int(q.shape[0]), _p(q, _ip),
+                                     _p(out, _fp))
+    return out

@@ -21,6 +21,7 @@ namespace r2x {
 constexpr int LT = 16;            // output tile edge
 constexpr int LH = 5;             // window half width
 constexpr int LE = LT + 2 * LH;   // 26: tile + halo
+constexpr int IMAGE_LOSS_MAX_H = 65535 * LT;   // rows of LT-pixel CTAs are grid.y, at most 65535
 
 struct SsimWindow { float g[11]; };
 
@@ -233,6 +234,7 @@ size_t image_loss_scratch_bytes(int H, int W) {
 int launch_image_loss(cudaStream_t st, int H, int W, const float* image, const float* target, float w_l1,
                       float w_dssim, float* loss_out, float* grad_out, void* scratch, size_t scratch_bytes) {
     if (H <= 0 || W <= 0) return fail_msg(R2X_ERR_INVALID, "r2x_image_loss: bad H/W");
+    if (H > IMAGE_LOSS_MAX_H) return fail_msg(R2X_ERR_INVALID, "r2x_image_loss: H too large (grid.y = ceil(H / 16) <= 65535)");
     if (!image || !target || !loss_out || !scratch) return fail_msg(R2X_ERR_INVALID, "r2x_image_loss: null pointer");
     if (scratch_bytes < image_loss_scratch_bytes(H, W)) return fail_msg(R2X_ERR_INVALID, "r2x_image_loss: scratch too small");
     static const SsimWindow win = make_window();
@@ -264,6 +266,8 @@ int launch_image_loss_views(cudaStream_t st, int N, int H, int W, const float* i
                             float w_dssim, float* loss_out, float* grad_out, void* scratch, size_t scratch_bytes) {
     if (N < 1 || N > 65535) return fail_msg(R2X_ERR_INVALID, "r2x_image_loss_views: bad N (need 1 <= N <= 65535)");
     if (H <= 0 || W <= 0) return fail_msg(R2X_ERR_INVALID, "r2x_image_loss_views: bad H/W");
+    if (H > IMAGE_LOSS_MAX_H)
+        return fail_msg(R2X_ERR_INVALID, "r2x_image_loss_views: H too large (grid.y = ceil(H / 16) <= 65535)");
     if (!images || !targets || !loss_out || !scratch) return fail_msg(R2X_ERR_INVALID, "r2x_image_loss_views: null pointer");
     if (scratch_bytes < image_loss_views_scratch_bytes(N, H, W))
         return fail_msg(R2X_ERR_INVALID, "r2x_image_loss_views: scratch too small");
@@ -349,14 +353,17 @@ int launch_tv3d(cudaStream_t st, int nx, int ny, int nz, const float* vol, int r
     if (scratch_bytes < tv3d_scratch_bytes(nx, ny, nz)) return fail_msg(R2X_ERR_INVALID, "r2x_tv3d_loss: scratch too small");
     const size_t n = (size_t)nx * ny * nz;
     const int nblk = (int)((n + 255) / 256);
-    float scale = 1.f;
+    // A 1x1x1 volume has no differences: its mean is 0 / 0 = NaN, as the reference's, but every voxel's gradient is an
+    // empty sum, which autograd gives as 0.  So the loss takes 1 / 0 = inf and the gradient a scale of 0 (0 * inf is NaN).
+    float loss_scale = 1.f, grad_scale = 1.f;
     if (reduction_mean) {
         const double tot = (double)(nx - 1) * ny * nz + (double)nx * (ny - 1) * nz + (double)nx * ny * (nz - 1);
-        scale = (float)(1.0 / tot);
+        loss_scale = (float)(1.0 / tot);
+        grad_scale = tot > 0.0 ? loss_scale : 0.f;
     }
     float* partial = (float*)(((size_t)scratch + 255) & ~(size_t)255);
-    tv3d_kernel<<<nblk, 256, 0, st>>>(nx, ny, nz, vol, scale, grad_out, partial);
-    tv3d_reduce_kernel<<<1, 1024, 0, st>>>(nblk, partial, scale, loss_out);
+    tv3d_kernel<<<nblk, 256, 0, st>>>(nx, ny, nz, vol, grad_scale, grad_out, partial);
+    tv3d_reduce_kernel<<<1, 1024, 0, st>>>(nblk, partial, loss_scale, loss_out);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }
