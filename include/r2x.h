@@ -526,6 +526,39 @@ int r2x_projection_prepare_shape(int H0, int W0, int subsample, int* out_hw);
 int r2x_projection_prepare(void* stream, int n_views, int H0, int W0, int subsample, const double* img,
                            double proj_rescale, double object_scale, float* out);
 
+/* ---- cubic B-spline zoom of a placed volume (r2_gaussian_b200/resample.py, process_raw_data.py) ------------------ */
+/* A placed volume V[shape] is a source volume set at `offset` and normalised:
+ *   V[p] = (float64(src[p - offset]) - lo) / (hi - lo)   where p - offset lies in src_shape, else 0,
+ * both operations in float64, one rounding each.  src is device memory of element type `dtype`, read at
+ * sum_a q[a] * src_strides[a] (elements; a transposed host array keeps its strides).  A positive offset pads with zeros
+ * (expand_to_cube), a negative one crops (crop_to_cube), lo = 0, hi = 1 passes the values through unchanged.
+ * r2x_volume_place writes V (float64, C order) to out.
+ * r2x_zoom_cubic writes scipy.ndimage.zoom(V, zoom, order=3, mode="nearest") to out[out0, out1, out2] (float64): V padded
+ * by 12 edge voxels per side into `workspace`, the cubic B-spline prefilter along each axis in place (gain 6, pole
+ * sqrt(3) - 2, mirror start value), then output index o maps to x = o (n - 1) / (out - 1) + 12 (factor 1 when
+ * out = 1) and sums the 4 x 4 x 4 coefficients floor(x) - 1 .. floor(x) + 2 with the cubic B-spline weights.  The
+ * caller chooses out = int(round(n * zoom)) per axis and uses r2x_volume_place when every factor is exactly 1 (scipy
+ * returns a copy there).  r2x_zoom_workspace_bytes(shape) = (shape + 24)^3 * 8 bytes, 0 for a bad shape; no GPU needed.
+ * Arguments are checked before any CUDA work (non-NULL pointers, dtype, src_shape >= 1, strides >= 0, shape and out
+ * sizes in [1, 32768], lo and hi finite with hi > lo, workspace large enough).  64-bit indexing, no atomics, bitwise
+ * reproducible.  Asynchronous on `stream`. */
+#define R2X_PLACE_U8 0
+#define R2X_PLACE_U16 1
+#define R2X_PLACE_F64 2
+typedef struct r2x_place_desc {
+    const void* src;            /* device                                        */
+    int dtype;                  /* R2X_PLACE_U8, R2X_PLACE_U16 or R2X_PLACE_F64   */
+    int src_shape[3];
+    long long src_strides[3];   /* in elements, >= 0                             */
+    int shape[3];               /* the placed volume                             */
+    int offset[3];              /* its index of source voxel (0, 0, 0)           */
+    double lo, hi;
+} r2x_place_desc;
+size_t r2x_zoom_workspace_bytes(int n0, int n1, int n2);
+int r2x_volume_place(void* stream, const r2x_place_desc* desc, double* out);
+int r2x_zoom_cubic(void* stream, const r2x_place_desc* desc, int out0, int out1, int out2, void* workspace,
+                   size_t workspace_bytes, double* out);
+
 /* ---- multi-GPU exchange step: one-shot sum over NVLink peer memory ------------------------------ */
 /* The Gaussian-sharded projector (one process per GPU, every rank renders its index shard) needs ONE exchange per
  * projection: the sum of the per-rank partial detector images (BASELINE north_star; the reference itself is

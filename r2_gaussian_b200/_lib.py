@@ -103,6 +103,9 @@ PROTOTYPES = {
     "r2x_tv_value": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _sz]),
     "r2x_projection_prepare_shape": (_i, [_i, _i, _i, C.POINTER(_i)]),
     "r2x_projection_prepare": (_i, [_vp, _i, _i, _i, _i, _vp, C.c_double, C.c_double, _vp]),
+    "r2x_zoom_workspace_bytes": (_sz, [_i, _i, _i]),
+    "r2x_volume_place": (_i, [_vp, _vp, _vp]),
+    "r2x_zoom_cubic": (_i, [_vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "r2x_peer_alloc": (_i, [_sz, C.POINTER(_vp)]),
     "r2x_peer_free": (_i, [_vp]),
     "r2x_ipc_export": (_i, [_vp, _vp]),
@@ -127,6 +130,11 @@ class AdamGroup(C.Structure):
     """Mirror of `r2x_adam_group` (include/r2x.h)."""
     _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
                 ("numel", C.c_longlong), ("lr", C.c_float)]
+
+class PlaceDesc(C.Structure):
+    """Mirror of `r2x_place_desc` (include/r2x.h)."""
+    _fields_ = [("src", C.c_void_p), ("dtype", C.c_int), ("src_shape", C.c_int * 3), ("src_strides", C.c_longlong * 3),
+                ("shape", C.c_int * 3), ("offset", C.c_int * 3), ("lo", C.c_double), ("hi", C.c_double)]
 
 _lock = threading.Lock()
 _lib = None
