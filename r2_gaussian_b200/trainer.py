@@ -179,6 +179,20 @@ def derived_settings(scanner_cfg: dict, model: ModelParams, opt: OptimizationPar
             "tv_vol_sVoxel": [float(d) * n for d in scanner_cfg["dVoxel"]]}
 
 
+def evaluation_cameras(scene: Scene, pose=None, detector=None) -> list:
+    """[("train", cams), ("test", cams)]: the cameras `evaluate` renders.  `pose` (a PoseCorrection over the train
+    views, row = cam.uid): train views carry their corrections, test views keep their nominal poses.  `detector` (a
+    DetectorOffset): both splits carry the offset."""
+    out = []
+    for name, cams in (("train", scene.getTrainCameras()), ("test", scene.getTestCameras())):
+        if cams and name == "train" and pose is not None:
+            cams = [pose.device_camera(c, c.uid, POSE_ANCHOR) for c in cams]
+        if cams and detector is not None:
+            cams = detector.cameras(cams)
+        out.append((name, cams))
+    return out
+
+
 @torch.no_grad()
 def evaluate(scene: Scene, gaussians: GaussianModel, pipe, with_ssim: bool = True, pose=None, detector=None) -> dict:
     """3-D PSNR / SSIM of the queried volume and 2-D PSNR / SSIM of the rendered train and test views, with the
@@ -190,13 +204,9 @@ def evaluate(scene: Scene, gaussians: GaussianModel, pipe, with_ssim: bool = Tru
     out = {"psnr_3d": metric_vol(scene.vol_gt, vol, "psnr")[0]}
     if with_ssim:
         out["ssim_3d"] = metric_vol(scene.vol_gt, vol, "ssim")[0]
-    for name, cams in (("train", scene.getTrainCameras()), ("test", scene.getTestCameras())):
+    for name, cams in evaluation_cameras(scene, pose, detector):
         if not cams:
             continue
-        if name == "train" and pose is not None:
-            cams = [pose.device_camera(c, c.uid, POSE_ANCHOR) for c in cams]
-        if detector is not None:
-            cams = detector.cameras(cams)
         imgs = torch.concat([render(c, gaussians, pipe)["render"] for c in cams], 0).permute(1, 2, 0)
         gts = torch.concat([c.original_image.to(imgs.device) for c in cams], 0).permute(1, 2, 0)
         out[f"psnr_2d_{name}"] = metric_proj(gts, imgs, "psnr")[0]
