@@ -559,6 +559,46 @@ int r2x_volume_place(void* stream, const r2x_place_desc* desc, double* out);
 int r2x_zoom_cubic(void* stream, const r2x_place_desc* desc, int out0, int out1, int out2, void* workspace,
                    size_t workspace_bytes, double* out);
 
+/* ---- isosurface of a volume: marching cubes (r2_gaussian_b200/mesh.py, extract_mesh.py) ------------------------- */
+/* Replaces skimage.measure.marching_cubes in the reference's create_vol_mesh (r2_gaussian/utils/plot_utils.py).
+ * vol[nx,ny,nz] (device, float32, z fastest) is sampled at the integer index points (i, j, k); level is finite.
+ *   inside   a sample is inside iff v > level (strict; NaN is outside).
+ *   cubes    cube s = (i, j, k) for i < nx-1, j < ny-1, k < nz-1; corner b in 0..7 sits at s + (b&1, b>>1&1, b>>2&1);
+ *            the case is the 8-bit mask of its inside corners.  Cube edges are numbered axis-major: 0-3 along x (lower
+ *            corners 0, 2, 4, 6), 4-7 along y (0, 1, 4, 5), 8-11 along z (0, 1, 2, 3).  A grid edge is owned by its
+ *            lower sample and axis (s, a) and is cut iff exactly one end is inside.
+ *   vertex   a = v[p0] (lower end), b = v[p1]; t = (level - a) / (b - a) in float32 (IEEE division); the vertex is p0
+ *            except along axis a, where it is float32(p0[a]) + t.  No FMA: a numpy float32 statement gives the same
+ *            bits.  Index space.  A vertex may land on a sample that equals level; degenerate triangles are kept.
+ *   table    generated on the host by a rule, checked, and copied to __constant__ memory on first use per device:
+ *            1. face rule: on each cube face, each maximal run of inside corners along the face's 4-cycle is cut off
+ *               by one segment joining the two cut edges that bound it (diagonal inside corners are separated, diagonal
+ *               outside corners joined).  Two cubes sharing a face derive the same segments: no cracks.
+ *            2. the segments chain into closed loops (each cut edge ends one segment and starts one).
+ *            3. every triangle is counter-clockwise seen from the outside region (values <= level): (v1-v0)x(v2-v0)
+ *               points from inside to outside; a closed surface around a high-valued blob has positive signed volume.
+ *            4. loops in order of their smallest edge; each is a fan from the first vertex, walking the loop in its
+ *               direction from its smallest edge, whose fan diagonals join no two edges of a common cube face.
+ *            A table without such an apex for some loop, or with more than 5 triangles in a case, is refused.
+ *   order    vertices by owning sample (i ny + j) nz + k, then axis x < y < z; triangles by cube (linear index of its
+ *            lower sample), then table order.  verts float32 [V,3] (x = i, y = j, z = k), faces int32 [T,3].
+ * r2x_marching_cubes_table copies the table out (no GPU): ntri[256], edges[256][15], -1 padded.
+ * r2x_marching_cubes_count classifies every sample and writes totals_dev[2] (device) = {V, T} in 64 bits.
+ * r2x_marching_cubes_emit, on the scratch the count pass just filled, scans the per-word counts and writes the mesh;
+ * every write is bounded by the V and T it is given (wrong totals give a short mesh, never an out-of-bounds write),
+ * and V or T >= 2^31 returns R2X_ERR_OVERFLOW before any work.  Vertex ids come from the scans: the mesh is indexed and
+ * shared, with no welding pass.  Scratch (r2x_marching_cubes_scratch_bytes, no GPU; 0 for a bad grid): 5 uint32 words
+ * per 32 samples, 0.625 bytes per sample, plus 8 bytes per 32768 samples and under 2 KiB; the count pass fills 0.375 bytes
+ * per sample of it (inside bits and two per-word counts).  Arguments are checked before any CUDA work (non-NULL
+ * pointers, each size >= 1 -- an axis shorter than 2 has no cubes --, nx ny nz <= 2^31 - 1, finite level, enough
+ * scratch).  64-bit addressing, no atomics on the output, bitwise reproducible; asynchronous on `stream`. */
+int r2x_marching_cubes_table(int* ntri /* 256 */, signed char* edges /* 256 * 15 */);
+size_t r2x_marching_cubes_scratch_bytes(int nx, int ny, int nz);
+int r2x_marching_cubes_count(void* stream, int nx, int ny, int nz, const float* vol, float level, long long* totals_dev,
+                             void* scratch, size_t scratch_bytes);
+int r2x_marching_cubes_emit(void* stream, int nx, int ny, int nz, const float* vol, float level, long long V,
+                            long long T, float* verts, int* faces, void* scratch, size_t scratch_bytes);
+
 /* ---- multi-GPU exchange step: one-shot sum over NVLink peer memory ------------------------------ */
 /* The Gaussian-sharded projector (one process per GPU, every rank renders its index shard) needs ONE exchange per
  * projection: the sum of the per-rank partial detector images (BASELINE north_star; the reference itself is

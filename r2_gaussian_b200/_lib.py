@@ -106,6 +106,10 @@ PROTOTYPES = {
     "r2x_zoom_workspace_bytes": (_sz, [_i, _i, _i]),
     "r2x_volume_place": (_i, [_vp, _vp, _vp]),
     "r2x_zoom_cubic": (_i, [_vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
+    "r2x_marching_cubes_table": (_i, [_vp, _vp]),
+    "r2x_marching_cubes_scratch_bytes": (_sz, [_i, _i, _i]),
+    "r2x_marching_cubes_count": (_i, [_vp, _i, _i, _i, _vp, _f, _vp, _vp, _sz]),
+    "r2x_marching_cubes_emit": (_i, [_vp, _i, _i, _i, _vp, _f, _ll, _ll, _vp, _vp, _vp, _sz]),
     "r2x_peer_alloc": (_i, [_sz, C.POINTER(_vp)]),
     "r2x_peer_free": (_i, [_vp]),
     "r2x_ipc_export": (_i, [_vp, _vp]),
