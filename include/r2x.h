@@ -599,6 +599,47 @@ int r2x_marching_cubes_count(void* stream, int nx, int ny, int nz, const float* 
 int r2x_marching_cubes_emit(void* stream, int nx, int ny, int nz, const float* vol, float level, long long V,
                             long long T, float* verts, int* faces, void* scratch, size_t scratch_bytes);
 
+/* ---- volume rendering: emission-absorption and MIP ray casting (r2_gaussian_b200/volume_render.py, render_volume.py) */
+/* Replaces the pyvista / VTK volume plot of the reference's scripts/plot_volume.py.  Parity with VTK's pixels is not
+ * claimed.  vol[nx,ny,nz] (device, float32, z fastest), every axis >= 2.  Index space: sample vol[i,j,k] sits at the
+ * point (i, j, k); the field is the trilinear interpolant of the samples on the box B = [0,nx-1] x [0,ny-1] x [0,nz-1].
+ *   camera   cameras_dev (device, float32) holds R2X_VR_CAMERA_FLOATS = 16 floats per frame:
+ *            P[3] position, f[3] unit view direction, r[3] unit right, u[3] unit up, p pixel pitch, 3 unused.
+ *            The host builds them in float64 from a position P, focal point F and view-up U: f = normalize(F - P),
+ *            r = normalize(f x U), u = r x f; p = 2 tan(view_angle / 2) / H (perspective) or 2 S / H (parallel, S the
+ *            parallel scale: half the image height in voxels).  Pixel (row y from the top, column x) has offsets
+ *            a = ((x + 1/2) - W/2) p and b = ((H/2 - y) - 1/2) p.  Perspective: the ray leaves o = P along
+ *            d = normalize((f + a r) + b u); parallel (`parallel` = 1): it leaves o = (P + a r) + b u along d = f.
+ *   samples  [s_in, s_out] is the ray's parameter interval inside B (slab method, per axis (0 - o)/d and
+ *            ((n-1) - o)/d; an axis with d = 0 constrains nothing if 0 <= o <= n-1 and misses otherwise), with s_in
+ *            clamped to >= 0.  s_out < s_in misses.  Otherwise the samples are s_k = s_in + k step for
+ *            k = 0 .. floor((s_out - s_in) / step), each formed from k, at the point o + s_k d, clamped into B; the
+ *            cell is i0 = min(floor(p), n - 2) per axis, w = p - i0, and the value is the trilinear blend with weights
+ *            (1 - w, w) along each axis.  The ray set-up and sample points are float64 without FMA (a numpy float64
+ *            statement gives the same sample counts and points); w is rounded to float32 and everything after it is
+ *            float32.
+ *   transfer t = clamp((v - c0) * (1 / (c1 - c0)), 0, 1) (the reciprocal rounded once to float32); colour from the
+ *            K-entry RGB LUT lut_dev (device, float32 [K][3]): pos = t (K - 1), j = min(floor(pos), K - 2),
+ *            w = pos - j, colour = (1 - w) L[j] + w L[j+1]; K = 1 is a constant colour.  Opacity alpha_tf = t.
+ *   mode 0   composite: alpha = 1 - (1 - alpha_tf)^(step / unit) (unit: the opacity unit distance, in voxels); front
+ *            to back from C = 0, T = 1: C += T alpha colour, T *= 1 - alpha; the ray stops after the first sample
+ *            that leaves T < 2^-16.  RGB = C + T background, A = 1 - T.
+ *   mode 1   MIP: m = the largest sampled value; RGB = colour(t(m)), A = 1 for a ray that meets B.
+ *            A ray that misses B gets RGB = background, A = 0 in both modes.
+ *   output   out (device, float32) [n_frames, H, W, 4] RGBA.  No shading, no jitter, no texture filtering.
+ * One thread per pixel, R2X_VR_TILE x R2X_VR_TILE pixel tiles, frames on the grid's z dimension; no atomics, bitwise
+ * reproducible; asynchronous on `stream`.  background[3] is a host pointer.  Arguments are checked before any CUDA
+ * work: non-NULL pointers, nx ny nz >= 2, n_frames H W >= 1, parallel 0 or 1, mode 0 or 1, 1 <= K <= 4096, finite
+ * c0 < c1 with c1 - c0 a finite float, finite step > 0 with at most 2^31 - 1 samples along the box diagonal, finite unit > 0, a finite background,
+ * frames and pixel tiles per grid dimension <= 65535 (so n_frames H W 4 < 2^62 for the 64-bit output index). */
+#define R2X_VR_CAMERA_FLOATS 16
+#define R2X_VR_TILE 16
+#define R2X_VR_COMPOSITE 0
+#define R2X_VR_MIP 1
+int r2x_volume_render(void* stream, int nx, int ny, int nz, const float* vol, int n_frames, int H, int W,
+                      const float* cameras_dev, int parallel, int mode, float c0, float c1, const float* lut_dev, int K,
+                      float step, float unit, const float* background, float* out);
+
 /* ---- multi-GPU exchange step: one-shot sum over NVLink peer memory ------------------------------ */
 /* The Gaussian-sharded projector (one process per GPU, every rank renders its index shard) needs ONE exchange per
  * projection: the sum of the per-rank partial detector images (BASELINE north_star; the reference itself is

@@ -32,16 +32,28 @@ def parse_args(argv=None):
                                              "reconstruction or a trained model, written as binary PLY")
     ap.add_argument("--output", required=True, help="PLY file to write")
     ap.add_argument("--level", type=float, default=0.5, help="iso level: samples > level are inside (default 0.5)")
-    ap.add_argument("-s", "--source_path", default=None, help="scene directory or NAF pickle")
-    ap.add_argument("--vol", default=None, help=".npy volume [nx, ny, nz]")
-    ap.add_argument("-m", "--model_path", default=None, help="output directory of a trainer run")
-    ap.add_argument("--iteration", type=int, default=-1, help="with -m: saved iteration (-1: the last one)")
-    ap.add_argument("--resolution", type=int, default=None, help="with -m: query N^3 samples instead of nVoxel")
+    add_source_arguments(ap)
     a = ap.parse_args(argv)
     from .mesh import finite_level
 
     if not finite_level(a.level):
         ap.error(f"--level must be a finite float32, got {a.level}")
+    check_source_arguments(ap, a)
+    return a
+
+
+def add_source_arguments(ap):
+    """The volume source options: -s, --vol, -m, --iteration, --resolution."""
+    ap.add_argument("-s", "--source_path", default=None, help="scene directory or NAF pickle")
+    ap.add_argument("--vol", default=None, help=".npy volume [nx, ny, nz]")
+    ap.add_argument("-m", "--model_path", default=None, help="output directory of a trainer run")
+    ap.add_argument("--iteration", type=int, default=-1, help="with -m: saved iteration (-1: the last one)")
+    ap.add_argument("--resolution", type=int, default=None, help="with -m: query N^3 samples instead of nVoxel")
+
+
+def check_source_arguments(ap, a):
+    """Refuse (ap.error) conflicting or missing sources, options that do not apply to the source, missing paths and a
+    missing --output directory."""
     if a.model_path is not None and a.vol is not None:
         ap.error("give either -m or --vol, not both")
     if a.model_path is None and a.vol is None and a.source_path is None:
@@ -58,7 +70,6 @@ def parse_args(argv=None):
     out_dir = os.path.dirname(os.path.abspath(a.output))
     if not os.path.isdir(out_dir):
         ap.error(f"--output: directory {out_dir} does not exist")
-    return a
 
 
 def _read_volume(path: str) -> np.ndarray:
