@@ -15,6 +15,10 @@ Two layers, as the kernels split the work:
   regularisations (of det2^2, mu and the projective w), x_grad_mul / y_grad_mul at the 1.3 tanfov clamp, the
   parallel-beam constant J, scale_modifier (dL/dscale is with respect to the modified scale, as the reference's) and
   the cov3D_precomp path.
+* The matrix gradients (make_pose_chain).  The same chain (_chain_core) continued to one Gaussian's contribution to
+  dL/dviewmatrix and dL/dprojmatrix in the layout of the rasterizer's pose rows, with the same frozen decisions; its
+  inputs are those of make_chain and PNK more rounding knobs.  tests/test_pose_grad_float64_cpu.py checks it against
+  autograd of a float64 forward and against central differences where the clamp is active.
 
 The bar (reference).  The chain is linear in the moments.  A float32 kernel that sums the pairs and runs the chain
 well is off from y64 by a small multiple of u = 2^-24 of
@@ -164,85 +168,96 @@ def _sigma6(s, q):
     return _six(R @ (s * s).diag() @ R.T)
 
 
+def _chain_core(m, p, W, H, tanfovx, tanfovy, mode, scale_modifier, precomp, eps):
+    """The reference's backward of one Gaussian from its moments m to dL/dhat and dL/dt (zero in parallel beam), and
+    the intermediates the 3-D mean and the matrix gradients go on from, as a dict.  eps: the backward's two 1e-7
+    regularisations, of det2^2 and of mu (0 gives the exact derivative of the frozen forward)."""
+    import torch
+
+    hx, hy = W / (2.0 * tanfovx), H / (2.0 * tanfovy)
+    S0, Sx, Sy, Sxx, Sxy, Syy = m[0], m[1], m[2], m[3], m[4], m[5]
+    mean, sc, q, c6 = p[0:3], p[3:6], p[6:10], p[10:16]
+    A, B, Cc, rho, mu = p[16], p[17], p[18], p[19], p[20]
+    view, proj = p[21:37], p[37:53]
+    kM, kV, kh, kd2, kd3, kmu = p[53:62].reshape(3, 3), p[62:68], p[68:74], p[74], p[75], p[76]
+    w = rho * mu
+    g2x = w * (-A * Sx - B * Sy) * (0.5 * W)
+    g2y = w * (-Cc * Sy - B * Sx) * (0.5 * H)
+    dcx, dcy, dcz = -0.5 * w * Sxx, -w * Sxy, -0.5 * w * Syy
+    dmu = rho * S0
+    dop = mu * S0
+    s_eff = scale_modifier * sc
+    V = _sym6(kV * (c6 if precomp else _sigma6(s_eff, q)))
+    V4 = view.reshape(4, 4)                          # V4[k][r] = view[4k + r]
+    Rv = V4[:3, :3].T                                # t = Rv mean + V4[3, :3]
+    t = Rv @ mean + V4[3, :3]
+    tx, ty, tz = t[0], t[1], t[2]
+    zero, one = torch.zeros_like(tz), torch.ones_like(tz)
+    if mode == 1:
+        limx, limy = 1.3 * tanfovx, 1.3 * tanfovy
+        txtz, tytz = tx / tz, ty / tz
+        xgm = ((txtz >= -limx) & (txtz <= limx)).to(t.dtype)
+        ygm = ((tytz >= -limy) & (tytz <= limy)).to(t.dtype)
+        tx = tz * txtz.clamp(-limx, limx)
+        ty = tz * tytz.clamp(-limy, limy)
+        l = torch.sqrt(tx * tx + ty * ty + tz * tz)
+        J = torch.stack([torch.stack([hx / tz, zero, -hx * tx / (tz * tz)]),
+                         torch.stack([zero, hy / tz, -hy * ty / (tz * tz)]),
+                         torch.stack([tx / l, ty / l, tz / l])])
+    else:
+        J = torch.stack([torch.stack([hx + zero, zero, zero]), torch.stack([zero, hy + zero, zero]),
+                         torch.stack([zero, zero, one])])
+    M = kM * (J @ Rv)
+    hat = _sym6(kh * _six(M @ V @ M.T))
+    a, b, d = hat[0, 0], hat[0, 1], hat[1, 1]
+    det2 = kd2 * (a * d - b * b)
+    K, det3 = _adj_det(hat)
+    det3 = kd3 * det3
+    musq = 2 * math.pi * det3 / det2
+    muv = kmu * torch.sqrt(torch.clamp(musq, min=0.0))
+    inv = 1.0 / (det2 * det2 + eps)
+    adj = torch.stack([torch.stack([d, -b]), torch.stack([-b, a])])
+    Gc = torch.stack([torch.stack([dcx, 0.5 * dcy]), torch.stack([0.5 * dcy, dcz])])
+    T = adj @ Gc @ adj
+    pi_mu = math.pi / (muv + eps)
+    ratio = det3 / det2
+    ddet3 = torch.stack([K[0, 0], 2 * K[0, 1], 2 * K[0, 2], K[1, 1], 2 * K[1, 2], K[2, 2]])
+    ddet2 = torch.stack([d, -2 * b, zero, a, zero, zero])
+    dh = pi_mu * (ddet3 - ratio * ddet2) / det2 * dmu
+    dh = dh + torch.stack([-inv * T[0, 0], -inv * (T[0, 1] + T[1, 0]), zero, -inv * T[1, 1], zero, zero])
+    D = torch.stack([torch.stack([dh[0], 0.5 * dh[1], 0.5 * dh[2]]),
+                     torch.stack([0.5 * dh[1], dh[3], 0.5 * dh[4]]),
+                     torch.stack([0.5 * dh[2], 0.5 * dh[4], dh[5]])])
+    dt = torch.zeros_like(mean)
+    if mode == 1:
+        dJ = 2.0 * (D @ M @ V) @ Rv.T                # dL/dJ = (dL/dM) Rv^T, dL/dM = 2 D M V
+        rz = 1.0 / tz
+        rl, rl3 = 1.0 / l, 1.0 / (l * l * l)
+        tdot = tx * dJ[2, 0] + ty * dJ[2, 1] + tz * dJ[2, 2]
+        dtx = xgm * (-hx * rz * rz * dJ[0, 2] + rl * dJ[2, 0] - rl3 * tx * tdot)
+        dty = ygm * (-hy * rz * rz * dJ[1, 2] + rl * dJ[2, 1] - rl3 * ty * tdot)
+        dtz = (-rz * rz * (hx * dJ[0, 0] + hy * dJ[1, 1]) + 2 * rz ** 3 * (hx * tx * dJ[0, 2] + hy * ty * dJ[1, 2])
+               + rl * dJ[2, 2] - rl3 * tz * tdot)
+        dt = torch.stack([dtx, dty, dtz])
+    P4 = proj.reshape(4, 4)                          # P4[k][r] = proj[4k + r]
+    hom = P4[:3, :].T @ mean + P4[3, :]
+    m_w = 1.0 / (hom[3] + 1e-7)                      # the forward's own 1e-7 (not a regularisation of the backward)
+    return dict(g2x=g2x, g2y=g2y, dop=dop, dmu=dmu, mean=mean, sc=sc, q=q, s_eff=s_eff, V=V, Rv=Rv, J=J, M=M, D=D,
+                dt=dt, P4=P4, hom=hom, m_w=m_w)
+
+
 def make_chain(W, H, tanfovx, tanfovy, mode, scale_modifier=1.0, precomp=False):
     """chain(m [6], p [NP]) -> y (the outputs of OUT_KEYS concatenated), for one Gaussian, float64 torch."""
     import torch
     from torch.func import grad
 
-    hx, hy = W / (2.0 * tanfovx), H / (2.0 * tanfovy)
-
     def chain(m, p):
-        S0, Sx, Sy, Sxx, Sxy, Syy = m[0], m[1], m[2], m[3], m[4], m[5]
-        mean, sc, q, c6 = p[0:3], p[3:6], p[6:10], p[10:16]
-        A, B, Cc, rho, mu = p[16], p[17], p[18], p[19], p[20]
-        view, proj = p[21:37], p[37:53]
-        kM, kV, kh, kd2, kd3, kmu = p[53:62].reshape(3, 3), p[62:68], p[68:74], p[74], p[75], p[76]
-        w = rho * mu
-        g2x = w * (-A * Sx - B * Sy) * (0.5 * W)
-        g2y = w * (-Cc * Sy - B * Sx) * (0.5 * H)
-        dcx, dcy, dcz = -0.5 * w * Sxx, -w * Sxy, -0.5 * w * Syy
-        dmu = rho * S0
-        dop = mu * S0
-        s_eff = scale_modifier * sc
-        V = _sym6(kV * (c6 if precomp else _sigma6(s_eff, q)))
-        V4 = view.reshape(4, 4)                          # V4[k][r] = view[4k + r]
-        Rv = V4[:3, :3].T                                # t = Rv mean + V4[3, :3]
-        t = Rv @ mean + V4[3, :3]
-        tx, ty, tz = t[0], t[1], t[2]
-        zero, one = torch.zeros_like(tz), torch.ones_like(tz)
-        if mode == 1:
-            limx, limy = 1.3 * tanfovx, 1.3 * tanfovy
-            txtz, tytz = tx / tz, ty / tz
-            xgm = ((txtz >= -limx) & (txtz <= limx)).to(t.dtype)
-            ygm = ((tytz >= -limy) & (tytz <= limy)).to(t.dtype)
-            tx = tz * txtz.clamp(-limx, limx)
-            ty = tz * tytz.clamp(-limy, limy)
-            l = torch.sqrt(tx * tx + ty * ty + tz * tz)
-            J = torch.stack([torch.stack([hx / tz, zero, -hx * tx / (tz * tz)]),
-                             torch.stack([zero, hy / tz, -hy * ty / (tz * tz)]),
-                             torch.stack([tx / l, ty / l, tz / l])])
-        else:
-            J = torch.stack([torch.stack([hx + zero, zero, zero]), torch.stack([zero, hy + zero, zero]),
-                             torch.stack([zero, zero, one])])
-        M = kM * (J @ Rv)
-        hat = _sym6(kh * _six(M @ V @ M.T))
-        a, b, d = hat[0, 0], hat[0, 1], hat[1, 1]
-        det2 = kd2 * (a * d - b * b)
-        K, det3 = _adj_det(hat)
-        det3 = kd3 * det3
-        musq = 2 * math.pi * det3 / det2
-        muv = kmu * torch.sqrt(torch.clamp(musq, min=0.0))
-        inv = 1.0 / (det2 * det2 + 1e-7)
-        adj = torch.stack([torch.stack([d, -b]), torch.stack([-b, a])])
-        Gc = torch.stack([torch.stack([dcx, 0.5 * dcy]), torch.stack([0.5 * dcy, dcz])])
-        T = adj @ Gc @ adj
-        pi_mu = math.pi / (muv + 1e-7)
-        ratio = det3 / det2
-        ddet3 = torch.stack([K[0, 0], 2 * K[0, 1], 2 * K[0, 2], K[1, 1], 2 * K[1, 2], K[2, 2]])
-        ddet2 = torch.stack([d, -2 * b, zero, a, zero, zero])
-        dh = pi_mu * (ddet3 - ratio * ddet2) / det2 * dmu
-        dh = dh + torch.stack([-inv * T[0, 0], -inv * (T[0, 1] + T[1, 0]), zero, -inv * T[1, 1], zero, zero])
-        D = torch.stack([torch.stack([dh[0], 0.5 * dh[1], 0.5 * dh[2]]),
-                         torch.stack([0.5 * dh[1], dh[3], 0.5 * dh[4]]),
-                         torch.stack([0.5 * dh[2], 0.5 * dh[4], dh[5]])])
+        c = _chain_core(m, p, W, H, tanfovx, tanfovy, mode, scale_modifier, precomp, 1e-7)
+        g2x, g2y, M, D, P4, m_w, q, s_eff = c["g2x"], c["g2y"], c["M"], c["D"], c["P4"], c["m_w"], c["q"], c["s_eff"]
         G3 = M.T @ D @ M                                 # dL/dSigma, full symmetric
         dcov = torch.stack([G3[0, 0], 2 * G3[0, 1], 2 * G3[0, 2], G3[1, 1], 2 * G3[1, 2], G3[2, 2]])
-        dmean = torch.zeros_like(mean)
-        if mode == 1:
-            dJ = 2.0 * (D @ M @ V) @ Rv.T                # dL/dJ = (dL/dM) Rv^T, dL/dM = 2 D M V
-            rz = 1.0 / tz
-            l = torch.sqrt(tx * tx + ty * ty + tz * tz)
-            rl, rl3 = 1.0 / l, 1.0 / (l * l * l)
-            tdot = tx * dJ[2, 0] + ty * dJ[2, 1] + tz * dJ[2, 2]
-            dtx = xgm * (-hx * rz * rz * dJ[0, 2] + rl * dJ[2, 0] - rl3 * tx * tdot)
-            dty = ygm * (-hy * rz * rz * dJ[1, 2] + rl * dJ[2, 1] - rl3 * ty * tdot)
-            dtz = (-rz * rz * (hx * dJ[0, 0] + hy * dJ[1, 1]) + 2 * rz ** 3 * (hx * tx * dJ[0, 2] + hy * ty * dJ[1, 2])
-                   + rl * dJ[2, 2] - rl3 * tz * tdot)
-            dmean = Rv.T @ torch.stack([dtx, dty, dtz])
-        P4 = proj.reshape(4, 4)                          # P4[k][r] = proj[4k + r]
-        hom = P4[:3, :].T @ mean + P4[3, :]
-        m_w = 1.0 / (hom[3] + 1e-7)
-        mul1, mul2 = hom[0] * m_w * m_w, hom[1] * m_w * m_w
+        dmean = c["Rv"].T @ c["dt"]
+        mul1, mul2 = c["hom"][0] * m_w * m_w, c["hom"][1] * m_w * m_w
         dmean = dmean + torch.stack([(P4[k, 0] * m_w - P4[k, 3] * mul1) * g2x + (P4[k, 1] * m_w - P4[k, 3] * mul2) * g2y
                                      for k in range(3)])
         if precomp:
@@ -250,9 +265,52 @@ def make_chain(W, H, tanfovx, tanfovy, mode, scale_modifier=1.0, precomp=False):
         else:
             ds = grad(lambda s: (dcov * _sigma6(s, q)).sum())(s_eff)
             dr = grad(lambda qq: (dcov * _sigma6(s_eff, qq)).sum())(q)
-        return torch.cat([torch.stack([g2x, g2y, dop, dmu]), dmean, dcov, ds, dr])
+        return torch.cat([torch.stack([g2x, g2y, c["dop"], c["dmu"]]), dmean, dcov, ds, dr])
 
     return chain
+
+
+# ---- the matrix gradients ------------------------------------------------------------------------------------------
+# One Gaussian's contribution to dL/dviewmatrix and dL/dprojmatrix, laid out as the rasterizer's pose rows (POSE_N = 24
+# floats, include/r2x.h): pose[3a + b] = dL/dview[4a + b] (a < 4: a = 3 is the translation column), pose[12 + 3a + j]
+# = dL/dproj[4a + (0, 1, 3)[j]].  With the chain's D = dL/dhat and dt = dL/dt (x_grad_mul / y_grad_mul, J at the
+# clamped t, the parallel-beam constant J):
+#     t_b = sum_a view[4a + b] p_a + view[12 + b]          -> dt_b p_a,  dt_b
+#     M[i][a] = sum_b J[i][b] view[4a + b]                 -> sum_i (2 D M Sigma)[i][a] J[i][b]
+#     ndc = (hom_x, hom_y) / (hom_w + 1e-7), hom = P^T [p, 1] -> g2x m_w, g2y m_w, -(g2x hom_x + g2y hom_y) m_w^2
+# times [p, 1]_a.  Four more rounding knobs (PNK, after the chain's NP inputs) are unit factors on the two view terms
+# and on m_w and the w term: the float32 sums of the kernel round each of them.
+POSE_N = 24
+PNK = 4
+POSE_KEYS = ("view_rot", "view_trans", "proj")
+POSE_SLICES = {"view_rot": slice(0, 9), "view_trans": slice(9, 12), "proj": slice(12, 24)}
+
+
+def make_pose_chain(W, H, tanfovx, tanfovy, mode, scale_modifier=1.0, precomp=False, eps=1e-7):
+    """chain(m [6], p [NP + PNK]) -> the POSE_N matrix-gradient contributions of one Gaussian, float64 torch.
+    eps = 0: the exact derivative of the frozen forward (no regularisations)."""
+    import torch
+
+    def chain(m, p):
+        c = _chain_core(m, p[:NP], W, H, tanfovx, tanfovy, mode, scale_modifier, precomp, eps)
+        kt, kM, kw, kgw = p[NP], p[NP + 1], p[NP + 2], p[NP + 3]
+        mean, dt, J = c["mean"], c["dt"], c["J"]
+        dM = 2.0 * (c["D"] @ c["M"] @ c["V"])           # dL/dM
+        rot = kt * (mean[:, None] * dt[None, :]) + kM * (dM.T @ J)    # [a][b]
+        m_w = kw * c["m_w"]
+        hom = c["hom"]
+        gw = kgw * -(c["g2x"] * hom[0] + c["g2y"] * hom[1]) * m_w * m_w
+        ph = torch.cat([mean, torch.ones_like(mean[:1])])
+        pj = ph[:, None] * torch.stack([c["g2x"] * m_w, c["g2y"] * m_w, gw])[None, :]    # [a][j]
+        return torch.cat([rot.reshape(9), dt, pj.reshape(12)])
+
+    return chain
+
+
+def pose_chain_inputs(*args):
+    """chain_inputs(...) followed by the PNK pose knobs (all 1): [P, NP + PNK]."""
+    p = chain_inputs(*args)
+    return np.concatenate([p, np.ones((len(p), PNK))], 1)
 
 
 def chain_inputs(means, scales, rots, cov3D, conic_opacity, mu, view, proj):
