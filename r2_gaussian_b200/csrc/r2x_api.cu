@@ -786,7 +786,10 @@ int r2x_raster_forward_async_raw(void* stream, int P, int W, int H, const float*
                                  const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
                                  float tan_fovy, int mode, float* out_color, int* radii, void* geom_buf, void* image_buf,
                                  void* binning_buf, long long capacity, uint32_t* status_dev, const r2x_activation* act) {
-    if (!act || !raw_scales || !raw_rotations) return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward_async_raw: null argument");
+    // P == 0 (an empty shard of a Gaussian-sharded run) passes null parameter pointers: the call below zeroes
+    // the output and status and reads no parameter
+    if (!act || (P > 0 && (!raw_scales || !raw_rotations)))
+        return fail_msg(R2X_ERR_INVALID, "r2x_raster_forward_async_raw: null argument");
     ActScope scope(act);
     return r2x_raster_forward_async(stream, P, W, H, means3D, raw_density, raw_scales, scale_modifier, raw_rotations, nullptr,
                                     viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, 0, mode, out_color, radii, geom_buf,
@@ -799,7 +802,8 @@ int r2x_raster_backward_raw(void* stream, int P, long long R, int W, int H, cons
                             const void* geom_buf, const void* binning_buf, const void* image_buf, void* scratch,
                             const float* dL_dpix, float* dL_dmean2D, float* dL_draw_density, float* dL_dmean3D,
                             float* dL_dcov3D, float* dL_draw_scale, float* dL_draw_rot, int mode, const r2x_activation* act) {
-    if (!act || !raw_scales || !raw_rotations) return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward_raw: null argument");
+    if (!act || (P > 0 && (!raw_scales || !raw_rotations)))
+        return fail_msg(R2X_ERR_INVALID, "r2x_raster_backward_raw: null argument");
     ActScope scope(act);
     return r2x_raster_backward(stream, P, R, W, H, means3D, raw_scales, scale_modifier, raw_rotations, nullptr, viewmatrix,
                                projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buf, binning_buf, image_buf, scratch,
@@ -873,7 +877,8 @@ int r2x_voxel_forward_async_raw(void* stream, int P, int nx, int ny, int nz, flo
                                 float* out_volume, int* radii_x, int* radii_y, int* radii_z, void* geom_buf,
                                 void* image_buf, void* binning_buf, long long capacity, uint32_t* status_dev,
                                 const r2x_activation* act) {
-    if (!act || !raw_scales || !raw_rotations) return fail_msg(R2X_ERR_INVALID, "r2x_voxel_forward_async_raw: null argument");
+    if (!act || (P > 0 && (!raw_scales || !raw_rotations)))
+        return fail_msg(R2X_ERR_INVALID, "r2x_voxel_forward_async_raw: null argument");
     ActScope scope(act);
     return r2x_voxel_forward_async(stream, P, nx, ny, nz, sx, sy, sz, cx, cy, cz, means3D, raw_density, raw_scales,
                                    scale_modifier, raw_rotations, nullptr, 0, out_volume, radii_x, radii_y, radii_z, geom_buf,
@@ -886,7 +891,8 @@ int r2x_voxel_backward_raw(void* stream, int P, long long R, int nx, int ny, int
                            const void* geom_buf, const void* binning_buf, const void* image_buf, void* scratch,
                            const float* dL_dvol, float* dL_draw_density, float* dL_dmean3D, float* dL_dcov3D,
                            float* dL_draw_scale, float* dL_draw_rot, const r2x_activation* act) {
-    if (!act || !raw_scales || !raw_rotations) return fail_msg(R2X_ERR_INVALID, "r2x_voxel_backward_raw: null argument");
+    if (!act || (P > 0 && (!raw_scales || !raw_rotations)))
+        return fail_msg(R2X_ERR_INVALID, "r2x_voxel_backward_raw: null argument");
     ActScope scope(act);
     return r2x_voxel_backward(stream, P, R, nx, ny, nz, sx, sy, sz, cx, cy, cz, means3D, raw_scales, scale_modifier,
                               raw_rotations, nullptr, radii_x, radii_y, radii_z, geom_buf, binning_buf, image_buf, scratch,
