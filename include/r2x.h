@@ -507,6 +507,25 @@ size_t r2x_tv_value_scratch_bytes(int nx, int ny, int nz);
 int r2x_tv_value(void* stream, int nx, int ny, int nz, const float* x, double* out, void* scratch,
                  size_t scratch_bytes);
 
+/* ---- one Chambolle-Pock iteration for data-constrained TV (cp_tv, r2_gaussian_b200/recon.py and tv.py) ---------- */
+/* Chambolle-Pock (primal-dual hybrid gradient) on  minimise TV(x) subject to |A x - b| <= eps, x in C,  with
+ * K = [A; nu grad] (the grad / div = -grad^T of r2x_tv_prox).  The data dual q and its prox stay with the caller, in
+ * projection space; this call is the rest of the iteration, given g = A^T q (r2x_volume_backproject of the new q):
+ *   p_out    = P_{1/nu}(p + sigma nu grad xbar)                   per voxel: u, scaled by (1/nu) / |u| when |u| > 1/nu
+ *   x_out    = P_C(x - tau g + tau nu div p_out)                  C = {x >= 0} when nonneg (u < 0 ? 0 : u), else all
+ *   xbar_out = 2 x_out - x                                        (one fmaf)
+ * x, xbar, g, x_out, xbar_out are float32 [nx,ny,nz] (z fastest); p, p_out are float32 [3,nx,ny,nz] (component a at
+ * a * nx*ny*nz + voxel).  One launch (tv_cp_kernel in csrc/r2x_tv.cu): a CTA owns a 4 x 8 x 32 tile, holds xbar on the
+ * tile's [-1, T] box and p_out on its [-1, T - 1] box in shared memory, and writes all three outputs of the tile;
+ * 44 bytes per voxel.  p and xbar are read across tile edges, so the outputs are the caller's ping-pong buffers: no
+ * output may overlap an input or another output (inputs may overlap each other, e.g. x == xbar).  No scratch.
+ * tau, sigma, nu finite and > 0, and sigma nu, tau nu, 1 / nu finite (float32, rounded once from double).  No
+ * atomics, bitwise reproducible; arguments are checked before any CUDA work; asynchronous on `stream`.
+ * Limits: nx <= 262140, ny <= 524280. */
+int r2x_tv_cp_step(void* stream, int nx, int ny, int nz, const float* x, const float* xbar, const float* p,
+                   const float* g, float tau, float sigma, float nu, int nonneg, float* x_out, float* xbar_out,
+                   float* p_out);
+
 /* ---- real-scan projection preparation (r2_gaussian_b200/generate_real_data.py) ---------------------------------- */
 /* Replaces the reference's per-view numpy + cv2 chain (data_generator/real_dataset/generate_data.py:91-109).
  * img[n_views, H0, W0] (device, float64: the processed scan's `img` arrays) -> out[n_views, H, W] (device, float32):

@@ -101,6 +101,7 @@ PROTOTYPES = {
     "r2x_tv_prox": (_i, [_vp, _i, _i, _i, _vp, _f, _i, _i, _vp, _vp, _sz]),
     "r2x_tv_value_scratch_bytes": (_sz, [_i, _i, _i]),
     "r2x_tv_value": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _sz]),
+    "r2x_tv_cp_step": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _f, _f, _i, _vp, _vp, _vp]),
     "r2x_projection_prepare_shape": (_i, [_i, _i, _i, C.POINTER(_i)]),
     "r2x_projection_prepare": (_i, [_vp, _i, _i, _i, _i, _vp, C.c_double, C.c_double, _vp]),
     "r2x_zoom_workspace_bytes": (_sz, [_i, _i, _i]),

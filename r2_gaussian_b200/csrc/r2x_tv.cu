@@ -16,6 +16,13 @@
 // from L2.  A last launch (tv_primal_kernel) writes x from p_niter.  Weight 0 skips the dual entirely: x = P_C(v),
 // bit for bit.  P_C(u) = (u < 0 ? 0 : u).  Everything is elementwise or a fixed stencil: no atomics, bitwise
 // reproducible.
+//
+// r2x_tv_cp_step is the volume part of one Chambolle-Pock iteration of cp_tv (recon.py): from x, xbar, p and
+// g = A^T q it writes p+ = P_{1/nu}(p + sigma nu grad xbar), x+ = P_C(x - tau g + tau nu div p+) and xbar+ = 2 x+ - x
+// in one launch (tv_cp_kernel) on the same 4 x 8 x 32 tiles: xbar on the tile's [-1, T] box, p+ on its [-1, T - 1]
+// box (the -1 layer is a neighbour's p+, recomputed here with the same instructions, so it is the value that neighbour
+// writes), then div p+ and the primal on the tile.  Bytes per voxel: x, xbar, g read (12), p read (12), x+, xbar+
+// written (8), p+ written (12) = 44; halo re-reads come from L2.
 #include <cmath>
 #include <cstdint>
 
@@ -121,6 +128,73 @@ __global__ void __launch_bounds__(TV_THREADS) tv_primal_kernel(int nx, int ny, i
     out[i] = proj_c(fmaf(-w, d, v[i]), nonneg);
 }
 
+constexpr int CP_PX = TV_TX + 1, CP_PY = TV_TY + 1, CP_PZ = TV_TZ + 1;   // p+ on the tile's [-1, T - 1] box
+constexpr int CP_PBOX = CP_PX * CP_PY * CP_PZ;
+
+// one Chambolle-Pock iteration after the data dual; xbar is staged on the [-1, T] box (the TV_R* box of tv_fgp_kernel)
+__global__ void __launch_bounds__(TV_THREADS) tv_cp_kernel(int nx, int ny, int nz, const float* __restrict__ x,
+                                                           const float* __restrict__ xbar, const float* __restrict__ p,
+                                                           const float* __restrict__ g, float tau, float sn, float tn,
+                                                           float pmax, float pmax2, int nonneg,
+                                                           float* __restrict__ x_out, float* __restrict__ xbar_out,
+                                                           float* __restrict__ p_out) {
+    __shared__ float xb[TV_RBOX];
+    __shared__ float pp[3][CP_PBOX];
+    const size_t nvox = (size_t)nx * ny * nz;
+    const int X0 = blockIdx.z * TV_TX, Y0 = blockIdx.y * TV_TY, Z0 = blockIdx.x * TV_TZ;
+    for (int e = threadIdx.x; e < TV_RBOX; e += TV_THREADS) {
+        const int lz = e % TV_RZ, t = e / TV_RZ, ly = t % TV_RY, lx = t / TV_RY;
+        const int X = X0 + lx - 1, Y = Y0 + ly - 1, Z = Z0 + lz - 1;
+        const bool in = X >= 0 && X < nx && Y >= 0 && Y < ny && Z >= 0 && Z < nz;
+        xb[e] = in ? xbar[((size_t)X * ny + Y) * nz + Z] : 0.0f;
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < CP_PBOX; e += TV_THREADS) {
+        const int lz = e % CP_PZ, t = e / CP_PZ, ly = t % CP_PY, lx = t / CP_PY;
+        const int X = X0 + lx - 1, Y = Y0 + ly - 1, Z = Z0 + lz - 1;
+        float u0 = 0.0f, u1 = 0.0f, u2 = 0.0f;
+        if (X >= 0 && X < nx && Y >= 0 && Y < ny && Z >= 0 && Z < nz) {
+            const int c = (lx * TV_RY + ly) * TV_RZ + lz;                  // the same voxel in the xbar box
+            const float x0 = xb[c];
+            const float g0 = X < nx - 1 ? xb[c + TV_RY * TV_RZ] - x0 : 0.0f;
+            const float g1 = Y < ny - 1 ? xb[c + TV_RZ] - x0 : 0.0f;
+            const float g2 = Z < nz - 1 ? xb[c + 1] - x0 : 0.0f;
+            const size_t i = ((size_t)X * ny + Y) * nz + Z;
+            u0 = fmaf(sn, g0, p[i]);
+            u1 = fmaf(sn, g1, p[nvox + i]);
+            u2 = fmaf(sn, g2, p[2 * nvox + i]);
+            const float n2 = fmaf(u2, u2, fmaf(u1, u1, u0 * u0));
+            if (n2 > pmax2) {
+                const float s = pmax / sqrtf(n2);
+                u0 *= s;
+                u1 *= s;
+                u2 *= s;
+            }
+        }
+        pp[0][e] = u0;
+        pp[1][e] = u1;
+        pp[2][e] = u2;
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < TV_TX * TV_TY * TV_TZ; e += TV_THREADS) {
+        const int lz = e % TV_TZ, t = e / TV_TZ, ly = t % TV_TY, lx = t / TV_TY;
+        const int X = X0 + lx, Y = Y0 + ly, Z = Z0 + lz;
+        if (!(X < nx && Y < ny && Z < nz)) continue;
+        const int c = ((lx + 1) * CP_PY + ly + 1) * CP_PZ + lz + 1;
+        float d = (X < nx - 1 ? pp[0][c] : 0.0f) - (X > 0 ? pp[0][c - CP_PY * CP_PZ] : 0.0f);
+        d += (Y < ny - 1 ? pp[1][c] : 0.0f) - (Y > 0 ? pp[1][c - CP_PZ] : 0.0f);
+        d += (Z < nz - 1 ? pp[2][c] : 0.0f) - (Z > 0 ? pp[2][c - 1] : 0.0f);
+        const size_t i = ((size_t)X * ny + Y) * nz + Z;
+        const float xv = x[i];
+        const float xp = proj_c(fmaf(tn, d, fmaf(-tau, g[i], xv)), nonneg);
+        x_out[i] = xp;
+        xbar_out[i] = fmaf(2.0f, xp, -xv);
+        p_out[i] = pp[0][c];
+        p_out[nvox + i] = pp[1][c];
+        p_out[2 * nvox + i] = pp[2][c];
+    }
+}
+
 constexpr int TVV_THREADS = 256;
 constexpr int TVV_MAX_BLOCKS = 1024;
 constexpr long long TVV_PER_BLOCK = 8 * TVV_THREADS;
@@ -173,6 +247,14 @@ __global__ void __launch_bounds__(TVV_THREADS) tv_value_final_kernel(int nb, con
 
 bool bad_grid(int nx, int ny, int nz) {
     return nx < 1 || ny < 1 || nz < 1 || (nx + TV_TX - 1) / TV_TX > 65535 || (ny + TV_TY - 1) / TV_TY > 65535;
+}
+
+bool finite_positive(double v) { return v > 0.0 && std::isfinite(v); }
+
+// [a, a + na) and [b, b + nb) (in floats) share an address
+bool overlap(const float* a, size_t na, const float* b, size_t nb) {
+    const uintptr_t a0 = (uintptr_t)a, b0 = (uintptr_t)b;
+    return a0 < b0 + nb * sizeof(float) && b0 < a0 + na * sizeof(float);
 }
 
 }  // namespace
@@ -242,6 +324,41 @@ int r2x_tv_value(void* stream, int nx, int ny, int nz, const float* x, double* o
     tv_value_partial_kernel<<<nb, TVV_THREADS, 0, st>>>(nx, ny, nz, chunk, x, (double*)scratch);
     R2X_CUDA_OK(cudaGetLastError());
     tv_value_final_kernel<<<1, TVV_THREADS, 0, st>>>(nb, (const double*)scratch, out);
+    R2X_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int r2x_tv_cp_step(void* stream, int nx, int ny, int nz, const float* x, const float* xbar, const float* p,
+                   const float* g, float tau, float sigma, float nu, int nonneg, float* x_out, float* xbar_out,
+                   float* p_out) {
+    using namespace r2x;
+    if (bad_grid(nx, ny, nz))
+        return fail_msg(R2X_ERR_INVALID, "r2x_tv_cp_step: bad grid (each size >= 1, nx <= 262140, ny <= 524280)");
+    if (!x || !xbar || !p || !g || !x_out || !xbar_out || !p_out)
+        return fail_msg(R2X_ERR_INVALID, "r2x_tv_cp_step: bad pointer (NULL)");
+    const double sn = (double)sigma * nu, tn = (double)tau * nu, pmax = 1.0 / (double)nu;
+    if (!finite_positive(tau) || !finite_positive(sigma) || !finite_positive(nu) || !finite_positive((float)sn) ||
+        !finite_positive((float)tn) || !finite_positive((float)pmax))
+        return fail_msg(R2X_ERR_INVALID,
+                        "r2x_tv_cp_step: bad step (tau, sigma, nu, sigma nu, tau nu and 1 / nu finite and > 0)");
+    if (nonneg != 0 && nonneg != 1) return fail_msg(R2X_ERR_INVALID, "r2x_tv_cp_step: bad nonneg (0 or 1)");
+    const size_t nvox = (size_t)nx * ny * nz;
+    const float* ins[4] = {x, xbar, g, p};
+    const size_t in_n[4] = {nvox, nvox, nvox, 3 * nvox};
+    float* outs[3] = {x_out, xbar_out, p_out};
+    const size_t out_n[3] = {nvox, nvox, 3 * nvox};
+    for (int o = 0; o < 3; ++o) {
+        for (int k = 0; k < 4; ++k)
+            if (overlap(outs[o], out_n[o], ins[k], in_n[k]))
+                return fail_msg(R2X_ERR_INVALID, "r2x_tv_cp_step: bad alias (an output overlaps an input)");
+        for (int k = o + 1; k < 3; ++k)
+            if (overlap(outs[o], out_n[o], outs[k], out_n[k]))
+                return fail_msg(R2X_ERR_INVALID, "r2x_tv_cp_step: bad alias (two outputs overlap)");
+    }
+    const dim3 grid((nz + TV_TZ - 1) / TV_TZ, (ny + TV_TY - 1) / TV_TY, (nx + TV_TX - 1) / TV_TX);
+    tv_cp_kernel<<<grid, TV_THREADS, 0, (cudaStream_t)stream>>>(nx, ny, nz, x, xbar, p, g, tau, (float)sn, (float)tn,
+                                                                (float)pmax, (float)(pmax * pmax), nonneg, x_out,
+                                                                xbar_out, p_out);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }

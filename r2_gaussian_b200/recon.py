@@ -1,11 +1,12 @@
 """Traditional CT reconstructions on the GPU -- FDK, SART / OS-SART and CGLS, what the reference obtains from TIGRE's
 `algs` (`r2_gaussian/utils/ct_utils.py::recon_volume` / `run_ct_recon_algs`, `scripts/run_traditional_methods.py`),
-and the TV-regularised FISTA-TV.
+the TV-regularised FISTA-TV and the data-constrained TV reconstruction cp_tv.
 
     x, l2 = cgls(projs, angles, scanner_cfg, niter=60)
     x = sart(projs, angles, scanner_cfg, niter=20, lmbda=1.0, lmbda_red=0.999, blocksize=1, nonneg=True)
     x, history = fista_tv(projs, angles, scanner_cfg, niter=FISTA_NITER, lmbda=FISTA_LAMBDA, tviter=20, nonneg=True)
-    x = recon_volume(projs, angles, scanner_cfg, method)           # fdk | cgls | sart | ossart | fista_tv
+    x, history = cp_tv(projs, angles, scanner_cfg, niter=CP_NITER, epsilon=None, epsilon_ratio=0.15, nonneg=True)
+    x = recon_volume(projs, angles, scanner_cfg, method)           # fdk | cgls | sart | ossart | fista_tv | cp_tv
 
 `projs` is a CUDA [N, H, W] tensor in the dataset layout (scene units, as the readers return it) and `scanner_cfg` the
 scaled dict of `dataset.read_scene`; volumes are [nx, ny, nz] in the voxelizer's layout.  A is `projector.project`
@@ -44,8 +45,31 @@ history[k] = {"data": 1/2 |A x_k - b|^2, "tv": TV(x_k), "F": data + lmbda tv} (o
 recognised convex baseline (TIGRE's algorithm collection has a FISTA with a TV proximal step); ASD-POCS, whose adaptive
 step and stop rules are defined by TIGRE's implementation, is not what it computes.
 
-Parity with TIGRE's binaries is not pinned (as for FDK and the projector).  ASD-POCS / OS-ASD-POCS are not built;
-`fista_tv` is the TV-regularised method this project offers.
+cp_tv solves the data-constrained TV problem that the reference's ASD-POCS baseline targets,
+    minimise  TV(x)   subject to   |A x - b| <= epsilon,   x >= 0   (nonneg=False drops the constraint)
+with the same isotropic TV, by Chambolle-Pock (primal-dual hybrid gradient, as Sidky, Jorgensen and Pan 2012 use it
+for CT) on K = [A; nu grad] (grad / div = -grad^T of csrc/r2x_tv.cu).  Step sizes: L >= |A|^2 (the Schur bound, as for
+FISTA-TV, or `L=`), nu = sqrt(L / 12) so that |K|^2 <= L + 12 nu^2 = 2 L, tau = sigma = 0.99 / sqrt(2 L), so
+tau sigma |K|^2 <= 0.98 < 1.  From x_0 = xbar_0 = 0, q_0 = 0 ([N, H, W]) and p_0 = 0 ([3, nx, ny, nz]); per iteration:
+    1. u = q + sigma (A xbar - b),  q = max(1 - sigma epsilon / |u|, 0) u     (prox of sigma F*, F the indicator of the
+       epsilon-ball around b; |u| a float64 reduction in a fixed order, as `_dot`)
+    2. p = P_{1/nu}(p + sigma nu grad xbar)                                    (per voxel onto |p_i| <= 1/nu)
+    3. x+ = P_C(x - tau A^T q + tau nu div p)                                  (C = {x >= 0} or everything)
+    4. xbar = 2 x+ - x,  x = x+
+Step 1 runs in projection space in torch, in the scaled form v = q / sigma + (A xbar - b), q / sigma =
+max(1 - epsilon / |v|, 0) v (the same q), so that epsilon >= |b| gives q = 0 exactly and x stays exactly 0; steps 2-4
+are one launch of `tv.tv_cp_step` (r2x_tv_cp_step) given A^T q.  history[k] = {"residual": |A x_k - b|, "tv": TV(x_k)};
+A xbar is then 2 A x_k - A x_{k-1} from the history's projections (A is linear), so an iteration costs one A and one
+A^T.  `cp_tv` takes epsilon = epsilon_ratio |A FDK(b) - b| by default (the reference's asd_pocs rule, 0.15, with this
+project's FDK and projector); the ratio has no units.  Convergence with these steps is slow: on the noisy 256^3 scene
+of DESIGN §8 the residual is still 4.7 epsilon after CP_NITER = 300 iterations (4.6 after 600), although 3D PSNR is
+within 1.1 dB of FISTA-TV's there; the Schur L is 1.67 |A|^2 on that geometry, and tau = sigma is not tuned to the
+scale of b.  So at the default iteration count the volume is a TV-regularised iterate on its way to the constrained
+optimum, not that optimum; `history` shows how far the residual is from epsilon.
+
+Parity with TIGRE's binaries is not pinned (as for FDK and the projector).  ASD-POCS / OS-ASD-POCS are not built:
+their adaptive step and stop rules are defined by TIGRE's implementation.  `cp_tv` solves their convex problem and
+`fista_tv` the TV-regularised least-squares one.
 
     python -m r2_gaussian_b200.recon -s <scene> -m <output> [--methods fdk,sart,cgls] [--short_scan]
         [--use_offDetector [--half_fan]] [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
@@ -53,7 +77,8 @@ Parity with TIGRE's binaries is not pinned (as for FDK and the projector).  ASD-
 mirrors `scripts/run_traditional_methods.py`: it reconstructs the scene's train views with each method, scores the
 volume against `vol_gt` with `metrics.metric_vol` and writes, per method, `<output>/<method>/ct_gt.npy`, `ct_pred.npy`,
 `eval_3d.yml` (method, psnr_3d, ssim_3d, ssim_3d_x/y/z, duration (sec), duration (min); fdk under `--short_scan`
-also `short_scan: true`, and `filter: <name>` under a `--fdk_filter` other than ram_lak) and the test views
+also `short_scan: true`, and `filter: <name>` under a `--fdk_filter` other than ram_lak; cp_tv ends with `epsilon` and
+`residual`, the final |A x - b|) and the test views
 `projs/{i:05d}_render.npy` (projections of the reconstruction) and `projs/{i:05d}_gt.npy`, plus `<output>/eval_3d.yml`
 keyed by method.  PNG slices and projections are not written (matplotlib is not a dependency of this project).
 `--short_scan` reconstructs fdk with Parker redundancy weights (`fdk.fdk(short_scan=True)`), for scenes whose train
@@ -76,7 +101,7 @@ import time
 import numpy as np
 import torch
 
-METHODS = ("fdk", "sart", "ossart", "cgls", "fista_tv")
+METHODS = ("fdk", "sart", "ossart", "cgls", "fista_tv", "cp_tv")
 NOT_BUILT = ("asd_pocs", "os_asd_pocs")
 # iteration counts and parameters of ct_utils.recon_volume / run_ct_recon_algs
 CGLS_NITER = 60
@@ -86,6 +111,9 @@ OSSART_BLOCKSIZE = 10
 FISTA_NITER = 50
 FISTA_LAMBDA = 1e-3
 FISTA_TVITER = 20
+# cp_tv defaults: the reference's asd_pocs epsilon ratio; CP_NITER from the convergence curve of DESIGN §8
+CP_NITER = 300
+CP_EPSILON_RATIO = 0.15
 
 
 def _dot(a: torch.Tensor, b: torch.Tensor) -> float:
@@ -186,6 +214,61 @@ def fista_tv_solve(b: torch.Tensor, A, At, shape, niter: int, lmbda: float, tvit
     return x_prev, history
 
 
+def _check_cp(niter, epsilon, L):
+    if int(niter) != niter or niter < 1:
+        raise ValueError(f"cp_tv: niter must be an integer >= 1, got {niter}")
+    if epsilon is not None and not (float(epsilon) >= 0.0 and math.isfinite(float(epsilon))):
+        raise ValueError(f"cp_tv: epsilon must be finite and >= 0, got {epsilon}")
+    if L is not None and not (float(L) > 0.0 and math.isfinite(float(L))):
+        raise ValueError(f"cp_tv: L must be finite and > 0, got {L}")
+
+
+def cp_step_sizes(L: float) -> tuple[float, float, float]:
+    """(tau, sigma, nu) of cp_tv for L >= |A|^2: nu = sqrt(L / 12), tau = sigma = 0.99 / sqrt(2 L)."""
+    tau = 0.99 / math.sqrt(2.0 * L)
+    return tau, tau, math.sqrt(L / 12.0)
+
+
+def cp_tv_solve(b: torch.Tensor, A, At, shape, niter: int, epsilon: float, L=None, nonneg: bool = True, step=None,
+                tv=None):
+    """Chambolle-Pock for min TV(x) s.t. |A x - b| <= epsilon (and x >= 0 when nonneg) from x = 0, over the callables
+    A(x, views) / At(y, views, weights); `shape` is the volume's.  `step(x, xbar, p, g, tau, sigma, nu, nonneg)` and
+    `tv(x)` default to the GPU `tv.tv_cp_step` / `tv.tv_value`.  Returns (x, history)."""
+    _check_cp(niter, epsilon, L)
+    if epsilon is None:
+        raise ValueError("cp_tv: epsilon must be given")
+    if step is None:
+        from .tv import tv_cp_step as step
+    if tv is None:
+        from .tv import tv_value as tv
+    everything = slice(None)
+    if L is None:
+        L = schur_lipschitz(b, A, At, shape)
+        if not L > 0.0:
+            raise ValueError("cp_tv: A 1 or A^T 1 is zero: no ray meets the volume")
+    tau, sigma, nu = cp_step_sizes(float(L))
+    epsilon = float(epsilon)
+    x = torch.zeros(tuple(shape), dtype=b.dtype, device=b.device)
+    xbar = x
+    p = torch.zeros((3,) + tuple(shape), dtype=b.dtype, device=b.device)
+    y = torch.zeros_like(b)                               # q / sigma
+    ax = torch.zeros_like(b)                              # A x_k (A 0 = 0)
+    ax_bar = ax                                           # A xbar_k
+    history = []
+    for _ in range(niter):
+        v = ax_bar.sub(b).add_(y)
+        norm = _dot(v, v) ** 0.5
+        y = torch.zeros_like(v) if norm <= epsilon else v.mul_(1.0 - epsilon / norm)
+        g = At(y.mul(sigma), everything, False)
+        x_next, xbar, p = step(x, xbar, p, g, tau, sigma, nu, nonneg)
+        ax_next = A(x_next, everything)
+        r = ax_next.sub(b)
+        history.append({"residual": _dot(r, r) ** 0.5, "tv": float(tv(x_next))})
+        ax_bar = ax_next.mul(2.0).sub_(ax)
+        x, ax = x_next, ax_next
+    return x, history
+
+
 def _operator(projs, angles, scanner_cfg, use_offDetector: bool = False):
     from .projector import CTOperator
 
@@ -221,6 +304,34 @@ def fista_tv(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = FISTA_
     return fista_tv_solve(b, op.A, op.At, op.nvox, niter, lmbda, tviter, L, nonneg)
 
 
+def _check_ratio(epsilon_ratio):
+    if not (float(epsilon_ratio) >= 0.0 and math.isfinite(float(epsilon_ratio))):
+        raise ValueError(f"cp_tv: epsilon_ratio must be finite and >= 0, got {epsilon_ratio}")
+
+
+def cp_tv_epsilon(projs: torch.Tensor, angles, scanner_cfg: dict, epsilon_ratio: float = CP_EPSILON_RATIO,
+                  use_offDetector: bool = False) -> float:
+    """epsilon_ratio |A FDK(b) - b|, the reference's asd_pocs tolerance, with this project's FDK and projector."""
+    from .fdk import fdk
+
+    _check_ratio(epsilon_ratio)
+    op, b = _operator(projs, angles, scanner_cfg, use_offDetector)
+    r = op.A(fdk(b, angles, scanner_cfg, use_offDetector=use_offDetector)).sub_(b)
+    return float(epsilon_ratio) * _dot(r, r) ** 0.5
+
+
+def cp_tv(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = CP_NITER, epsilon=None,
+          epsilon_ratio: float = CP_EPSILON_RATIO, L=None, nonneg: bool = True, use_offDetector: bool = False):
+    """Data-constrained TV (Chambolle-Pock) on the GPU projector pair and the GPU step kernel; epsilon=None takes
+    `cp_tv_epsilon(..., epsilon_ratio)`.  Returns (volume, history)."""
+    _check_cp(niter, epsilon, L)
+    _check_ratio(epsilon_ratio)
+    op, b = _operator(projs, angles, scanner_cfg, use_offDetector)
+    if epsilon is None:
+        epsilon = cp_tv_epsilon(b, angles, scanner_cfg, epsilon_ratio, use_offDetector)
+    return cp_tv_solve(b, op.A, op.At, op.nvox, niter, epsilon, L, nonneg)
+
+
 def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, short_scan: bool = False,
                  use_offDetector: bool = False, half_fan: bool = False, fdk_filter: str | None = None) -> torch.Tensor:
     """The reconstructions of ct_utils.recon_volume / run_ct_recon_algs with their iteration counts.  `short_scan`
@@ -248,6 +359,8 @@ def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, sh
         return sart(projs, angles, scanner_cfg, SART_NITER, blocksize=OSSART_BLOCKSIZE, use_offDetector=off)
     if method == "fista_tv":
         return fista_tv(projs, angles, scanner_cfg, use_offDetector=off)[0]
+    if method == "cp_tv":
+        return cp_tv(projs, angles, scanner_cfg, use_offDetector=off)[0]
     raise ValueError(f"recon_volume: unknown method {method!r} (supported: {', '.join(METHODS)})")
 
 
@@ -287,7 +400,8 @@ def _parse_methods(text: str) -> list[str]:
 
 
 def main(argv=None) -> dict:
-    ap = argparse.ArgumentParser(description="Traditional CT reconstructions (FDK, SART, OS-SART, CGLS, FISTA-TV) of a scene")
+    ap = argparse.ArgumentParser(description="Traditional CT reconstructions (FDK, SART, OS-SART, CGLS, FISTA-TV, "
+                                             "CP-TV) of a scene")
     ap.add_argument("-s", "--source_path", required=True, help="scene directory or NAF pickle")
     ap.add_argument("-m", "--model_path", required=True, help="output directory")
     ap.add_argument("--methods", default="fdk,sart,cgls", help=f"comma-separated subset of {','.join(METHODS)}")
@@ -329,8 +443,14 @@ def main(argv=None) -> dict:
         short_scan = a.short_scan and method == "fdk"
         half_fan = a.half_fan and method == "fdk"
         fdk_filter = a.fdk_filter if method == "fdk" else None
-        pred = recon_volume(projs_train, train_angles, cfg, method, short_scan=short_scan,
-                            use_offDetector=a.use_offDetector, half_fan=half_fan, fdk_filter=fdk_filter)
+        extra = {}
+        if method == "cp_tv":
+            eps = cp_tv_epsilon(projs_train, train_angles, cfg, use_offDetector=a.use_offDetector)
+            pred, hist = cp_tv(projs_train, train_angles, cfg, epsilon=eps, use_offDetector=a.use_offDetector)
+            extra = {"epsilon": eps, "residual": hist[-1]["residual"]}
+        else:
+            pred = recon_volume(projs_train, train_angles, cfg, method, short_scan=short_scan,
+                                use_offDetector=a.use_offDetector, half_fan=half_fan, fdk_filter=fdk_filter)
         torch.cuda.synchronize()
         duration = time.time() - t0
         ct_pred = pred.cpu().numpy()
@@ -349,6 +469,7 @@ def main(argv=None) -> dict:
             report["filter"] = fdk_filter
         if a.use_offDetector:
             report["use_offDetector"] = True
+        report.update(extra)
         with open(os.path.join(save, "eval_3d.yml"), "w") as f:
             yaml.dump(report, f, default_flow_style=False, sort_keys=False)
         if test_angles:
