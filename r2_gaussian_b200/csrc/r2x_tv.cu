@@ -245,8 +245,16 @@ __global__ void __launch_bounds__(TVV_THREADS) tv_value_final_kernel(int nb, con
     if (threadIdx.x == 0) out[0] = s[0];
 }
 
+// tiles of t voxels along an axis of n voxels, in 64 bits: n + t - 1 is past INT_MAX for n within a tile of it
+inline long long tiles(int n, int t) { return ((long long)n + t - 1) / t; }
+
 bool bad_grid(int nx, int ny, int nz) {
-    return nx < 1 || ny < 1 || nz < 1 || (nx + TV_TX - 1) / TV_TX > 65535 || (ny + TV_TY - 1) / TV_TY > 65535;
+    return nx < 1 || ny < 1 || nz < 1 || tiles(nx, TV_TX) > 65535 || tiles(ny, TV_TY) > 65535;
+}
+
+// the tv_fgp_kernel / tv_cp_kernel grid of a grid that passed bad_grid: z tiles on x (up to 2^26), y on y, x on z
+dim3 tile_grid(int nx, int ny, int nz) {
+    return dim3((unsigned)tiles(nz, TV_TZ), (unsigned)tiles(ny, TV_TY), (unsigned)tiles(nx, TV_TX));
 }
 
 bool finite_positive(double v) { return v > 0.0 && std::isfinite(v); }
@@ -289,7 +297,7 @@ int r2x_tv_prox(void* stream, int nx, int ny, int nz, const float* v, float weig
     }
     float* buf[3] = {(float*)scratch, (float*)scratch + 3 * nvox, (float*)scratch + 6 * nvox};
     const float step = (float)(1.0 / (12.0 * (double)weight));
-    const dim3 grid((nz + TV_TZ - 1) / TV_TZ, (ny + TV_TY - 1) / TV_TY, (nx + TV_TX - 1) / TV_TX);
+    const dim3 grid = tile_grid(nx, ny, nz);
     double t = 1.0, t_prev = 1.0;   // t_k and t_{k-1} of the launch computing p_k
     for (int k = 1; k <= niter; ++k) {
         const int mode = k == 1 ? 0 : (k == 2 ? 1 : 2);
@@ -355,7 +363,7 @@ int r2x_tv_cp_step(void* stream, int nx, int ny, int nz, const float* x, const f
             if (overlap(outs[o], out_n[o], outs[k], out_n[k]))
                 return fail_msg(R2X_ERR_INVALID, "r2x_tv_cp_step: bad alias (two outputs overlap)");
     }
-    const dim3 grid((nz + TV_TZ - 1) / TV_TZ, (ny + TV_TY - 1) / TV_TY, (nx + TV_TX - 1) / TV_TX);
+    const dim3 grid = tile_grid(nx, ny, nz);
     tv_cp_kernel<<<grid, TV_THREADS, 0, (cudaStream_t)stream>>>(nx, ny, nz, x, xbar, p, g, tau, (float)sn, (float)tn,
                                                                 (float)pmax, (float)(pmax * pmax), nonneg, x_out,
                                                                 xbar_out, p_out);

@@ -169,7 +169,9 @@ int r2x_volume_render(void* stream, int nx, int ny, int nz, const float* vol, in
     if ((uintptr_t)out % 16) return bad("pointer (out is not 16-byte aligned)");
     if (nx < 2 || ny < 2 || nz < 2) return bad("grid (each axis needs >= 2 samples)");
     if (n_frames < 1 || H < 1 || W < 1) return bad("image (n_frames, H and W must be >= 1)");
-    if (n_frames > VR_MAX_GRID || (H + VR_TILE - 1) / VR_TILE > VR_MAX_GRID || (W + VR_TILE - 1) / VR_TILE > VR_MAX_GRID)
+    // pixel tiles in 64 bits: H + VR_TILE - 1 is past INT_MAX for H within a tile of it
+    const long long tiles_y = ((long long)H + VR_TILE - 1) / VR_TILE, tiles_x = ((long long)W + VR_TILE - 1) / VR_TILE;
+    if (n_frames > VR_MAX_GRID || tiles_y > VR_MAX_GRID || tiles_x > VR_MAX_GRID)
         return bad("image (frames and pixel tiles per grid dimension must be <= 65535)");
     if (parallel != 0 && parallel != 1) return bad("parallel (0 or 1)");
     if (mode != R2X_VR_COMPOSITE && mode != R2X_VR_MIP) return bad("mode (0 composite, 1 mip)");
@@ -191,7 +193,7 @@ int r2x_volume_render(void* stream, int nx, int ny, int nz, const float* vol, in
     q.nx = nx; q.ny = ny; q.nz = nz; q.H = H; q.W = W; q.parallel = parallel; q.mode = mode; q.K = K;
     q.c0 = c0; q.inv_range = inv_range; q.expo = expo; q.step = step;
     for (int c = 0; c < 3; ++c) q.bg[c] = background[c];
-    const dim3 grid((unsigned)((W + VR_TILE - 1) / VR_TILE), (unsigned)((H + VR_TILE - 1) / VR_TILE), (unsigned)n_frames);
+    const dim3 grid((unsigned)tiles_x, (unsigned)tiles_y, (unsigned)n_frames);
     volume_render_kernel<<<grid, dim3(VR_TILE, VR_TILE), 3 * K * sizeof(float), (cudaStream_t)stream>>>(
         q, vol, cameras_dev, lut_dev, out);
     R2X_CUDA_OK(cudaGetLastError());

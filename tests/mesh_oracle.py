@@ -123,9 +123,10 @@ def table():
     return _TABLE
 
 
-def marching_cubes(vol, level=0.5) -> tuple[np.ndarray, np.ndarray]:
+def marching_cubes(vol, level=0.5, x_offset: int = 0) -> tuple[np.ndarray, np.ndarray]:
     """(verts float32 [V, 3], faces int32 [T, 3]) of include/r2x.h's marching cubes; float64 input is rounded to
-    float32 first, level too."""
+    float32 first, level too.  With `x_offset`, `vol` is the slab of x-planes x_offset, x_offset + 1, ... of a larger
+    grid: vertex x coordinates are float32(x_offset + i) + t, as the full grid's."""
     v = np.ascontiguousarray(np.asarray(vol), dtype=np.float32)
     if v.ndim != 3:
         raise ValueError("marching_cubes: expected a 3-D volume")
@@ -148,7 +149,7 @@ def marching_cubes(vol, level=0.5) -> tuple[np.ndarray, np.ndarray]:
     x1 = v[p1[:, 0], p1[:, 1], p1[:, 2]]
     with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
         t = (lv - x0) / (x1 - x0)
-    verts = p0.astype(np.float32)
+    verts = (p0 + np.array([x_offset, 0, 0], np.int64)).astype(np.float32)
     rows = np.arange(len(a))
     verts[rows, a] = verts[rows, a] + t
     if min(nx, ny, nz) < 2:

@@ -11,12 +11,16 @@ import numpy as np
 T_STOP = 2.0 ** -16
 
 
-def ray_setup(rec, H, W, parallel, shape):
+def ray_setup(rec, H, W, parallel, shape, pixels=None):
     """(o [R, 3], d [R, 3], s_in [R], s_out [R], meets [R]) for the H * W rays of one float32 camera record,
-    row-major from the top-left pixel."""
+    row-major from the top-left pixel, or for the flat pixel indices `pixels` (y W + x) only."""
     rec = np.asarray(rec, np.float32).astype(np.float64)
     P, f, r, u, p = rec[0:3], rec[3:6], rec[6:9], rec[9:12], rec[12]
-    y, x = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
+    if pixels is None:
+        y, x = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
+    else:
+        px = np.asarray(pixels, np.int64)
+        y, x = (px // W).astype(np.float64), (px % W).astype(np.float64)
     a = (((x + 0.5) - 0.5 * W) * p).reshape(-1, 1)
     b = (((0.5 * H - y) - 0.5) * p).reshape(-1, 1)
     if parallel:
@@ -88,8 +92,9 @@ def lut_colour(lut, t):
 
 
 def render_frame(vol, rec, H, W, parallel, mode="composite", clim=(0.0, 1.0), lut=((0, 0, 0), (1, 1, 1)), step=0.5,
-                 unit=None, background=(0.0, 0.0, 0.0)):
-    """float64 [H, W, 4] RGBA of one camera record."""
+                 unit=None, background=(0.0, 0.0, 0.0), pixels=None):
+    """float64 [H, W, 4] RGBA of one camera record; with `pixels` (flat indices y W + x) float64 [len(pixels), 4] of
+    those pixels only, so that a subset of a 10^6-row image stays cheap."""
     vol = np.asarray(vol, np.float32)
     shape = vol.shape
     n_ = np.asarray(shape, np.float64)
@@ -97,7 +102,7 @@ def render_frame(vol, rec, H, W, parallel, mode="composite", clim=(0.0, 1.0), lu
         unit = float(np.linalg.norm(n_ - 1) / (n_.mean() - 1))
     step64, expo = rec_step(step), rec_step(step) / rec_step(unit)
     bg = np.asarray(background, np.float32).astype(np.float64)
-    o, d, s0, s1, meets = ray_setup(rec, H, W, parallel, shape)
+    o, d, s0, s1, meets = ray_setup(rec, H, W, parallel, shape, pixels)
     n = sample_counts(s0, s1, meets, step)
     R = len(o)
     hi = n_ - 1
@@ -132,7 +137,7 @@ def render_frame(vol, rec, H, W, parallel, mode="composite", clim=(0.0, 1.0), lu
     else:
         out[meets, :3] = C[meets] + T[meets, None] * bg
         out[meets, 3] = 1.0 - T[meets]
-    return out.reshape(H, W, 4)
+    return out if pixels is not None else out.reshape(H, W, 4)
 
 
 def render(vol, cameras, **kw):
