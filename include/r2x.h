@@ -659,6 +659,78 @@ int r2x_volume_render(void* stream, int nx, int ny, int nz, const float* vol, in
                       const float* cameras_dev, int parallel, int mode, float c0, float c1, const float* lut_dev, int K,
                       float step, float unit, const float* background, float* out);
 
+/* ---- scene view: depth-tested triangles and line segments (r2_gaussian_b200/scene_view.py, visualize_scene.py) ---- */
+/* Replaces the open3d window of the reference's scripts/visualize_scene.py with a headless rasterizer.  Pixel parity
+ * with open3d is not claimed.  Everything is in scene units.
+ *   input    n_prims primitives; primitive i has pos[i] (device, float64 [3][3]: three points, a segment uses the first
+ *            two), meta[i] (device, int32 [2]: kind, texture index) and attr[i] (device, float32 [R2X_SV_ATTR = 12]):
+ *              R2X_SV_FLAT     0 triangle, colour attr[0:3]
+ *              R2X_SV_MESH     1 triangle, base colour attr[0:3], per-vertex normals attr[3:6], [6:9], [9:12] (world)
+ *              R2X_SV_TEXTURED 2 triangle, per-vertex texture coordinates (u, v) in attr[3:5], [5:7], [7:9]
+ *              R2X_SV_LINE     3 segment pos[i][0] -> pos[i][1], colour attr[0:3], width w = attr[3] pixels (> 0)
+ *            tex (device, float32 [n_tex][tex_h][tex_w]) and lut (device, float32 [K][3]) serve textured triangles.
+ *   camera   cameras (device, float32) holds R2X_SV_CAMERA_FLOATS = 16 floats per frame, the record of the volume
+ *            renderer (P, f, r, u, pitch p; `parallel` selects the projection), read as float64.  Camera coordinates of
+ *            a point X: d = X - P, (x, y, z) = (d.r, d.u, d.f), each dot product ((d0 a0 + d1 a1) + d2 a2).
+ *            Screen: sx = W/2 + x / q, sy = H/2 - y / q with q = z p (perspective) or q = p (parallel); pixel (column x,
+ *            row y from the top) has its centre at (x + 1/2, y + 1/2).
+ *   clip     in camera coordinates, against 5 planes in order, inside iff the value is >= 0: z - near; and the guard band
+ *            G = R2X_SV_GUARD = 2^20 pixels: g - x, g + x, g - y, g + y with g = G p z (perspective) or G p (parallel).
+ *            A triangle is clipped Sutherland-Hodgman (vertices in order, each edge a -> b keeps a if inside and adds the
+ *            cut if the two sides differ); every cut point is formed from the edge's inside end A to its outside end B:
+ *            t = dA / (dA - dB), A + t (B - A), so two triangles that share an edge get the same cut points.  The
+ *            polygon (3 to 8 vertices; fewer than 3 is nothing) is the fan (0, k, k+1).  A segment keeps the part
+ *            inside every plane, its outside end replaced by the cut.  Anything wholly behind the near plane is dropped.
+ *   snap     screen points are snapped to 1/256 pixel: X = rint(256 sx), Y = rint(256 sy) (int64, ties to even).
+ *   coverage triangle (fan triangle A, B, C; zero area dropped; negative area: B and C swapped, both windings drawn):
+ *            pixel centre p = (256 x + 128, 256 y + 128) is covered iff for each edge a -> b (A->B, B->C, C->A)
+ *            e = dx (py - ay) - dy (px - ax) with (dx, dy) = b - a is > 0, or = 0 on an edge with dy < 0 or (dy = 0 and
+ *            dx > 0) (top-left rule).  All int64, exact: two triangles sharing an edge never both cover a pixel and
+ *            never both miss one.  A polygon covers the union of its fan.
+ *            segment (ends a, b = the snapped points / 256, in pixels; c = pixel centre; all float64, round to nearest):
+ *            d = b - a, e = c - a, L = d.d, t = clamp((e.d) / L, 0, 1) (0 if L = 0), q = e - t d; covered iff
+ *            q.q <= r r with r = w / 2.
+ *   depth    triangle: with the camera-space plane n = (V1 - V0) x (V2 - V0), c = n.V0 of the unclipped vertices and the
+ *            pixel's a = ((x + 1/2) - W/2) p, b = ((H/2 - y) - 1/2) p: z = c / ((n0 a + n1 b) + n2) (perspective) or
+ *            ((c - n0 a) - n1 b) / n2 (parallel) -- perspective-correct.  Segment: 1/z = (1 - t)/za + t/zb
+ *            (perspective) or z = za + t (zb - za) (parallel), za, zb the clipped ends' depths.  z below near (or NaN)
+ *            becomes near; then rounded once to float32.
+ *   visible  each covered pixel does a 64-bit atomicMin of (float bits of z) << 32 | i into keys (device, uint64
+ *            [n_frames][H][W], all ones where nothing is drawn).  Positive floats order as their bits: the nearest
+ *            primitive wins and ties go to the lower id; the minimum does not depend on the order of the atomics.
+ *   shading  one thread per pixel decodes the id.  Flat triangles and segments: their colour.  Mesh and textured
+ *            triangles: the point P on the plane (perspective (a z, b z, z), parallel (a, b, z), z as above) has weights
+ *            w_v = n.((V_{v+1} - P) x (V_{v+2} - P)) / n.n (1/3 each if n.n = 0).  Mesh: N = sum w_v N_v, D = the
+ *            pixel's ray direction in world coordinates ((f + a r) + b u, or f), lambda = min(|N.D| / sqrt(N.N D.D), 1)
+ *            (0 if N = 0), colour = base (A + (1 - A) lambda) with A = R2X_SV_AMBIENT = 0.25: a two-sided headlight.
+ *            Textured: (u, v) = sum w_v uv_v, texel column min(max(floor(u tex_w), 0), tex_w - 1), row likewise from v
+ *            and tex_h, value t clamped to [0, 1] (NaN -> 0), colour from the LUT as the volume renderer maps t
+ *            (float32, no FMA).  Float64 until the colour is rounded to float32.  Uncovered: background[3] (host).
+ *   output   rgb (device, float32 [n_frames][H][W][3]).
+ * Work: a primitive whose clamped pixel box is at most R2X_SV_TILE = 16 pixels on each side is rasterized by one thread;
+ * a larger one is split into the 16 x 16 tiles of its box, one CTA (one thread per pixel) per tile.  Frames on the
+ * grid's z dimension.  Scratch (r2x_scene_raster_scratch_bytes, no GPU; 0 for bad sizes): 64 bytes plus 40 bytes per
+ * (primitive, frame).  Arguments are checked before any CUDA work: non-NULL pointers (tex only with n_tex > 0),
+ * 1 <= n_prims with n_prims n_frames <= 2^31 - 1, 1 <= n_frames <= 65535, 1 <= H, W <= R2X_SV_MAX_SIDE = 16384,
+ * texture sides 1 to 16384 with n_tex tex_h tex_w <= 2^31 - 1, 1 <= K <= 4096, parallel 0 or 1, finite near > 0, a
+ * finite background, enough scratch.  The contents of pos / meta / attr / tex (finite points, widths > 0, kinds,
+ * texture indices < n_tex) are the caller's to check.  Asynchronous on `stream`; two calls give the same bits. */
+#define R2X_SV_CAMERA_FLOATS 16
+#define R2X_SV_ATTR 12
+#define R2X_SV_TILE 16
+#define R2X_SV_MAX_SIDE 16384
+#define R2X_SV_GUARD 1048576.0
+#define R2X_SV_AMBIENT 0.25
+#define R2X_SV_FLAT 0
+#define R2X_SV_MESH 1
+#define R2X_SV_TEXTURED 2
+#define R2X_SV_LINE 3
+size_t r2x_scene_raster_scratch_bytes(int n_prims, int n_frames);
+int r2x_scene_raster(void* stream, int n_prims, const double* pos, const int* meta, const float* attr, int n_tex,
+                     int tex_h, int tex_w, const float* tex, const float* lut, int K, int n_frames, int H, int W,
+                     const float* cameras, int parallel, double near, const float* background,
+                     unsigned long long* keys, float* rgb, void* scratch, size_t scratch_bytes);
+
 /* ---- multi-GPU exchange step: one-shot sum over NVLink peer memory ------------------------------ */
 /* The Gaussian-sharded projector (one process per GPU, every rank renders its index shard) needs ONE exchange per
  * projection: the sum of the per-rank partial detector images (BASELINE north_star; the reference itself is

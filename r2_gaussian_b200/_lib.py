@@ -112,6 +112,9 @@ PROTOTYPES = {
     "r2x_marching_cubes_count": (_i, [_vp, _i, _i, _i, _vp, _f, _vp, _vp, _sz]),
     "r2x_marching_cubes_emit": (_i, [_vp, _i, _i, _i, _vp, _f, _ll, _ll, _vp, _vp, _vp, _sz]),
     "r2x_volume_render": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _i, _i, _f, _f, _vp, _i, _f, _f, _vp, _vp]),
+    "r2x_scene_raster_scratch_bytes": (_sz, [_i, _i]),
+    "r2x_scene_raster": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, C.c_double, _vp,
+                              _vp, _vp, _vp, _sz]),
     "r2x_peer_alloc": (_i, [_sz, C.POINTER(_vp)]),
     "r2x_peer_free": (_i, [_vp]),
     "r2x_ipc_export": (_i, [_vp, _vp]),
