@@ -659,7 +659,7 @@ int r2x_volume_render(void* stream, int nx, int ny, int nz, const float* vol, in
                       const float* cameras_dev, int parallel, int mode, float c0, float c1, const float* lut_dev, int K,
                       float step, float unit, const float* background, float* out);
 
-/* ---- scene view: depth-tested triangles and line segments (r2_gaussian_b200/scene_view.py, visualize_scene.py) ---- */
+/* ---- scene view: depth-tested triangles, line segments and ellipsoids (scene_view.py, visualize_scene.py) ---- */
 /* Replaces the open3d window of the reference's scripts/visualize_scene.py with a headless rasterizer.  Pixel parity
  * with open3d is not claimed.  Everything is in scene units.
  *   input    n_prims primitives; primitive i has pos[i] (device, float64 [3][3]: three points, a segment uses the first
@@ -668,6 +668,9 @@ int r2x_volume_render(void* stream, int nx, int ny, int nz, const float* vol, in
  *              R2X_SV_MESH     1 triangle, base colour attr[0:3], per-vertex normals attr[3:6], [6:9], [9:12] (world)
  *              R2X_SV_TEXTURED 2 triangle, per-vertex texture coordinates (u, v) in attr[3:5], [5:7], [7:9]
  *              R2X_SV_LINE     3 segment pos[i][0] -> pos[i][1], colour attr[0:3], width w = attr[3] pixels (> 0)
+ *              R2X_SV_ELLIPSOID 4 solid ellipsoid E = { c + R diag(s) v : |v| <= 1 } (the 1-sigma ellipsoid of
+ *                              Sigma = R S^2 R^T): centre c = pos[i][0], semi-axes s = pos[i][1] (all > 0; pos[i][2] is
+ *                              ignored), colour attr[0:3], quaternion (w, x, y, z) = attr[3:7] (non-zero)
  *            tex (device, float32 [n_tex][tex_h][tex_w]) and lut (device, float32 [K][3]) serve textured triangles.
  *   camera   cameras (device, float32) holds R2X_SV_CAMERA_FLOATS = 16 floats per frame, the record of the volume
  *            renderer (P, f, r, u, pitch p; `parallel` selects the projection), read as float64.  Camera coordinates of
@@ -706,6 +709,31 @@ int r2x_volume_render(void* stream, int nx, int ny, int nz, const float* vol, in
  *            Textured: (u, v) = sum w_v uv_v, texel column min(max(floor(u tex_w), 0), tex_w - 1), row likewise from v
  *            and tex_h, value t clamped to [0, 1] (NaN -> 0), colour from the LUT as the volume renderer maps t
  *            (float32, no FMA).  Float64 until the colour is rounded to float32.  Uncovered: background[3] (host).
+ *   ellipsoid (kind 4; float64, every operation rounded to nearest in the order written, dot products as above)
+ *            rotation  q = attr[3:7] read as float64, m = sqrt(((w w + x x) + y y) + z z), (w, x, y, z) /= m, and R is
+ *                      build_rotation's matrix: R00 = 1 - 2 (y y + z z), R01 = 2 (x y - w z), R02 = 2 (x z + w y),
+ *                      R10 = 2 (x y + w z), R11 = 1 - 2 (x x + z z), R12 = 2 (y z - w x), R20 = 2 (x z - w y),
+ *                      R21 = 2 (y z + w x), R22 = 1 - 2 (x x + y y); k_j = 1 / s_j.
+ *            ray       pixel (x, y) with a, b as below: perspective O = P, D = (f + a r) + b u; parallel
+ *                      O = (P + a r) + b u, D = f.  D.f is 1 up to the camera's rounding: the ray parameter is the depth.
+ *            hit       w = O - c; e_j = ((R0j w0 + R1j w1) + R2j w2) k_j, g_j likewise from D; A = g.g, B = g.e,
+ *                      C = e.e - 1, Delta = B B - A C.  Covered iff Delta >= 0 and the larger root is >= near, with the
+ *                      roots t1 = h / A and t2 = C / h (t2 = t1 if h = 0), h = -(B + copysign(sqrt(Delta), B)); z is
+ *                      the smaller root if it is >= near, else the larger (a camera inside, or an ellipsoid cut by the
+ *                      near plane, sees the inside surface).  The key is written as for the other kinds.
+ *            box       c' = the camera coordinates of c; M_ij = ((r_0 R0j + r_1 R1j) + r_2 R2j) s_j with the camera
+ *                      rows r, u, f for i = 0, 1, 2; S_kl = (M_k0 M_l0 + M_k1 M_l1) + M_k2 M_l2 (Sigma in camera
+ *                      coordinates).  Nothing if c'_z + sqrt(S_zz) < near.  Perspective with c'_z - sqrt(S_zz) < near,
+ *                      or with a2 = c'_z c'_z - S_zz not > 0: the whole frame.  Perspective otherwise: in x the tangent
+ *                      planes through the camera, b1 = c'_x c'_z - S_xz, c0 = c'_x c'_x - S_xx,
+ *                      d = sqrt(max(b1 b1 - a2 c0, 0)), alpha = (b1 -+ d) / a2, sx = W/2 + alpha / p; in y likewise
+ *                      from c'_y, S_yz, S_yy, sy = H/2 - beta / p.  Parallel: sx = W/2 + (c'_x -+ sqrt(S_xx)) / p,
+ *                      sy = H/2 - (c'_y +- sqrt(S_yy)) / p.  Pixel box: columns min(max(floor(sx_lo) - 1, 0), W) to
+ *                      max(min(floor(sx_hi) + 1, W - 1), -1), rows likewise (empty if reversed).
+ *            shading   the hit is recomputed from the id: H = O + z D (per component O_i + z D_i), v = H - c,
+ *                      m_j = (R0j v0 + R1j v1) + R2j v2, n_i = (R_i0 (m_0 k_0) k_0 + R_i1 (m_1 k_1) k_1) + R_i2 (m_2 k_2) k_2
+ *                      (n = R diag(1/s^2) R^T (H - c)), lambda = min(|n.D| / sqrt(n.n D.D), 1) (0 if n = 0), colour =
+ *                      base (A + (1 - A) lambda): the mesh's headlight.
  *   output   rgb (device, float32 [n_frames][H][W][3]).
  * Work: a primitive whose clamped pixel box is at most R2X_SV_TILE = 16 pixels on each side is rasterized by one thread;
  * a larger one is split into the 16 x 16 tiles of its box, one CTA (one thread per pixel) per tile.  Frames on the
@@ -714,7 +742,7 @@ int r2x_volume_render(void* stream, int nx, int ny, int nz, const float* vol, in
  * 1 <= n_prims with n_prims n_frames <= 2^31 - 1, 1 <= n_frames <= 65535, 1 <= H, W <= R2X_SV_MAX_SIDE = 16384,
  * texture sides 1 to 16384 with n_tex tex_h tex_w <= 2^31 - 1, 1 <= K <= 4096, parallel 0 or 1, finite near > 0, a
  * finite background, enough scratch.  The contents of pos / meta / attr / tex (finite points, widths > 0, kinds,
- * texture indices < n_tex) are the caller's to check.  Asynchronous on `stream`; two calls give the same bits. */
+ * texture indices < n_tex, semi-axes > 0, non-zero quaternions) are the caller's to check.  Asynchronous on `stream`; two calls give the same bits. */
 #define R2X_SV_CAMERA_FLOATS 16
 #define R2X_SV_ATTR 12
 #define R2X_SV_TILE 16
@@ -725,6 +753,7 @@ int r2x_volume_render(void* stream, int nx, int ny, int nz, const float* vol, in
 #define R2X_SV_MESH 1
 #define R2X_SV_TEXTURED 2
 #define R2X_SV_LINE 3
+#define R2X_SV_ELLIPSOID 4
 size_t r2x_scene_raster_scratch_bytes(int n_prims, int n_frames);
 int r2x_scene_raster(void* stream, int n_prims, const double* pos, const int* meta, const float* attr, int n_tex,
                      int tex_h, int tex_w, const float* tex, const float* lut, int K, int n_frames, int H, int W,

@@ -117,9 +117,87 @@ __device__ __forceinline__ float depth_key_f(const SvParams& q, double z) {
     return __double2float_rn(z >= q.near ? z : q.near);   // NaN -> near
 }
 
+// an ellipsoid: centre, rotation (columns: the axes), semi-axes and their inverses
+struct Ell {
+    double c[3], R[3][3], s[3], k[3];
+};
+
+__device__ void load_ell(const double* __restrict__ pos, const float* __restrict__ attr, int id, Ell& E) {
+    const double* X = pos + (size_t)id * 9;
+    const float* at = attr + (size_t)id * R2X_SV_ATTR;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        E.c[i] = __ldg(X + i);
+        E.s[i] = __ldg(X + 3 + i);
+        E.k[i] = ddiv(1.0, E.s[i]);
+    }
+    double w = __ldg(at + 3), x = __ldg(at + 4), y = __ldg(at + 5), z = __ldg(at + 6);
+    const double m = __dsqrt_rn(dadd(dadd(dadd(dmul(w, w), dmul(x, x)), dmul(y, y)), dmul(z, z)));
+    w = ddiv(w, m); x = ddiv(x, m); y = ddiv(y, m); z = ddiv(z, m);
+    E.R[0][0] = dsub(1.0, dmul(2.0, dadd(dmul(y, y), dmul(z, z))));
+    E.R[0][1] = dmul(2.0, dsub(dmul(x, y), dmul(w, z)));
+    E.R[0][2] = dmul(2.0, dadd(dmul(x, z), dmul(w, y)));
+    E.R[1][0] = dmul(2.0, dadd(dmul(x, y), dmul(w, z)));
+    E.R[1][1] = dsub(1.0, dmul(2.0, dadd(dmul(x, x), dmul(z, z))));
+    E.R[1][2] = dmul(2.0, dsub(dmul(y, z), dmul(w, x)));
+    E.R[2][0] = dmul(2.0, dsub(dmul(x, z), dmul(w, y)));
+    E.R[2][1] = dmul(2.0, dadd(dmul(y, z), dmul(w, x)));
+    E.R[2][2] = dsub(1.0, dmul(2.0, dadd(dmul(x, x), dmul(y, y))));
+}
+
+// o = diag(k) R^T v: v in the ellipsoid's unit-sphere frame
+__device__ __forceinline__ void ell_local(const Ell& E, const double* v, double* o) {
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+        o[j] = dmul(dadd(dadd(dmul(E.R[0][j], v[0]), dmul(E.R[1][j], v[1])), dmul(E.R[2][j], v[2])), E.k[j]);
+}
+
+// the ray O + t D of pixel (x, y); t is the camera depth
+__device__ __forceinline__ void pixel_ray(const SvParams& q, const Cam& k, int x, int y, double* O, double* D) {
+    double a, b;
+    pixel_ab(q, k, x, y, a, b);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        if (q.parallel) {
+            O[i] = dadd(dadd(k.P[i], dmul(a, k.r[i])), dmul(b, k.u[i]));
+            D[i] = k.f[i];
+        } else {
+            O[i] = k.P[i];
+            D[i] = dadd(dadd(k.f[i], dmul(a, k.r[i])), dmul(b, k.u[i]));
+        }
+    }
+}
+
+// whether the ray hits the ellipsoid at a depth >= near, and the depth of the visible surface
+__device__ __forceinline__ bool ell_hit(const SvParams& q, const Ell& E, const double* O, const double* D, double& z) {
+    const double w[3] = {dsub(O[0], E.c[0]), dsub(O[1], E.c[1]), dsub(O[2], E.c[2])};
+    double e[3], g[3];
+    ell_local(E, w, e);
+    ell_local(E, D, g);
+    const double A = dot3(g, g), B = dot3(g, e), C = dsub(dot3(e, e), 1.0);
+    const double disc = dsub(dmul(B, B), dmul(A, C));
+    if (!(disc >= 0.0)) return false;
+    const double h = -dadd(B, copysign(__dsqrt_rn(disc), B));   // no cancellation
+    const double t1 = ddiv(h, A), t2 = h != 0.0 ? ddiv(C, h) : t1;
+    const double lo = fmin(t1, t2), hi = fmax(t1, t2);
+    if (!(hi >= q.near)) return false;
+    z = lo >= q.near ? lo : hi;
+    return true;
+}
+
+// the image-plane range (b1 -+ d) / a2 of the two tangent planes through the camera along one screen axis
+__device__ __forceinline__ void tangent_range(double cx, double cz, double sxz, double sxx, double a2, double& lo,
+                                              double& hi) {
+    const double b1 = dsub(dmul(cx, cz), sxz), c0 = dsub(dmul(cx, cx), sxx);
+    const double d = __dsqrt_rn(fmax(dsub(dmul(b1, b1), dmul(a2, c0)), 0.0));
+    lo = ddiv(dsub(b1, d), a2);
+    hi = ddiv(dadd(b1, d), a2);
+}
+
 // a primitive in one frame, ready for the pixel test
 struct Geom {
-    bool line;
+    bool line, ell;
+    Ell E;                           // ellipsoid
     int nv;                          // triangle: clipped polygon size (0: nothing left); line: 2 or 0
     long long X[SV_MAX_POLY], Y[SV_MAX_POLY];
     double V[3][3];                  // triangle: camera-space vertices (unclipped), for the plane
@@ -133,8 +211,58 @@ __device__ __forceinline__ long long floor256(long long v) { return v >> 8; }   
 __device__ void build_geom(const SvParams& q, const Cam& k, const double* __restrict__ pos, const int* __restrict__ meta,
                            const float* __restrict__ attr, int id, Geom& g) {
     const double* X = pos + (size_t)id * 9;
-    g.line = __ldg(meta + 2 * (size_t)id) == R2X_SV_LINE;
+    const int kind = __ldg(meta + 2 * (size_t)id);
+    g.line = kind == R2X_SV_LINE;
+    g.ell = kind == R2X_SV_ELLIPSOID;
     g.x0 = 0; g.y0 = 0; g.x1 = -1; g.y1 = -1;
+    if (g.ell) {
+        g.nv = 0;
+        load_ell(pos, attr, id, g.E);
+        double cc[3], M[3][3];
+        to_cam(k, X, cc);
+        const double* rows[3] = {k.r, k.u, k.f};
+#pragma unroll
+        for (int i = 0; i < 3; ++i)
+#pragma unroll
+            for (int j = 0; j < 3; ++j)
+                M[i][j] = dmul(dadd(dadd(dmul(rows[i][0], g.E.R[0][j]), dmul(rows[i][1], g.E.R[1][j])),
+                                    dmul(rows[i][2], g.E.R[2][j])), g.E.s[j]);
+        double S[3][3];   // Sigma in camera coordinates
+#pragma unroll
+        for (int a = 0; a < 3; ++a)
+#pragma unroll
+            for (int b = 0; b < 3; ++b)
+                S[a][b] = dadd(dadd(dmul(M[a][0], M[b][0]), dmul(M[a][1], M[b][1])), dmul(M[a][2], M[b][2]));
+        const double sz = __dsqrt_rn(S[2][2]);
+        if (dadd(cc[2], sz) < q.near) return;
+        g.nv = 1;
+        double lx, hx, ly, hy;
+        if (q.parallel) {
+            const double sx = __dsqrt_rn(S[0][0]), sy = __dsqrt_rn(S[1][1]);
+            lx = dadd(0.5 * q.W, ddiv(dsub(cc[0], sx), k.p));
+            hx = dadd(0.5 * q.W, ddiv(dadd(cc[0], sx), k.p));
+            ly = dsub(0.5 * q.H, ddiv(dadd(cc[1], sy), k.p));
+            hy = dsub(0.5 * q.H, ddiv(dsub(cc[1], sy), k.p));
+        } else {
+            const double a2 = dsub(dmul(cc[2], cc[2]), S[2][2]);
+            if (!(dsub(cc[2], sz) >= q.near) || !(a2 > 0.0)) {   // the camera is inside or near it: every pixel
+                g.x0 = 0; g.y0 = 0; g.x1 = q.W - 1; g.y1 = q.H - 1;
+                return;
+            }
+            double lo, hi;
+            tangent_range(cc[0], cc[2], S[0][2], S[0][0], a2, lo, hi);
+            lx = dadd(0.5 * q.W, ddiv(lo, k.p));
+            hx = dadd(0.5 * q.W, ddiv(hi, k.p));
+            tangent_range(cc[1], cc[2], S[1][2], S[1][1], a2, lo, hi);
+            ly = dsub(0.5 * q.H, ddiv(hi, k.p));
+            hy = dsub(0.5 * q.H, ddiv(lo, k.p));
+        }
+        g.x0 = (int)fmin(fmax(dsub(floor(lx), 1.0), 0.0), (double)q.W);
+        g.x1 = (int)fmax(fmin(dadd(floor(hx), 1.0), (double)(q.W - 1)), -1.0);
+        g.y0 = (int)fmin(fmax(dsub(floor(ly), 1.0), 0.0), (double)q.H);
+        g.y1 = (int)fmax(fmin(dadd(floor(hy), 1.0), (double)(q.H - 1)), -1.0);
+        return;
+    }
     if (g.line) {
         double a[3], b[3];
         to_cam(k, X, a);
@@ -248,6 +376,11 @@ __device__ __forceinline__ double tri_depth(const SvParams& q, const Geom& g, do
 // whether (x, y) is covered, and its depth
 __device__ __forceinline__ bool cover(const SvParams& q, const Cam& k, const Geom& g, int x, int y, double& z) {
     double a, b;
+    if (g.ell) {
+        double O[3], D[3];
+        pixel_ray(q, k, x, y, O, D);
+        return ell_hit(q, g.E, O, D, z);
+    }
     if (g.line) {
         const double cx = (double)x + 0.5, cy = (double)y + 0.5;
         const double dx = dsub(g.bx, g.ax), dy = dsub(g.by, g.ay), ex = dsub(cx, g.ax), ey = dsub(cy, g.ay);
@@ -376,6 +509,14 @@ __global__ void __launch_bounds__(SV_THREADS) sv_tile_kernel(SvParams q, const d
     }
 }
 
+// the two-sided headlight shade A + (1 - A) min(|N.D| / sqrt(N.N D.D), 1) of normal N along the ray D (A if N = 0)
+__device__ __forceinline__ double headlight(const double* N, const double* D) {
+    const double nn = dot3(N, N), dd = dot3(D, D);
+    double lam = 0.0;
+    if (nn > 0.0) lam = fmin(fabs(ddiv(dot3(N, D), __dsqrt_rn(dmul(nn, dd)))), 1.0);
+    return dadd(R2X_SV_AMBIENT, dmul(1.0 - R2X_SV_AMBIENT, lam));
+}
+
 __device__ __forceinline__ float fblend(float a, float b, float w) {
     return __fadd_rn(__fmul_rn(__fsub_rn(1.0f, w), a), __fmul_rn(w, b));
 }
@@ -399,6 +540,22 @@ __global__ void __launch_bounds__(SV_THREADS) sv_resolve_kernel(SvParams q, cons
         const float* at = attr + (size_t)id * R2X_SV_ATTR;
         if (kind == R2X_SV_LINE || kind == R2X_SV_FLAT) {
             out[0] = __ldg(at); out[1] = __ldg(at + 1); out[2] = __ldg(at + 2);
+        } else if (kind == R2X_SV_ELLIPSOID) {
+            const Cam k = load_cam(cameras, frame);
+            Ell E;
+            load_ell(pos, attr, id, E);
+            double O[3], D[3], z, shade = R2X_SV_AMBIENT;
+            pixel_ray(q, k, x, y, O, D);
+            if (ell_hit(q, E, O, D, z)) {   // always, for the id that won the pixel
+                double v[3], m[3], n[3];
+                for (int i = 0; i < 3; ++i) v[i] = dsub(dadd(O[i], dmul(z, D[i])), E.c[i]);
+                ell_local(E, v, m);
+                for (int j = 0; j < 3; ++j) m[j] = dmul(m[j], E.k[j]);
+                for (int i = 0; i < 3; ++i)
+                    n[i] = dadd(dadd(dmul(E.R[i][0], m[0]), dmul(E.R[i][1], m[1])), dmul(E.R[i][2], m[2]));
+                shade = headlight(n, D);
+            }
+            for (int i = 0; i < 3; ++i) out[i] = __double2float_rn(dmul((double)__ldg(at + i), shade));
         } else {
             const Cam k = load_cam(cameras, frame);
             const double* X = pos + (size_t)id * 9;
@@ -441,10 +598,7 @@ __global__ void __launch_bounds__(SV_THREADS) sv_resolve_kernel(SvParams q, cons
                 double D[3];   // the headlight: along the pixel's ray, in world coordinates
                 for (int i = 0; i < 3; ++i)
                     D[i] = q.parallel ? k.f[i] : dadd(dadd(k.f[i], dmul(a, k.r[i])), dmul(b, k.u[i]));
-                const double nn = dot3(N, N), dd = dot3(D, D);
-                double lam = 0.0;
-                if (nn > 0.0) lam = fmin(fabs(ddiv(dot3(N, D), __dsqrt_rn(dmul(nn, dd)))), 1.0);
-                const double shade = dadd(R2X_SV_AMBIENT, dmul(1.0 - R2X_SV_AMBIENT, lam));
+                const double shade = headlight(N, D);
                 for (int i = 0; i < 3; ++i) out[i] = __double2float_rn(dmul((double)__ldg(at + i), shade));
             } else {   // textured
                 const double tu = dadd(dadd(dmul(w[0], (double)__ldg(at + 3)), dmul(w[1], (double)__ldg(at + 5))),

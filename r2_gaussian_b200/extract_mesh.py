@@ -98,14 +98,12 @@ def load_volume(a):
     return _model_volume(a)
 
 
-def _model_volume(a):
-    import torch
-
+def load_model(a):
+    """(source label, GaussianModel of the saved iteration, scanner_cfg of the model's scene, recorded settings) of
+    -m: the scene is the one the model was trained on unless -s names another."""
     from .dataset import read_scene
     from .gaussian_model import GaussianModel
-    from .render_query import query
     from .test import load_settings, resolve_iteration
-    from .trainer import PipelineParams
 
     try:
         settings = load_settings(a.model_path)
@@ -118,14 +116,24 @@ def _model_volume(a):
     if not os.path.exists(source):
         raise SystemExit(f"the model's scene {source} does not exist; pass -s")
     cfg = dict(read_scene(source, eval=False).scanner_cfg)
+    gaussians = GaussianModel(None)
+    gaussians.load_ply(pickle_path)
+    return f"model@{iteration}", gaussians, cfg, settings
+
+
+def _model_volume(a):
+    import torch
+
+    from .render_query import query
+    from .trainer import PipelineParams
+
+    source, gaussians, cfg, settings = load_model(a)
     if a.resolution is not None:
         cfg["nVoxel"] = [int(a.resolution)] * 3
     pipe = PipelineParams(**{k: settings[k] for k in PipelineParams.__dataclass_fields__ if k in settings})
-    gaussians = GaussianModel(None)
-    gaussians.load_ply(pickle_path)
     with torch.no_grad():
         vol = query(gaussians, cfg["offOrigin"], cfg["nVoxel"], cfg["sVoxel"], pipe)["vol"]
-    return f"model@{iteration}", vol, cfg
+    return source, vol, cfg
 
 
 def main(argv=None) -> dict:

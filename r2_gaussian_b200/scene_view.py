@@ -1,5 +1,6 @@
-"""Scene view on the GPU: a depth-tested rasterizer for triangles and line segments over the C ABI (r2x_scene_raster,
-csrc/r2x_scene.cu), and the glyphs of the reference's `scripts/visualize_scene.py`.
+"""Scene view on the GPU: a depth-tested rasterizer for triangles, line segments and ellipsoids over the C ABI
+(r2x_scene_raster, csrc/r2x_scene.cu), the glyphs of the reference's `scripts/visualize_scene.py`, and a trained
+model's Gaussians as ellipsoids (the reference's `show_gaussians`).
 
     prims = concat(mesh_triangles(verts, faces, vol, cfg), box(cfg["offOrigin"], cfg["sVoxel"], RED),
                    camera_glyph(cam, 1.0, colour, image=cam.original_image[0]))
@@ -11,8 +12,9 @@ near plane and a 2^20-pixel guard band; vertices snapped to 1/256 pixel and int6
 rule, so coverage is exact; lines cover the pixels whose centre lies within w/2 pixels of the projected segment;
 perspective-correct float64 depth rounded to float32 in a 64-bit atomicMin with the primitive id, so the nearest
 primitive wins, ties go to the lower id and two calls give the same bits.  Mesh triangles get a two-sided headlight
-Lambert shade from gradient vertex normals, image planes a nearest-texel lookup through a LUT.  There is no CPU
-fallback.
+Lambert shade from gradient vertex normals, image planes a nearest-texel lookup through a LUT.  Ellipsoids are
+analytic: each pixel's ray meets the quadric in float64 (exact silhouette and depth, one record per ellipsoid), shaded
+with the same headlight from the analytic normal.  There is no CPU fallback.
 """
 from __future__ import annotations
 
@@ -23,7 +25,7 @@ import numpy as np
 
 from .volume_render import Camera, look_at, lut_from
 
-FLAT, MESH, TEXTURED, LINE = 0, 1, 2, 3     # R2X_SV_FLAT, _MESH, _TEXTURED, _LINE
+FLAT, MESH, TEXTURED, LINE, ELLIPSOID = 0, 1, 2, 3, 4   # R2X_SV_FLAT, _MESH, _TEXTURED, _LINE, _ELLIPSOID
 ATTR = 12                                    # R2X_SV_ATTR
 MAX_SIDE = 16384                             # R2X_SV_MAX_SIDE
 NEAR = 1e-3
@@ -217,6 +219,66 @@ def mesh_triangles(verts, faces, vol, scanner_cfg: dict | None = None, colour=ME
     return Primitives(pos[f].contiguous(), meta, attr, None)
 
 
+def ellipsoids(centres, axes, quaternions, colours, device=None) -> Primitives:
+    """Solid ellipsoids { c + R diag(s) v : |v| <= 1 }: centres and semi-axes [n, 3], quaternions [n, 4] in the
+    model's (w, x, y, z) order (R is `gaussian_utils.build_rotation`'s; the kernel normalises them), colours [n, 3]
+    or one colour.  Built on the device from tensors or arrays, with no per-ellipsoid host work."""
+    import torch
+    dev = _device(device)
+    c = torch.as_tensor(centres, device=dev).detach().to(torch.float64).reshape(-1, 3)
+    n = c.shape[0]
+    s = torch.as_tensor(axes, device=dev).detach().to(torch.float64).reshape(n, 3)
+    q = torch.as_tensor(quaternions, device=dev).detach().to(torch.float32).reshape(n, 4)
+    col = torch.as_tensor(colours, device=dev).detach().to(torch.float32)
+    pos = torch.zeros((n, 3, 3), dtype=torch.float64, device=dev)
+    pos[:, 0], pos[:, 1] = c, s
+    meta = torch.zeros((n, 2), dtype=torch.int32, device=dev)
+    meta[:, 0] = ELLIPSOID
+    attr = torch.zeros((n, ATTR), dtype=torch.float32, device=dev)
+    attr[:, 0:3] = col.reshape(-1, 3).expand(n, 3)
+    attr[:, 3:7] = q
+    return Primitives(pos, meta, attr, None)
+
+
+SORT_GAUSSIANS = ("no", "density", "scale")
+
+
+def gaussian_ellipsoids(gaussians, n_gaussian: int | None = None, sort_gaussians: str = "no"):
+    """(Primitives, indices): the 1-sigma ellipsoids of a model's Gaussians by the rules of the reference's
+    `show_gaussians`, on the model's device.  Keeps the Gaussians whose density (`get_density[:, 0]`) is not 0; sorts
+    them by density ("density") or by the mean activated scale ((s0 + s1) + s2) / 3 in float32 ("scale"), largest
+    first, or keeps the model's order ("no"); draws the first `n_gaussian` (all if None or more than there are).  The
+    sort is stable, so ties keep the model's order; the reference's `argsort()[::-1]` may order exact ties differently.
+    Each is gray at t = density * (0.95 / max density) in float32 (the maximum over every kept Gaussian, as the
+    reference's vertex colour) and oriented by `get_rotation` in the model's (w, x, y, z) order -- the orientation the
+    rasterizer and voxelizer use.  `indices` (int64, on the device) are the drawn Gaussians' rows in the model."""
+    import torch
+    if sort_gaussians not in SORT_GAUSSIANS:
+        raise ValueError(f"sort_gaussians must be one of {SORT_GAUSSIANS}, got {sort_gaussians!r}")
+    if n_gaussian is not None and int(n_gaussian) < 1:
+        raise ValueError(f"n_gaussian must be >= 1 or None, got {n_gaussian}")
+    with torch.no_grad():
+        dens = gaussians.get_density[:, 0].detach()
+        idx = torch.nonzero(dens != 0).squeeze(1)
+        if idx.numel() == 0:
+            raise ValueError("gaussian_ellipsoids: every Gaussian has density 0; nothing to draw")
+        kept = dens[idx]
+        scale = torch.tensor(0.95, dtype=torch.float32, device=dens.device) / kept.max().to(torch.float32)
+        if sort_gaussians != "no":
+            if sort_gaussians == "density":
+                key = kept
+            else:
+                s = gaussians.get_scaling.detach()[idx].to(torch.float32)
+                key = ((s[:, 0] + s[:, 1]) + s[:, 2]) / 3.0
+            idx = idx[torch.sort(key, descending=True, stable=True).indices]
+        if n_gaussian is not None:
+            idx = idx[:int(n_gaussian)]
+        grey = (dens[idx].to(torch.float32) * scale)[:, None].expand(-1, 3)
+        prims = ellipsoids(gaussians.get_xyz.detach()[idx], gaussians.get_scaling.detach()[idx],
+                           gaussians.get_rotation.detach()[idx], grey, device=dens.device)
+    return prims, idx
+
+
 def concat(*parts) -> Primitives:
     """One primitive list, in the order given (ties in depth go to the earlier part); textures are stacked and their
     indices renumbered.  Textures of one list share a size."""
@@ -239,10 +301,21 @@ def concat(*parts) -> Primitives:
 
 
 def points(prims: Primitives) -> np.ndarray:
-    """Every point a primitive uses (two per segment, three per triangle), float64 [M, 3]."""
-    pos = prims.pos.detach().cpu().numpy()
-    line = prims.meta[:, 0].cpu().numpy() == LINE
-    return np.concatenate([pos[line, :2].reshape(-1, 3), pos[~line].reshape(-1, 3)])
+    """Every point a primitive uses (two per segment, three per triangle), float64 [M, 3]; an ellipsoid gives the two
+    opposite corners of its axis-aligned bounding box (half sides sqrt(sum_j (R_ij s_j)^2))."""
+    import torch
+
+    from .gaussian_utils import build_rotation
+    kind = prims.meta[:, 0]
+    ell = kind == ELLIPSOID
+    pos = prims.pos.detach()
+    parts = [pos[kind == LINE, :2].reshape(-1, 3), pos[(kind != LINE) & ~ell].reshape(-1, 3)]
+    if bool(ell.any()):
+        e = pos[ell]
+        R = build_rotation(prims.attr[ell, 3:7].detach().to(torch.float64))
+        half = torch.sqrt(((R * e[:, 1, None, :]) ** 2).sum(2))
+        parts += [e[:, 0] - half, e[:, 0] + half]
+    return torch.cat(parts).cpu().numpy()
 
 
 def default_view(prims: Primitives, width: int, height: int, view_angle: float = 30.0) -> Camera:
@@ -286,10 +359,16 @@ def _check(prims: Primitives):
     if prims.attr.dtype != torch.float32 or tuple(prims.attr.shape) != (n, ATTR):
         raise ValueError(f"render: attr must be float32 [n, {ATTR}]")
     kind = prims.meta[:, 0]
-    if not bool(((kind >= FLAT) & (kind <= LINE)).all()):
-        raise ValueError("render: a primitive kind is not 0 (flat), 1 (mesh), 2 (textured) or 3 (line)")
+    if not bool(((kind >= FLAT) & (kind <= ELLIPSOID)).all()):
+        raise ValueError("render: a primitive kind is not 0 (flat), 1 (mesh), 2 (textured), 3 (line) or 4 (ellipsoid)")
     if not bool(torch.isfinite(prims.pos).all()) or not bool(torch.isfinite(prims.attr).all()):
         raise ValueError("render: positions and attributes must be finite")
+    ell = kind == ELLIPSOID
+    if bool(ell.any()):
+        if not bool((prims.pos[ell, 1] > 0).all()):
+            raise ValueError("render: every ellipsoid semi-axis must be finite and > 0")
+        if not bool((prims.attr[ell, 3:7] != 0).any(1).all()):
+            raise ValueError("render: an ellipsoid's quaternion is all zero")
     w = prims.attr[:, 3][kind == LINE]
     if w.numel() and not bool((w > 0).all()):
         raise ValueError("render: every line width must be > 0")

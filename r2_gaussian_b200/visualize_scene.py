@@ -10,12 +10,18 @@ SOURCE is one of (as in `extract_mesh`)
                                          the trained model's query() mesh, its cameras with the learned pose and detector
                                          corrections, and (thinner) the nominal cameras
 
+    -m <model> --gaussians [--n_gaussian N] [--sort_gaussians {no,density,scale}]
+                                         the trained model's Gaussians as shaded 1-sigma ellipsoids (the reference's
+                                         show_gaussians) instead of a mesh: those of non-zero density, optionally sorted
+                                         by density or mean scale (largest first), the first N of them, gray by density
+
 Drawn: the marching-cubes mesh at --mc_thresh (0.5), the volume's box (red), the unit box [-1, 1]^3 (blue), a frame at
 offOrigin, and per drawn train view its frustum in a colour from --cmap, its projection on the image plane (at depth
 --cam_scale, or with --true_detector at the detector: DSD from the source, sDetector in size, the offset honoured) and a
 small frame.  Without --camera the view is `scene_view.default_view`; --orbit N turns it about the scan axis (+z) and
 writes <stem>_0000.png ...; --save_npy also writes the float frames [N, H, W, 3] to <stem>.npy.  Prints one JSON line:
-source, triangles, lines, cameras, frames, width, height, seconds, outputs.  GPU only.
+source, triangles, lines, cameras, frames, width, height, seconds, outputs (and with --gaussians: gaussians, the number
+drawn).  GPU only.
 """
 from __future__ import annotations
 
@@ -28,7 +34,8 @@ import time
 
 import numpy as np
 
-from .extract_mesh import add_source_arguments, check_source_arguments, load_volume
+from .extract_mesh import add_source_arguments, check_source_arguments, load_model, load_volume
+from .scene_view import SORT_GAUSSIANS
 
 CAMERA_LUT = np.array([[0.0, 0.0, 1.0], [1.0, 0.0, 0.0]])   # blue -> red: the default camera colours
 
@@ -57,6 +64,12 @@ def parse_args(argv=None):
     ap.add_argument("--supersample", type=int, default=1, help="k x k box-filter supersampling (default 1: off)")
     ap.add_argument("--background", type=float, nargs=3, default=[1.0, 1.0, 1.0], metavar=("R", "G", "B"))
     ap.add_argument("--save_npy", action="store_true", help="also write the float RGB frames to <stem>.npy")
+    ap.add_argument("--gaussians", action="store_true",
+                    help="with -m: draw the model's Gaussians as ellipsoids instead of the density's mesh")
+    ap.add_argument("--n_gaussian", type=int, default=None, help="with --gaussians: draw at most N (default: all)")
+    ap.add_argument("--sort_gaussians", default=None, choices=SORT_GAUSSIANS,
+                    help="with --gaussians: which N to draw -- the first in the model ('no', the default), the densest "
+                         "or the largest")
     a = ap.parse_args(argv)
     from .mesh import finite_level
     from .scene_view import MAX_SIDE
@@ -92,6 +105,17 @@ def parse_args(argv=None):
             ap.error(f"--camera: {e}")
     if (a.true_detector or a.use_offDetector) and a.source_path is None and a.model_path is None:
         ap.error("--true_detector and --use_offDetector need cameras: give -s <scene> or -m <model>")
+    if a.gaussians:
+        if a.model_path is None:
+            ap.error("--gaussians draws a trained model's Gaussians: give -m <model>")
+        if a.resolution is not None or a.vol is not None:
+            ap.error("--gaussians draws no volume: --resolution and --vol do not apply")
+        if a.n_gaussian is not None and a.n_gaussian < 1:
+            ap.error(f"--n_gaussian must be >= 1, got {a.n_gaussian}")
+    elif a.n_gaussian is not None or a.sort_gaussians is not None:
+        ap.error("--n_gaussian and --sort_gaussians apply to --gaussians")
+    if a.sort_gaussians is None:
+        a.sort_gaussians = "no"
     return a
 
 
@@ -136,13 +160,19 @@ def _cameras(a):
     return list(zip(nominal, corrected))[::a.views], scene
 
 
-def build(a, vol, cfg):
-    """(primitives, report counts) of everything the CLI draws."""
+def build(a, vol, cfg, gaussians=None):
+    """(primitives, triangles, cameras, Gaussians drawn or None) of everything the CLI draws: the mesh of `vol`, or
+    with `gaussians` (a GaussianModel) their ellipsoids."""
     from .mesh import marching_cubes
-    from .scene_view import (BLUE, LINE_WIDTH, RED, axes, box, camera_glyph, concat, mesh_triangles)
+    from .scene_view import (BLUE, LINE_WIDTH, RED, axes, box, camera_glyph, concat, gaussian_ellipsoids,
+                             mesh_triangles)
 
-    verts, faces = marching_cubes(vol, a.mc_thresh)
-    parts = [mesh_triangles(verts, faces, vol, cfg)]
+    if gaussians is None:
+        verts, faces = marching_cubes(vol, a.mc_thresh)
+        parts, n_tris, n_gauss = [mesh_triangles(verts, faces, vol, cfg)], int(faces.shape[0]), None
+    else:
+        ell, _ = gaussian_ellipsoids(gaussians, a.n_gaussian, a.sort_gaussians)
+        parts, n_tris, n_gauss = [ell], 0, len(ell)
     if cfg is not None:
         parts += [box(cfg["offOrigin"], cfg["sVoxel"], RED), box((0, 0, 0), (2, 2, 2), BLUE),
                   axes(cfg["offOrigin"], float(cfg["sVoxel"][0]) / 2)]
@@ -158,7 +188,7 @@ def build(a, vol, cfg):
         parts.append(camera_glyph(cam, a.cam_scale, col, image=img, plane_depth=depth))
         if a.model_path is not None:
             parts.append(camera_glyph(nom, a.cam_scale, col, plane_depth=depth, width=LINE_WIDTH / 2))
-    return concat(*parts), int(faces.shape[0]), len(pairs)
+    return concat(*parts), n_tris, len(pairs), n_gauss
 
 
 def run(argv=None):
@@ -172,9 +202,13 @@ def run(argv=None):
     from .scene_view import LINE, default_view, render, scan_orbit
     from .volume_render import look_at, to_uint8, write_png
 
-    source, vol, cfg = load_volume(a)
+    if a.gaussians:
+        source, gaussians, cfg, _ = load_model(a)
+        vol = None
+    else:
+        (source, vol, cfg), gaussians = load_volume(a), None
     try:
-        prims, n_tris, n_cams = build(a, vol, cfg)
+        prims, n_tris, n_cams, n_gauss = build(a, vol, cfg, gaussians)
     except ValueError as e:
         raise SystemExit(str(e)) from e
     if a.camera is not None:
@@ -198,6 +232,8 @@ def run(argv=None):
     report = {"source": source, "triangles": n_tris, "lines": int((prims.meta[:, 0] == LINE).sum()),
               "cameras": n_cams, "frames": len(cams), "width": a.width, "height": a.height, "seconds": seconds,
               "outputs": outputs}
+    if n_gauss is not None:
+        report["gaussians"] = n_gauss
     print(json.dumps(report))
     return report, frames, prims, cams
 
