@@ -492,7 +492,7 @@ __global__ void __launch_bounds__(SV_THREADS) sv_tile_kernel(SvParams q, const d
     for (long long t = blockIdx.x; t < total; t += gridDim.x) {
         int lo = 0, hi = nrec - 1;   // the last record whose base <= t
         while (lo < hi) {
-            const int mid = (lo + hi + 1) >> 1;
+            const int mid = lo + ((hi - lo + 1) >> 1);   // lo + hi + 1 passes INT_MAX past 2^30 records
             if (rec[mid].base <= t) lo = mid;
             else hi = mid - 1;
         }
