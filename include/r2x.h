@@ -340,6 +340,33 @@ size_t r2x_detector_offset_grad_scratch_bytes(int P, int n_views);
 int r2x_detector_offset_grad(void* stream, int P, int n_views, int W, const float* dL_dmean2D, float* dL_doffset,
                              void* scratch, size_t scratch_bytes);
 
+/* ---- horizontal detector offset from the projections (detector.estimate_offset) ------------------------------------
+ * The model.  A circular scan measures most rays twice.  Image column c of a view sees the detector coordinate
+ * u = du (c - (W - 1) / 2 - sigma): sigma is the column shift of the rotation axis from the detector centre (the
+ * caller's candidate, the DetectorOffset s minus the scanner file's t_u).  Column pitch du = sDetector_u / nDetector_u.
+ *   parallel beam (mode 0): P(beta, u) = P(beta + pi, -u) in every row, so for a pair (i, j) with beta_j - beta_i = pi
+ *     the sample m (0 <= m < W) of row r compares view i at column m + sigma with view j at column W - 1 - m + sigma,
+ *     rows row_lo .. row_lo + n_rows - 1 (both columns carry the same fraction, so both see the same interpolation);
+ *   cone beam (mode 1): in the mid-plane, P(beta, gamma) = P(beta + pi - 2 gamma, -gamma) with gamma = atan(u / DSD)
+ *     and gamma > 0 towards larger column index, so a pair (i, j) with d = beta_j - beta_i in [0, 2 pi) shares the one
+ *     ray at t = DSD tan((pi - d) / 2) / du pixels from the axis: view i at column (W - 1) / 2 + t + sigma against view
+ *     j at column (W - 1) / 2 - t + sigma, both in image row (H - 1) / 2 + t_v (n_rows must be 1).
+ * Every value is linear in the column and (cone beam) the row, formed in float64 from the float32 projections; a
+ * sample counts when both of its columns lie in [0, W - 1] (and its row in [0, H - 1]).  For each of the K candidate
+ * shifts sigma[k] (host-free: device float64) the entry point writes
+ *   num[k] = sum (a - b)^2,   den[k] = sum (a^2 + b^2),   count[k] = the number of valid samples
+ * over the pair table pair_views int32 [n_pairs, 2] (view i, view j; 0 <= i, j < N, the caller's promise) and
+ * pair_dbeta float64 [n_pairs] (beta_j - beta_i; read in cone beam only).  projs is float32 [N, H, W].
+ * Two launches: per candidate, a fixed grid of contiguous sample chunks summed in a fixed tree into `scratch`
+ * (>= r2x_detector_offset_cost_scratch_bytes bytes), then the chunks of each candidate added in order: no atomics,
+ * two calls give the same bits.  Limits: 1 <= K <= 65535, n_pairs x n_rows x (W or 1) samples < 2^62; anything else
+ * is refused before any CUDA work.  Asynchronous. */
+size_t r2x_detector_offset_cost_scratch_bytes(int mode, int W, int n_pairs, int n_rows, int K);
+int r2x_detector_offset_cost(void* stream, int mode, int N, int H, int W, const float* projs, int n_pairs,
+                             const int* pair_views, const double* pair_dbeta, double DSD, double du, double t_v,
+                             int row_lo, int n_rows, int K, const double* sigma, double* num, double* den,
+                             long long* count, void* scratch, size_t scratch_bytes);
+
 int r2x_voxel_forward_async_raw(void* stream, int P, int nx, int ny, int nz, float sx, float sy, float sz, float cx,
                                 float cy, float cz, const float* means3D, const float* raw_density,
                                 const float* raw_scales, float scale_modifier, const float* raw_rotations,

@@ -80,6 +80,9 @@ PROTOTYPES = {
     "r2x_detector_offset_apply": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
     "r2x_detector_offset_grad_scratch_bytes": (_sz, [_i, _i]),
     "r2x_detector_offset_grad": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _sz]),
+    "r2x_detector_offset_cost_scratch_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "r2x_detector_offset_cost": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp, _vp, C.c_double, C.c_double, C.c_double, _i,
+                                      _i, _i, _vp, _vp, _vp, _vp, _vp, _sz]),
     "r2x_voxel_forward_async_raw": (_i, [_vp, _i, _i, _i, _i, _f, _f, _f, _f, _f, _f, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp,
                                          _vp, _vp, _vp, _ll, _vp, _vp]),
     "r2x_voxel_backward_raw": (_i, [_vp, _i, _ll, _i, _i, _i, _f, _f, _f, _f, _f, _f, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp,

@@ -177,9 +177,16 @@ class Camera:
 
 class Scene:
     def __init__(self, source_path: str, model_path: str = "", eval: bool = True, shuffle: bool = True, device="cuda",
-                 data_device=None, use_offDetector: bool = False):
+                 data_device=None, use_offDetector: bool = False, offDetector_u: float | None = None):
+        """`offDetector_u` (scene units) replaces the scanner's offDetector[0] in a copy of its config, the one every
+        camera and `scanner_cfg` then carry (with `use_offDetector`, e.g. an estimated offset)."""
         self.model_path = model_path
         info = read_scene(source_path, eval)
+        if offDetector_u is not None:
+            from .detector import with_offDetector_u
+            info.scanner_cfg = with_offDetector_u(info.scanner_cfg, offDetector_u)
+            for c in info.train_cameras + info.test_cameras:
+                c.scanner_cfg = info.scanner_cfg
         if shuffle:
             random.shuffle(info.train_cameras)
             random.shuffle(info.test_cameras)

@@ -2,8 +2,8 @@
 
     python -m r2_gaussian_b200.initialize_pcd --data <scene dir | NAF pickle> [--output init.npy]
         [--recon_method random|fdk|cgls|fista_tv|volume] [--recon recon.npy] [--n_points 50000] [--density_thresh 0.05]
-        [--density_rescale 0.15] [--random_density_max 1.0] [--evaluate] [--short_scan] [--use_offDetector [--half_fan]]
-        [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
+        [--density_rescale 0.15] [--random_density_max 1.0] [--evaluate] [--short_scan] [--use_offDetector]
+        [--estimate_offDetector] [--half_fan] [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
 
 `random` draws positions uniformly in the volume and densities in [0, random_density_max) with numpy's global
 generator seeded with 0, exactly like the reference.  `fdk` reconstructs the volume from the train views with the
@@ -16,7 +16,10 @@ the flag is refused with any other method.  `--use_offDetector` reconstructs thr
 adds half-fan redundancy weights to that FDK for a full circle whose detector is shifted sideways (`fdk.fdk(...,
 half_fan=True)`; fdk only, not with --short_scan).  `--fdk_filter NAME` gives that FDK one of TIGRE's windowed ramp
 filters (`fdk.fdk(filter=NAME)`): the reference's FDK takes its window from the scanner's `filter`, this one only on
-request, and without the flag a scanner whose `filter` names a window is refused (fdk only).  `cgls` does the same with 60 CGLS iterations over the GPU projector pair
+request, and without the flag a scanner whose `filter` names a window is refused (fdk only).
+`--estimate_offDetector` (fdk, cgls and fista_tv) first measures the horizontal detector offset from the train views
+(`detector.estimate_offset`, on top of the file's offset under `--use_offDetector`) and reconstructs with a copy of the
+scanner whose offDetector[0] is that total, as `--use_offDetector` would; `--half_fan` then needs no `--use_offDetector`.  `cgls` does the same with 60 CGLS iterations over the GPU projector pair
 (`r2_gaussian_b200.recon`, the reference's `algs.cgls`); it also needs a CUDA device.  `fista_tv` does the same with
 the TV-regularised FISTA-TV of `r2_gaussian_b200.recon` at its default settings (CUDA as well).  `volume` samples a reconstruction made elsewhere (`--recon`, an .npy in the scene's
 voxel grid) the same way.  Writes [n_points, 4] = (x, y, z, density) in the scene's normalised [-1,1]^3 coordinates to
@@ -33,7 +36,7 @@ import os
 import numpy as np
 
 from .dataset import init_point_cloud, read_scene
-from .recon import add_fdk_filter_flag, check_fdk_flags
+from .recon import add_estimate_flag, add_fdk_filter_flag, check_fdk_flags
 from .trainer import default_init_path
 
 # A filtered backprojection from a handful of views is dominated by streaks, and thresholding it gives no useful
@@ -109,12 +112,16 @@ def main(argv=None) -> str:
                     help="with --recon_method fdk and --use_offDetector: half-fan redundancy weights for a full circle "
                          "with the detector shifted sideways")
     add_fdk_filter_flag(ap, "with --recon_method fdk: the ramp filter")
+    add_estimate_flag(ap, "with --recon_method fdk, cgls or fista_tv: reconstruct")
     a = ap.parse_args(argv)
     check_fdk_flags(a, a.recon_method == "fdk", f"{{flag}} applies to --recon_method fdk only, not {a.recon_method}: "
                     "the iterative methods need no redundancy weights")
     if a.use_offDetector and a.recon_method not in ("fdk", "cgls", "fista_tv"):
         raise SystemExit(f"--use_offDetector applies to --recon_method fdk, cgls or fista_tv, not {a.recon_method}: "
                          "no projections are reconstructed")
+    if a.estimate_offDetector and a.recon_method not in ("fdk", "cgls", "fista_tv"):
+        raise SystemExit(f"--estimate_offDetector applies to --recon_method fdk, cgls or fista_tv, not "
+                         f"{a.recon_method}: no projections are reconstructed")
     if a.recon_method in ("fdk", "cgls", "fista_tv"):
         _require_cuda_for(a.recon_method)
     np.random.seed(0)                                    # initialize_pcd.py:23
@@ -133,7 +140,12 @@ def main(argv=None) -> str:
     os.makedirs(os.path.dirname(out) or ".", exist_ok=True)
     if a.recon_method in ("fdk", "cgls", "fista_tv"):
         # no draws from numpy's generator before np.random.choice
-        recon = recon_train_views(info, a.recon_method, a.short_scan, a.use_offDetector, a.half_fan, a.fdk_filter)
+        use_off = a.use_offDetector
+        if a.estimate_offDetector:
+            from .estimate_offset import estimated_scanner
+            info.scanner_cfg, _ = estimated_scanner(info, a.use_offDetector)
+            use_off = True
+        recon = recon_train_views(info, a.recon_method, a.short_scan, use_off, a.half_fan, a.fdk_filter)
     pts = init_point_cloud(info.scanner_cfg, a.n_points, recon=recon, density_thresh=a.density_thresh,
                            density_rescale=a.density_rescale, random_density_max=a.random_density_max)
     np.save(out, pts)

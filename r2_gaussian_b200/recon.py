@@ -72,7 +72,7 @@ their adaptive step and stop rules are defined by TIGRE's implementation.  `cp_t
 `fista_tv` the TV-regularised least-squares one.
 
     python -m r2_gaussian_b200.recon -s <scene> -m <output> [--methods fdk,sart,cgls] [--short_scan]
-        [--use_offDetector [--half_fan]] [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
+        [--use_offDetector] [--estimate_offDetector] [--half_fan] [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
 
 mirrors `scripts/run_traditional_methods.py`: it reconstructs the scene's train views with each method, scores the
 volume against `vol_gt` with `metrics.metric_vol` and writes, per method, `<output>/<method>/ct_gt.npy`, `ct_pred.npy`,
@@ -86,7 +86,10 @@ views cover less than a full circle; it is refused when --methods has no fdk.  `
 reprojects every method through the scanner's offDetector (without it a non-zero offset is refused by the projector
 pair and ignored by fdk); `--half_fan` (with it, fdk only, not with --short_scan) adds half-fan redundancy weights for
 a full circle whose detector is shifted sideways.  The reports add `half_fan: true` / `use_offDetector: true` only when
-those flags are on.  `--fdk_filter NAME` reconstructs fdk with one of TIGRE's windowed ramp filters
+those flags are on.  `--estimate_offDetector` measures the horizontal detector offset from the train views
+(`detector.estimate_offset`, on top of the file's offset under `--use_offDetector`) and runs every method, and the
+test-view projections, with a copy of the scanner whose offDetector[0] is that total; `--half_fan` then needs no
+`--use_offDetector`, and the reports add `estimated_offset_px` and `offDetector_u` (the file's units).  `--fdk_filter NAME` reconstructs fdk with one of TIGRE's windowed ramp filters
 (`fdk.fdk(filter=NAME)`, overriding the scanner's `filter`); it is refused when --methods has no fdk.  Without it fdk
 refuses a scanner whose `filter` names a window.
 """
@@ -371,8 +374,9 @@ def check_fdk_flags(args, fdk_selected: bool, not_fdk: str):
                      ("--fdk_filter", args.fdk_filter is not None)):
         if on and not fdk_selected:
             raise SystemExit(not_fdk.format(flag=flag))
-    if args.half_fan and not args.use_offDetector:
-        raise SystemExit("--half_fan needs --use_offDetector: the half-fan weights follow the detector offset")
+    if args.half_fan and not (args.use_offDetector or getattr(args, "estimate_offDetector", False)):
+        raise SystemExit("--half_fan needs --use_offDetector (or --estimate_offDetector): the half-fan weights follow "
+                         "the detector offset")
     if args.half_fan and args.short_scan:
         raise SystemExit("--half_fan and --short_scan cannot be combined (half-fan weights need a full circle)")
 
@@ -384,6 +388,13 @@ def add_fdk_filter_flag(ap, help_text: str):
     ap.add_argument("--fdk_filter", default=None, choices=FILTERS, metavar="NAME",
                     help=f"{help_text}: {', '.join(FILTERS)} (TIGRE's names; default: the scanner's filter, which must "
                          "then be null or ram_lak)")
+
+
+def add_estimate_flag(ap, what: str):
+    """--estimate_offDetector on a CLI's parser."""
+    ap.add_argument("--estimate_offDetector", default=False, action="store_true",
+                    help=f"estimate the horizontal detector offset from the train views (detector.estimate_offset; "
+                         f"relative to the scanner's offDetector under --use_offDetector) and {what} through it")
 
 
 def _parse_methods(text: str) -> list[str]:
@@ -413,6 +424,7 @@ def main(argv=None) -> dict:
                     help="with --use_offDetector: reconstruct fdk with half-fan redundancy weights (a full circle with "
                          "the detector shifted sideways)")
     add_fdk_filter_flag(ap, "reconstruct fdk with this ramp filter")
+    add_estimate_flag(ap, "reconstruct and reproject every method")
     a = ap.parse_args(argv)
     methods = _parse_methods(a.methods)
     check_fdk_flags(a, "fdk" in methods, "{flag} applies to the fdk method, which --methods does not include (the "
@@ -432,6 +444,11 @@ def main(argv=None) -> dict:
     train_angles = [c.angle for c in info.train_cameras]
     test_angles = [c.angle for c in info.test_cameras]
     vol_gt = np.asarray(info.vol, np.float32)
+    use_off, estimate = a.use_offDetector, None
+    if a.estimate_offDetector:
+        from .estimate_offset import estimated_scanner
+        cfg, estimate = estimated_scanner(info, a.use_offDetector)
+        use_off = True
     out = {}
     print(f"Run traditional algorithms on {os.path.basename(source)}")
     for method in methods:
@@ -445,12 +462,12 @@ def main(argv=None) -> dict:
         fdk_filter = a.fdk_filter if method == "fdk" else None
         extra = {}
         if method == "cp_tv":
-            eps = cp_tv_epsilon(projs_train, train_angles, cfg, use_offDetector=a.use_offDetector)
-            pred, hist = cp_tv(projs_train, train_angles, cfg, epsilon=eps, use_offDetector=a.use_offDetector)
+            eps = cp_tv_epsilon(projs_train, train_angles, cfg, use_offDetector=use_off)
+            pred, hist = cp_tv(projs_train, train_angles, cfg, epsilon=eps, use_offDetector=use_off)
             extra = {"epsilon": eps, "residual": hist[-1]["residual"]}
         else:
             pred = recon_volume(projs_train, train_angles, cfg, method, short_scan=short_scan,
-                                use_offDetector=a.use_offDetector, half_fan=half_fan, fdk_filter=fdk_filter)
+                                use_offDetector=use_off, half_fan=half_fan, fdk_filter=fdk_filter)
         torch.cuda.synchronize()
         duration = time.time() - t0
         ct_pred = pred.cpu().numpy()
@@ -469,11 +486,14 @@ def main(argv=None) -> dict:
             report["filter"] = fdk_filter
         if a.use_offDetector:
             report["use_offDetector"] = True
+        if estimate is not None:
+            report["estimated_offset_px"] = estimate["offset_px"]
+            report["offDetector_u"] = estimate["offDetector_u"] / info.scene_scale
         report.update(extra)
         with open(os.path.join(save, "eval_3d.yml"), "w") as f:
             yaml.dump(report, f, default_flow_style=False, sort_keys=False)
         if test_angles:
-            render = project(pred, test_angles, cfg, use_offDetector=a.use_offDetector).cpu().numpy()
+            render = project(pred, test_angles, cfg, use_offDetector=use_off).cpu().numpy()
             for i, cam in enumerate(info.test_cameras):
                 np.save(os.path.join(save, "projs", f"{i:05d}_render.npy"), render[i])
                 np.save(os.path.join(save, "projs", f"{i:05d}_gt.npy"), np.asarray(cam.image, np.float32))

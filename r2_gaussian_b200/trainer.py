@@ -42,6 +42,13 @@ and the native step see it too.  With `--detector_offset_refine` the learned off
 file's units.  The rasterizer clamps each Gaussian's EWA Jacobian at 1.3 tan_fov about the axis, as the reference does,
 so with an offset of more than 0.15 W a Gaussian whose centre projects beyond that clamp gets a clamped footprint.
 Without the switch the offset is ignored (the reference's render() has none) and nothing changes.
+
+`--estimate_offDetector` measures the horizontal detector offset from the train views before training
+(`detector.estimate_offset`, relative to the file's offset under `--use_offDetector`, else to a centred detector) and
+trains as `--use_offDetector` would on a copy of the scanner whose offDetector[0] is the estimated total
+(`dataset.Scene(offDetector_u=...)`).  With `--detector_offset_refine` the learned offset acts on top of the estimate.
+Each save then writes `detector_offset.yml` with `estimate_px` / `estimate_scene` next to the learned offset (if any)
+and the total `offDetector_u`; the printed result adds `detector_estimate_px`.
 """
 from __future__ import annotations
 
@@ -263,7 +270,8 @@ def render_batch(cams, gaussians: GaussianModel) -> dict:
 def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, testing_iterations=(),
              saving_iterations=(), checkpoint_iterations=(), checkpoint: str | None = None, init_points=None,
              log=print, pose_params: PoseParams | None = None, batch_size: int = 1,
-             detector_params: DetectorParams | None = None, use_offDetector: bool = False) -> dict:
+             detector_params: DetectorParams | None = None, use_offDetector: bool = False,
+             estimate_offDetector: bool = False) -> dict:
     first_iter = 0
     refine = pose_params is not None and pose_params.pose_refine
     if refine and world_info()[1] > 1:
@@ -277,8 +285,19 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
     why = batch_refusal(B, refine, world_info()[1], bool(getattr(pipe, "compute_cov3D_python", False)))
     if why is not None:
         raise ValueError(why)
+    estimate = off_u = None
+    if estimate_offDetector:
+        # the offset measured from the train views, on top of the file's under use_offDetector, becomes the scene's
+        from .dataset import read_scene
+        from .estimate_offset import estimate_scene
+        info = read_scene(model.source_path, eval=False)
+        estimate = estimate_scene(info, use_offDetector)
+        off_u, use_offDetector = estimate["offDetector_u"], True
+        log(f"estimated detector offset: {estimate['offset_px']:+.4f} px, offDetector_u = "
+            f"{off_u / info.scene_scale:.6g} ({estimate['n_pairs']} conjugate pairs)")
     scene = Scene(model.source_path, model.model_path, eval=model.eval, shuffle=False, device="cuda",
-                  data_device=model.data_device, use_offDetector=use_offDetector)
+                  data_device=model.data_device, use_offDetector=use_offDetector, offDetector_u=off_u)
+    scene.offset_estimate = estimate
     cfg = scene.scanner_cfg
     if B > len(scene.getTrainCameras()):
         raise ValueError(f"--batch_size {B} exceeds the scene's {len(scene.getTrainCameras())} train views")
@@ -535,7 +554,7 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
                         scene.save(iteration, queryfunc)
                         if corr is not None:
                             save_train_poses(scene, corr, iteration)
-                        if det is not None:
+                        if det is not None or estimate is not None:
                             save_detector_offset(scene, det, iteration)
                     else:
                         save_sharded(scene, gaussians, iteration, queryfunc, rank)
@@ -586,6 +605,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
     if det is not None:
         history["detector"] = det
         history["detector_offset_px"] = float(det.offset.detach()[0])
+    if estimate is not None:
+        history["detector_estimate_px"] = estimate["offset_px"]
     return history
 
 
@@ -602,15 +623,22 @@ def save_train_poses(scene: Scene, corr, iteration: int):
 
 @torch.no_grad()
 def save_detector_offset(scene: Scene, det, iteration: int):
-    """`point_cloud/iteration_<N>/detector_offset.yml`: the learned offset in pixels and in scene units at the detector,
-    and the sign convention in words."""
+    """`point_cloud/iteration_<N>/detector_offset.yml`: the learned offset (`det`, or None) in pixels and in scene units
+    at the detector, and the sign convention in words; under `--estimate_offDetector` also the estimate
+    (`estimate_px`, `estimate_scene`, relative to the file's offset or a centred detector)."""
     import yaml
-    doc = {"offset_px": float(det.offset.detach()[0]), "offset_scene": det.scene_units(scene.scanner_cfg),
-           "sign_convention": SIGN_CONVENTION}
+    doc = {}
+    if det is not None:
+        doc = {"offset_px": float(det.offset.detach()[0]), "offset_scene": det.scene_units(scene.scanner_cfg)}
+    doc["sign_convention"] = SIGN_CONVENTION
+    est = getattr(scene, "offset_estimate", None)
+    if est is not None:
+        doc["estimate_px"], doc["estimate_scene"] = est["offset_px"], est["offset_scene"]
     if getattr(scene, "use_offDetector", False):
-        # the learned offset acts on top of the scanner file's: the total, back in the file's units
+        # the learned offset acts on top of the scanner file's (or the estimate's): the total, in the file's units
         cfg = scene.scanner_cfg
-        doc["offDetector_u"] = (float(cfg.get("offDetector", [0.0, 0.0])[0]) - det.scene_units(cfg)) / scene.scene_scale
+        learned = det.scene_units(cfg) if det is not None else 0.0
+        doc["offDetector_u"] = (float(cfg.get("offDetector", [0.0, 0.0])[0]) - learned) / scene.scene_scale
     with open(os.path.join(scene.model_path, f"point_cloud/iteration_{iteration}", "detector_offset.yml"), "w") as f:
         yaml.dump(doc, f, default_flow_style=False, sort_keys=False)
 
@@ -732,6 +760,9 @@ def parse_args(argv=None):
                     help="train views per optimizer step (1 .. number of train views); schedules stay in steps")
     ap.add_argument("--use_offDetector", action="store_true",
                     help="train through the scanner's offDetector (every camera's projection matrix carries it)")
+    ap.add_argument("--estimate_offDetector", action="store_true",
+                    help="estimate the horizontal detector offset from the train views (on top of the file's under "
+                         "--use_offDetector) and train through it")
     a = ap.parse_args(argv)
     pick = lambda cls: cls(**{k: getattr(a, k) for k in cls.__dataclass_fields__})
     model, pipe, opt, pose = pick(ModelParams), pick(PipelineParams), pick(OptimizationParams), pick(PoseParams)
@@ -768,7 +799,8 @@ def main(argv=None):
                         "checkpoint_iterations": a.checkpoint_iterations, "start_checkpoint": a.start_checkpoint,
                         "quiet": False, "config": None, "detect_anomaly": False,
                         **({"batch_size": a.batch_size} if a.batch_size > 1 else {}),
-                        **({"use_offDetector": True} if a.use_offDetector else {})}, pose, a.detector_params)
+                        **({"use_offDetector": True} if a.use_offDetector else {}),
+                        **({"estimate_offDetector": True} if a.estimate_offDetector else {})}, pose, a.detector_params)
     random.seed(a.seed), np.random.seed(a.seed), torch.manual_seed(a.seed)     # safe_state (`general_utils.py:61-63`)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if world > 1:                      # launched by torchrun: one process per GPU, Gaussians sharded by index
@@ -783,7 +815,8 @@ def main(argv=None):
             enable_peer_exchange(True)
     hist = training(model, opt, pipe, set(a.test_iterations) | {opt.iterations}, set(a.save_iterations),
                     set(a.checkpoint_iterations), a.start_checkpoint, pose_params=pose, batch_size=a.batch_size,
-                    detector_params=a.detector_params, use_offDetector=a.use_offDetector)
+                    detector_params=a.detector_params, use_offDetector=a.use_offDetector,
+                    estimate_offDetector=a.estimate_offDetector)
     final = hist["eval"].get(opt.iterations, {})
     if world > 1:
         import torch.distributed as dist
@@ -803,6 +836,8 @@ def main(argv=None):
                       "repeated_iterations": hist.get("repeated_iterations", 0),
                       "gaussians": hist["gaussians"], **({"batch_size": a.batch_size} if a.batch_size > 1 else {}),
                       **({"detector_offset_px": hist["detector_offset_px"]} if "detector_offset_px" in hist else {}),
+                      **({"detector_estimate_px": hist["detector_estimate_px"]} if "detector_estimate_px" in hist
+                         else {}),
                       **final}))
 
 
