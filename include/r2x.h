@@ -514,6 +514,38 @@ int r2x_volume_backproject(void* stream, int n_views, int H, int W, const float*
                            float cz, float step, float* out_volume, float* out_weight, void* scratch,
                            size_t scratch_bytes);
 
+/* Per-view geometry (helical scans, calibrated benches; scene.view_scanner).  r2x_fdk_views, r2x_volume_project_views
+ * and r2x_volume_backproject_views are r2x_fdk, r2x_volume_project and r2x_volume_backproject with the scalars
+ * tan_fovx, tan_fovy, shift_u, shift_v and dso replaced by one row per view of the table view_geometry, device float64
+ * [N, 5] (row-major):
+ *   column 0  tan_fovx of view v   (tan of half its horizontal FoV, sDetector_u / 2 / DSD_v; parallel beam: 1)
+ *   column 1  tan_fovy of view v   (sDetector_v / 2 / DSD_v; parallel beam: 1)
+ *   column 2  shift_u of view v    (its offDetector_u in pixels, t_u of scene.detector_shift)
+ *   column 3  shift_v of view v    (its offDetector_v in pixels)
+ *   column 4  dso of view v        (its DSO: FDK's isocentre pitch and (DSO / z_view)^2 weight; unread by the projector
+ *                                   pair, whose rays need only the view matrix and the FoV)
+ * Every value is rounded to float32 where it is read, as the scalar entry points' float arguments are, so view v is
+ * bit for bit the scalar call with its values, and a table whose rows all equal the scalars is bit for bit the scalar
+ * entry point.  A view's DSO and its volume position offOrigin_v live in its view matrix: the camera of view v is the
+ * nominal one at DSO_v translated by offOrigin - offOrigin_v, with the grid kept at (cx, cy, cz) (scene.make_view).
+ * view_geometry_host is the same table in host memory: it is checked before any CUDA work (present, every value finite,
+ * tan_fov > 0 (always for the projector pair, cone beam for FDK), dso > 0 in cone beam) and the device copy matching it
+ * is the caller's promise.  r2x_fdk_views takes R2X_FDK_PLAIN with any filter field; Parker and half-fan weights assume
+ * one fixed circle and are refused, as is a NULL table.  Otherwise each behaves, and is limited, as its scalar entry. */
+int r2x_fdk_views(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                  const float* projmatrices, int mode, int weighting, int nx, int ny, int nz, float sx, float sy,
+                  float sz, float cx, float cy, float cz, const double* view_geometry,
+                  const double* view_geometry_host, float* out_volume, void* scratch, size_t scratch_bytes);
+int r2x_volume_project_views(void* stream, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
+                             float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
+                             int mode, float step, const double* view_geometry, const double* view_geometry_host,
+                             float* out_projs);
+int r2x_volume_backproject_views(void* stream, int n_views, int H, int W, const float* projs,
+                                 const float* viewmatrices, const float* projmatrices, int mode, int nx, int ny,
+                                 int nz, float sx, float sy, float sz, float cx, float cy, float cz, float step,
+                                 const double* view_geometry, const double* view_geometry_host, float* out_volume,
+                                 float* out_weight, void* scratch, size_t scratch_bytes);
+
 /* ---- isotropic total variation on a volume (FISTA-TV, r2_gaussian_b200/recon.py and tv.py) --------------------- */
 /* Volumes are float32 [nx,ny,nz] (z fastest).  grad x = forward differences along x, y, z, 0 across the last index;
  *   TV(x) = sum over voxels of sqrt(dx^2 + dy^2 + dz^2)      (isotropic; not the anisotropic r2x_tv3d_loss)

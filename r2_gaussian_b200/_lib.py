@@ -100,6 +100,12 @@ PROTOTYPES = {
     "r2x_volume_backproject_scratch_bytes": (_sz, [_i, _i, _i]),
     "r2x_volume_backproject": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _f, _f, _i, _i, _i, _f, _f, _f, _f, _f,
                                     _f, _f, _vp, _vp, _vp, _sz]),
+    "r2x_fdk_views": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _f, _f, _f, _vp, _vp, _vp, _vp,
+                           _sz]),
+    "r2x_volume_project_views": (_i, [_vp, _i, _i, _i, _vp, _f, _f, _f, _f, _f, _f, _i, _i, _i, _vp, _i, _f, _vp, _vp,
+                                      _vp]),
+    "r2x_volume_backproject_views": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _f, _f, _f, _f, _f,
+                                          _vp, _vp, _vp, _vp, _vp, _sz]),
     "r2x_tv_prox_scratch_bytes": (_sz, [_i, _i, _i]),
     "r2x_tv_prox": (_i, [_vp, _i, _i, _i, _vp, _f, _i, _i, _vp, _vp, _sz]),
     "r2x_tv_value_scratch_bytes": (_sz, [_i, _i, _i]),

@@ -9,7 +9,9 @@
 //                              (g_x, g_y, g_z, k0) and (s_x, s_y, s_z, k1), so the gather sees the projector's float32
 //                              sample positions p_k = fma(k, s, g) and k range by construction, for a detector offset
 //                              by (t_u, t_v) pixels as well; the gather below finds each voxel's footprint through the
-//                              caller's offset projmatrices, so it stays the transpose of the offset projector.
+//                              caller's offset projmatrices, so it stays the transpose of the offset projector.  With
+//                              a per-view geometry table each view's rays take its row (project_ray_setup), and the
+//                              caller's per-view projmatrices carry its FoV and offset.
 //   volume_backproject_kernel  a thread owns one voxel x; a CTA is 32 voxels along z (the lanes) x 4 along y.  Per view
 //                              (index order; projmatrix / viewmatrix rows staged in shared memory per chunk) the 8
 //                              corners of x's open support box (x-1, x+1)^3 go through projmatrix and the rasterizer's
@@ -44,17 +46,18 @@ size_t backproject_scratch_bytes(int N, int H, int W) {
     return bp_al256((size_t)(N < BP_CHUNK ? N : BP_CHUNK) * H * W * 2 * sizeof(float4)) + 256;
 }
 
-template <bool CONE>
+template <bool CONE, bool TABLE>
 __global__ void __launch_bounds__(BP_RAYS_THREADS) backproject_rays_kernel(
     int H, int W, const float* __restrict__ viewm, int nx, int ny, int nz, float sx, float sy, float sz, float cx,
-    float cy, float cz, float tanx, float tany, float step, ProjShift shift, float4* __restrict__ rays) {
+    float cy, float cz, float tanx, float tany, float step, ProjShift shift, const double* __restrict__ vg,
+    float4* __restrict__ rays) {
     const long long p = (long long)blockIdx.x * BP_RAYS_THREADS + threadIdx.x;
     const long long HW = (long long)H * W;
     if (p >= HW) return;
     const int view = blockIdx.y;
     const int v = (int)(p / W), u = (int)(p % W);
-    const ProjRay r = project_ray_setup<CONE>(viewm, view, u, v, H, W, nx, ny, nz, sx, sy, sz, cx, cy, cz, tanx, tany,
-                                              step, shift);
+    const ProjRay r = project_ray_setup<CONE, TABLE>(viewm, view, u, v, H, W, nx, ny, nz, sx, sy, sz, cx, cy, cz, tanx, tany,
+                                              step, shift, vg);
     long long k0 = r.k0, k1 = r.k1;
     if (k0 > k1) {
         k0 = 1; k1 = 0;                                                   // the ray misses the box
@@ -207,8 +210,8 @@ static int backproject_validate(int N, int H, int W, const float* projs, const f
 template <bool CONE>
 static int backproject_launch(cudaStream_t st, int N, int H, int W, const float* projs, const float* viewm,
                               const float* projm, float tanx, float tany, int nx, int ny, int nz, float sx, float sy,
-                              float sz, float cx, float cy, float cz, float step, ProjShift shift, float* out,
-                              float* wgt, float4* rays) {
+                              float sz, float cx, float cy, float cz, float step, ProjShift shift,
+                              const double* vg, float* out, float* wgt, float4* rays) {
     const float dx = sx / nx, dy = sy / ny, dz = sz / nz;
     const float ox = cx - 0.5f * sx + 0.5f * dx, oy = cy - 0.5f * sy + 0.5f * dy, oz = cz - 0.5f * sz + 0.5f * dz;
     const long long HW = (long long)H * W;
@@ -216,9 +219,10 @@ static int backproject_launch(cudaStream_t st, int N, int H, int W, const float*
     for (int v0 = 0; v0 < N; v0 += BP_CHUNK) {
         const int nc = min(BP_CHUNK, N - v0);
         const float* vm = viewm + (size_t)v0 * 16;
+        const double* g = vg ? vg + (size_t)v0 * VG_COLS : nullptr;
         const dim3 rgrid((unsigned)((HW + BP_RAYS_THREADS - 1) / BP_RAYS_THREADS), nc);
-        backproject_rays_kernel<CONE><<<rgrid, BP_RAYS_THREADS, 0, st>>>(H, W, vm, nx, ny, nz, sx, sy, sz, cx, cy, cz,
-                                                                         tanx, tany, step, shift, rays);
+        (g ? backproject_rays_kernel<CONE, true> : backproject_rays_kernel<CONE, false>)<<<rgrid, BP_RAYS_THREADS, 0, st>>>(
+            H, W, vm, nx, ny, nz, sx, sy, sz, cx, cy, cz, tanx, tany, step, shift, g, rays);
         R2X_CUDA_OK(cudaGetLastError());
         const int first = v0 == 0;
         const float scale = v0 + nc == N ? step : 1.0f;   // partial sums stay unscaled between chunks
@@ -234,6 +238,19 @@ static int backproject_launch(cudaStream_t st, int N, int H, int W, const float*
         R2X_CUDA_OK(cudaGetLastError());
     }
     return 0;
+}
+
+static int backproject_run(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                           const float* projmatrices, float tan_fovx, float tan_fovy, int mode, ProjShift shift,
+                           int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy, float cz,
+                           float step, const double* vg, float* out_volume, float* out_weight, void* scratch) {
+    const cudaStream_t st = (cudaStream_t)stream;
+    float4* rays = (float4*)(((size_t)scratch + 255) & ~(size_t)255);
+    if (mode == 1)
+        return backproject_launch<true>(st, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, nx, ny,
+                                        nz, sx, sy, sz, cx, cy, cz, step, shift, vg, out_volume, out_weight, rays);
+    return backproject_launch<false>(st, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, nx, ny,
+                                     nz, sx, sy, sz, cx, cy, cz, step, shift, vg, out_volume, out_weight, rays);
 }
 
 }  // namespace r2x
@@ -255,14 +272,31 @@ int r2x_volume_backproject(void* stream, int n_views, int H, int W, const float*
         return rc;
     if (!(std::isfinite(shift_u) && std::isfinite(shift_v)))
         return fail_msg(R2X_ERR_INVALID, "r2x_volume_backproject: bad shift (must be finite)");
-    const ProjShift shift = proj_shift(shift_u, shift_v, H, W);
-    const cudaStream_t st = (cudaStream_t)stream;
-    float4* rays = (float4*)(((size_t)scratch + 255) & ~(size_t)255);
-    if (mode == 1)
-        return backproject_launch<true>(st, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, nx, ny,
-                                        nz, sx, sy, sz, cx, cy, cz, step, shift, out_volume, out_weight, rays);
-    return backproject_launch<false>(st, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, nx, ny,
-                                     nz, sx, sy, sz, cx, cy, cz, step, shift, out_volume, out_weight, rays);
+    return backproject_run(stream, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode,
+                           proj_shift(shift_u, shift_v, H, W), nx, ny, nz, sx, sy, sz, cx, cy, cz, step, nullptr,
+                           out_volume, out_weight, scratch);
+}
+
+int r2x_volume_backproject_views(void* stream, int n_views, int H, int W, const float* projs,
+                                 const float* viewmatrices, const float* projmatrices, int mode, int nx, int ny,
+                                 int nz, float sx, float sy, float sz, float cx, float cy, float cz, float step,
+                                 const double* view_geometry, const double* view_geometry_host, float* out_volume,
+                                 float* out_weight, void* scratch, size_t scratch_bytes) {
+    using namespace r2x;
+    if (mode != 0 && mode != 1)
+        return fail_msg(R2X_ERR_INVALID, "r2x_volume_backproject: bad mode (0 = parallel, 1 = cone)");
+    if (n_views < 1) return fail_msg(R2X_ERR_INVALID, "r2x_volume_backproject: bad N/H/W (each must be >= 1)");
+    if (int rc = view_geometry_check("r2x_volume_backproject_views", n_views, mode, view_geometry, view_geometry_host,
+                                     true))
+        return rc;
+    // the scalars stand in for the table in the shared checks; the ray setup reads every view's row
+    const float tanx = (float)view_geometry_host[VG_TANX], tany = (float)view_geometry_host[VG_TANY];
+    if (int rc = backproject_validate(n_views, H, W, projs, viewmatrices, projmatrices, tanx, tany, mode, nx, ny, nz,
+                                      sx, sy, sz, cx, cy, cz, step, out_volume, scratch, scratch_bytes))
+        return rc;
+    return backproject_run(stream, n_views, H, W, projs, viewmatrices, projmatrices, tanx, tany, mode,
+                           ProjShift{0.0, 0.0}, nx, ny, nz, sx, sy, sz, cx, cy, cz, step, view_geometry, out_volume,
+                           out_weight, scratch);
 }
 
 }  // extern "C"

@@ -29,6 +29,9 @@
 //                           projmatrices.  The scale is pi / N, or 1 for Parker weights (they hold each view's
 //                           interval).
 //
+// With a per-view geometry table (r2x_fdk_views) the filter kernels take each row's tan_fov, offset and isocentre pitch
+// from its view's row (fdk_view_row) and the backprojection each view's DSO; without one, the scalars.
+//
 // The float64 NumPy statements of the same definitions are oracle/fdk_oracle.py (plain),
 // tests/fdk_short_scan_oracle.py (short scan, Parker weights) and tests/offset_detector_oracle.py (offset detector,
 // half-fan weights).
@@ -37,6 +40,7 @@
 
 #include "../../include/r2x.h"
 #include "r2x_common.cuh"
+#include "r2x_project.cuh"
 
 namespace r2x {
 
@@ -56,13 +60,15 @@ size_t fdk_scratch_bytes(int N, int H, int W) {
 static size_t fdk_filter_smem(int W) { return (size_t)(3 * W + (W + 1) / 2) * sizeof(float); }
 static size_t fdk_window_smem(int W) { return (size_t)(2 * W) * sizeof(float); }
 
-template <bool CONE>
+// TABLE: each view's DSO from its row of the per-view geometry table `vg`; without it `dso` for every view.
+template <bool CONE, bool TABLE>
 __global__ void __launch_bounds__(FDK_BX * FDK_BY) fdk_backproject_kernel(
     int N, int H, int W, const float* __restrict__ q, const float* __restrict__ viewm, const float* __restrict__ projm,
     float dso, int nx, int ny, int nz, float ox, float oy, float oz, float dx, float dy, float dz, float scale,
-    float* __restrict__ vol) {
-    // per view: projmatrix rows 0, 1, 3 and viewmatrix row 2 as (m[r], m[4+r], m[8+r], m[12+r])
+    float* __restrict__ vol, const double* __restrict__ vg) {
+    // per view: projmatrix rows 0, 1, 3 and viewmatrix row 2 as (m[r], m[4+r], m[8+r], m[12+r]), and its DSO
     __shared__ float4 mat[FDK_VCHUNK][4];
+    __shared__ float vdso[TABLE ? FDK_VCHUNK : 1];
     const int y = blockIdx.x * FDK_BX + threadIdx.x;
     const int x = blockIdx.y * FDK_BY + threadIdx.y;
     const int z0 = blockIdx.z * FDK_ZR;
@@ -85,6 +91,7 @@ __global__ void __launch_bounds__(FDK_BX * FDK_BY) fdk_backproject_kernel(
             const int rr = slot == 3 ? 2 : (slot == 2 ? 3 : slot);
             mat[v][slot] = make_float4(m[rr], m[4 + rr], m[8 + rr], m[12 + rr]);
         }
+        if (CONE && TABLE && tid < nc) vdso[tid] = (float)vg[(size_t)(c0 + tid) * VG_COLS + VG_DSO];
         __syncthreads();
         if (!live) continue;
         for (int v = 0; v < nc; ++v) {
@@ -106,7 +113,7 @@ __global__ void __launch_bounds__(FDK_BX * FDK_BY) fdk_backproject_kernel(
                 if (CONE) {
                     const float zv = fmaf(fk, sv, av);
                     if (!(zv > 0.0f)) continue;
-                    const float u = dso * __frcp_rn(zv);
+                    const float u = (TABLE ? vdso[v] : dso) * __frcp_rn(zv);
                     w = u * u;
                 }
                 const float pw = __frcp_rn(fmaf(fk, sw, aw));
@@ -174,6 +181,23 @@ struct FdkWeights {
     float fan = 1.0f, hf_inv_delta = 1.0f, hf_sigma = 1.0f;   // HALF_FAN: a = ndc_x * fan, 1 / delta, sign(t_u)
 };
 
+// isocentre pitch: cone dDetector_u * DSO / DSD = 2 tan_fovx DSO / W; parallel 2 / W (ndc [-1,1] = scene [-1,1])
+__host__ __device__ inline double fdk_pitch(int W, float tanx, int mode, float dso) {
+    return mode == 1 ? 2.0 * (double)tanx * (double)dso / W : 2.0 / W;
+}
+
+// A per-view table row's filter arguments, rounded and derived exactly as r2x_fdk derives the scalar ones on the host
+// (float32 arguments, su / sv and 1 / pitch in float64 rounded once), so a view filters bit for bit as a scalar call
+// with its values.
+__device__ __forceinline__ void fdk_view_row(const double* __restrict__ row, int H, int W, int cone, float& tanx,
+                                             float& tany, float& inv_delta, float& su, float& sv) {
+    tanx = (float)row[VG_TANX];
+    tany = (float)row[VG_TANY];
+    su = (float)(2.0 * (double)(float)row[VG_SHIFT_U] / W);
+    sv = (float)(-2.0 * (double)(float)row[VG_SHIFT_V] / H);
+    inv_delta = (float)(1.0 / fdk_pitch(W, tanx, cone, (float)row[VG_DSO]));
+}
+
 // Step 1 of FDK on detector row r (view * H + row) of a detector offset by (t_u, t_v) pixels (zero when centred): each
 // pixel's cosine weight (cone beam) at its ndc moved by (su, sv) = (2 t_u / W, -2 t_v / H), then WEIGHT's redundancy
 // weight: PARKER its Parker weight at fan angle -atan(a) (cone; 0 for parallel beam) times its view's angular interval,
@@ -207,14 +231,16 @@ __device__ __forceinline__ void fdk_weight_row(size_t r, int H, int W, const flo
 // Steps 1-2 of FDK with the band-limited Ram-Lak filter, one CTA per detector row: fdk_weight_row, the row staged in
 // shared memory between two rows of zeros and filtered with the Ram-Lak taps (shift-invariant, so the same for any
 // offset).
-template <int WEIGHT>
+template <int WEIGHT, bool TABLE>
 __global__ void __launch_bounds__(256) fdk_filter_kernel(int H, int W, const float* __restrict__ projs, float tanx,
                                                          float tany, int cone, float inv_delta, float su, float sv,
-                                                         FdkWeights fw, float* __restrict__ q) {
+                                                         FdkWeights fw, const double* __restrict__ vg,
+                                                         float* __restrict__ q) {
     extern __shared__ float sm[];
     float* row = sm;              // [3W]: zeros | weighted row | zeros
     float* g = sm + 3 * W;        // [(W+1)/2]: g[m] = 1 / (pi^2 (2m+1)^2)
     const size_t r = blockIdx.x;  // view * H + detector row
+    if (TABLE) fdk_view_row(vg + (r / H) * VG_COLS, H, W, cone, tanx, tany, inv_delta, su, sv);
     fdk_weight_row<WEIGHT>(r, H, W, projs, tanx, tany, cone, su, sv, fw, [&](int j, float p) {
         row[j] = 0.0f;
         row[W + j] = p;
@@ -263,14 +289,16 @@ __device__ __forceinline__ double fdk_window_tap(int k) {
 // pixels j - k and j + k both lie in the row for k <= near = min(j, W-1-j), one of them up to far = max(j, W-1-j);
 // the sum runs from k = far down to 1, smallest taps first (as fdk_filter_kernel's), with no bounds checks in either
 // loop.
-template <int WEIGHT, int WINDOW>
+template <int WEIGHT, int WINDOW, bool TABLE>
 __global__ void __launch_bounds__(256) fdk_window_kernel(int H, int W, const float* __restrict__ projs, float tanx,
                                                          float tany, int cone, float inv_delta, float su, float sv,
-                                                         FdkWeights fw, float* __restrict__ q) {
+                                                         FdkWeights fw, const double* __restrict__ vg,
+                                                         float* __restrict__ q) {
     extern __shared__ float sm[];
     float* row = sm;              // [W]: weighted row
     float* h = sm + W;            // [W]: h[k]
     const size_t r = blockIdx.x;  // view * H + detector row
+    if (TABLE) fdk_view_row(vg + (r / H) * VG_COLS, H, W, cone, tanx, tany, inv_delta, su, sv);
     fdk_weight_row<WEIGHT>(r, H, W, projs, tanx, tany, cone, su, sv, fw, [&](int j, float p) { row[j] = p; });
     for (int k = threadIdx.x; k < W; k += blockDim.x) h[k] = (float)fdk_window_tap<WINDOW>(k);
     __syncthreads();
@@ -285,52 +313,50 @@ __global__ void __launch_bounds__(256) fdk_window_kernel(int H, int W, const flo
     }
 }
 
-// isocentre pitch: cone dDetector_u * DSO / DSD = 2 tan_fovx DSO / W; parallel 2 / W (ndc [-1,1] = scene [-1,1])
-static double fdk_pitch(int W, float tanx, int mode, float dso) {
-    return mode == 1 ? 2.0 * (double)tanx * (double)dso / W : 2.0 / W;
-}
+using FdkFilterKernel = void (*)(int, int, const float*, float, float, int, float, float, float, FdkWeights,
+                                 const double*, float*);
 
-using FdkFilterKernel = void (*)(int, int, const float*, float, float, int, float, float, float, FdkWeights, float*);
-
-template <int WEIGHT>
+template <int WEIGHT, bool TABLE>
 static FdkFilterKernel fdk_filter_for(int window) {
     switch (window) {
-        case R2X_FDK_SHEPP_LOGAN: return fdk_window_kernel<WEIGHT, R2X_FDK_SHEPP_LOGAN>;
-        case R2X_FDK_COSINE: return fdk_window_kernel<WEIGHT, R2X_FDK_COSINE>;
-        case R2X_FDK_HAMMING: return fdk_window_kernel<WEIGHT, R2X_FDK_HAMMING>;
-        case R2X_FDK_HANN: return fdk_window_kernel<WEIGHT, R2X_FDK_HANN>;
-        default: return fdk_filter_kernel<WEIGHT>;
+        case R2X_FDK_SHEPP_LOGAN: return fdk_window_kernel<WEIGHT, R2X_FDK_SHEPP_LOGAN, TABLE>;
+        case R2X_FDK_COSINE: return fdk_window_kernel<WEIGHT, R2X_FDK_COSINE, TABLE>;
+        case R2X_FDK_HAMMING: return fdk_window_kernel<WEIGHT, R2X_FDK_HAMMING, TABLE>;
+        case R2X_FDK_HANN: return fdk_window_kernel<WEIGHT, R2X_FDK_HANN, TABLE>;
+        default: return fdk_filter_kernel<WEIGHT, TABLE>;
     }
 }
 
 // window: R2X_FDK_RAM_LAK or one of the windowed filters (r2x_fdk's filter field)
 static int fdk_filter(cudaStream_t st, int weighting, int window, int N, int H, int W, const float* projs, float tanx,
-                      float tany, int mode, float dso, float su, float sv, const FdkWeights& fw, float* q) {
-    auto kernel = weighting == R2X_FDK_PARKER     ? fdk_filter_for<R2X_FDK_PARKER>(window)
-                  : weighting == R2X_FDK_HALF_FAN ? fdk_filter_for<R2X_FDK_HALF_FAN>(window)
-                                                  : fdk_filter_for<R2X_FDK_PLAIN>(window);
+                      float tany, int mode, float dso, float su, float sv, const FdkWeights& fw, const double* vg,
+                      float* q) {
+    // a table comes with R2X_FDK_PLAIN only (r2x_fdk_views)
+    auto kernel = vg                              ? fdk_filter_for<R2X_FDK_PLAIN, true>(window)
+                  : weighting == R2X_FDK_PARKER   ? fdk_filter_for<R2X_FDK_PARKER, false>(window)
+                  : weighting == R2X_FDK_HALF_FAN ? fdk_filter_for<R2X_FDK_HALF_FAN, false>(window)
+                                                  : fdk_filter_for<R2X_FDK_PLAIN, false>(window);
     const size_t smem = window == R2X_FDK_RAM_LAK ? fdk_filter_smem(W) : fdk_window_smem(W);
     if (smem > 48 * 1024)
         R2X_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<(unsigned)((long long)N * H), 256, smem, st>>>(H, W, projs, tanx, tany, mode,
-                                                            (float)(1.0 / fdk_pitch(W, tanx, mode, dso)), su, sv, fw, q);
+                                                            (float)(1.0 / fdk_pitch(W, tanx, mode, dso)), su, sv, fw, vg,
+                                                            q);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }
 
 static int fdk_backproject(cudaStream_t st, int N, int H, int W, const float* q, const float* viewm, const float* projm,
-                           int mode, float dso, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy,
-                           float cz, float scale, float* vol) {
+                           int mode, float dso, const double* vg, int nx, int ny, int nz, float sx, float sy,
+                           float sz, float cx, float cy, float cz, float scale, float* vol) {
     const float dx = sx / nx, dy = sy / ny, dz = sz / nz;
     const float ox = cx - 0.5f * sx + 0.5f * dx, oy = cy - 0.5f * sy + 0.5f * dy, oz = cz - 0.5f * sz + 0.5f * dz;
     const dim3 grid((ny + FDK_BX - 1) / FDK_BX, (nx + FDK_BY - 1) / FDK_BY, (nz + FDK_ZR - 1) / FDK_ZR);
     const dim3 block(FDK_BX, FDK_BY);
-    if (mode == 1)
-        fdk_backproject_kernel<true><<<grid, block, 0, st>>>(N, H, W, q, viewm, projm, dso, nx, ny, nz, ox, oy, oz, dx, dy,
-                                                            dz, scale, vol);
-    else
-        fdk_backproject_kernel<false><<<grid, block, 0, st>>>(N, H, W, q, viewm, projm, dso, nx, ny, nz, ox, oy, oz, dx,
-                                                             dy, dz, scale, vol);
+    // parallel beam reads no DSO
+    auto kernel = mode == 1 ? (vg ? fdk_backproject_kernel<true, true> : fdk_backproject_kernel<true, false>)
+                            : fdk_backproject_kernel<false, false>;
+    kernel<<<grid, block, 0, st>>>(N, H, W, q, viewm, projm, dso, nx, ny, nz, ox, oy, oz, dx, dy, dz, scale, vol, vg);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -355,17 +381,12 @@ static int fdk_validate(int N, int H, int W, const float* projs, const float* vi
     return 0;
 }
 
-}  // namespace r2x
-
-extern "C" {
-
-size_t r2x_fdk_scratch_bytes(int n_views, int H, int W) { return r2x::fdk_scratch_bytes(n_views, H, W); }
-
-int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
-            const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
-            int weighting, const float* view_weights, float arc, float dso, int nx, int ny, int nz, float sx, float sy,
-            float sz, float cx, float cy, float cz, float* out_volume, void* scratch, size_t scratch_bytes) {
-    using namespace r2x;
+// r2x_fdk, and r2x_fdk_views with the scalars standing in for its table (vg) in the checks
+static int fdk_run(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                   const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
+                   int weighting, const float* view_weights, float arc, float dso, int nx, int ny, int nz, float sx,
+                   float sy, float sz, float cx, float cy, float cz, float* out_volume, void* scratch,
+                   size_t scratch_bytes, const double* vg) {
     if (int rc = fdk_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode, dso, nx, ny,
                               nz, sx, sy, sz, out_volume, scratch, scratch_bytes))
         return rc;
@@ -407,12 +428,47 @@ int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const f
     const cudaStream_t st = (cudaStream_t)stream;
     float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
     const float su = (float)(2.0 * (double)shift_u / W), sv = (float)(-2.0 * (double)shift_v / H);
-    if (int rc = fdk_filter(st, weighting, window, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, su, sv, fw, q))
+    if (int rc = fdk_filter(st, weighting, window, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, su, sv, fw, vg,
+                            q))
         return rc;
     // Parker's dbeta_v already holds each view's share of the arc
     const float scale = weighting == R2X_FDK_PARKER ? 1.0f : (float)(pi / n_views);
-    return fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, nx, ny, nz, sx, sy, sz, cx, cy,
-                           cz, scale, out_volume);
+    return fdk_backproject(st, n_views, H, W, q, viewmatrices, projmatrices, mode, dso, vg, nx, ny, nz, sx, sy, sz, cx,
+                           cy, cz, scale, out_volume);
+}
+
+}  // namespace r2x
+
+extern "C" {
+
+size_t r2x_fdk_scratch_bytes(int n_views, int H, int W) { return r2x::fdk_scratch_bytes(n_views, H, W); }
+
+int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+            const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
+            int weighting, const float* view_weights, float arc, float dso, int nx, int ny, int nz, float sx, float sy,
+            float sz, float cx, float cy, float cz, float* out_volume, void* scratch, size_t scratch_bytes) {
+    return r2x::fdk_run(stream, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode, shift_u,
+                        shift_v, weighting, view_weights, arc, dso, nx, ny, nz, sx, sy, sz, cx, cy, cz, out_volume,
+                        scratch, scratch_bytes, nullptr);
+}
+
+int r2x_fdk_views(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                  const float* projmatrices, int mode, int weighting, int nx, int ny, int nz, float sx, float sy,
+                  float sz, float cx, float cy, float cz, const double* view_geometry,
+                  const double* view_geometry_host, float* out_volume, void* scratch, size_t scratch_bytes) {
+    using namespace r2x;
+    if (mode != 0 && mode != 1) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad mode (0 = parallel, 1 = cone)");
+    if (n_views < 1) return fail_msg(R2X_ERR_INVALID, "r2x_fdk: bad N/H/W (each must be >= 1)");
+    if ((weighting & 0xff) == R2X_FDK_PARKER || (weighting & 0xff) == R2X_FDK_HALF_FAN)
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk_views: bad weighting (Parker and half-fan weights assume one fixed "
+                                         "circle; a per-view table takes R2X_FDK_PLAIN only)");
+    if (int rc = view_geometry_check("r2x_fdk_views", n_views, mode, view_geometry, view_geometry_host, false))
+        return rc;
+    const double* row0 = view_geometry_host;
+    return fdk_run(stream, n_views, H, W, projs, viewmatrices, projmatrices, (float)row0[VG_TANX],
+                   (float)row0[VG_TANY], mode, (float)row0[VG_SHIFT_U], (float)row0[VG_SHIFT_V], weighting, nullptr,
+                   0.0f, (float)row0[VG_DSO], nx, ny, nz, sx, sy, sz, cx, cy, cz, out_volume, scratch, scratch_bytes,
+                   view_geometry);
 }
 
 int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, float tan_fovx, float tan_fovy,
@@ -424,7 +480,7 @@ int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, 
         return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_filter: bad DSO / tan_fov");
     if (!projs || !filtered) return r2x::fail_msg(R2X_ERR_INVALID, "r2x_fdk_filter: bad pointer (NULL)");
     return r2x::fdk_filter((cudaStream_t)stream, R2X_FDK_PLAIN, R2X_FDK_RAM_LAK, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso,
-                           0.0f, 0.0f, r2x::FdkWeights(), filtered);
+                           0.0f, 0.0f, r2x::FdkWeights(), nullptr, filtered);
 }
 
 int r2x_fdk_backproject(void* stream, int n_views, int H, int W, const float* filtered, const float* viewmatrices,
@@ -433,8 +489,9 @@ int r2x_fdk_backproject(void* stream, int n_views, int H, int W, const float* fi
     if (int rc = r2x::fdk_validate(n_views, H, W, filtered, viewmatrices, projmatrices, 1.0f, 1.0f,
                                    mode, dso, nx, ny, nz, sx, sy, sz, out_volume, filtered, (size_t)-1))
         return rc;
-    return r2x::fdk_backproject((cudaStream_t)stream, n_views, H, W, filtered, viewmatrices, projmatrices, mode, dso, nx,
-                                ny, nz, sx, sy, sz, cx, cy, cz, (float)(3.141592653589793 / n_views), out_volume);
+    return r2x::fdk_backproject((cudaStream_t)stream, n_views, H, W, filtered, viewmatrices, projmatrices, mode, dso,
+                                nullptr, nx, ny, nz, sx, sy, sz, cx, cy, cz, (float)(3.141592653589793 / n_views),
+                                out_volume);
 }
 
 }  // extern "C"

@@ -14,7 +14,8 @@
 //                          g_k = fma(k, step, g_c) in float32, floor, 8 predicated __ldg loads, float32 sum in k order.
 //                          The 32 x 8 tile is staged in shared memory so the [N,H,W] rows are stored in whole sectors.
 //                          No atomics: the projections are bitwise reproducible.  A detector offset by (t_u, t_v)
-//                          pixels (TIGRE's geo.offDetector) only moves the pixel's ndc in the float64 setup.
+//                          pixels (TIGRE's geo.offDetector) only moves the pixel's ndc in the float64 setup.  With a
+//                          per-view geometry table the setup takes the view's tan_fov and shift from it.
 //
 // The float64 NumPy statement of the same definition is oracle/projector_oracle.py.
 #include <cmath>
@@ -29,19 +30,19 @@ namespace r2x {
 constexpr int PRJ_BV = 32, PRJ_BU = 8;   // CTA: 32 detector rows (lanes) x 8 detector columns
 constexpr int PRJ_MAX_VIEWS = 65535;     // views per launch (grid.z); more are launched in chunks
 
-template <bool CONE>
+template <bool CONE, bool TABLE>
 __global__ void __launch_bounds__(PRJ_BV * PRJ_BU) volume_project_kernel(
     const float* __restrict__ vol, int nx, int ny, int nz, float sx, float sy, float sz, float cx, float cy, float cz,
     int H, int W, const float* __restrict__ viewm, float tanx, float tany, float step, ProjShift shift,
-    float* __restrict__ out) {
+    const double* __restrict__ vg, float* __restrict__ out) {
     __shared__ float tile[PRJ_BV][PRJ_BU + 1];
     const int v = blockIdx.y * PRJ_BV + threadIdx.x;   // detector row
     const int u = blockIdx.x * PRJ_BU + threadIdx.y;   // detector column
     const int view = blockIdx.z;
     float acc = 0.0f;
     if (v < H && u < W) {
-        const ProjRay ray = project_ray_setup<CONE>(viewm, view, u, v, H, W, nx, ny, nz, sx, sy, sz, cx, cy, cz, tanx,
-                                                    tany, step, shift);
+        const ProjRay ray = project_ray_setup<CONE, TABLE>(viewm, view, u, v, H, W, nx, ny, nz, sx, sy, sz, cx, cy, cz, tanx,
+                                                    tany, step, shift, vg);
         const long long sy_ = nz, sx_ = (long long)ny * nz;
         for (long long k = ray.k0; k <= ray.k1; ++k) {
             const float fk = (float)k;
@@ -96,6 +97,26 @@ static int project_validate(int nx, int ny, int nz, const float* volume, float s
     return 0;
 }
 
+static int project_launch(cudaStream_t st, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
+                          float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
+                          float tan_fovx, float tan_fovy, int mode, ProjShift shift, float step, const double* vg,
+                          float* out_projs) {
+    const dim3 block(PRJ_BV, PRJ_BU);
+    for (int v0 = 0; v0 < n_views; v0 += PRJ_MAX_VIEWS) {
+        const int nv = min(PRJ_MAX_VIEWS, n_views - v0);
+        const dim3 grid((W + PRJ_BU - 1) / PRJ_BU, (H + PRJ_BV - 1) / PRJ_BV, nv);
+        const float* vm = viewmatrices + (size_t)v0 * 16;
+        const double* g = vg ? vg + (size_t)v0 * VG_COLS : nullptr;
+        float* o = out_projs + (size_t)v0 * H * W;
+        auto kernel = mode == 1 ? (g ? volume_project_kernel<true, true> : volume_project_kernel<true, false>)
+                                : (g ? volume_project_kernel<false, true> : volume_project_kernel<false, false>);
+        kernel<<<grid, block, 0, st>>>(volume, nx, ny, nz, sx, sy, sz, cx, cy, cz, H, W, vm, tan_fovx, tan_fovy, step,
+                                       shift, g, o);
+        R2X_CUDA_OK(cudaGetLastError());
+    }
+    return 0;
+}
+
 }  // namespace r2x
 
 extern "C" {
@@ -110,23 +131,28 @@ int r2x_volume_project(void* stream, int nx, int ny, int nz, const float* volume
         return rc;
     if (!(std::isfinite(shift_u) && std::isfinite(shift_v)))
         return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad shift (must be finite)");
-    const ProjShift shift = proj_shift(shift_u, shift_v, H, W);
-    const cudaStream_t st = (cudaStream_t)stream;
-    const dim3 block(PRJ_BV, PRJ_BU);
-    for (int v0 = 0; v0 < n_views; v0 += PRJ_MAX_VIEWS) {
-        const int nv = min(PRJ_MAX_VIEWS, n_views - v0);
-        const dim3 grid((W + PRJ_BU - 1) / PRJ_BU, (H + PRJ_BV - 1) / PRJ_BV, nv);
-        const float* vm = viewmatrices + (size_t)v0 * 16;
-        float* o = out_projs + (size_t)v0 * H * W;
-        if (mode == 1)
-            volume_project_kernel<true><<<grid, block, 0, st>>>(volume, nx, ny, nz, sx, sy, sz, cx, cy, cz, H, W, vm,
-                                                                tan_fovx, tan_fovy, step, shift, o);
-        else
-            volume_project_kernel<false><<<grid, block, 0, st>>>(volume, nx, ny, nz, sx, sy, sz, cx, cy, cz, H, W, vm,
-                                                                 tan_fovx, tan_fovy, step, shift, o);
-        R2X_CUDA_OK(cudaGetLastError());
-    }
-    return 0;
+    return project_launch((cudaStream_t)stream, nx, ny, nz, volume, sx, sy, sz, cx, cy, cz, n_views, H, W,
+                          viewmatrices, tan_fovx, tan_fovy, mode, proj_shift(shift_u, shift_v, H, W), step, nullptr,
+                          out_projs);
+}
+
+int r2x_volume_project_views(void* stream, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
+                             float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
+                             int mode, float step, const double* view_geometry, const double* view_geometry_host,
+                             float* out_projs) {
+    using namespace r2x;
+    if (mode != 0 && mode != 1) return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad mode (0 = parallel, 1 = cone)");
+    if (n_views < 1) return fail_msg(R2X_ERR_INVALID, "r2x_volume_project: bad N/H/W (each must be >= 1)");
+    if (int rc = view_geometry_check("r2x_volume_project_views", n_views, mode, view_geometry, view_geometry_host,
+                                     true))
+        return rc;
+    // the scalars stand in for the table in the shared checks; the kernels read every view's row
+    const float tanx = (float)view_geometry_host[VG_TANX], tany = (float)view_geometry_host[VG_TANY];
+    if (int rc = project_validate(nx, ny, nz, volume, sx, sy, sz, cx, cy, cz, n_views, H, W, viewmatrices, tanx, tany,
+                                  mode, step, out_projs))
+        return rc;
+    return project_launch((cudaStream_t)stream, nx, ny, nz, volume, sx, sy, sz, cx, cy, cz, n_views, H, W,
+                          viewmatrices, tanx, tany, mode, ProjShift{0.0, 0.0}, step, view_geometry, out_projs);
 }
 
 }  // extern "C"

@@ -3,6 +3,7 @@
 #pragma once
 
 #include <cmath>
+#include <cstdio>
 
 namespace r2x {
 
@@ -23,15 +24,54 @@ struct ProjShift {
     double su, sv;
 };
 
-static inline ProjShift proj_shift(float tu, float tv, int H, int W) {
+__host__ __device__ inline ProjShift proj_shift(float tu, float tv, int H, int W) {
     return {2.0 * (double)tu / W, 2.0 * (double)tv / H};
 }
 
-template <bool CONE>
+// Columns of a per-view geometry table row (include/r2x.h): float64 [N, VG_COLS].
+constexpr int VG_COLS = 5, VG_TANX = 0, VG_TANY = 1, VG_SHIFT_U = 2, VG_SHIFT_V = 3, VG_DSO = 4;
+
+// Host check of a per-view geometry table (the host copy of the device table the kernels read) before any CUDA work:
+// present, every value finite once rounded to float32 as the kernels round it, tan_fov > 0 (cone beam, or always when
+// `tan_always`), dso > 0 in cone beam.  Returns 0 or the fail_msg code.
+static inline int view_geometry_check(const char* who, int N, int mode, const double* dev, const double* host,
+                                      bool tan_always) {
+    char msg[192];
+    if (!dev || !host) {
+        std::snprintf(msg, sizeof msg, "%s: bad pointer (view_geometry NULL)", who);
+        return fail_msg(R2X_ERR_INVALID, msg);
+    }
+    for (int v = 0; v < N; ++v) {
+        const double* row = host + (size_t)v * VG_COLS;
+        const char* bad = nullptr;
+        for (int c = 0; c < VG_COLS; ++c)
+            if (!std::isfinite((float)row[c])) bad = "values must be finite";
+        if (!bad && (mode == 1 || tan_always) && !((float)row[VG_TANX] > 0.0f && (float)row[VG_TANY] > 0.0f))
+            bad = "tan_fov must be > 0";
+        if (!bad && mode == 1 && !((float)row[VG_DSO] > 0.0f)) bad = "cone beam needs dso > 0";
+        if (bad) {
+            std::snprintf(msg, sizeof msg, "%s: bad view_geometry (view %d: %s)", who, v, bad);
+            return fail_msg(R2X_ERR_INVALID, msg);
+        }
+    }
+    return 0;
+}
+
+// TABLE: the view's tan_fov and shift come from its row of the per-view geometry table `vg` (include/r2x.h), rounded
+// to float32 as the scalar entry points' arguments are, so a view is bit for bit the scalar call with its values.
+// Without TABLE, `vg` is not read and the code is the scalar setup's.
+template <bool CONE, bool TABLE>
 __device__ __forceinline__ ProjRay project_ray_setup(const float* __restrict__ viewm, int view, int u, int v, int H,
                                                      int W, int nx, int ny, int nz, float sx, float sy, float sz,
                                                      float cx, float cy, float cz, float tanx, float tany,
-                                                     float step, ProjShift shift) {
+                                                     float step, ProjShift shift,
+                                                     const double* __restrict__ vg) {
+    if (TABLE) {
+        const double* row = vg + (size_t)view * VG_COLS;
+        tanx = (float)row[VG_TANX];
+        tany = (float)row[VG_TANY];
+        shift = proj_shift((float)row[VG_SHIFT_U], (float)row[VG_SHIFT_V], H, W);
+    }
     // world -> camera: rotation Rw[r][c] = m[4c + r], translation T[r] = m[12 + r] (column-major flat)
     const float* m = viewm + (size_t)view * 16;
     double Rw[3][3], T[3];

@@ -21,12 +21,13 @@ import math
 import os
 import pickle
 import random
+import warnings
 from dataclasses import dataclass, field
 
 import numpy as np
 import torch
 
-from .scene import angle2pose, detector_shift, projection_matrix, shifted_projection_matrix
+from .scene import VIEW_KEYS, camera_pose, detector_shift, projection_matrix, shifted_projection_matrix, view_scanner
 
 MODE_ID = {"parallel": 0, "cone": 1}
 _LENGTH_KEYS = ("dVoxel", "sVoxel", "sDetector", "dDetector", "offOrigin", "offDetector", "DSD", "DSO")
@@ -47,6 +48,7 @@ class CameraInfo:
     height: int
     mode: int
     scanner_cfg: dict
+    view_geometry: dict = field(default_factory=dict)   # the frame's VIEW_KEYS overrides, in scene units
 
 
 @dataclass
@@ -67,7 +69,7 @@ def _rescale(cfg: dict) -> float:
 
 
 def _camera_info(uid, angle, image, name, path, cfg) -> CameraInfo:
-    w2c = np.linalg.inv(angle2pose(cfg["DSO"], angle))
+    w2c = np.linalg.inv(camera_pose(cfg, angle))
     # dDetector / sDetector are [v, u]
     fov_x = math.atan2(cfg["sDetector"][1] / 2, cfg["DSD"]) * 2
     fov_y = math.atan2(cfg["sDetector"][0] / 2, cfg["DSD"]) * 2
@@ -85,7 +87,15 @@ def scale_scanner(cfg: dict) -> float:
     return _rescale(cfg)
 
 
-def read_blender(path: str, eval: bool = True) -> SceneInfo:
+def frame_geometry(frame: dict, scale: float) -> dict:
+    """A projection frame's per-view overrides (`scene.VIEW_KEYS`), rescaled by `scale` as `_rescale` rescales the
+    scanner's lengths."""
+    return {k: (np.asarray(frame[k], dtype=np.float64) * scale).tolist() for k in VIEW_KEYS if k in frame}
+
+
+def read_blender(path: str, eval: bool = True, use_view_geometry: bool = False) -> SceneInfo:
+    """`use_view_geometry` builds each camera from its frame's overrides (`scene.view_scanner`); without it they are
+    only recorded in `CameraInfo.view_geometry`, with one warning naming the flag when a frame carries any."""
     with open(os.path.join(path, "meta_data.json")) as f:
         meta = json.load(f)
     cfg = meta["scanner"]
@@ -95,8 +105,14 @@ def read_blender(path: str, eval: bool = True) -> SceneInfo:
         offset = len(meta["proj_train"]) if split == "test" else 0
         for i, frame in enumerate(meta["proj_" + split]):
             p = os.path.join(path, frame["file_path"])
-            cams[split].append(_camera_info(i + offset, frame["angle"], np.load(p) * scale,
-                                            os.path.basename(p).split(".")[0], p, cfg))
+            geo = frame_geometry(frame, scale)
+            info = _camera_info(i + offset, frame["angle"], np.load(p) * scale, os.path.basename(p).split(".")[0], p,
+                                view_scanner(cfg, geo) if use_view_geometry else cfg)
+            info.view_geometry = geo
+            cams[split].append(info)
+    if not use_view_geometry and any(c.view_geometry for c in cams["train"] + cams["test"]):
+        warnings.warn(f"{path}: its projection frames carry per-view geometry ({', '.join(VIEW_KEYS)}), which is "
+                      "ignored: pass --use_view_geometry (use_view_geometry=True) to use it", stacklevel=2)
     vol = np.load(os.path.join(path, meta["vol"])).astype(np.float32)
     return SceneInfo(cams["train"], cams["test"], vol, cfg, scale)
 
@@ -126,9 +142,10 @@ def read_naf(path: str, eval: bool = True) -> SceneInfo:
     return SceneInfo(cams["train"], cams["test"], np.asarray(data["image"], dtype=np.float32), cfg, scale)
 
 
-def read_scene(source_path: str, eval: bool = True) -> SceneInfo:
+def read_scene(source_path: str, eval: bool = True, use_view_geometry: bool = False) -> SceneInfo:
+    """`use_view_geometry`: each camera from its frame's per-view geometry (`read_blender`; NAF pickles carry none)."""
     if os.path.exists(os.path.join(source_path, "meta_data.json")):
-        return read_blender(source_path, eval)
+        return read_blender(source_path, eval, use_view_geometry)
     if source_path.split(".")[-1] in ("pickle", "pkl"):
         return read_naf(source_path, eval)
     raise ValueError(f"Could not recognize scene type: {source_path}.")
@@ -142,6 +159,19 @@ def train_view_count(source_path: str) -> int:
     if source_path.split(".")[-1] in ("pickle", "pkl"):
         with open(source_path, "rb") as f:
             return int(pickle.load(f)["numTrain"])
+    raise ValueError(f"Could not recognize scene type: {source_path}.")
+
+
+def train_view_dsd(source_path: str) -> list[float]:
+    """Each train view's DSD under per-view geometry (its frame's, else the scanner's; file units), without reading
+    the projections.  NAF pickles carry one DSD."""
+    if os.path.exists(os.path.join(source_path, "meta_data.json")):
+        with open(os.path.join(source_path, "meta_data.json")) as f:
+            meta = json.load(f)
+        return [float(fr.get("DSD", meta["scanner"]["DSD"])) for fr in meta["proj_train"]]
+    if source_path.split(".")[-1] in ("pickle", "pkl"):
+        with open(source_path, "rb") as f:
+            return [float(pickle.load(f)["DSD"])]
     raise ValueError(f"Could not recognize scene type: {source_path}.")
 
 
@@ -177,11 +207,19 @@ class Camera:
 
 class Scene:
     def __init__(self, source_path: str, model_path: str = "", eval: bool = True, shuffle: bool = True, device="cuda",
-                 data_device=None, use_offDetector: bool = False, offDetector_u: float | None = None):
+                 data_device=None, use_offDetector: bool = False, offDetector_u: float | None = None,
+                 use_view_geometry: bool = False):
         """`offDetector_u` (scene units) replaces the scanner's offDetector[0] in a copy of its config, the one every
-        camera and `scanner_cfg` then carry (with `use_offDetector`, e.g. an estimated offset)."""
+        camera and `scanner_cfg` then carry (with `use_offDetector`, e.g. an estimated offset).  `use_view_geometry`
+        builds every camera from its frame's per-view DSO, DSD, offOrigin and offDetector (`scene.view_scanner`) and
+        implies `use_offDetector`; `scanner_cfg`, `bbox` and the grid stay the scanner's."""
+        if use_view_geometry and offDetector_u is not None:
+            raise ValueError("Scene: offDetector_u (an estimated offset of one fixed circle) cannot be combined with "
+                             "use_view_geometry")
+        use_offDetector = bool(use_offDetector or use_view_geometry)
+        self.use_view_geometry = bool(use_view_geometry)
         self.model_path = model_path
-        info = read_scene(source_path, eval)
+        info = read_scene(source_path, eval, use_view_geometry)
         if offDetector_u is not None:
             from .detector import with_offDetector_u
             info.scanner_cfg = with_offDetector_u(info.scanner_cfg, offDetector_u)
@@ -235,15 +273,16 @@ def init_point_cloud(scanner_cfg: dict, n_points: int, recon: np.ndarray | None 
 
 def write_blender(path: str, scanner: dict, train: list, test: list, vol: np.ndarray):
     """Write a scene in the reference's directory format.  `train` / `test`: lists of (angle, projection[H,W]) in
-    the scanner's own (unscaled) units; `scanner` as in `data_generator/synthetic_dataset/scanner/*.yml`."""
+    the scanner's own (unscaled) units, or (angle, projection, overrides) with a dict of the frame's per-view geometry
+    (`scene.VIEW_KEYS`, unscaled); `scanner` as in `data_generator/synthetic_dataset/scanner/*.yml`."""
     os.makedirs(path, exist_ok=True)
     meta = {"scanner": scanner, "vol": "vol_gt.npy", "bbox": [[-1, -1, -1], [1, 1, 1]], "proj_train": [], "proj_test": []}
     np.save(os.path.join(path, "vol_gt.npy"), np.asarray(vol, dtype=np.float32))
     for split, frames in (("train", train), ("test", test)):
         os.makedirs(os.path.join(path, "proj_" + split), exist_ok=True)
-        for i, (angle, proj) in enumerate(frames):
+        for i, (angle, proj, *overrides) in enumerate(frames):
             rel = os.path.join("proj_" + split, f"proj_{split}_{i:04d}.npy")
             np.save(os.path.join(path, rel), np.asarray(proj, dtype=np.float32))
-            meta["proj_" + split].append({"file_path": rel, "angle": float(angle)})
+            meta["proj_" + split].append({"file_path": rel, "angle": float(angle), **(overrides[0] if overrides else {})})
     with open(os.path.join(path, "meta_data.json"), "w") as f:
         json.dump(meta, f, indent=1)

@@ -36,6 +36,12 @@ detector is shifted sideways to widen the field of view: rays near the axis are 
 and Wang's (2002) redundancy weights (`half_fan_weight`) give each its share, where the plain FDK would reconstruct the
 outer part at about half its density.  It refuses a centred axis, an axis not strictly inside the detector, views that
 do not cover a full circle and a short scan.  The float64 statement is tests/offset_detector_oracle.py.
+
+`view_geometry=` (one dict per view, as for `projector.project`) reconstructs a calibrated circle whose DSO, DSD and
+offDetector are measured per view (r2x_fdk_views: each view's cosine weight, isocentre pitch and (DSO / z)^2 weight
+from its own row of the table).  It implies `use_offDetector`.  FDK has no helical weighting, so a table whose
+offOrigin varies between views (a helical scan) is refused, as are `short_scan` and `half_fan`: cgls, sart, fista_tv
+and cp_tv (`recon`) are exact for any geometry.
 """
 from __future__ import annotations
 
@@ -46,7 +52,7 @@ import numpy as np
 import torch
 
 from ._lib import check, load
-from .scene import MODE_CONE, detector_shift, make_view
+from .scene import MODE_CONE, detector_shift, make_view, view_scanner
 
 # the scanner filters fdk reconstructs without its `filter` keyword
 SUPPORTED_FILTERS = (None, "ram_lak")
@@ -140,9 +146,31 @@ def check_filter(filter, scanner_cfg: dict) -> str:
     raise ValueError(f"fdk: the scanner's filter {filt!r} is not supported (supported: null, {', '.join(FILTERS)})")
 
 
+def helical(scanner_cfg: dict, view_geometry) -> bool:
+    """Whether the volume's position offOrigin varies between the views of a per-view geometry."""
+    pos = np.array([view_scanner(scanner_cfg, g or {}).get("offOrigin_view", scanner_cfg["offOrigin"])
+                    for g in view_geometry], np.float64).reshape(-1, 3)
+    return bool(len(pos) and np.any(pos != pos[0]))
+
+
+def check_view_geometry(scanner_cfg: dict, view_geometry, short_scan: bool = False, half_fan: bool = False):
+    """The refusals of fdk's per-view geometry: Parker or half-fan weights, and an offOrigin that varies between
+    views (no helical weighting)."""
+    for flag, on in (("short_scan", short_scan), ("half_fan", half_fan)):
+        if on:
+            raise ValueError(f"fdk: {flag} cannot be combined with view_geometry (its redundancy weights assume one fixed "
+                             "circle)")
+    if helical(scanner_cfg, view_geometry):
+        raise ValueError("fdk: the views' offOrigin varies (a helical scan) and FDK has no helical weighting: "
+                         "reconstruct with cgls, sart, fista_tv or cp_tv, which are exact for any geometry")
+
+
 def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool = False, use_offDetector: bool = False,
-        half_fan: bool = False, filter: str | None = None) -> torch.Tensor:
+        half_fan: bool = False, filter: str | None = None, view_geometry=None) -> torch.Tensor:
     filt = check_filter(filter, scanner_cfg)
+    if view_geometry is not None:
+        check_view_geometry(scanner_cfg, view_geometry, short_scan, half_fan)
+        use_offDetector = True
     if half_fan and not use_offDetector:
         raise ValueError("fdk: half_fan needs use_offDetector=True (the half-fan weights follow the detector offset)")
     if half_fan and short_scan:
@@ -176,7 +204,12 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool =
         raise ValueError(f"fdk: projections are {H}x{W}, scanner nDetector is {list(scanner_cfg['nDetector'])}")
     if N == 0:
         raise ValueError("fdk: no projections")
-    views = [make_view(scanner_cfg, float(a), use_offDetector) for a in angles]
+    table = None
+    if view_geometry is not None:
+        from .projector import view_table
+        views, table = view_table(angles, scanner_cfg, view_geometry)
+    else:
+        views = [make_view(scanner_cfg, float(a), use_offDetector) for a in angles]
     mode = views[0].mode
     weighting, view_weights, arc = (R2X_FDK_HALF_FAN if half_fan else R2X_FDK_PLAIN), None, 0.0
     if short_scan:
@@ -196,9 +229,15 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool =
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
         vw = None if view_weights is None else torch.from_numpy(view_weights.astype(np.float32)).to(dev)
-        rc = lib.r2x_fdk(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), float(views[0].tanfovx),
-                         float(views[0].tanfovy), int(mode), t_u, t_v, weighting | (FILTERS.index(filt) << 8),
-                         None if vw is None else vw.data_ptr(), float(arc), float(scanner_cfg["DSO"]), nx, ny, nz, sx,
-                         sy, sz, cx, cy, cz, vol.data_ptr(), scratch.data_ptr(), nbytes)
+        if table is not None:
+            table_dev = torch.from_numpy(table).to(dev)
+            rc = lib.r2x_fdk_views(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), int(mode),
+                                   weighting | (FILTERS.index(filt) << 8), nx, ny, nz, sx, sy, sz, cx, cy, cz,
+                                   table_dev.data_ptr(), table.ctypes.data, vol.data_ptr(), scratch.data_ptr(), nbytes)
+        else:
+            rc = lib.r2x_fdk(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), float(views[0].tanfovx),
+                             float(views[0].tanfovy), int(mode), t_u, t_v, weighting | (FILTERS.index(filt) << 8),
+                             None if vw is None else vw.data_ptr(), float(arc), float(scanner_cfg["DSO"]), nx, ny, nz,
+                             sx, sy, sz, cx, cy, cz, vol.data_ptr(), scratch.data_ptr(), nbytes)
     check(rc, "r2x_fdk")
     return vol

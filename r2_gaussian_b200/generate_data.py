@@ -1,7 +1,7 @@
 """Synthetic CT scene from a volume -- the reference's `data_generator/synthetic_dataset/generate_data.py`.
 
     python -m r2_gaussian_b200.generate_data --vol X.npy --scanner cone_beam.yml --output DIR
-        [--n_train 50] [--n_test 100] [--seed 0] [--use_offDetector]
+        [--n_train 50] [--n_test 100] [--seed 0] [--use_offDetector] [--helical_travel Z | --view_geometry FILE.json]
 
 Reads the scanner configuration (the reference's yml format), projects the volume on the GPU with
 `projector.project` (the reference uses TIGRE's `Ax`) at the train angles linspace(0, totalAngle, n_train + 1)[:-1]
@@ -17,6 +17,17 @@ generator; the projector is defined by render()'s geometry, not bit-identical to
 `scene.detector_shift`'s).  The reference's real-data generator takes the same offset on its command line; here it is
 the scanner file's `offDetector` ([u, v], in the file's units), written unchanged into `meta_data.json`, so the scene
 is then reconstructed and trained with the same switch.
+
+Per-view geometry (`scene.view_scanner`; the scene is then used with `--use_view_geometry`):
+  * `--helical_travel Z` moves the volume along the rotation axis during the train arc, a helical scan:
+    offOrigin_z(beta) = offOrigin_z + Z ((beta - startAngle) / totalAngle - 1/2), in the scanner file's units, with
+    totalAngle free to exceed 360 (several turns).  The test angles are drawn over the same arc, and every frame is
+    written with its `offOrigin`.
+  * `--view_geometry FILE.json` takes any other table, e.g. a calibration: {"train": [...], "test": [...]} with one
+    dict per view of `scene.VIEW_KEYS` overrides (DSO, DSD, offOrigin [x, y, z], offDetector [u, v]; file units).
+    Each list must hold --n_train / --n_test entries.  The frames are written with their overrides.
+Either projects through the per-view table (`projector.project(..., view_geometry=...)`), which implies
+`--use_offDetector`.
 """
 from __future__ import annotations
 
@@ -48,6 +59,45 @@ def train_angles(cfg: dict, n_train: int) -> np.ndarray:
 
 def draw_test_angles(cfg: dict, n_test: int, rng: np.random.RandomState) -> np.ndarray:
     return np.sort(rng.rand(n_test) * 2.0 * np.pi) + cfg["startAngle"] / 180 * np.pi    # the full circle, always
+
+
+def helical_offsets(cfg: dict, angles, travel: float) -> list[dict]:
+    """{"offOrigin": [x, y, z]} per angle (radians) of a helical scan: the scanner's offOrigin with z moved by
+    travel ((beta - startAngle) / totalAngle - 1/2), beta the angle in degrees."""
+    off = [float(v) for v in cfg.get("offOrigin", [0.0, 0.0, 0.0])]
+    frac = (np.degrees(np.asarray(angles, np.float64)) - float(cfg["startAngle"])) / float(cfg["totalAngle"]) - 0.5
+    return [{"offOrigin": [off[0], off[1], off[2] + float(travel) * float(f)]} for f in frac]
+
+
+def draw_arc_angles(cfg: dict, n_test: int, rng: np.random.RandomState) -> np.ndarray:
+    """n_test sorted random angles (radians) over the train arc [startAngle, startAngle + totalAngle)."""
+    return np.sort(rng.rand(n_test) * (cfg["totalAngle"] / 180 * np.pi)) + cfg["startAngle"] / 180 * np.pi
+
+
+def read_view_geometry(path: str, n_train: int, n_test: int) -> dict:
+    """The {"train": [...], "test": [...]} override file of --view_geometry, after the refusals."""
+    import json
+
+    from .scene import VIEW_KEYS
+
+    with open(path) as f:
+        table = json.load(f)
+    if not isinstance(table, dict) or set(table) != {"train", "test"}:
+        raise SystemExit(f"--view_geometry {path}: expected an object with the keys 'train' and 'test'")
+    for split, n in (("train", n_train), ("test", n_test)):
+        rows = table[split]
+        if not isinstance(rows, list) or len(rows) != n:
+            raise SystemExit(f"--view_geometry {path}: {split} holds {len(rows) if isinstance(rows, list) else '?'} "
+                             f"entries, --n_{split} is {n}")
+        for i, row in enumerate(rows):
+            unknown = sorted(set(row) - set(VIEW_KEYS)) if isinstance(row, dict) else ["(not an object)"]
+            if unknown:
+                raise SystemExit(f"--view_geometry {path}: {split}[{i}] has unknown keys {unknown} "
+                                 f"(supported: {', '.join(VIEW_KEYS)})")
+            for k, size in (("offOrigin", 3), ("offDetector", 2)):
+                if k in row and np.asarray(row[k]).shape != (size,):
+                    raise SystemExit(f"--view_geometry {path}: {split}[{i}].{k} must hold {size} numbers")
+    return table
 
 
 def shift_projections(case_path: str, columns: int, empty: float = 1e-6) -> None:
@@ -91,18 +141,28 @@ def main(argv=None) -> str:
     ap.add_argument("--seed", default=0, type=int, help="Seed of the noise and of the test angles.")
     ap.add_argument("--use_offDetector", default=False, action="store_true",
                     help="Project through the scanner's offDetector (else a non-zero offDetector is refused).")
+    ap.add_argument("--helical_travel", default=None, type=float,
+                    help="Move the volume this far along z (scanner units) over the train arc: a helical scan.")
+    ap.add_argument("--view_geometry", default=None, type=str,
+                    help="JSON file {\"train\": [...], \"test\": [...]} of per-view DSO, DSD, offOrigin, offDetector.")
     a = ap.parse_args(argv)
 
     import torch
     import yaml
 
-    from .dataset import scale_scanner, write_blender
+    from .dataset import frame_geometry, scale_scanner, write_blender
     from .projector import project
 
     with open(a.scanner) as f:
         cfg = yaml.safe_load(f)
+    if a.helical_travel is not None and a.view_geometry is not None:
+        raise SystemExit("--helical_travel and --view_geometry cannot be combined: give the helix in the file")
+    if a.helical_travel is not None and not np.isfinite(a.helical_travel):
+        raise SystemExit(f"--helical_travel must be finite, got {a.helical_travel}")
+    table = read_view_geometry(a.view_geometry, a.n_train, a.n_test) if a.view_geometry else None
+    per_view = table is not None or a.helical_travel is not None
     off = [float(v) for v in cfg.get("offDetector", [0.0, 0.0])]
-    if any(v != 0.0 for v in off) and not a.use_offDetector:
+    if any(v != 0.0 for v in off) and not (a.use_offDetector or per_view):
         raise SystemExit(f"the scanner's offDetector is {off}: pass --use_offDetector to project through the offset "
                          "detector (and use it again to reconstruct and train on the scene)")
     if not torch.cuda.is_available():
@@ -121,14 +181,31 @@ def main(argv=None) -> str:
 
     dvol = torch.from_numpy(vol).cuda()
     angles_train = train_angles(cfg, a.n_train)
-    projs_train = (project(dvol, angles_train, scaled, a.use_offDetector) / scene_scale).cpu().numpy()
+    rows = {"train": table["train"] if table else None, "test": table["test"] if table else None}
+    if a.helical_travel is not None:
+        rows["train"] = helical_offsets(cfg, angles_train, a.helical_travel)
+
+    def views(split):   # the split's overrides in scene units (frame_geometry), or None: the scalar path
+        return None if rows[split] is None else [frame_geometry(r, scene_scale) for r in rows[split]]
+
+    projs_train = (project(dvol, angles_train, scaled, a.use_offDetector, views("train")) / scene_scale).cpu().numpy()
     if cfg.get("noise", False):
         projs_train = add_noise(projs_train, cfg["possion_noise"], cfg["gaussian_noise"], rng)
-    angles_test = draw_test_angles(cfg, a.n_test, rng)
-    projs_test = (project(dvol, angles_test, scaled, a.use_offDetector) / scene_scale).cpu().numpy()
+    if a.helical_travel is not None:
+        angles_test = draw_arc_angles(cfg, a.n_test, rng)
+        rows["test"] = helical_offsets(cfg, angles_test, a.helical_travel)
+    else:
+        angles_test = draw_test_angles(cfg, a.n_test, rng)
+    projs_test = (project(dvol, angles_test, scaled, a.use_offDetector, views("test")) / scene_scale).cpu().numpy()
+
+    def frames(angles, projs, split):
+        if rows[split] is None:
+            return list(zip(angles, projs))
+        return list(zip(angles, projs, rows[split]))
 
     case_path = os.path.join(a.output, case_name)
-    write_blender(case_path, cfg, list(zip(angles_train, projs_train)), list(zip(angles_test, projs_test)), vol)
+    write_blender(case_path, cfg, frames(angles_train, projs_train, "train"), frames(angles_test, projs_test, "test"),
+                  vol)
     print(f"Generate data for case {case_name} complete!")
     return case_path
 

@@ -16,6 +16,10 @@ definition is in include/r2x.h.  A scanner whose `offDetector` is not zero is re
 which projects through the offset detector (the shift_u / shift_v of r2x_volume_project / r2x_volume_backproject,
 TIGRE's `geo.offDetector`; the convention is `scene.detector_shift`'s) and matches a render() whose cameras carry the
 same offset (`dataset.Scene(use_offDetector=True)`, `scene.make_view(..., use_offDetector=True)`).
+`view_geometry=` (one dict per angle: a projection frame's overrides in scene units, `CameraInfo.view_geometry`, or a
+`scene.view_scanner` dict) gives every view its own DSO, DSD, offOrigin and offDetector, as a helical scan or a
+calibrated bench measures them; it implies `use_offDetector` and runs the `_views` entry points with the per-view table
+of `view_table`.  Without it the scalar entry points run as before.
 `backproject` sums every (ray, sample, voxel) triple `project` uses, with the same
 weight, so <project(x), y> = <x, backproject(y)> up to float32 rounding.  Both run on the current stream; no CPU
 fallback.  `CTOperator` binds the pair to one set of angles for repeated use (the iterative solvers).
@@ -26,7 +30,7 @@ import numpy as np
 import torch
 
 from ._lib import check, load
-from .scene import detector_shift, make_view
+from .scene import detector_shift, make_view, view_scanner
 
 DEFAULT_ACCURACY = 0.5
 
@@ -50,18 +54,42 @@ def _check_geometry(what: str, scanner_cfg: dict, use_offDetector: bool = False)
     return accuracy
 
 
-def project(volume: torch.Tensor, angles, scanner_cfg: dict, use_offDetector: bool = False) -> torch.Tensor:
+def view_table(angles, scanner_cfg: dict, view_geometry) -> tuple[list, np.ndarray]:
+    """(views, table) of a per-view geometry: each angle's `scene.make_view` of `scene.view_scanner(scanner_cfg, g)`
+    with its detector offset, and the float64 [N, 5] table of the `_views` entry points (include/r2x.h): tan_fovx,
+    tan_fovy, shift_u, shift_v (`scene.detector_shift` of the view) and DSO.  Refuses a length mismatch and values the
+    entry points would refuse."""
+    angles = np.asarray(angles, dtype=np.float64).reshape(-1)
+    view_geometry = list(view_geometry)
+    if len(view_geometry) != len(angles):
+        raise ValueError(f"view_geometry: {len(view_geometry)} entries for {len(angles)} angles")
+    cfgs = [view_scanner(scanner_cfg, g or {}) for g in view_geometry]
+    views = [make_view(c, float(a), True) for c, a in zip(cfgs, angles)]
+    table = np.array([[v.tanfovx, v.tanfovy, *detector_shift(c), float(c["DSO"])] for v, c in zip(views, cfgs)],
+                     dtype=np.float64).reshape(-1, 5)
+    for c in cfgs:
+        off, pos = c.get("offDetector", [0.0, 0.0]), c.get("offOrigin_view", c["offOrigin"])
+        if not np.all(np.isfinite(np.asarray([c["DSO"], c["DSD"], *off, *pos], np.float64))):
+            raise ValueError(f"view_geometry: values must be finite, got DSO {c['DSO']}, DSD {c['DSD']}, offDetector "
+                             f"{off}, offOrigin {pos}")
+        if c["mode"] == "cone" and not (float(c["DSO"]) > 0.0 and float(c["DSD"]) > 0.0):
+            raise ValueError(f"view_geometry: cone beam needs DSO > 0 and DSD > 0, got {c['DSO']} and {c['DSD']}")
+    return views, np.ascontiguousarray(table)
+
+
+def project(volume: torch.Tensor, angles, scanner_cfg: dict, use_offDetector: bool = False,
+            view_geometry=None) -> torch.Tensor:
     nvox = tuple(int(v) for v in scanner_cfg["nVoxel"])
     if tuple(getattr(volume, "shape", ())) != nvox:
         raise ValueError(f"project: volume shape {tuple(getattr(volume, 'shape', ()))} is not the scanner's nVoxel "
                          f"{list(nvox)}")
-    _check_geometry("project", scanner_cfg, use_offDetector)
+    _check_geometry("project", scanner_cfg, use_offDetector or view_geometry is not None)
     if not isinstance(volume, torch.Tensor) or volume.device.type != "cuda":
         raise RuntimeError("project: volume must be a CUDA tensor (this build has no CPU fallback; "
                            f"got {getattr(volume, 'device', type(volume))})")
     if np.asarray(angles, dtype=np.float64).size == 0:
         raise ValueError("project: no angles")
-    return CTOperator(angles, scanner_cfg, volume.device, use_offDetector).A(volume)
+    return CTOperator(angles, scanner_cfg, volume.device, use_offDetector, view_geometry).A(volume)
 
 
 class CTOperator:
@@ -70,14 +98,19 @@ class CTOperator:
     the angle list) and `At(y, views, weights)` backprojects their [n, H, W] projections, returning (A_views^T y,
     A_views^T 1) when `weights` is true.  Inputs are used as float32 contiguous tensors on the operator's device.
     `use_offDetector` binds the offset-detector pair (both directions, and the offset projmatrices the backprojector's
-    footprints need)."""
+    footprints need).  `view_geometry` binds the per-view pair (`view_table`; implies `use_offDetector`)."""
 
-    def __init__(self, angles, scanner_cfg: dict, device, use_offDetector: bool = False):
+    def __init__(self, angles, scanner_cfg: dict, device, use_offDetector: bool = False, view_geometry=None):
+        use_offDetector = use_offDetector or view_geometry is not None
         accuracy = _check_geometry("backproject", scanner_cfg, use_offDetector)
         angles = np.asarray(angles, dtype=np.float64).reshape(-1)
         if len(angles) == 0:
             raise ValueError("backproject: no angles")
-        views = [make_view(scanner_cfg, float(a), use_offDetector) for a in angles]
+        self.table = None
+        if view_geometry is not None:
+            views, self.table = view_table(angles, scanner_cfg, view_geometry)
+        else:
+            views = [make_view(scanner_cfg, float(a), use_offDetector) for a in angles]
         self.shift = detector_shift(scanner_cfg) if use_offDetector else (0.0, 0.0)
         self.device = torch.device(device)
         self.nvox = tuple(int(v) for v in scanner_cfg["nVoxel"])
@@ -88,7 +121,13 @@ class CTOperator:
         self.mode, self.tanx, self.tany = int(views[0].mode), float(views[0].tanfovx), float(views[0].tanfovy)
         self.vm = torch.from_numpy(np.stack([v.viewmatrix.reshape(16) for v in views])).to(self.device)
         self.pm = torch.from_numpy(np.stack([v.projmatrix.reshape(16) for v in views])).to(self.device)
+        if self.table is not None:
+            self.table_dev = torch.from_numpy(self.table).to(self.device)
         self.lib = load()
+
+    def _table(self, v0: int):
+        """(device, host) pointers of the per-view table from view v0."""
+        return self.table_dev[v0].data_ptr(), self.table.ctypes.data + v0 * self.table.strides[0]
 
     def _views(self, views: slice) -> tuple[int, int]:
         v0, v1, stride = views.indices(self.N)
@@ -104,9 +143,14 @@ class CTOperator:
                 raise ValueError(f"project: volume shape {tuple(vol.shape)} is not the scanner's nVoxel {list(self.nvox)}")
             out = torch.empty((n, self.H, self.W), dtype=torch.float32, device=self.device)
             stream = torch.cuda.current_stream(self.device).cuda_stream
-            rc = self.lib.r2x_volume_project(stream, *self.nvox, vol.data_ptr(), *self.size, *self.centre, n, self.H,
-                                             self.W, self.vm[v0].data_ptr(), self.tanx, self.tany, self.mode,
-                                             *self.shift, self.step, out.data_ptr())
+            if self.table is not None:
+                rc = self.lib.r2x_volume_project_views(stream, *self.nvox, vol.data_ptr(), *self.size, *self.centre, n,
+                                                       self.H, self.W, self.vm[v0].data_ptr(), self.mode, self.step,
+                                                       *self._table(v0), out.data_ptr())
+            else:
+                rc = self.lib.r2x_volume_project(stream, *self.nvox, vol.data_ptr(), *self.size, *self.centre, n,
+                                                 self.H, self.W, self.vm[v0].data_ptr(), self.tanx, self.tany,
+                                                 self.mode, *self.shift, self.step, out.data_ptr())
         check(rc, "r2x_volume_project")
         return out
 
@@ -122,18 +166,27 @@ class CTOperator:
             nbytes = int(self.lib.r2x_volume_backproject_scratch_bytes(n, self.H, self.W))
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
             stream = torch.cuda.current_stream(self.device).cuda_stream
-            rc = self.lib.r2x_volume_backproject(stream, n, self.H, self.W, projs.data_ptr(), self.vm[v0].data_ptr(),
-                                                 self.pm[v0].data_ptr(), self.tanx, self.tany, self.mode, *self.shift,
-                                                 *self.nvox, *self.size, *self.centre, self.step, vol.data_ptr(),
-                                                 wgt.data_ptr() if weights else None, scratch.data_ptr(), nbytes)
+            if self.table is not None:
+                rc = self.lib.r2x_volume_backproject_views(stream, n, self.H, self.W, projs.data_ptr(),
+                                                           self.vm[v0].data_ptr(), self.pm[v0].data_ptr(), self.mode,
+                                                           *self.nvox, *self.size, *self.centre, self.step,
+                                                           *self._table(v0), vol.data_ptr(),
+                                                           wgt.data_ptr() if weights else None, scratch.data_ptr(),
+                                                           nbytes)
+            else:
+                rc = self.lib.r2x_volume_backproject(stream, n, self.H, self.W, projs.data_ptr(),
+                                                     self.vm[v0].data_ptr(), self.pm[v0].data_ptr(), self.tanx,
+                                                     self.tany, self.mode, *self.shift, *self.nvox, *self.size,
+                                                     *self.centre, self.step, vol.data_ptr(),
+                                                     wgt.data_ptr() if weights else None, scratch.data_ptr(), nbytes)
         check(rc, "r2x_volume_backproject")
         return (vol, wgt) if weights else vol
 
 
 def backproject(projections: torch.Tensor, angles, scanner_cfg: dict, weights: bool = False,
-                use_offDetector: bool = False):
-    """A^T projections for the projector of `project(., angles, scanner_cfg, use_offDetector)`: [nx, ny, nz], or
-    (volume, A^T 1) when `weights` is true."""
+                use_offDetector: bool = False, view_geometry=None):
+    """A^T projections for the projector of `project(., angles, scanner_cfg, use_offDetector, view_geometry)`:
+    [nx, ny, nz], or (volume, A^T 1) when `weights` is true."""
     shape = tuple(getattr(projections, "shape", ()))
     if len(shape) != 3:
         raise ValueError(f"backproject: expected projections of shape [N, H, W], got {shape}")
@@ -143,8 +196,9 @@ def backproject(projections: torch.Tensor, angles, scanner_cfg: dict, weights: b
     det = (int(scanner_cfg["nDetector"][0]), int(scanner_cfg["nDetector"][1]))
     if shape[1:] != det:
         raise ValueError(f"backproject: projections are {shape[1]}x{shape[2]}, scanner nDetector is {list(det)}")
-    _check_geometry("backproject", scanner_cfg, use_offDetector)
+    _check_geometry("backproject", scanner_cfg, use_offDetector or view_geometry is not None)
     if not isinstance(projections, torch.Tensor) or projections.device.type != "cuda":
         raise RuntimeError("backproject: projections must be a CUDA tensor (this build has no CPU fallback; "
                            f"got {getattr(projections, 'device', type(projections))})")
-    return CTOperator(angles, scanner_cfg, projections.device, use_offDetector).At(projections, slice(None), weights)
+    return CTOperator(angles, scanner_cfg, projections.device, use_offDetector, view_geometry).At(projections,
+                                                                                                 slice(None), weights)

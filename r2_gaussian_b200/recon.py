@@ -73,6 +73,7 @@ their adaptive step and stop rules are defined by TIGRE's implementation.  `cp_t
 
     python -m r2_gaussian_b200.recon -s <scene> -m <output> [--methods fdk,sart,cgls] [--short_scan]
         [--use_offDetector] [--estimate_offDetector] [--half_fan] [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
+        [--use_view_geometry]
 
 mirrors `scripts/run_traditional_methods.py`: it reconstructs the scene's train views with each method, scores the
 volume against `vol_gt` with `metrics.metric_vol` and writes, per method, `<output>/<method>/ct_gt.npy`, `ct_pred.npy`,
@@ -91,7 +92,10 @@ those flags are on.  `--estimate_offDetector` measures the horizontal detector o
 test-view projections, with a copy of the scanner whose offDetector[0] is that total; `--half_fan` then needs no
 `--use_offDetector`, and the reports add `estimated_offset_px` and `offDetector_u` (the file's units).  `--fdk_filter NAME` reconstructs fdk with one of TIGRE's windowed ramp filters
 (`fdk.fdk(filter=NAME)`, overriding the scanner's `filter`); it is refused when --methods has no fdk.  Without it fdk
-refuses a scanner whose `filter` names a window.
+refuses a scanner whose `filter` names a window.  `--use_view_geometry` reconstructs and reprojects every method
+through each view's own DSO, DSD, offOrigin and offDetector (the frames' keys, `scene.view_scanner`; reports add
+`use_view_geometry: true`); fdk then refuses a helical scan (an offOrigin that varies), and the flag is refused with
+--estimate_offDetector, --half_fan and --short_scan, which assume one fixed circle.
 """
 from __future__ import annotations
 
@@ -272,38 +276,40 @@ def cp_tv_solve(b: torch.Tensor, A, At, shape, niter: int, epsilon: float, L=Non
     return x, history
 
 
-def _operator(projs, angles, scanner_cfg, use_offDetector: bool = False):
+def _operator(projs, angles, scanner_cfg, use_offDetector: bool = False, view_geometry=None):
     from .projector import CTOperator
 
     if not isinstance(projs, torch.Tensor) or projs.device.type != "cuda":
         raise RuntimeError("recon: projections must be a CUDA tensor (this build has no CPU fallback; "
                            f"got {getattr(projs, 'device', type(projs))})")
-    op = CTOperator(angles, scanner_cfg, projs.device, use_offDetector)
+    op = CTOperator(angles, scanner_cfg, projs.device, use_offDetector, view_geometry)
     b = projs.detach().to(torch.float32).contiguous()
     if tuple(b.shape) != (op.N, op.H, op.W):
         raise ValueError(f"recon: projections {list(b.shape)} do not match {op.N} angles of {op.H}x{op.W} pixels")
     return op, b
 
 
-def cgls(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = CGLS_NITER, use_offDetector: bool = False):
+def cgls(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = CGLS_NITER, use_offDetector: bool = False,
+         view_geometry=None):
     """CGLS on the GPU projector pair; returns (volume, l2 per iteration)."""
-    op, b = _operator(projs, angles, scanner_cfg, use_offDetector)
+    op, b = _operator(projs, angles, scanner_cfg, use_offDetector, view_geometry)
     return cgls_solve(b, op.A, op.At, niter)
 
 
 def sart(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = SART_NITER, lmbda: float = 1.0,
          lmbda_red: float = 0.999, blocksize: int = 1, nonneg: bool = True,
-         use_offDetector: bool = False) -> torch.Tensor:
+         use_offDetector: bool = False, view_geometry=None) -> torch.Tensor:
     """SART (blocksize 1) or OS-SART on the GPU projector pair."""
-    op, b = _operator(projs, angles, scanner_cfg, use_offDetector)
+    op, b = _operator(projs, angles, scanner_cfg, use_offDetector, view_geometry)
     return sart_solve(b, op.A, op.At, op.nvox, niter, lmbda, lmbda_red, blocksize, nonneg)
 
 
 def fista_tv(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = FISTA_NITER, lmbda: float = FISTA_LAMBDA,
-             tviter: int = FISTA_TVITER, nonneg: bool = True, L=None, use_offDetector: bool = False):
+             tviter: int = FISTA_TVITER, nonneg: bool = True, L=None, use_offDetector: bool = False,
+             view_geometry=None):
     """FISTA-TV on the GPU projector pair and the GPU TV prox; returns (volume, history)."""
     _check_fista(niter, lmbda, tviter, L)
-    op, b = _operator(projs, angles, scanner_cfg, use_offDetector)
+    op, b = _operator(projs, angles, scanner_cfg, use_offDetector, view_geometry)
     return fista_tv_solve(b, op.A, op.At, op.nvox, niter, lmbda, tviter, L, nonneg)
 
 
@@ -313,34 +319,41 @@ def _check_ratio(epsilon_ratio):
 
 
 def cp_tv_epsilon(projs: torch.Tensor, angles, scanner_cfg: dict, epsilon_ratio: float = CP_EPSILON_RATIO,
-                  use_offDetector: bool = False) -> float:
-    """epsilon_ratio |A FDK(b) - b|, the reference's asd_pocs tolerance, with this project's FDK and projector."""
-    from .fdk import fdk
+                  use_offDetector: bool = False, view_geometry=None) -> float:
+    """epsilon_ratio |A FDK(b) - b|, the reference's asd_pocs tolerance, with this project's FDK and projector.  FDK
+    has no helical weighting, so a per-view geometry whose offOrigin varies takes the CGLS volume in FDK's place."""
+    from .fdk import fdk, helical
 
     _check_ratio(epsilon_ratio)
-    op, b = _operator(projs, angles, scanner_cfg, use_offDetector)
-    r = op.A(fdk(b, angles, scanner_cfg, use_offDetector=use_offDetector)).sub_(b)
+    op, b = _operator(projs, angles, scanner_cfg, use_offDetector, view_geometry)
+    if view_geometry is not None and helical(scanner_cfg, view_geometry):
+        x0 = cgls_solve(b, op.A, op.At, CGLS_NITER)[0]
+    else:
+        x0 = fdk(b, angles, scanner_cfg, use_offDetector=use_offDetector, view_geometry=view_geometry)
+    r = op.A(x0).sub_(b)
     return float(epsilon_ratio) * _dot(r, r) ** 0.5
 
 
 def cp_tv(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = CP_NITER, epsilon=None,
-          epsilon_ratio: float = CP_EPSILON_RATIO, L=None, nonneg: bool = True, use_offDetector: bool = False):
+          epsilon_ratio: float = CP_EPSILON_RATIO, L=None, nonneg: bool = True, use_offDetector: bool = False,
+          view_geometry=None):
     """Data-constrained TV (Chambolle-Pock) on the GPU projector pair and the GPU step kernel; epsilon=None takes
     `cp_tv_epsilon(..., epsilon_ratio)`.  Returns (volume, history)."""
     _check_cp(niter, epsilon, L)
     _check_ratio(epsilon_ratio)
-    op, b = _operator(projs, angles, scanner_cfg, use_offDetector)
+    op, b = _operator(projs, angles, scanner_cfg, use_offDetector, view_geometry)
     if epsilon is None:
-        epsilon = cp_tv_epsilon(b, angles, scanner_cfg, epsilon_ratio, use_offDetector)
+        epsilon = cp_tv_epsilon(b, angles, scanner_cfg, epsilon_ratio, use_offDetector, view_geometry)
     return cp_tv_solve(b, op.A, op.At, op.nvox, niter, epsilon, L, nonneg)
 
 
 def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, short_scan: bool = False,
-                 use_offDetector: bool = False, half_fan: bool = False, fdk_filter: str | None = None) -> torch.Tensor:
+                 use_offDetector: bool = False, half_fan: bool = False, fdk_filter: str | None = None,
+                 view_geometry=None) -> torch.Tensor:
     """The reconstructions of ct_utils.recon_volume / run_ct_recon_algs with their iteration counts.  `short_scan`
     selects the Parker-weighted FDK, `half_fan` the half-fan-weighted one and `fdk_filter` FDK's ramp filter
     (`fdk.fdk(filter=...)`); all three apply to method fdk only.  `use_offDetector` reconstructs through the scanner's
-    offDetector (every method)."""
+    offDetector (every method), `view_geometry` through each view's own geometry (every method; `projector.project`)."""
     for flag, on in (("short_scan", short_scan), ("half_fan", half_fan)):
         if on and method != "fdk":
             raise ValueError(f"recon_volume: {flag} applies to fdk only, not {method!r} (the iterative methods need no "
@@ -353,17 +366,19 @@ def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, sh
         from .fdk import fdk
 
         return fdk(projs, angles, scanner_cfg, short_scan=short_scan, use_offDetector=off, half_fan=half_fan,
-                   filter=fdk_filter)
+                   filter=fdk_filter, view_geometry=view_geometry)
+    vg = view_geometry
     if method == "cgls":
-        return cgls(projs, angles, scanner_cfg, CGLS_NITER, use_offDetector=off)[0]
+        return cgls(projs, angles, scanner_cfg, CGLS_NITER, use_offDetector=off, view_geometry=vg)[0]
     if method == "sart":
-        return sart(projs, angles, scanner_cfg, SART_NITER, use_offDetector=off)
+        return sart(projs, angles, scanner_cfg, SART_NITER, use_offDetector=off, view_geometry=vg)
     if method == "ossart":
-        return sart(projs, angles, scanner_cfg, SART_NITER, blocksize=OSSART_BLOCKSIZE, use_offDetector=off)
+        return sart(projs, angles, scanner_cfg, SART_NITER, blocksize=OSSART_BLOCKSIZE, use_offDetector=off,
+                    view_geometry=vg)
     if method == "fista_tv":
-        return fista_tv(projs, angles, scanner_cfg, use_offDetector=off)[0]
+        return fista_tv(projs, angles, scanner_cfg, use_offDetector=off, view_geometry=vg)[0]
     if method == "cp_tv":
-        return cp_tv(projs, angles, scanner_cfg, use_offDetector=off)[0]
+        return cp_tv(projs, angles, scanner_cfg, use_offDetector=off, view_geometry=vg)[0]
     raise ValueError(f"recon_volume: unknown method {method!r} (supported: {', '.join(METHODS)})")
 
 
@@ -397,6 +412,31 @@ def add_estimate_flag(ap, what: str):
                          f"relative to the scanner's offDetector under --use_offDetector) and {what} through it")
 
 
+def add_view_geometry_flag(ap, what: str):
+    """--use_view_geometry on a CLI's parser."""
+    ap.add_argument("--use_view_geometry", default=False, action="store_true",
+                    help=f"{what} through each view's own DSO, DSD, offOrigin and offDetector (the projection frames' "
+                         "keys; helical scans, calibrated benches); implies --use_offDetector")
+
+
+def check_view_geometry_flags(args):
+    """The refusals of --use_view_geometry that every CLI shares; checked before any CUDA work."""
+    if not getattr(args, "use_view_geometry", False):
+        return
+    for flag, on in (("--estimate_offDetector", getattr(args, "estimate_offDetector", False)),
+                     ("--half_fan", getattr(args, "half_fan", False)),
+                     ("--short_scan", getattr(args, "short_scan", False))):
+        if on:
+            why = ("the conjugate-ray estimate assumes one fixed circle" if flag == "--estimate_offDetector" else
+                   "its redundancy weights assume one fixed circle")
+            raise SystemExit(f"{flag} cannot be combined with --use_view_geometry: {why}")
+
+
+def view_geometry_of(cameras, on: bool):
+    """The per-view geometry (`CameraInfo.view_geometry`) of `cameras` under --use_view_geometry, else None."""
+    return [c.view_geometry for c in cameras] if on else None
+
+
 def _parse_methods(text: str) -> list[str]:
     methods = [m.strip() for m in text.split(",") if m.strip()]
     for m in methods:
@@ -425,10 +465,12 @@ def main(argv=None) -> dict:
                          "the detector shifted sideways)")
     add_fdk_filter_flag(ap, "reconstruct fdk with this ramp filter")
     add_estimate_flag(ap, "reconstruct and reproject every method")
+    add_view_geometry_flag(ap, "reconstruct and reproject every method")
     a = ap.parse_args(argv)
     methods = _parse_methods(a.methods)
     check_fdk_flags(a, "fdk" in methods, "{flag} applies to the fdk method, which --methods does not include (the "
                     "iterative methods need no redundancy weights)")
+    check_view_geometry_flags(a)
     if not torch.cuda.is_available():
         raise SystemExit("the reconstructions need a CUDA device: they run on the GPU and have no CPU fallback")
     import yaml
@@ -438,13 +480,15 @@ def main(argv=None) -> dict:
     from .projector import project
 
     source = os.path.abspath(a.source_path)
-    info = read_scene(source, eval=True)
+    info = read_scene(source, eval=True, use_view_geometry=a.use_view_geometry)
     cfg = info.scanner_cfg
+    vg_train = view_geometry_of(info.train_cameras, a.use_view_geometry)
+    vg_test = view_geometry_of(info.test_cameras, a.use_view_geometry)
     projs_train = torch.from_numpy(np.stack([np.asarray(c.image, np.float32) for c in info.train_cameras])).cuda()
     train_angles = [c.angle for c in info.train_cameras]
     test_angles = [c.angle for c in info.test_cameras]
     vol_gt = np.asarray(info.vol, np.float32)
-    use_off, estimate = a.use_offDetector, None
+    use_off, estimate = a.use_offDetector or a.use_view_geometry, None
     if a.estimate_offDetector:
         from .estimate_offset import estimated_scanner
         cfg, estimate = estimated_scanner(info, a.use_offDetector)
@@ -462,12 +506,14 @@ def main(argv=None) -> dict:
         fdk_filter = a.fdk_filter if method == "fdk" else None
         extra = {}
         if method == "cp_tv":
-            eps = cp_tv_epsilon(projs_train, train_angles, cfg, use_offDetector=use_off)
-            pred, hist = cp_tv(projs_train, train_angles, cfg, epsilon=eps, use_offDetector=use_off)
+            eps = cp_tv_epsilon(projs_train, train_angles, cfg, use_offDetector=use_off, view_geometry=vg_train)
+            pred, hist = cp_tv(projs_train, train_angles, cfg, epsilon=eps, use_offDetector=use_off,
+                               view_geometry=vg_train)
             extra = {"epsilon": eps, "residual": hist[-1]["residual"]}
         else:
             pred = recon_volume(projs_train, train_angles, cfg, method, short_scan=short_scan,
-                                use_offDetector=use_off, half_fan=half_fan, fdk_filter=fdk_filter)
+                                use_offDetector=use_off, half_fan=half_fan, fdk_filter=fdk_filter,
+                                view_geometry=vg_train)
         torch.cuda.synchronize()
         duration = time.time() - t0
         ct_pred = pred.cpu().numpy()
@@ -486,6 +532,8 @@ def main(argv=None) -> dict:
             report["filter"] = fdk_filter
         if a.use_offDetector:
             report["use_offDetector"] = True
+        if a.use_view_geometry:
+            report["use_view_geometry"] = True
         if estimate is not None:
             report["estimated_offset_px"] = estimate["offset_px"]
             report["offDetector_u"] = estimate["offDetector_u"] / info.scene_scale
@@ -493,7 +541,7 @@ def main(argv=None) -> dict:
         with open(os.path.join(save, "eval_3d.yml"), "w") as f:
             yaml.dump(report, f, default_flow_style=False, sort_keys=False)
         if test_angles:
-            render = project(pred, test_angles, cfg, use_offDetector=use_off).cpu().numpy()
+            render = project(pred, test_angles, cfg, use_offDetector=use_off, view_geometry=vg_test).cpu().numpy()
             for i, cam in enumerate(info.test_cameras):
                 np.save(os.path.join(save, "projs", f"{i:05d}_render.npy"), render[i])
                 np.save(os.path.join(save, "projs", f"{i:05d}_gt.npy"), np.asarray(cam.image, np.float32))

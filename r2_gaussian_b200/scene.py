@@ -121,12 +121,45 @@ class View:
     FoVy: float = 0.0
 
 
+# the keys a projection frame of meta_data.json may carry to override the scanner for that view (scanner units)
+VIEW_KEYS = ("DSO", "DSD", "offOrigin", "offDetector")
+
+
+def view_scanner(scanner: dict, frame: dict) -> dict:
+    """The scanner of one view: a copy of `scanner` with the frame's `VIEW_KEYS` overrides.  `DSO`, `DSD` and
+    `offDetector` replace the scanner's.  The frame's `offOrigin` is where the volume sits during the view (TIGRE's
+    per-angle `geo.offOrigin`); the reconstruction grid stays at the scanner's `offOrigin`, so it goes to
+    `offOrigin_view` and `camera_pose` translates the camera by offOrigin - offOrigin_view.  A view_scanner dict is a
+    valid frame: its own `offOrigin_view` (else `offOrigin`) is taken as the view's."""
+    cfg = dict(scanner)
+    for k in ("DSO", "DSD"):
+        if k in frame:
+            cfg[k] = float(frame[k])
+    if "offDetector" in frame:
+        cfg["offDetector"] = [float(v) for v in frame["offDetector"]]
+    pos = frame.get("offOrigin_view", frame.get("offOrigin"))
+    if pos is not None:
+        cfg["offOrigin_view"] = [float(v) for v in pos]
+    return cfg
+
+
+def camera_pose(scanner: dict, angle: float) -> np.ndarray:
+    """Camera-to-world of the view at `angle`: `angle2pose` at the scanner's DSO, translated by offOrigin -
+    offOrigin_view when `view_scanner` set a volume position (a zero translation changes no bit)."""
+    c2w = angle2pose(scanner["DSO"], angle)
+    if "offOrigin_view" in scanner:
+        t = (np.asarray(scanner["offOrigin"], np.float64) - np.asarray(scanner["offOrigin_view"], np.float64))
+        if np.any(t != 0.0):
+            c2w[:3, 3] += t
+    return c2w
+
+
 def make_view(scanner: dict, angle: float, use_offDetector: bool = False) -> View:
     """The view at `angle`.  `use_offDetector` puts the scanner's offDetector into the projection matrix
     (`detector_shift`, `shifted_projection_matrix`); off, or with a zero offset, the view is bit for bit the centred
-    one."""
+    one.  A `view_scanner` dict gives that view's camera (`camera_pose`)."""
     mode = MODE_CONE if scanner["mode"] == "cone" else MODE_PARALLEL
-    c2w = angle2pose(scanner["DSO"], angle)
+    c2w = camera_pose(scanner, angle)
     w2c = np.linalg.inv(c2w)
     R = w2c[:3, :3].T  # stored transposed, dataset_readers.py:123-125
     T = w2c[:3, 3]

@@ -4,7 +4,7 @@
         [--skip_render_test] [--skip_recon] [--quiet]
 
 Settings come from what `trainer` recorded: `<model>/cfg_args.json`, plus the run options only the flat
-`<model>/cfg_args` carries (such as `use_offDetector`); without the JSON, `cfg_args` alone, the `Namespace(...)` repr,
+`<model>/cfg_args` carries (such as `use_offDetector` and `use_view_geometry`); without the JSON, `cfg_args` alone, the `Namespace(...)` repr,
 read with `ast` (never evaluated).  Options given on the command line win over the file.  `--iteration -1` loads the
 largest N among `<model>/point_cloud/iteration_N/` (the reference's `searchForMaxIteration`).
 
@@ -40,7 +40,7 @@ import numpy as np
 
 from .trainer import ModelParams, PipelineParams
 
-SETTING_FLAGS = ("source_path", "data_device", "compute_cov3D_python", "debug", "use_offDetector")
+SETTING_FLAGS = ("source_path", "data_device", "compute_cov3D_python", "debug", "use_offDetector", "use_view_geometry")
 
 
 def parse_cfg_args(text: str) -> dict:
@@ -109,6 +109,8 @@ def parse_args(argv=None):
     ap.add_argument("--debug", action="store_const", const=True, default=None)
     ap.add_argument("--use_offDetector", action="store_const", const=True, default=None,
                     help="evaluate through the scanner's offDetector (default: as the model was trained)")
+    ap.add_argument("--use_view_geometry", action="store_const", const=True, default=None,
+                    help="evaluate through each view's own geometry (default: as the model was trained)")
     ap.add_argument("--iteration", default=-1, type=int, help="saved iteration to evaluate (-1: the last one)")
     ap.add_argument("--skip_render_train", action="store_true", default=False)
     ap.add_argument("--skip_render_test", action="store_true", default=False)
@@ -254,7 +256,8 @@ def testing(model_path: str, settings: dict, iteration: int = -1, skip_render_tr
     pick = lambda cls: cls(**{k: settings[k] for k in cls.__dataclass_fields__ if k in settings})
     model, pipe = pick(ModelParams), pick(PipelineParams)
     scene = Scene(settings["source_path"], model_path, eval=model.eval, shuffle=False, device="cuda",
-                  data_device=model.data_device, use_offDetector=bool(settings.get("use_offDetector", False)))
+                  data_device=model.data_device, use_offDetector=bool(settings.get("use_offDetector", False)),
+                  use_view_geometry=bool(settings.get("use_view_geometry", False)))
     gaussians = GaussianModel(None)
     gaussians.load_ply(pickle_path)
     scene.gaussians = gaussians

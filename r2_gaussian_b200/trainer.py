@@ -49,6 +49,12 @@ trains as `--use_offDetector` would on a copy of the scanner whose offDetector[0
 (`dataset.Scene(offDetector_u=...)`).  With `--detector_offset_refine` the learned offset acts on top of the estimate.
 Each save then writes `detector_offset.yml` with `estimate_px` / `estimate_scene` next to the learned offset (if any)
 and the total `offDetector_u`; the printed result adds `detector_estimate_px`.
+
+`--use_view_geometry` trains through each view's own DSO, DSD, offOrigin and offDetector, read from the projection
+frames (`dataset.Scene(use_view_geometry=True)`, `scene.view_scanner`): a helical scan or a calibrated bench.  It implies
+`--use_offDetector` and is recorded in `cfg_args`.  `--pose_refine` and `--detector_offset_refine` act on top of it.
+It is refused with `--estimate_offDetector` (the estimate assumes one fixed circle), with Gaussian sharding, and with
+`--batch_size` > 1 when the train views' DSD differ (a batch shares one field of view).
 """
 from __future__ import annotations
 
@@ -222,6 +228,25 @@ def evaluate(scene: Scene, gaussians: GaussianModel, pipe, with_ssim: bool = Tru
     return out
 
 
+def view_geometry_refusal(use_view_geometry: bool, estimate_offDetector: bool, world: int, batch_size: int,
+                          source_path: str) -> str | None:
+    """Why `--use_view_geometry` cannot be used with these settings (None: it can).  Checked before any CUDA work."""
+    if not use_view_geometry:
+        return None
+    if estimate_offDetector:
+        return ("--estimate_offDetector cannot be combined with --use_view_geometry: the conjugate-ray estimate assumes "
+                "one fixed circle")
+    if world > 1:
+        return "--use_view_geometry is not supported with Gaussian sharding (WORLD_SIZE > 1): train on one GPU"
+    if batch_size > 1:
+        from .dataset import train_view_dsd
+        dsd = train_view_dsd(source_path)
+        if len(set(dsd)) > 1:
+            return (f"--batch_size {batch_size} needs one field of view for every train view, but under "
+                    f"--use_view_geometry their DSD varies ({min(dsd):g} to {max(dsd):g}): use --batch_size 1")
+    return None
+
+
 def batch_refusal(batch_size: int, pose_refine: bool, world: int, compute_cov3D_python: bool) -> str | None:
     """Why `--batch_size` cannot be used with these settings (None: it can).  Checked before any CUDA work."""
     if batch_size < 1:
@@ -271,8 +296,12 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
              saving_iterations=(), checkpoint_iterations=(), checkpoint: str | None = None, init_points=None,
              log=print, pose_params: PoseParams | None = None, batch_size: int = 1,
              detector_params: DetectorParams | None = None, use_offDetector: bool = False,
-             estimate_offDetector: bool = False) -> dict:
+             estimate_offDetector: bool = False, use_view_geometry: bool = False) -> dict:
     first_iter = 0
+    why = view_geometry_refusal(use_view_geometry, estimate_offDetector, world_info()[1], int(batch_size),
+                                model.source_path)
+    if why is not None:
+        raise ValueError(why)
     refine = pose_params is not None and pose_params.pose_refine
     if refine and world_info()[1] > 1:
         raise RuntimeError("--pose_refine is not supported with Gaussian sharding (WORLD_SIZE > 1): every rank would "
@@ -296,7 +325,8 @@ def training(model: ModelParams, opt: OptimizationParams, pipe: PipelineParams, 
         log(f"estimated detector offset: {estimate['offset_px']:+.4f} px, offDetector_u = "
             f"{off_u / info.scene_scale:.6g} ({estimate['n_pairs']} conjugate pairs)")
     scene = Scene(model.source_path, model.model_path, eval=model.eval, shuffle=False, device="cuda",
-                  data_device=model.data_device, use_offDetector=use_offDetector, offDetector_u=off_u)
+                  data_device=model.data_device, use_offDetector=use_offDetector, offDetector_u=off_u,
+                  use_view_geometry=use_view_geometry)
     scene.offset_estimate = estimate
     cfg = scene.scanner_cfg
     if B > len(scene.getTrainCameras()):
@@ -763,6 +793,9 @@ def parse_args(argv=None):
     ap.add_argument("--estimate_offDetector", action="store_true",
                     help="estimate the horizontal detector offset from the train views (on top of the file's under "
                          "--use_offDetector) and train through it")
+    ap.add_argument("--use_view_geometry", action="store_true",
+                    help="train through each view's own DSO, DSD, offOrigin and offDetector (the projection frames' "
+                         "keys; helical scans, calibrated benches); implies --use_offDetector")
     a = ap.parse_args(argv)
     pick = lambda cls: cls(**{k: getattr(a, k) for k in cls.__dataclass_fields__})
     model, pipe, opt, pose = pick(ModelParams), pick(PipelineParams), pick(OptimizationParams), pick(PoseParams)
@@ -775,6 +808,12 @@ def parse_args(argv=None):
         ap.error(why)
     a.detector_params = pick(DetectorParams)
     why = detector_refusal(a.detector_params.detector_offset_refine, pose.pose_refine, world)
+    if why is not None:
+        ap.error(why)
+    try:
+        why = view_geometry_refusal(a.use_view_geometry, a.estimate_offDetector, world, a.batch_size, a.source_path)
+    except (OSError, ValueError, KeyError) as e:
+        why = f"--use_view_geometry: cannot read the train views of {a.source_path}: {e}"
     if why is not None:
         ap.error(why)
     if a.batch_size > 1:
@@ -800,7 +839,8 @@ def main(argv=None):
                         "quiet": False, "config": None, "detect_anomaly": False,
                         **({"batch_size": a.batch_size} if a.batch_size > 1 else {}),
                         **({"use_offDetector": True} if a.use_offDetector else {}),
-                        **({"estimate_offDetector": True} if a.estimate_offDetector else {})}, pose, a.detector_params)
+                        **({"estimate_offDetector": True} if a.estimate_offDetector else {}),
+                        **({"use_view_geometry": True} if a.use_view_geometry else {})}, pose, a.detector_params)
     random.seed(a.seed), np.random.seed(a.seed), torch.manual_seed(a.seed)     # safe_state (`general_utils.py:61-63`)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if world > 1:                      # launched by torchrun: one process per GPU, Gaussians sharded by index
@@ -816,7 +856,7 @@ def main(argv=None):
     hist = training(model, opt, pipe, set(a.test_iterations) | {opt.iterations}, set(a.save_iterations),
                     set(a.checkpoint_iterations), a.start_checkpoint, pose_params=pose, batch_size=a.batch_size,
                     detector_params=a.detector_params, use_offDetector=a.use_offDetector,
-                    estimate_offDetector=a.estimate_offDetector)
+                    estimate_offDetector=a.estimate_offDetector, use_view_geometry=a.use_view_geometry)
     final = hist["eval"].get(opt.iterations, {})
     if world > 1:
         import torch.distributed as dist

@@ -18,7 +18,7 @@ SOURCE is one of (as in `extract_mesh`)
 Drawn: the marching-cubes mesh at --mc_thresh (0.5), the volume's box (red), the unit box [-1, 1]^3 (blue), a frame at
 offOrigin, and per drawn train view its frustum in a colour from --cmap, its projection on the image plane (at depth
 --cam_scale, or with --true_detector at the detector: DSD from the source, sDetector in size, the offset honoured) and a
-small frame.  Without --camera the view is `scene_view.default_view`; --orbit N turns it about the scan axis (+z) and
+small frame (--use_view_geometry: each view's own source and detector).  Without --camera the view is `scene_view.default_view`; --orbit N turns it about the scan axis (+z) and
 writes <stem>_0000.png ...; --save_npy also writes the float frames [N, H, W, 3] to <stem>.npy.  Prints one JSON line:
 source, triangles, lines, cameras, frames, width, height, seconds, outputs (and with --gaussians: gaussians, the number
 drawn).  GPU only.
@@ -46,6 +46,9 @@ def parse_args(argv=None):
     ap.add_argument("--output", required=True, help="PNG file to write (with --orbit: the stem of the frame files)")
     add_source_arguments(ap)
     ap.add_argument("--use_offDetector", action="store_true", help="cameras with the scanner's detector offset")
+    ap.add_argument("--use_view_geometry", action="store_true",
+                    help="each camera at its own source and detector (the frames' per-view DSO, DSD, offOrigin, "
+                         "offDetector: a helix shows as one); implies --use_offDetector")
     ap.add_argument("--mc_thresh", type=float, default=0.5, help="marching-cubes level of the mesh (default 0.5)")
     ap.add_argument("--cam_scale", type=float, default=1.0, help="size of the camera glyphs (default 1.0)")
     ap.add_argument("--width", type=int, default=1000, help="image width in pixels (default 1000)")
@@ -103,8 +106,8 @@ def parse_args(argv=None):
             look_at(a.camera[0:3], a.camera[3:6], a.camera[6:9], a.width, a.height, a.view_angle)
         except ValueError as e:
             ap.error(f"--camera: {e}")
-    if (a.true_detector or a.use_offDetector) and a.source_path is None and a.model_path is None:
-        ap.error("--true_detector and --use_offDetector need cameras: give -s <scene> or -m <model>")
+    if (a.true_detector or a.use_offDetector or a.use_view_geometry) and a.source_path is None and a.model_path is None:
+        ap.error("--true_detector, --use_offDetector and --use_view_geometry need cameras: give -s <scene> or -m <model>")
     if a.gaussians:
         if a.model_path is None:
             ap.error("--gaussians draws a trained model's Gaussians: give -m <model>")
@@ -138,7 +141,8 @@ def _cameras(a):
     if a.model_path is None:
         if a.source_path is None:
             return [], None
-        scene = Scene(a.source_path, eval=False, shuffle=False, device="cuda", use_offDetector=a.use_offDetector)
+        scene = Scene(a.source_path, eval=False, shuffle=False, device="cuda", use_offDetector=a.use_offDetector,
+                      use_view_geometry=a.use_view_geometry)
         cams = scene.getTrainCameras()
         return [(c, c) for c in cams[::a.views]], scene
     from .test import correction_modules, load_settings, resolve_iteration
@@ -147,7 +151,8 @@ def _cameras(a):
     settings = load_settings(a.model_path)
     source = a.source_path or settings.get("source_path")
     off = a.use_offDetector or bool(settings.get("use_offDetector", False))
-    scene = Scene(source, eval=False, shuffle=False, device="cuda", use_offDetector=off)
+    per_view = a.use_view_geometry or bool(settings.get("use_view_geometry", False))
+    scene = Scene(source, eval=False, shuffle=False, device="cuda", use_offDetector=off, use_view_geometry=per_view)
     _, pickle_path = resolve_iteration(a.model_path, a.iteration)
     try:
         pose, det = correction_modules(os.path.dirname(pickle_path), scene)
@@ -185,6 +190,8 @@ def build(a, vol, cfg, gaussians=None):
     for i, (nom, cam) in enumerate(pairs):
         col = camera_colour(a.lut, i * a.views, n_all)
         img = None if a.no_images else cam.original_image[0]
+        if depth is not None and scene.use_view_geometry:   # the view's own DSD, from its field of view
+            depth = float(scene.scanner_cfg["sDetector"][1]) / 2.0 / math.tan(float(nom.FoVx) / 2.0)
         parts.append(camera_glyph(cam, a.cam_scale, col, image=img, plane_depth=depth))
         if a.model_path is not None:
             parts.append(camera_glyph(nom, a.cam_scale, col, plane_depth=depth, width=LINE_WIDTH / 2))
