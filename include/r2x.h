@@ -536,6 +536,41 @@ int r2x_fdk_views(void* stream, int n_views, int H, int W, const float* projs, c
                   const float* projmatrices, int mode, int weighting, int nx, int ny, int nz, float sx, float sy,
                   float sz, float cx, float cy, float cz, const double* view_geometry,
                   const double* view_geometry_host, float* out_volume, void* scratch, size_t scratch_bytes);
+/* Helical FDK (Tang et al. 2006, "A three-dimensional-weighted cone beam filtered backprojection (CB-FBP) algorithm for
+ * image reconstruction in volumetric CT -- helical scanning", Phys. Med. Biol. 51:855), in native cone-beam geometry on
+ * the flat detector; float64 statement in tests/fdk_helical_oracle.py.  Cone beam only.
+ *   Helix.  One DSO, one DSD, a centred detector and one offOrigin x / y; the volume position's z is affine in each
+ *     view's unwrapped angle beta, so in the grid frame (scene.camera_pose) the source of view v is at
+ *     (DSO cos beta + c_x, DSO sin beta + c_y, z_s(beta)), z_s(beta) = z0 + pitch * beta (pitch signed, per radian;
+ *     0 is a circle).  beta[N] (device) and beta_host[N] are the views' angles, strictly increasing; the caller sorts
+ *     the views (and their projections and matrices) into that order.  The arc is [beta_lo, beta_hi) with
+ *     beta_lo <= beta[0], beta[N-1] < beta_hi and beta_hi - beta_lo >= 2 pi; dbeta[N] (device) is each view's
+ *     quadrature interval (fdk.helix_views: between the midpoints of its neighbours, beta_lo and beta_hi at the ends).
+ *   Filter.  Steps 1-2 of r2x_fdk with R2X_FDK_PLAIN and the filter field of `weighting` (no other bits).
+ *   Conjugates.  For voxel x and view beta: d = the in-plane vector from the source to x, L = |d|, gamma its fan angle
+ *     from the central ray, signed so that the source at beta + pi + 2 gamma lies on the same in-plane line (R2X_FDK_PARKER's
+ *     convention).  K(beta, x) = {(beta + 2 pi m, L)} u {(beta + pi + 2 gamma + 2 pi m, 2 DSO cos(gamma) - L)} over the
+ *     integers m with beta_lo <= beta_k < beta_hi (a conjugate with 2 DSO cos(gamma) - L <= 0 does not exist; a view
+ *     with L cos(gamma) <= 0 gets weight 0), each with its detector row nu_k = (Z - z_s(beta_k)) / (L_k cos(gamma)
+ *     tan_fovy); nu_0 is minus the ndc row at which the view samples x.
+ *   Weight.  W_Q(nu) = 1 for |nu| <= Q, cos^2(pi/2 (|nu| - Q) / (1 - Q)) for Q < |nu| < 1, 0 for |nu| >= 1 (the last
+ *     rule first: Q = 1 gives 1 inside the detector, 0 on and beyond its edge); 0 <= Q <= 1.
+ *     w(beta, x) = W_Q(nu_0) / sum_{k in K} W_Q(nu_k) (0 when W_Q(nu_0) = 0).
+ *   Backprojection.  out_volume(x) = sum over views in index order of dbeta_v * w(beta_v, x) * U^2 * Qf_v(x), with Qf_v
+ *     sampled and U = DSO / z_view as in step 3 of r2x_fdk.  With pitch 0, Q = 1 and a full circle, a voxel whose two
+ *     conjugate rays both hit the detector gets w = 1/2 and dbeta = 2 pi / N: the plain FDK's pi / N.
+ * Each CTA visits only the views whose source height lies within (DSO + the grid's largest in-plane radius about
+ * (c_x, c_y)) * tan_fovy of its voxels (widened by 1e-3): the others have W_Q(nu_0) = 0 there, so the skip drops exact
+ * zeros.  Refuses, before any CUDA work: parallel beam, NULL pointers, a non-finite helix, Q outside [0, 1], beta_host
+ * not finite and strictly increasing, beta outside [beta_lo, beta_hi), an arc shorter than 2 pi (within 1e-6), any
+ * weighting bit but the filter field, and what r2x_fdk refuses.  Deterministic (no atomics).  `scratch` holds
+ * r2x_fdk_scratch_bytes(N, H, W).  Asynchronous on `stream`.  Limits as r2x_fdk's. */
+int r2x_fdk_helical(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                    const float* projmatrices, float tan_fovx, float tan_fovy, int mode, int weighting, float dso,
+                    const double* beta, const double* dbeta, const double* beta_host, double z0, double pitch,
+                    double beta_lo, double beta_hi, double c_x, double c_y, float q, int nx, int ny, int nz, float sx,
+                    float sy, float sz, float cx, float cy, float cz, float* out_volume, void* scratch,
+                    size_t scratch_bytes);
 int r2x_volume_project_views(void* stream, int nx, int ny, int nz, const float* volume, float sx, float sy, float sz,
                              float cx, float cy, float cz, int n_views, int H, int W, const float* viewmatrices,
                              int mode, float step, const double* view_geometry, const double* view_geometry_host,

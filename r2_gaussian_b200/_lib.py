@@ -102,6 +102,9 @@ PROTOTYPES = {
                                     _f, _f, _vp, _vp, _vp, _sz]),
     "r2x_fdk_views": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _f, _f, _f, _vp, _vp, _vp, _vp,
                            _sz]),
+    "r2x_fdk_helical": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _i, _f, _vp, _vp, _vp, C.c_double, C.c_double,
+                             C.c_double, C.c_double, C.c_double, C.c_double, _f, _i, _i, _i, _f, _f, _f, _f, _f, _f, _vp,
+                             _vp, _sz]),
     "r2x_volume_project_views": (_i, [_vp, _i, _i, _i, _vp, _f, _f, _f, _f, _f, _f, _i, _i, _i, _vp, _i, _f, _vp, _vp,
                                       _vp]),
     "r2x_volume_backproject_views": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _f, _f, _f, _f, _f,

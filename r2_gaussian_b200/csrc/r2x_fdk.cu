@@ -29,12 +29,17 @@
 //                           projmatrices.  The scale is pi / N, or 1 for Parker weights (they hold each view's
 //                           interval).
 //
+//   fdk_helical_kernel      r2x_fdk_helical's backprojection of a helical scan (Tang et al. 2006): the same sample
+//                           and U^2 weight, times each view's interval dbeta_v and its 3-D redundancy weight
+//                           W_Q(nu_0) / sum over the turns and conjugate rays of the voxel's in-plane line of W_Q(nu_k);
+//                           each CTA visits only the views within vertical reach of its z-run.
+//
 // With a per-view geometry table (r2x_fdk_views) the filter kernels take each row's tan_fov, offset and isocentre pitch
 // from its view's row (fdk_view_row) and the backprojection each view's DSO; without one, the scalars.
 //
 // The float64 NumPy statements of the same definitions are oracle/fdk_oracle.py (plain),
-// tests/fdk_short_scan_oracle.py (short scan, Parker weights) and tests/offset_detector_oracle.py (offset detector,
-// half-fan weights).
+// tests/fdk_short_scan_oracle.py (short scan, Parker weights), tests/offset_detector_oracle.py (offset detector,
+// half-fan weights) and tests/fdk_helical_oracle.py (helical weights).
 #include <cmath>
 #include <cstdint>
 
@@ -437,6 +442,264 @@ static int fdk_run(void* stream, int n_views, int H, int W, const float* projs, 
                            cy, cz, scale, out_volume);
 }
 
+// ---- helical FDK (r2x_fdk_helical): Tang et al. 2006's 3-D redundancy weight in the backprojection ----------------
+
+// The scalars of a helical backprojection: the helix z_s(beta) = z0 + h beta (z0 in float64, the kernel forms each
+// view's z_s in float64 and rounds it once), the arc [beta_lo, beta_lo + arc), the rotation centre (c_x, c_y), and the
+// weight W_Q's Q with band = 1 / (2 (1 - Q)) (0 for Q = 1).  reach bounds |Z - z_s(beta_v)| below which a view can
+// reach a voxel: (DSO + the grid's largest in-plane radius about the centre) * tan_fovy, widened by 1e-3.
+struct FdkHelix {
+    double z0 = 0.0, h = 0.0, beta_lo = 0.0, c_x = 0.0, c_y = 0.0;
+    float arc = 0.0f, dso = 0.0f, tany = 0.0f, q = 1.0f, band = 0.0f, reach = 0.0f;
+};
+
+// W_Q(nu): 1 for |nu| <= Q, cos^2(pi/2 (|nu| - Q) / (1 - Q)) up to 1, 0 from |nu| = 1 on.
+__device__ __forceinline__ float fdk_helix_wq(float nu, float q, float band) {
+    const float a = fabsf(nu);
+    if (a >= 1.0f) return 0.0f;
+    if (a <= q) return 1.0f;
+    const float c = cospif((a - q) * band);
+    return c * c;
+}
+
+// view v's source height z_s(beta_v), rounded once; the window search and the staging both read it from here, so
+// both see the same value.
+__device__ __forceinline__ float fdk_helix_zs(const double* __restrict__ beta, int v, const FdkHelix& hx) {
+    return (float)fma(hx.h, beta[v], hx.z0);
+}
+
+// First view index in [0, N) whose key sgn * z_s(beta_v) is > lo (strict) or >= lo; the keys do not decrease with v.
+__device__ __forceinline__ int fdk_helix_search(const double* __restrict__ beta, int N, const FdkHelix& hx, float sgn,
+                                                float lo, bool strict) {
+    int a = 0, b = N;
+    while (a < b) {
+        const int m = (a + b) >> 1;
+        const float key = sgn * fdk_helix_zs(beta, m, hx);
+        if (strict ? key > lo : key >= lo) b = m;
+        else a = m + 1;
+    }
+    return a;
+}
+
+// Helical FDK backprojection, one thread per (x, y) column and FDK_ZR voxels along z as fdk_backproject_kernel, each
+// view sampled as there and weighted by dbeta_v * w(beta_v, x) * U^2.  The CTA loops over the contiguous views whose
+// source height lies within `reach` of its z-run (found by binary search; a view outside it has W_Q(nu_0) = 0 at every
+// voxel of the CTA, so the skip drops exact zeros).  Per (column, view) it sets up gamma, L and the candidates' m
+// ranges once (only the turns whose source lies within vertical reach of the run), then per voxel sums W_Q over them.
+__global__ void __launch_bounds__(FDK_BX * FDK_BY) fdk_helical_kernel(
+    int N, int H, int W, const float* __restrict__ q, const float* __restrict__ viewm, const float* __restrict__ projm,
+    const double* __restrict__ beta, const double* __restrict__ dbeta, FdkHelix hx, int nx, int ny, int nz, float ox,
+    float oy, float oz, float dx, float dy, float dz, float* __restrict__ vol) {
+    // per view: projmatrix rows 0, 1, 3 and viewmatrix row 2 as fdk_backproject_kernel's; the source (S_x, S_y) and
+    // (cos beta, sin beta); z_s, beta - beta_lo and dbeta
+    __shared__ float4 mat[FDK_VCHUNK][4];
+    __shared__ float4 src[FDK_VCHUNK];
+    __shared__ float4 hel[FDK_VCHUNK];
+    const int y = blockIdx.x * FDK_BX + threadIdx.x;
+    const int x = blockIdx.y * FDK_BY + threadIdx.y;
+    const int z0 = blockIdx.z * FDK_ZR;
+    const int tid = threadIdx.y * FDK_BX + threadIdx.x;
+    const bool live = x < nx && y < ny;
+    const float X = fmaf((float)x, dx, ox), Y = fmaf((float)y, dy, oy), Z0 = fmaf((float)z0, dz, oz);
+    const float Z1 = fmaf((float)(FDK_ZR - 1), dz, Z0);   // the run's last voxel (past nz too: only widens the bounds)
+    const float half_w = 0.5f * (float)W, half_h = 0.5f * (float)H;
+    const float cen_w = 0.5f * (float)(W - 1), cen_h = 0.5f * (float)(H - 1);
+    const size_t view_stride = (size_t)H * W;
+    const float two_pi = 6.28318530717958648f, pi = 3.14159265358979324f;
+    const float turn = (float)(6.283185307179586 * hx.h);   // z_s gained per turn
+    float acc[FDK_ZR];
+#pragma unroll
+    for (int k = 0; k < FDK_ZR; ++k) acc[k] = 0.0f;
+
+    // the view window: z_s(beta_v) within reach of [Z0, Z1]; z_s is monotone in v (sign sgn), constant for h = 0
+    int vb = 0, ve = N;
+    if (hx.h != 0.0) {
+        const float sgn = hx.h > 0.0 ? 1.0f : -1.0f;
+        const float lo = sgn > 0.0f ? Z0 - hx.reach : -(Z1 + hx.reach);
+        const float hi = sgn > 0.0f ? Z1 + hx.reach : -(Z0 - hx.reach);
+        vb = fdk_helix_search(beta, N, hx, sgn, lo, true);
+        ve = fdk_helix_search(beta, N, hx, sgn, hi, false);
+    }
+
+    for (int c0 = vb; c0 < ve; c0 += FDK_VCHUNK) {
+        const int nc = min(FDK_VCHUNK, ve - c0);
+        __syncthreads();
+        for (int e = tid; e < nc * 4; e += FDK_BX * FDK_BY) {
+            const int v = e >> 2, slot = e & 3;
+            const float* m = (slot == 3 ? viewm : projm) + (size_t)(c0 + v) * 16;
+            const int rr = slot == 3 ? 2 : (slot == 2 ? 3 : slot);
+            mat[v][slot] = make_float4(m[rr], m[4 + rr], m[8 + rr], m[12 + rr]);
+        }
+        if (tid < nc) {
+            const double b = beta[c0 + tid];
+            double sb, cb;
+            sincos(b, &sb, &cb);
+            src[tid] = make_float4((float)fma((double)hx.dso, cb, hx.c_x), (float)fma((double)hx.dso, sb, hx.c_y),
+                                   (float)cb, (float)sb);
+            hel[tid] = make_float4(fdk_helix_zs(beta, c0 + tid, hx), (float)(b - hx.beta_lo), (float)dbeta[c0 + tid],
+                                   0.0f);
+        }
+        __syncthreads();
+        if (!live) continue;
+        for (int v = 0; v < nc; ++v) {
+            const float4 S = src[v], G = hel[v];
+            const float zs = G.x, brel = G.y;
+            // in-plane: d = x - source; zin = L cos(gamma) along the central ray -(cos beta, sin beta), sg = L sin(gamma)
+            const float ddx = X - S.x, ddy = Y - S.y;
+            const float zin = -fmaf(S.z, ddx, S.w * ddy);
+            if (!(zin > 0.0f)) continue;
+            const float inv0 = __frcp_rn(zin * hx.tany);
+            // nu_0 is affine in z: all of the run off the detector on one side gives W_Q(nu_0) = 0 at every voxel
+            const float nu_a = (Z0 - zs) * inv0, nu_b = (Z1 - zs) * inv0;
+            if ((nu_a >= 1.0f && nu_b >= 1.0f) || (nu_a <= -1.0f && nu_b <= -1.0f)) continue;
+            const float sg = fmaf(S.w, ddx, -S.z * ddy);
+            const float gam = atan2f(sg, zin);
+            const float l2 = fmaf(zin, zin, sg * sg);
+            // the conjugate's L_c cos(gamma) = 2 DSO cos^2(gamma) - L cos(gamma); none when the voxel is off the circle
+            const float zc = 2.0f * hx.dso * zin * (zin / l2) - zin;
+            const float invc = zc > 0.0f ? __frcp_rn(zc * hx.tany) : 0.0f;
+            const float cbase = fmaf(2.0f, gam, pi);   // conjugate at beta + pi + 2 gamma + 2 pi m
+            // m ranges: beta_k in [beta_lo, beta_lo + arc), and (h != 0) source within reach of the run
+            float dlo = ceilf(-brel / two_pi), dhi = ceilf((hx.arc - brel) / two_pi) - 1.0f;
+            float clo = ceilf(-(brel + cbase) / two_pi), chi = ceilf((hx.arc - brel - cbase) / two_pi) - 1.0f;
+            if (turn != 0.0f) {
+                const float r0 = zin * hx.tany, rc = zc * hx.tany;
+                const float a0 = (Z0 - zs - r0) / turn, b0 = (Z1 - zs + r0) / turn;
+                dlo = fmaxf(dlo, floorf(fminf(a0, b0)));
+                dhi = fminf(dhi, ceilf(fmaxf(a0, b0)));
+                const float ac = (Z0 - zs - rc) / turn - cbase / two_pi, bc = (Z1 - zs + rc) / turn - cbase / two_pi;
+                clo = fmaxf(clo, floorf(fminf(ac, bc)));
+                chi = fminf(chi, ceilf(fmaxf(ac, bc)));
+            }
+            if (!(invc > 0.0f)) chi = clo - 1.0f;
+            const int mdl = (int)dlo, mdh = (int)dhi, mcl = (int)clo, mch = (int)chi;
+            float wsum[FDK_ZR];
+#pragma unroll
+            for (int k = 0; k < FDK_ZR; ++k) wsum[k] = 0.0f;
+            for (int m = mdl; m <= mdh; ++m) {
+                const float zk = fmaf((float)m, turn, zs);
+#pragma unroll
+                for (int k = 0; k < FDK_ZR; ++k)
+                    wsum[k] += fdk_helix_wq((fmaf((float)k, dz, Z0) - zk) * inv0, hx.q, hx.band);
+            }
+            for (int m = mcl; m <= mch; ++m) {
+                const float zk = fmaf(fmaf((float)m, two_pi, cbase), (float)hx.h, zs);
+#pragma unroll
+                for (int k = 0; k < FDK_ZR; ++k)
+                    wsum[k] += fdk_helix_wq((fmaf((float)k, dz, Z0) - zk) * invc, hx.q, hx.band);
+            }
+            const float4 P0 = mat[v][0], P1 = mat[v][1], P3 = mat[v][2], V2 = mat[v][3];
+            const float ax = fmaf(P0.z, Z0, fmaf(P0.y, Y, fmaf(P0.x, X, P0.w)));
+            const float ay = fmaf(P1.z, Z0, fmaf(P1.y, Y, fmaf(P1.x, X, P1.w)));
+            const float aw = fmaf(P3.z, Z0, fmaf(P3.y, Y, fmaf(P3.x, X, P3.w))) + 1e-7f;  // the rasterizer's divide
+            const float sx = P0.z * dz, sy = P1.z * dz, sw = P3.z * dz;
+            const float av = fmaf(V2.z, Z0, fmaf(V2.y, Y, fmaf(V2.x, X, V2.w))), sv = V2.z * dz;
+            const float* qv = q + (size_t)(c0 + v) * view_stride;
+#pragma unroll
+            for (int k = 0; k < FDK_ZR; ++k) {
+                const float fk = (float)k;
+                const float w0 = fdk_helix_wq((fmaf(fk, dz, Z0) - zs) * inv0, hx.q, hx.band);
+                if (!(w0 > 0.0f)) continue;        // wsum >= w0 > 0 from here on
+                const float zv = fmaf(fk, sv, av);
+                if (!(zv > 0.0f)) continue;
+                const float u = hx.dso * __frcp_rn(zv);
+                const float w = u * u * (G.z * (w0 / wsum[k]));
+                const float pw = __frcp_rn(fmaf(fk, sw, aw));
+                const float px = fmaf(fmaf(fk, sx, ax) * pw, half_w, cen_w);
+                const float py = fmaf(fmaf(fk, sy, ay) * pw, half_h, cen_h);
+                if (!(px > -1.0f && px < (float)W && py > -1.0f && py < (float)H)) continue;
+                const float fx0 = floorf(px), fy0 = floorf(py);
+                const int ix = (int)fx0, iy = (int)fy0;
+                const float fx = px - fx0, fy = py - fy0;
+                const long long base = (long long)iy * W + ix;
+                float s00 = 0.0f, s01 = 0.0f, s10 = 0.0f, s11 = 0.0f;
+                if (iy >= 0) {
+                    if (ix >= 0) s00 = __ldg(qv + base);
+                    if (ix + 1 < W) s01 = __ldg(qv + base + 1);
+                }
+                if (iy + 1 < H) {
+                    if (ix >= 0) s10 = __ldg(qv + base + W);
+                    if (ix + 1 < W) s11 = __ldg(qv + base + W + 1);
+                }
+                const float top = fmaf(fx, s01 - s00, s00), bot = fmaf(fx, s11 - s10, s10);
+                acc[k] = fmaf(w, fmaf(fy, bot - top, top), acc[k]);
+            }
+        }
+    }
+    if (!live) return;
+    float* out = vol + ((size_t)x * ny + y) * nz;
+#pragma unroll
+    for (int k = 0; k < FDK_ZR; ++k)
+        if (z0 + k < nz) out[z0 + k] = acc[k];
+}
+
+// r2x_fdk_helical: the checks (all before any CUDA work), then the plain filter and the helical backprojection.
+static int fdk_helical_run(void* stream, int N, int H, int W, const float* projs, const float* viewm, const float* projm,
+                           float tanx, float tany, int mode, int weighting, float dso, const double* beta,
+                           const double* dbeta, const double* beta_host, double z0, double pitch, double beta_lo,
+                           double beta_hi, double c_x, double c_y, float q_param, int nx, int ny, int nz, float sx,
+                           float sy, float sz, float cx, float cy, float cz, float* out, void* scratch,
+                           size_t scratch_bytes) {
+    if (mode != 1)
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk_helical: bad mode (cone beam only; parallel-beam helices are not "
+                                         "supported)");
+    if (int rc = fdk_validate(N, H, W, projs, viewm, projm, tanx, tany, mode, dso, nx, ny, nz, sx, sy, sz, out, scratch,
+                              scratch_bytes))
+        return rc;
+    if (!beta || !dbeta || !beta_host) return fail_msg(R2X_ERR_INVALID, "r2x_fdk_helical: bad pointer (beta, dbeta or "
+                                                                        "beta_host NULL)");
+    if (weighting < 0 || (weighting & 0xff) != R2X_FDK_PLAIN || (weighting & ~0xff) > R2X_FDK_HANN)
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk_helical: bad weighting (the filter field only: 0x000 = Ram-Lak, "
+                                         "0x100 = Shepp-Logan, 0x200 = cosine, 0x300 = Hamming, 0x400 = Hann)");
+    const double h[6] = {z0, pitch, beta_lo, beta_hi, c_x, c_y};
+    for (double v : h)
+        if (!std::isfinite(v))
+            return fail_msg(R2X_ERR_INVALID, "r2x_fdk_helical: bad helix (z0, pitch, beta_lo, beta_hi, c_x, c_y must "
+                                             "be finite)");
+    if (!(q_param >= 0.0f && q_param <= 1.0f)) return fail_msg(R2X_ERR_INVALID, "r2x_fdk_helical: bad Q (needs 0 <= Q "
+                                                                                 "<= 1)");
+    for (int v = 0; v < N; ++v)
+        if (!std::isfinite(beta_host[v]) || (v > 0 && !(beta_host[v] > beta_host[v - 1])))
+            return fail_msg(R2X_ERR_INVALID, "r2x_fdk_helical: bad beta (must be finite and strictly increasing)");
+    if (!(beta_lo <= beta_host[0] && beta_host[N - 1] < beta_hi))
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk_helical: bad arc (needs beta_lo <= beta[0] and beta[N-1] < beta_hi)");
+    const double two_pi = 6.283185307179586;
+    if (!(beta_hi - beta_lo >= two_pi - 1e-6))
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk_helical: bad arc (beta_hi - beta_lo must be at least 2 pi; a circular "
+                                         "short scan takes R2X_FDK_PARKER)");
+    const float dx = sx / nx, dy = sy / ny, dz = sz / nz;
+    const float ox = cx - 0.5f * sx + 0.5f * dx, oy = cy - 0.5f * sy + 0.5f * dy, oz = cz - 0.5f * sz + 0.5f * dz;
+    // the grid's largest in-plane radius about the rotation centre: the farthest corner voxel centre
+    double rmax = 0.0;
+    for (int i = 0; i < 4; ++i) {
+        const double gx = (double)ox + (i & 1 ? (double)(nx - 1) * dx : 0.0) - c_x;
+        const double gy = (double)oy + (i & 2 ? (double)(ny - 1) * dy : 0.0) - c_y;
+        rmax = std::fmax(rmax, std::sqrt(gx * gx + gy * gy));
+    }
+    FdkHelix hx;
+    hx.z0 = z0;
+    hx.h = pitch;
+    hx.beta_lo = beta_lo;
+    hx.c_x = c_x;
+    hx.c_y = c_y;
+    hx.arc = (float)(beta_hi - beta_lo);
+    hx.dso = dso;
+    hx.tany = tany;
+    hx.q = q_param;
+    hx.band = q_param < 1.0f ? (float)(0.5 / (1.0 - (double)q_param)) : 0.0f;
+    hx.reach = (float)(((double)dso + rmax) * (double)tany * (1.0 + 1e-3));
+    const cudaStream_t st = (cudaStream_t)stream;
+    float* qf = (float*)(((size_t)scratch + 255) & ~(size_t)255);
+    if (int rc = fdk_filter(st, R2X_FDK_PLAIN, weighting & ~0xff, N, H, W, projs, tanx, tany, mode, dso, 0.0f, 0.0f,
+                            FdkWeights(), nullptr, qf))
+        return rc;
+    const dim3 grid((ny + FDK_BX - 1) / FDK_BX, (nx + FDK_BY - 1) / FDK_BY, (nz + FDK_ZR - 1) / FDK_ZR);
+    fdk_helical_kernel<<<grid, dim3(FDK_BX, FDK_BY), 0, st>>>(N, H, W, qf, viewm, projm, beta, dbeta, hx, nx, ny, nz,
+                                                              ox, oy, oz, dx, dy, dz, out);
+    R2X_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace r2x
 
 extern "C" {
@@ -469,6 +732,17 @@ int r2x_fdk_views(void* stream, int n_views, int H, int W, const float* projs, c
                    (float)row0[VG_TANY], mode, (float)row0[VG_SHIFT_U], (float)row0[VG_SHIFT_V], weighting, nullptr,
                    0.0f, (float)row0[VG_DSO], nx, ny, nz, sx, sy, sz, cx, cy, cz, out_volume, scratch, scratch_bytes,
                    view_geometry);
+}
+
+int r2x_fdk_helical(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                    const float* projmatrices, float tan_fovx, float tan_fovy, int mode, int weighting, float dso,
+                    const double* beta, const double* dbeta, const double* beta_host, double z0, double pitch,
+                    double beta_lo, double beta_hi, double c_x, double c_y, float q, int nx, int ny, int nz, float sx,
+                    float sy, float sz, float cx, float cy, float cz, float* out_volume, void* scratch,
+                    size_t scratch_bytes) {
+    return r2x::fdk_helical_run(stream, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode,
+                                weighting, dso, beta, dbeta, beta_host, z0, pitch, beta_lo, beta_hi, c_x, c_y, q, nx,
+                                ny, nz, sx, sy, sz, cx, cy, cz, out_volume, scratch, scratch_bytes);
 }
 
 int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, float tan_fovx, float tan_fovy,

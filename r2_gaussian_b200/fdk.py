@@ -39,9 +39,18 @@ do not cover a full circle and a short scan.  The float64 statement is tests/off
 
 `view_geometry=` (one dict per view, as for `projector.project`) reconstructs a calibrated circle whose DSO, DSD and
 offDetector are measured per view (r2x_fdk_views: each view's cosine weight, isocentre pitch and (DSO / z)^2 weight
-from its own row of the table).  It implies `use_offDetector`.  FDK has no helical weighting, so a table whose
+from its own row of the table).  It implies `use_offDetector`.  Plain FDK has no helical weighting, so a table whose
 offOrigin varies between views (a helical scan) is refused, as are `short_scan` and `half_fan`: cgls, sart, fista_tv
-and cp_tv (`recon`) are exact for any geometry.
+and cp_tv (`recon`) are exact for any geometry, and `helical=True` is FDK's approximate answer.
+
+`helical=True` (with `view_geometry`) reconstructs a helical scan with Tang et al.'s (2006) three-dimensional weighted
+FDK (r2x_fdk_helical; model in include/r2x.h, float64 statement in tests/fdk_helical_oracle.py).  The filter is the
+plain FDK's (any `filter=`); the backprojection weights each view of a voxel by W_Q of its detector row over the sum of
+W_Q over every measurement of the same in-plane line (its other turns and its conjugate rays), where W_Q is 1 within
+`helical_q` of the detector's centre (as a fraction of its half-height) and falls as cos^2 to 0 at its edge.
+`helix_views` fits the helix z_s = z0 + h beta to the views; it needs one DSO and DSD, a centred detector, one
+offOrigin x / y, an arc of at least 360 degrees and cone beam.  The views are reconstructed in beta order.  Pitch 0 (a
+circle of 360 degrees or more) is allowed.  `helical` is refused with `short_scan` and `half_fan`.
 """
 from __future__ import annotations
 
@@ -59,6 +68,10 @@ SUPPORTED_FILTERS = (None, "ram_lak")
 # the filters of the `filter` keyword (TIGRE's names); r2x_fdk's filter field is the index << 8 (include/r2x.h)
 FILTERS = ("ram_lak", "shepp_logan", "cosine", "hamming", "hann")
 R2X_FDK_PLAIN, R2X_FDK_PARKER, R2X_FDK_HALF_FAN = 0, 1, 2   # r2x_fdk's weighting (include/r2x.h)
+# helical FDK: W_Q's default Q (DESIGN §8 measures psnr_3d against Q), and the largest residual of the helix fit, in
+# voxels along z
+HELICAL_Q = 0.75
+HELIX_FIT_TOLERANCE = 1e-3
 # slack on the arc refusals: a scan sampled at linspace(0, pi, n + 1)[:-1] covers pi only up to rounding
 ARC_TOLERANCE = 1e-9
 
@@ -153,24 +166,114 @@ def helical(scanner_cfg: dict, view_geometry) -> bool:
     return bool(len(pos) and np.any(pos != pos[0]))
 
 
-def check_view_geometry(scanner_cfg: dict, view_geometry, short_scan: bool = False, half_fan: bool = False):
+def check_view_geometry(scanner_cfg: dict, view_geometry, short_scan: bool = False, half_fan: bool = False,
+                        helical_fdk: bool = False):
     """The refusals of fdk's per-view geometry: Parker or half-fan weights, and an offOrigin that varies between
-    views (no helical weighting)."""
+    views without `helical_fdk` (the plain FDK has no helical weighting)."""
     for flag, on in (("short_scan", short_scan), ("half_fan", half_fan)):
         if on:
             raise ValueError(f"fdk: {flag} cannot be combined with view_geometry (its redundancy weights assume one fixed "
                              "circle)")
-    if helical(scanner_cfg, view_geometry):
+    if not helical_fdk and helical(scanner_cfg, view_geometry):
         raise ValueError("fdk: the views' offOrigin varies (a helical scan) and FDK has no helical weighting: "
-                         "reconstruct with cgls, sart, fista_tv or cp_tv, which are exact for any geometry")
+                         "reconstruct with cgls, sart, fista_tv or cp_tv, which are exact for any geometry, or pass "
+                         "helical=True for FDK's approximate helical weighting")
+
+
+class Helix:
+    """The helix of `helix_views`: `order` sorts the views into beta order; `beta` (float64, strictly increasing) and
+    `dbeta` are the sorted views' unwrapped angles and quadrature intervals; the source height is z0 + h beta over the
+    arc [beta_lo, beta_hi); (c_x, c_y) is the rotation centre in the grid frame."""
+
+    def __init__(self, order, beta, dbeta, z0, h, beta_lo, beta_hi, c_x, c_y):
+        self.order, self.beta, self.dbeta = order, beta, dbeta
+        self.z0, self.h, self.beta_lo, self.beta_hi, self.c_x, self.c_y = z0, h, beta_lo, beta_hi, c_x, c_y
+
+
+def helix_views(angles, scanner_cfg: dict, view_geometry) -> Helix:
+    """Fit a helix to a per-view geometry.  View v's source sits at (DSO cos a_v, DSO sin a_v) + (c_x, c_y) and at
+    height z_v = offOrigin_z - offOrigin_v,z (`scene.camera_pose`).  The views are sorted by z_v (then by angle mod
+    2 pi), their angles unwrapped in that order (reversed if they then decrease), and z = z0 + h beta is fitted by least
+    squares.  The arc runs half a mean step beyond the first and last view; dbeta_v runs between the midpoints of its
+    neighbours.  Refuses fewer than 2 views, parallel beam, DSO, DSD or offDetector that vary, a non-zero offDetector,
+    an x / y offOrigin that varies, angles that do not advance monotonically along z, a fit residual above
+    HELIX_FIT_TOLERANCE voxels and an arc shorter than 360 degrees."""
+    angles = np.asarray(angles, np.float64).reshape(-1)
+    view_geometry = list(view_geometry)
+    N = len(angles)
+    if len(view_geometry) != N:
+        raise ValueError(f"fdk helical: {len(view_geometry)} view_geometry entries for {N} angles")
+    if N < 2:
+        raise ValueError(f"fdk helical: needs at least 2 views, got {N}")
+    if scanner_cfg["mode"] != "cone":
+        raise ValueError("fdk helical: cone beam only (parallel-beam helices are not supported)")
+    cfgs = [view_scanner(scanner_cfg, g or {}) for g in view_geometry]
+    for key in ("DSO", "DSD"):
+        vals = np.array([float(c[key]) for c in cfgs])
+        if np.any(vals != vals[0]):
+            raise ValueError(f"fdk helical: the views' {key} varies ({vals.min():g} .. {vals.max():g}); the helical "
+                             "weights need one circle radius and one detector distance")
+    off = np.array([[float(v) for v in c.get("offDetector", [0.0, 0.0])] for c in cfgs]).reshape(-1, 2)
+    if np.any(off != off[0]):
+        raise ValueError("fdk helical: the views' offDetector varies; the helical weights need a centred detector")
+    if np.any(off != 0.0):
+        raise ValueError(f"fdk helical: the detector is offset (offDetector {off[0].tolist()}); the helical weights "
+                         "need a centred detector")
+    grid = np.asarray(scanner_cfg["offOrigin"], np.float64)
+    pos = np.array([c.get("offOrigin_view", scanner_cfg["offOrigin"]) for c in cfgs], np.float64).reshape(-1, 3)
+    if not np.all(np.isfinite(pos)) or not np.all(np.isfinite(angles)):
+        raise ValueError("fdk helical: angles and offOrigin must be finite")
+    if np.any(pos[:, :2] != pos[0, :2]):
+        raise ValueError("fdk helical: the views' offOrigin x / y varies; a helix moves the volume along the rotation "
+                         "axis only")
+    z = grid[2] - pos[:, 2]
+    order = np.lexsort((np.mod(angles, 2.0 * math.pi), z))
+    beta = np.unwrap(angles[order])
+    if beta[-1] < beta[0]:
+        order, beta = order[::-1], beta[::-1]
+    if not np.all(np.diff(beta) > 0.0):
+        raise ValueError("fdk helical: the views' angles do not advance monotonically along the helix (sorted by the "
+                         "volume's z, the unwrapped angles must strictly increase or decrease)")
+    zs = z[order]
+    dz = float(scanner_cfg["sVoxel"][2]) / float(scanner_cfg["nVoxel"][2])
+    if np.max(np.abs(zs - zs.mean())) <= HELIX_FIT_TOLERANCE * dz:
+        h, z0 = 0.0, float(zs.mean())
+    else:
+        A = np.stack([np.ones(N), beta], 1)
+        (z0, h), *_ = np.linalg.lstsq(A, zs, rcond=None)
+        z0, h = float(z0), float(h)
+    resid = float(np.max(np.abs(zs - (z0 + h * beta))))
+    if resid > HELIX_FIT_TOLERANCE * dz:
+        raise ValueError(f"fdk helical: the volume's z is not affine in the view angle (a residual of {resid / dz:.3g} "
+                         f"voxels after fitting z = z0 + h beta; at most {HELIX_FIT_TOLERANCE:g})")
+    step = (beta[-1] - beta[0]) / (N - 1)
+    beta_lo, beta_hi = beta[0] - 0.5 * step, beta[-1] + 0.5 * step
+    if beta_hi - beta_lo < 2.0 * math.pi - ARC_TOLERANCE:
+        raise ValueError(f"fdk helical: the views cover an arc of {math.degrees(beta_hi - beta_lo):.2f} degrees; the "
+                         "helical weights need at least 360 (a circular short scan takes short_scan=True)")
+    edges = np.concatenate([[beta_lo], 0.5 * (beta[1:] + beta[:-1]), [beta_hi]])
+    c = grid[:2] - pos[0, :2]
+    return Helix(order, beta, np.diff(edges), z0, h, float(beta_lo), float(beta_hi), float(c[0]), float(c[1]))
 
 
 def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool = False, use_offDetector: bool = False,
-        half_fan: bool = False, filter: str | None = None, view_geometry=None) -> torch.Tensor:
+        half_fan: bool = False, filter: str | None = None, view_geometry=None, helical: bool = False,
+        helical_q: float = HELICAL_Q) -> torch.Tensor:
     filt = check_filter(filter, scanner_cfg)
+    if helical:
+        for flag, on in (("short_scan", short_scan), ("half_fan", half_fan)):
+            if on:
+                raise ValueError(f"fdk: helical cannot be combined with {flag} (its redundancy weights assume one fixed "
+                                 "circle)")
+        if view_geometry is None:
+            raise ValueError("fdk: helical needs view_geometry (the helix is read from the views' offOrigin)")
+        if not (isinstance(helical_q, (int, float)) and 0.0 <= float(helical_q) <= 1.0):
+            raise ValueError(f"fdk: helical_q must be in [0, 1], got {helical_q!r}")
     if view_geometry is not None:
-        check_view_geometry(scanner_cfg, view_geometry, short_scan, half_fan)
+        check_view_geometry(scanner_cfg, view_geometry, short_scan, half_fan, helical)
         use_offDetector = True
+    if helical:
+        return _fdk_helical(projections, angles, scanner_cfg, filt, list(view_geometry), float(helical_q))
     if half_fan and not use_offDetector:
         raise ValueError("fdk: half_fan needs use_offDetector=True (the half-fan weights follow the detector offset)")
     if half_fan and short_scan:
@@ -240,4 +343,46 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool =
                              None if vw is None else vw.data_ptr(), float(arc), float(scanner_cfg["DSO"]), nx, ny, nz,
                              sx, sy, sz, cx, cy, cz, vol.data_ptr(), scratch.data_ptr(), nbytes)
     check(rc, "r2x_fdk")
+    return vol
+
+
+def _fdk_helical(projections, angles, scanner_cfg: dict, filt: str, view_geometry, q: float) -> torch.Tensor:
+    """fdk(helical=True) after the keyword refusals: the helix fit, the views in beta order, r2x_fdk_helical."""
+    hx = helix_views(angles, scanner_cfg, view_geometry)
+    if not isinstance(projections, torch.Tensor) or projections.device.type != "cuda":
+        raise RuntimeError("fdk: projections must be a CUDA tensor (this build has no CPU fallback; "
+                           f"got {getattr(projections, 'device', type(projections))})")
+    if projections.dim() != 3:
+        raise ValueError(f"fdk: expected projections of shape [N, H, W], got {tuple(projections.shape)}")
+    angles = np.asarray(angles, dtype=np.float64).reshape(-1)
+    N, H, W = (int(s) for s in projections.shape)
+    if len(angles) != N:
+        raise ValueError(f"fdk: {N} projections but {len(angles)} angles")
+    if (H, W) != (int(scanner_cfg["nDetector"][0]), int(scanner_cfg["nDetector"][1])):
+        raise ValueError(f"fdk: projections are {H}x{W}, scanner nDetector is {list(scanner_cfg['nDetector'])}")
+    from .projector import view_table
+    views, table = view_table(angles[hx.order], scanner_cfg, [view_geometry[i] for i in hx.order])
+    nx, ny, nz = (int(v) for v in scanner_cfg["nVoxel"])
+    sx, sy, sz = (float(v) for v in scanner_cfg["sVoxel"])
+    cx, cy, cz = (float(v) for v in scanner_cfg["offOrigin"])
+    dev = projections.device
+    lib = load()
+    with torch.cuda.device(dev):
+        order = torch.from_numpy(np.ascontiguousarray(hx.order)).to(dev)
+        projs = projections.detach().to(torch.float32).index_select(0, order).contiguous()
+        vm = torch.from_numpy(np.stack([v.viewmatrix.reshape(16) for v in views])).to(dev)
+        pm = torch.from_numpy(np.stack([v.projmatrix.reshape(16) for v in views])).to(dev)
+        beta_host = np.ascontiguousarray(hx.beta, np.float64)
+        beta = torch.from_numpy(beta_host).to(dev)
+        dbeta = torch.from_numpy(np.ascontiguousarray(hx.dbeta, np.float64)).to(dev)
+        vol = torch.empty((nx, ny, nz), dtype=torch.float32, device=dev)
+        nbytes = int(lib.r2x_fdk_scratch_bytes(N, H, W))
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        rc = lib.r2x_fdk_helical(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(),
+                                 float(table[0, 0]), float(table[0, 1]), int(views[0].mode), FILTERS.index(filt) << 8,
+                                 float(table[0, 4]), beta.data_ptr(), dbeta.data_ptr(), beta_host.ctypes.data, hx.z0,
+                                 hx.h, hx.beta_lo, hx.beta_hi, hx.c_x, hx.c_y, q, nx, ny, nz, sx, sy, sz, cx, cy, cz,
+                                 vol.data_ptr(), scratch.data_ptr(), nbytes)
+    check(rc, "r2x_fdk_helical")
     return vol

@@ -4,7 +4,7 @@
         [--recon_method random|fdk|cgls|fista_tv|volume] [--recon recon.npy] [--n_points 50000] [--density_thresh 0.05]
         [--density_rescale 0.15] [--random_density_max 1.0] [--evaluate] [--short_scan] [--use_offDetector]
         [--estimate_offDetector] [--half_fan] [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
-        [--use_view_geometry]
+        [--use_view_geometry [--helical [--helical_q Q]]]
 
 `random` draws positions uniformly in the volume and densities in [0, random_density_max) with numpy's global
 generator seeded with 0, exactly like the reference.  `fdk` reconstructs the volume from the train views with the
@@ -29,7 +29,9 @@ them on the scene grid and prints their 3D PSNR against the ground-truth volume 
 
 `--use_view_geometry` (fdk, cgls and fista_tv) reconstructs through each train view's own DSO, DSD, offOrigin and
 offDetector (`recon.recon_volume(view_geometry=...)`); the fdk default is refused for a helical scan, whose offOrigin
-varies, in favour of `--recon_method cgls`.
+varies, in favour of `--recon_method cgls`, unless `--helical` asks for the helically weighted FDK
+(`fdk.fdk(helical=True, helical_q=Q)`; fdk with --use_view_geometry only, not with --short_scan, --half_fan or
+--estimate_offDetector).  The helix is fitted (`fdk.helix_views`) before any CUDA work.
 
 The default `--recon_method` is `random` (the reference defaults to `fdk`).
 """
@@ -41,8 +43,8 @@ import os
 import numpy as np
 
 from .dataset import init_point_cloud, read_scene
-from .recon import (add_estimate_flag, add_fdk_filter_flag, add_view_geometry_flag, check_fdk_flags,
-                    check_view_geometry_flags, view_geometry_of)
+from .recon import (add_estimate_flag, add_fdk_filter_flag, add_helical_flags, add_view_geometry_flag, check_fdk_flags,
+                    check_helical_flags, check_view_geometry_flags, view_geometry_of)
 from .trainer import default_init_path
 
 # A filtered backprojection from a handful of views is dominated by streaks, and thresholding it gives no useful
@@ -59,7 +61,8 @@ def _require_cuda_for(method: str):
 
 
 def recon_train_views(info, method: str, short_scan: bool = False, use_offDetector: bool = False,
-                      half_fan: bool = False, fdk_filter: str | None = None, use_view_geometry: bool = False) -> np.ndarray:
+                      half_fan: bool = False, fdk_filter: str | None = None, use_view_geometry: bool = False,
+                      helical: bool = False, helical_q: float | None = None) -> np.ndarray:
     """`recon.recon_volume(..., method, short_scan, use_offDetector, half_fan, fdk_filter, view_geometry)` of the train
     views of a `read_scene` result, as a host float32 [nx, ny, nz] array."""
     import torch
@@ -69,7 +72,8 @@ def recon_train_views(info, method: str, short_scan: bool = False, use_offDetect
     projs = torch.from_numpy(np.stack([np.asarray(c.image, np.float32) for c in info.train_cameras])).cuda()
     vol = recon_volume(projs, [c.angle for c in info.train_cameras], info.scanner_cfg, method, short_scan=short_scan,
                        use_offDetector=use_offDetector, half_fan=half_fan, fdk_filter=fdk_filter,
-                       view_geometry=view_geometry_of(info.train_cameras, use_view_geometry))
+                       view_geometry=view_geometry_of(info.train_cameras, use_view_geometry), helical=helical,
+                       helical_q=helical_q)
     return vol.cpu().numpy()
 
 
@@ -121,7 +125,10 @@ def main(argv=None) -> str:
     add_fdk_filter_flag(ap, "with --recon_method fdk: the ramp filter")
     add_estimate_flag(ap, "with --recon_method fdk, cgls or fista_tv: reconstruct")
     add_view_geometry_flag(ap, "with --recon_method fdk, cgls or fista_tv: reconstruct")
+    add_helical_flags(ap)
     a = ap.parse_args(argv)
+    check_helical_flags(a, a.recon_method == "fdk", f"{{flag}} applies to --recon_method fdk only, not "
+                        f"{a.recon_method}: the iterative methods need no redundancy weights")
     check_view_geometry_flags(a)
     if a.use_view_geometry and a.recon_method not in ("fdk", "cgls", "fista_tv"):
         raise SystemExit(f"--use_view_geometry applies to --recon_method fdk, cgls or fista_tv, not {a.recon_method}: "
@@ -135,11 +142,18 @@ def main(argv=None) -> str:
         raise SystemExit(f"--estimate_offDetector applies to --recon_method fdk, cgls or fista_tv, not "
                          f"{a.recon_method}: no projections are reconstructed")
     if a.use_view_geometry and a.recon_method == "fdk":
-        from .fdk import helical
+        from .fdk import helical, helix_views
         scene = read_scene(os.path.abspath(a.data), eval=False, use_view_geometry=True)
-        if helical(scene.scanner_cfg, view_geometry_of(scene.train_cameras, True)):
+        if a.helical:
+            try:
+                helix_views([c.angle for c in scene.train_cameras], scene.scanner_cfg,
+                            view_geometry_of(scene.train_cameras, True))
+            except ValueError as e:
+                raise SystemExit(f"--helical: {e}") from e
+        elif helical(scene.scanner_cfg, view_geometry_of(scene.train_cameras, True)):
             raise SystemExit("--recon_method fdk cannot reconstruct a helical scan (the train views' offOrigin varies and "
-                             "FDK has no helical weighting): use --recon_method cgls (or fista_tv)")
+                             "FDK has no helical weighting): use --recon_method cgls (or fista_tv), or --helical for "
+                             "FDK's approximate helical weighting")
     if a.recon_method in ("fdk", "cgls", "fista_tv"):
         _require_cuda_for(a.recon_method)
     np.random.seed(0)                                    # initialize_pcd.py:23
@@ -164,7 +178,7 @@ def main(argv=None) -> str:
             info.scanner_cfg, _ = estimated_scanner(info, a.use_offDetector)
             use_off = True
         recon = recon_train_views(info, a.recon_method, a.short_scan, use_off or a.use_view_geometry, a.half_fan,
-                                  a.fdk_filter, a.use_view_geometry)
+                                  a.fdk_filter, a.use_view_geometry, a.helical, a.helical_q)
     pts = init_point_cloud(info.scanner_cfg, a.n_points, recon=recon, density_thresh=a.density_thresh,
                            density_rescale=a.density_rescale, random_density_max=a.random_density_max)
     np.save(out, pts)

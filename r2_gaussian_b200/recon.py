@@ -73,7 +73,7 @@ their adaptive step and stop rules are defined by TIGRE's implementation.  `cp_t
 
     python -m r2_gaussian_b200.recon -s <scene> -m <output> [--methods fdk,sart,cgls] [--short_scan]
         [--use_offDetector] [--estimate_offDetector] [--half_fan] [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
-        [--use_view_geometry]
+        [--use_view_geometry [--helical [--helical_q Q]]]
 
 mirrors `scripts/run_traditional_methods.py`: it reconstructs the scene's train views with each method, scores the
 volume against `vol_gt` with `metrics.metric_vol` and writes, per method, `<output>/<method>/ct_gt.npy`, `ct_pred.npy`,
@@ -95,7 +95,10 @@ test-view projections, with a copy of the scanner whose offDetector[0] is that t
 refuses a scanner whose `filter` names a window.  `--use_view_geometry` reconstructs and reprojects every method
 through each view's own DSO, DSD, offOrigin and offDetector (the frames' keys, `scene.view_scanner`; reports add
 `use_view_geometry: true`); fdk then refuses a helical scan (an offOrigin that varies), and the flag is refused with
---estimate_offDetector, --half_fan and --short_scan, which assume one fixed circle.
+--estimate_offDetector, --half_fan and --short_scan, which assume one fixed circle.  `--helical` (with it) reconstructs
+fdk with helical redundancy weights instead (`fdk.fdk(helical=True, helical_q=Q)`; the report adds `helical: true` and
+`helical_q`); it is refused without --use_view_geometry, when --methods has no fdk, and with --short_scan, --half_fan
+and --estimate_offDetector.  cp_tv's tolerance keeps the CGLS volume in the plain FDK's place on a helical scan.
 """
 from __future__ import annotations
 
@@ -349,12 +352,13 @@ def cp_tv(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = CP_NITER,
 
 def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, short_scan: bool = False,
                  use_offDetector: bool = False, half_fan: bool = False, fdk_filter: str | None = None,
-                 view_geometry=None) -> torch.Tensor:
+                 view_geometry=None, helical: bool = False, helical_q: float | None = None) -> torch.Tensor:
     """The reconstructions of ct_utils.recon_volume / run_ct_recon_algs with their iteration counts.  `short_scan`
-    selects the Parker-weighted FDK, `half_fan` the half-fan-weighted one and `fdk_filter` FDK's ramp filter
-    (`fdk.fdk(filter=...)`); all three apply to method fdk only.  `use_offDetector` reconstructs through the scanner's
-    offDetector (every method), `view_geometry` through each view's own geometry (every method; `projector.project`)."""
-    for flag, on in (("short_scan", short_scan), ("half_fan", half_fan)):
+    selects the Parker-weighted FDK, `half_fan` the half-fan-weighted one, `helical` (with `helical_q`, None for
+    fdk.HELICAL_Q) the helical one and `fdk_filter` FDK's ramp filter (`fdk.fdk(filter=...)`); all four apply to
+    method fdk only.  `use_offDetector` reconstructs through the scanner's offDetector (every method), `view_geometry`
+    through each view's own geometry (every method; `projector.project`)."""
+    for flag, on in (("short_scan", short_scan), ("half_fan", half_fan), ("helical", helical)):
         if on and method != "fdk":
             raise ValueError(f"recon_volume: {flag} applies to fdk only, not {method!r} (the iterative methods need no "
                              "redundancy weights)")
@@ -363,10 +367,11 @@ def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, sh
                          "ramp filter)")
     off = use_offDetector
     if method == "fdk":
-        from .fdk import fdk
+        from .fdk import HELICAL_Q, fdk
 
         return fdk(projs, angles, scanner_cfg, short_scan=short_scan, use_offDetector=off, half_fan=half_fan,
-                   filter=fdk_filter, view_geometry=view_geometry)
+                   filter=fdk_filter, view_geometry=view_geometry, helical=helical,
+                   helical_q=HELICAL_Q if helical_q is None else helical_q)
     vg = view_geometry
     if method == "cgls":
         return cgls(projs, angles, scanner_cfg, CGLS_NITER, use_offDetector=off, view_geometry=vg)[0]
@@ -403,6 +408,37 @@ def add_fdk_filter_flag(ap, help_text: str):
     ap.add_argument("--fdk_filter", default=None, choices=FILTERS, metavar="NAME",
                     help=f"{help_text}: {', '.join(FILTERS)} (TIGRE's names; default: the scanner's filter, which must "
                          "then be null or ram_lak)")
+
+
+def add_helical_flags(ap):
+    """--helical and --helical_q Q on a CLI's parser."""
+    from .fdk import HELICAL_Q
+
+    ap.add_argument("--helical", default=False, action="store_true",
+                    help="with --use_view_geometry: reconstruct fdk with helical redundancy weights (fdk.fdk(helical="
+                         "True); a helical scan, or a circle of 360 degrees or more)")
+    ap.add_argument("--helical_q", default=None, type=float, metavar="Q",
+                    help=f"with --helical: the fraction of the detector's half-height weighted fully before the "
+                         f"weights fall to 0 at its edge, in [0, 1] (default {HELICAL_Q})")
+
+
+def check_helical_flags(args, fdk_selected: bool, not_fdk: str):
+    """The refusals of --helical and --helical_q that the recon and initialize_pcd CLIs share, before any CUDA work;
+    `not_fdk` as for check_fdk_flags."""
+    if args.helical_q is not None and not args.helical:
+        raise SystemExit("--helical_q applies with --helical only")
+    if not args.helical:
+        return
+    if not fdk_selected:
+        raise SystemExit(not_fdk.format(flag="--helical"))
+    if not args.use_view_geometry:
+        raise SystemExit("--helical needs --use_view_geometry: the helix is read from the views' offOrigin")
+    for flag in ("--short_scan", "--half_fan", "--estimate_offDetector"):
+        if getattr(args, flag[2:], False):
+            raise SystemExit(f"--helical cannot be combined with {flag} (its weights or its estimate assume one fixed "
+                             "circle)")
+    if args.helical_q is not None and not 0.0 <= args.helical_q <= 1.0:
+        raise SystemExit(f"--helical_q must be in [0, 1], got {args.helical_q}")
 
 
 def add_estimate_flag(ap, what: str):
@@ -466,10 +502,13 @@ def main(argv=None) -> dict:
     add_fdk_filter_flag(ap, "reconstruct fdk with this ramp filter")
     add_estimate_flag(ap, "reconstruct and reproject every method")
     add_view_geometry_flag(ap, "reconstruct and reproject every method")
+    add_helical_flags(ap)
     a = ap.parse_args(argv)
     methods = _parse_methods(a.methods)
     check_fdk_flags(a, "fdk" in methods, "{flag} applies to the fdk method, which --methods does not include (the "
                     "iterative methods need no redundancy weights)")
+    check_helical_flags(a, "fdk" in methods, "{flag} applies to the fdk method, which --methods does not include (the "
+                        "iterative methods need no redundancy weights)")
     check_view_geometry_flags(a)
     if not torch.cuda.is_available():
         raise SystemExit("the reconstructions need a CUDA device: they run on the GPU and have no CPU fallback")
@@ -484,6 +523,12 @@ def main(argv=None) -> dict:
     cfg = info.scanner_cfg
     vg_train = view_geometry_of(info.train_cameras, a.use_view_geometry)
     vg_test = view_geometry_of(info.test_cameras, a.use_view_geometry)
+    if a.helical:
+        from .fdk import helix_views
+        try:
+            helix_views([c.angle for c in info.train_cameras], cfg, vg_train)
+        except ValueError as e:
+            raise SystemExit(f"--helical: {e}") from e
     projs_train = torch.from_numpy(np.stack([np.asarray(c.image, np.float32) for c in info.train_cameras])).cuda()
     train_angles = [c.angle for c in info.train_cameras]
     test_angles = [c.angle for c in info.test_cameras]
@@ -503,6 +548,7 @@ def main(argv=None) -> dict:
         t0 = time.time()
         short_scan = a.short_scan and method == "fdk"
         half_fan = a.half_fan and method == "fdk"
+        helical_fdk = a.helical and method == "fdk"
         fdk_filter = a.fdk_filter if method == "fdk" else None
         extra = {}
         if method == "cp_tv":
@@ -513,7 +559,7 @@ def main(argv=None) -> dict:
         else:
             pred = recon_volume(projs_train, train_angles, cfg, method, short_scan=short_scan,
                                 use_offDetector=use_off, half_fan=half_fan, fdk_filter=fdk_filter,
-                                view_geometry=vg_train)
+                                view_geometry=vg_train, helical=helical_fdk, helical_q=a.helical_q)
         torch.cuda.synchronize()
         duration = time.time() - t0
         ct_pred = pred.cpu().numpy()
@@ -528,6 +574,10 @@ def main(argv=None) -> dict:
             report["short_scan"] = True
         if half_fan:
             report["half_fan"] = True
+        if helical_fdk:
+            from .fdk import HELICAL_Q
+            report["helical"] = True
+            report["helical_q"] = float(HELICAL_Q if a.helical_q is None else a.helical_q)
         if fdk_filter not in (None, "ram_lak"):
             report["filter"] = fdk_filter
         if a.use_offDetector:
