@@ -461,6 +461,23 @@ int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const f
             const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
             int weighting, const float* view_weights, float arc, float dso, int nx, int ny, int nz, float sx, float sy,
             float sz, float cx, float cy, float cz, float* out_volume, void* scratch, size_t scratch_bytes);
+/* r2x_fdk of a laterally truncated scan (the object wider than the detector's field of view): r2x_fdk's arguments and
+ * scratch plus a pad of L = `pad` pixels, 0 <= L <= W, that extends each row past its edges before step 2 so that the
+ * filter does not see a step there (Ohnesorge et al., Med. Phys. 27(1), 2000; float64 statement in
+ * tests/fdk_pad_oracle.py).  Per detector row, after step 1 (cosine and any Parker weight), with r[0 .. W-1] the
+ * weighted row:
+ *   e[i] = r[i] for 0 <= i < W;  e[-k] = t_k r[k-1] and e[W-1+k] = t_k r[W-k] for k = 1 .. L, where
+ *   t_k = (1 + cos(pi k / (L + 1))) / 2: a mirror about each edge, rolled off to zero;
+ *   Q_j = (1 / D) sum_{i=-L}^{W-1+L} h[j-i] e[i] for 0 <= j < W, with the taps h of the filter field.
+ * Only Q_0 .. Q_{W-1} are written and backprojected (step 3 unchanged).  L = 0 is r2x_fdk bit for bit.  Refuses, before
+ * any CUDA work, pad < 0, pad > W, R2X_FDK_HALF_FAN (a shifted detector's truncation is deliberate and its weights
+ * handle it) and a padded row whose stage exceeds 227 KB of shared memory ((3 W + 2 L + ceil((W + L) / 2)) floats for
+ * Ram-Lak, (2 W + 3 L) for a window: any pad up to W = 9685), then everything r2x_fdk refuses. */
+int r2x_fdk_pad(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
+                int weighting, const float* view_weights, float arc, float dso, int nx, int ny, int nz, float sx,
+                float sy, float sz, float cx, float cy, float cz, float* out_volume, void* scratch, size_t scratch_bytes,
+                int pad);
 /* The two stages of r2x_fdk on their own (measurement; centred, R2X_FDK_PLAIN, Ram-Lak): filtered[N,H,W] = steps 1-2;
  * out_volume = step 3 of it. */
 int r2x_fdk_filter(void* stream, int n_views, int H, int W, const float* projs, float tan_fovx, float tan_fovy,

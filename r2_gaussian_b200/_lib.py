@@ -93,6 +93,8 @@ PROTOTYPES = {
     "r2x_fdk_scratch_bytes": (_sz, [_i, _i, _i]),
     "r2x_fdk": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _f, _f, _i, _vp, _f, _f, _i, _i, _i, _f, _f, _f, _f, _f,
                      _f, _vp, _vp, _sz]),
+    "r2x_fdk_pad": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _i, _f, _f, _i, _vp, _f, _f, _i, _i, _i, _f, _f, _f, _f,
+                         _f, _f, _vp, _vp, _sz, _i]),
     "r2x_fdk_filter": (_i, [_vp, _i, _i, _i, _vp, _f, _f, _i, _f, _vp]),
     "r2x_fdk_backproject": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _i, _f, _i, _i, _i, _f, _f, _f, _f, _f, _f, _vp]),
     "r2x_volume_project": (_i, [_vp, _i, _i, _i, _vp, _f, _f, _f, _f, _f, _f, _i, _i, _i, _vp, _f, _f, _i, _f, _f, _f,

@@ -64,6 +64,10 @@ size_t fdk_scratch_bytes(int N, int H, int W) {
 
 static size_t fdk_filter_smem(int W) { return (size_t)(3 * W + (W + 1) / 2) * sizeof(float); }
 static size_t fdk_window_smem(int W) { return (size_t)(2 * W) * sizeof(float); }
+// with a pad of L pixels (r2x_fdk_pad): the extended row takes 2 L more samples and the taps reach W - 1 + L
+static size_t fdk_filter_pad_smem(int W, int L) { return (size_t)(3 * W + 2 * L + (W + L + 1) / 2) * sizeof(float); }
+static size_t fdk_window_pad_smem(int W, int L) { return (size_t)(2 * W + 3 * L) * sizeof(float); }
+constexpr size_t FDK_SMEM_OPTIN = 227 * 1024;   // an sm_90 CTA's largest dynamic shared memory
 
 // TABLE: each view's DSO from its row of the per-view geometry table `vg`; without it `dso` for every view.
 template <bool CONE, bool TABLE>
@@ -233,35 +237,50 @@ __device__ __forceinline__ void fdk_weight_row(size_t r, int H, int W, const flo
     }
 }
 
+// The truncation pad of r2x_fdk_pad (model in include/r2x.h): weighted pixel j of a row e[0 .. W-1] is also mirrored
+// into the extension, e[-k] = t_k r[k-1] and e[W-1+k] = t_k r[W-k] for k = 1 .. L, with the roll-off
+// t_k = (1 + cos(pi k / (L + 1))) / 2 rounded once from float64.  Each pixel has at most one image on each side, so
+// the weighting pass writes the whole extended row with no extra barrier.
+__device__ __forceinline__ float fdk_pad_taper(int k, int L) {
+    return (float)(0.5 * (1.0 + cospi((double)k / (double)(L + 1))));
+}
+__device__ __forceinline__ void fdk_pad_mirror(float* __restrict__ e, int W, int L, int j, float p) {
+    if (j < L) e[-(j + 1)] = fdk_pad_taper(j + 1, L) * p;
+    if (W - j <= L) e[2 * W - 1 - j] = fdk_pad_taper(W - j, L) * p;
+}
+
 // Steps 1-2 of FDK with the band-limited Ram-Lak filter, one CTA per detector row: fdk_weight_row, the row staged in
 // shared memory between two rows of zeros and filtered with the Ram-Lak taps (shift-invariant, so the same for any
-// offset).
-template <int WEIGHT, bool TABLE>
+// offset).  PAD (r2x_fdk_pad): the row is extended by `pad` mirrored, rolled-off pixels on each side
+// (fdk_pad_mirror) before the zeros, and the taps reach W - 1 + pad; only the W measured pixels are written.
+template <int WEIGHT, bool TABLE, bool PAD = false>
 __global__ void __launch_bounds__(256) fdk_filter_kernel(int H, int W, const float* __restrict__ projs, float tanx,
                                                          float tany, int cone, float inv_delta, float su, float sv,
                                                          FdkWeights fw, const double* __restrict__ vg,
-                                                         float* __restrict__ q) {
+                                                         float* __restrict__ q, int pad) {
     extern __shared__ float sm[];
-    float* row = sm;              // [3W]: zeros | weighted row | zeros
-    float* g = sm + 3 * W;        // [(W+1)/2]: g[m] = 1 / (pi^2 (2m+1)^2)
-    const size_t r = blockIdx.x;  // view * H + detector row
+    const int L = PAD ? pad : 0;
+    float* row = sm;                  // [3W + 2L]: zeros | e[-L .. W-1+L] | zeros
+    float* g = sm + 3 * W + 2 * L;    // [(W+L+1)/2]: g[m] = 1 / (pi^2 (2m+1)^2)
+    const size_t r = blockIdx.x;      // view * H + detector row
     if (TABLE) fdk_view_row(vg + (r / H) * VG_COLS, H, W, cone, tanx, tany, inv_delta, su, sv);
     fdk_weight_row<WEIGHT>(r, H, W, projs, tanx, tany, cone, su, sv, fw, [&](int j, float p) {
         row[j] = 0.0f;
-        row[W + j] = p;
-        row[2 * W + j] = 0.0f;
+        row[W + L + j] = p;
+        row[2 * W + 2 * L + j] = 0.0f;
+        if (PAD) fdk_pad_mirror(row + W + L, W, L, j, p);
     });
-    for (int m = threadIdx.x; m < (W + 1) / 2; m += blockDim.x) {
+    for (int m = threadIdx.x; m < (W + L + 1) / 2; m += blockDim.x) {
         const float k = (float)(2 * m + 1);
         g[m] = 1.0f / (9.869604401089358f * k * k);
     }
     __syncthreads();
     for (int j = threadIdx.x; j < W; j += blockDim.x) {
-        const float* c = row + W + j;
+        const float* c = row + W + L + j;
         // smallest taps first: summed from k = 1 up, the accumulator is near r_j / 4 after a few taps and every tap
         // below half its ulp (k beyond ~3700) is lost, which truncated the filter on wide rows
         float acc = 0.0f;
-        for (int m = W / 2 - 1; m >= 0; --m) acc = fmaf(g[m], c[-(2 * m + 1)] + c[2 * m + 1], acc);
+        for (int m = (W + L) / 2 - 1; m >= 0; --m) acc = fmaf(g[m], c[-(2 * m + 1)] + c[2 * m + 1], acc);
         q[r * W + j] = fmaf(0.25f, c[0], -acc) * inv_delta;
     }
 }
@@ -293,24 +312,29 @@ __device__ __forceinline__ double fdk_window_tap(int k) {
 // h[0 .. W-1] rounded once from float64 next to it, then the linear convolution over the whole row.  Pixel j's partner
 // pixels j - k and j + k both lie in the row for k <= near = min(j, W-1-j), one of them up to far = max(j, W-1-j);
 // the sum runs from k = far down to 1, smallest taps first (as fdk_filter_kernel's), with no bounds checks in either
-// loop.
-template <int WEIGHT, int WINDOW, bool TABLE>
+// loop.  PAD (r2x_fdk_pad): the staged row is the extended row e[-pad .. W-1+pad] (fdk_pad_mirror), the taps run to
+// h[W-1+pad], and pixel j's partners reach j + pad to its left and W - 1 + pad - j to its right.
+template <int WEIGHT, int WINDOW, bool TABLE, bool PAD = false>
 __global__ void __launch_bounds__(256) fdk_window_kernel(int H, int W, const float* __restrict__ projs, float tanx,
                                                          float tany, int cone, float inv_delta, float su, float sv,
                                                          FdkWeights fw, const double* __restrict__ vg,
-                                                         float* __restrict__ q) {
+                                                         float* __restrict__ q, int pad) {
     extern __shared__ float sm[];
-    float* row = sm;              // [W]: weighted row
-    float* h = sm + W;            // [W]: h[k]
-    const size_t r = blockIdx.x;  // view * H + detector row
+    const int L = PAD ? pad : 0;
+    float* row = sm;                  // [W + 2L]: e[-L .. W-1+L]
+    float* h = sm + W + 2 * L;        // [W + L]: h[k]
+    const size_t r = blockIdx.x;      // view * H + detector row
     if (TABLE) fdk_view_row(vg + (r / H) * VG_COLS, H, W, cone, tanx, tany, inv_delta, su, sv);
-    fdk_weight_row<WEIGHT>(r, H, W, projs, tanx, tany, cone, su, sv, fw, [&](int j, float p) { row[j] = p; });
-    for (int k = threadIdx.x; k < W; k += blockDim.x) h[k] = (float)fdk_window_tap<WINDOW>(k);
+    fdk_weight_row<WEIGHT>(r, H, W, projs, tanx, tany, cone, su, sv, fw, [&](int j, float p) {
+        row[L + j] = p;
+        if (PAD) fdk_pad_mirror(row + L, W, L, j, p);
+    });
+    for (int k = threadIdx.x; k < W + L; k += blockDim.x) h[k] = (float)fdk_window_tap<WINDOW>(k);
     __syncthreads();
     for (int j = threadIdx.x; j < W; j += blockDim.x) {
-        const float* c = row + j;
-        const int near = min(j, W - 1 - j), far = max(j, W - 1 - j);
-        const int side = j < W - 1 - j ? 1 : -1;   // the partner that stays in the row beyond `near`
+        const float* c = row + L + j;
+        const int near = min(j + L, W - 1 + L - j), far = max(j + L, W - 1 + L - j);
+        const int side = j + L < W - 1 + L - j ? 1 : -1;   // the partner that stays in the row beyond `near`
         float acc = 0.0f;
         for (int k = far; k > near; --k) acc = fmaf(h[k], c[side * k], acc);
         for (int k = near; k > 0; --k) acc = fmaf(h[k], c[-k] + c[k], acc);
@@ -319,34 +343,43 @@ __global__ void __launch_bounds__(256) fdk_window_kernel(int H, int W, const flo
 }
 
 using FdkFilterKernel = void (*)(int, int, const float*, float, float, int, float, float, float, FdkWeights,
-                                 const double*, float*);
+                                 const double*, float*, int);
 
-template <int WEIGHT, bool TABLE>
+template <int WEIGHT, bool TABLE, bool PAD = false>
 static FdkFilterKernel fdk_filter_for(int window) {
     switch (window) {
-        case R2X_FDK_SHEPP_LOGAN: return fdk_window_kernel<WEIGHT, R2X_FDK_SHEPP_LOGAN, TABLE>;
-        case R2X_FDK_COSINE: return fdk_window_kernel<WEIGHT, R2X_FDK_COSINE, TABLE>;
-        case R2X_FDK_HAMMING: return fdk_window_kernel<WEIGHT, R2X_FDK_HAMMING, TABLE>;
-        case R2X_FDK_HANN: return fdk_window_kernel<WEIGHT, R2X_FDK_HANN, TABLE>;
-        default: return fdk_filter_kernel<WEIGHT, TABLE>;
+        case R2X_FDK_SHEPP_LOGAN: return fdk_window_kernel<WEIGHT, R2X_FDK_SHEPP_LOGAN, TABLE, PAD>;
+        case R2X_FDK_COSINE: return fdk_window_kernel<WEIGHT, R2X_FDK_COSINE, TABLE, PAD>;
+        case R2X_FDK_HAMMING: return fdk_window_kernel<WEIGHT, R2X_FDK_HAMMING, TABLE, PAD>;
+        case R2X_FDK_HANN: return fdk_window_kernel<WEIGHT, R2X_FDK_HANN, TABLE, PAD>;
+        default: return fdk_filter_kernel<WEIGHT, TABLE, PAD>;
     }
 }
 
-// window: R2X_FDK_RAM_LAK or one of the windowed filters (r2x_fdk's filter field)
+// the filter stage's dynamic shared memory with a pad of L pixels (the unpadded layouts at L = 0)
+static size_t fdk_filter_stage_smem(int window, int W, int L) {
+    if (L == 0) return window == R2X_FDK_RAM_LAK ? fdk_filter_smem(W) : fdk_window_smem(W);
+    return window == R2X_FDK_RAM_LAK ? fdk_filter_pad_smem(W, L) : fdk_window_pad_smem(W, L);
+}
+
+// window: R2X_FDK_RAM_LAK or one of the windowed filters (r2x_fdk's filter field); pad: r2x_fdk_pad's L (0 runs the
+// unpadded kernels; a pad comes without a table and without R2X_FDK_HALF_FAN)
 static int fdk_filter(cudaStream_t st, int weighting, int window, int N, int H, int W, const float* projs, float tanx,
                       float tany, int mode, float dso, float su, float sv, const FdkWeights& fw, const double* vg,
-                      float* q) {
+                      float* q, int pad = 0) {
     // a table comes with R2X_FDK_PLAIN only (r2x_fdk_views)
-    auto kernel = vg                              ? fdk_filter_for<R2X_FDK_PLAIN, true>(window)
+    auto kernel = pad > 0 ? (weighting == R2X_FDK_PARKER ? fdk_filter_for<R2X_FDK_PARKER, false, true>(window)
+                                                         : fdk_filter_for<R2X_FDK_PLAIN, false, true>(window))
+                  : vg                            ? fdk_filter_for<R2X_FDK_PLAIN, true>(window)
                   : weighting == R2X_FDK_PARKER   ? fdk_filter_for<R2X_FDK_PARKER, false>(window)
                   : weighting == R2X_FDK_HALF_FAN ? fdk_filter_for<R2X_FDK_HALF_FAN, false>(window)
                                                   : fdk_filter_for<R2X_FDK_PLAIN, false>(window);
-    const size_t smem = window == R2X_FDK_RAM_LAK ? fdk_filter_smem(W) : fdk_window_smem(W);
+    const size_t smem = fdk_filter_stage_smem(window, W, pad);
     if (smem > 48 * 1024)
         R2X_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<(unsigned)((long long)N * H), 256, smem, st>>>(H, W, projs, tanx, tany, mode,
                                                             (float)(1.0 / fdk_pitch(W, tanx, mode, dso)), su, sv, fw, vg,
-                                                            q);
+                                                            q, pad);
     R2X_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -391,7 +424,7 @@ static int fdk_run(void* stream, int n_views, int H, int W, const float* projs, 
                    const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
                    int weighting, const float* view_weights, float arc, float dso, int nx, int ny, int nz, float sx,
                    float sy, float sz, float cx, float cy, float cz, float* out_volume, void* scratch,
-                   size_t scratch_bytes, const double* vg) {
+                   size_t scratch_bytes, const double* vg, int pad = 0) {
     if (int rc = fdk_validate(n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode, dso, nx, ny,
                               nz, sx, sy, sz, out_volume, scratch, scratch_bytes))
         return rc;
@@ -434,7 +467,7 @@ static int fdk_run(void* stream, int n_views, int H, int W, const float* projs, 
     float* q = (float*)(((size_t)scratch + 255) & ~(size_t)255);
     const float su = (float)(2.0 * (double)shift_u / W), sv = (float)(-2.0 * (double)shift_v / H);
     if (int rc = fdk_filter(st, weighting, window, n_views, H, W, projs, tan_fovx, tan_fovy, mode, dso, su, sv, fw, vg,
-                            q))
+                            q, pad))
         return rc;
     // Parker's dbeta_v already holds each view's share of the arc
     const float scale = weighting == R2X_FDK_PARKER ? 1.0f : (float)(pi / n_views);
@@ -713,6 +746,24 @@ int r2x_fdk(void* stream, int n_views, int H, int W, const float* projs, const f
     return r2x::fdk_run(stream, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode, shift_u,
                         shift_v, weighting, view_weights, arc, dso, nx, ny, nz, sx, sy, sz, cx, cy, cz, out_volume,
                         scratch, scratch_bytes, nullptr);
+}
+
+int r2x_fdk_pad(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,
+                const float* projmatrices, float tan_fovx, float tan_fovy, int mode, float shift_u, float shift_v,
+                int weighting, const float* view_weights, float arc, float dso, int nx, int ny, int nz, float sx,
+                float sy, float sz, float cx, float cy, float cz, float* out_volume, void* scratch, size_t scratch_bytes,
+                int pad) {
+    using namespace r2x;
+    if (pad < 0 || pad > W) return fail_msg(R2X_ERR_INVALID, "r2x_fdk_pad: bad pad (needs 0 <= pad <= W)");
+    if (weighting >= 0 && (weighting & 0xff) == R2X_FDK_HALF_FAN)
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk_pad: bad weighting (no pad with R2X_FDK_HALF_FAN: an offset "
+                                         "detector's truncation is deliberate and its weights already handle it)");
+    if (W <= FDK_MAX_W && fdk_filter_stage_smem(weighting & ~0xff, W, pad) > FDK_SMEM_OPTIN)
+        return fail_msg(R2X_ERR_INVALID, "r2x_fdk_pad: bad pad (the padded row and its taps exceed 227 KB of shared "
+                                         "memory)");
+    return fdk_run(stream, n_views, H, W, projs, viewmatrices, projmatrices, tan_fovx, tan_fovy, mode, shift_u,
+                   shift_v, weighting, view_weights, arc, dso, nx, ny, nz, sx, sy, sz, cx, cy, cz, out_volume, scratch,
+                   scratch_bytes, nullptr, pad);
 }
 
 int r2x_fdk_views(void* stream, int n_views, int H, int W, const float* projs, const float* viewmatrices,

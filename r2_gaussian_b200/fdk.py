@@ -5,6 +5,7 @@
     vol = fdk(projections, angles, scanner_cfg, short_scan=True)   # Parker-weighted, for an arc short of 360 degrees
     vol = fdk(projections, angles, scanner_cfg, use_offDetector=True, half_fan=True)   # offset detector, 360 degrees
     vol = fdk(projections, angles, scanner_cfg, filter="hann")     # Hann-windowed ramp filter
+    vol = fdk(projections, angles, scanner_cfg, pad=0.5)           # object wider than the field of view
 
 `projections` is a CUDA float32 [N, H, W] tensor in the dataset layout (rows = v, columns = u, already multiplied by
 scene_scale); `scanner_cfg` is the scaled dict of `dataset.read_scene` / `Scene.scanner_cfg`.  The per-view geometry is
@@ -51,6 +52,15 @@ W_Q over every measurement of the same in-plane line (its other turns and its co
 `helix_views` fits the helix z_s = z0 + h beta to the views; it needs one DSO and DSD, a centred detector, one
 offOrigin x / y, an arc of at least 360 degrees and cone beam.  The views are reconstructed in beta order.  Pitch 0 (a
 circle of 360 degrees or more) is allowed.  `helical` is refused with `short_scan` and `half_fan`.
+
+`pad=F` (0 <= F <= 1) reconstructs a laterally truncated scan, one whose object is wider than the detector's field of
+view (r2x_fdk_pad; model in include/r2x.h, float64 statement in tests/fdk_pad_oracle.py).  Each weighted row is
+extended by L = round(F W) pixels on each side, a mirror of the row about its edge rolled off to zero by
+(1 + cos(pi k / (L + 1))) / 2, before the ramp filter; only the W measured pixels are backprojected.  Without it the
+filter sees a step at each edge of a truncated row, which shows as a bright rim at the edge of the field of view and
+cupping inside it.  It combines with any filter and with `short_scan`; it is refused with `half_fan` (the offset
+detector's truncation is deliberate and its weights handle it), `helical` and `view_geometry`.  pad=0 (the default)
+runs the unpadded FDK.
 """
 from __future__ import annotations
 
@@ -256,10 +266,32 @@ def helix_views(angles, scanner_cfg: dict, view_geometry) -> Helix:
     return Helix(order, beta, np.diff(edges), z0, h, float(beta_lo), float(beta_hi), float(c[0]), float(c[1]))
 
 
+def check_pad(pad, half_fan: bool = False, helical: bool = False, view_geometry=None) -> float:
+    """The refusals of fdk's `pad`: a number outside [0, 1], and a non-zero pad with half_fan, helical or
+    view_geometry (r2x_fdk_views and r2x_fdk_helical take no pad)."""
+    if isinstance(pad, bool) or not isinstance(pad, (int, float)) or not 0.0 <= float(pad) <= 1.0:
+        raise ValueError(f"fdk: pad must be a fraction of the detector width in [0, 1], got {pad!r}")
+    pad = float(pad)
+    if pad > 0.0:
+        for flag, on, why in (("half_fan", half_fan, "an offset detector's truncation is deliberate and its weights "
+                               "already handle it"),
+                              ("helical", helical, "the helical FDK has no truncation pad"),
+                              ("view_geometry", view_geometry is not None, "the per-view FDK has no truncation pad")):
+            if on:
+                raise ValueError(f"fdk: pad cannot be combined with {flag} ({why})")
+    return pad
+
+
+def pad_pixels(pad: float, W: int) -> int:
+    """L = round(pad W), halves rounded up: the pixels fdk(pad=...) adds on each side of a row of W."""
+    return int(math.floor(float(pad) * W + 0.5))
+
+
 def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool = False, use_offDetector: bool = False,
         half_fan: bool = False, filter: str | None = None, view_geometry=None, helical: bool = False,
-        helical_q: float = HELICAL_Q) -> torch.Tensor:
+        helical_q: float = HELICAL_Q, pad: float = 0.0) -> torch.Tensor:
     filt = check_filter(filter, scanner_cfg)
+    pad = check_pad(pad, half_fan, helical, view_geometry)
     if helical:
         for flag, on in (("short_scan", short_scan), ("half_fan", half_fan)):
             if on:
@@ -338,10 +370,12 @@ def fdk(projections: torch.Tensor, angles, scanner_cfg: dict, short_scan: bool =
                                    weighting | (FILTERS.index(filt) << 8), nx, ny, nz, sx, sy, sz, cx, cy, cz,
                                    table_dev.data_ptr(), table.ctypes.data, vol.data_ptr(), scratch.data_ptr(), nbytes)
         else:
-            rc = lib.r2x_fdk(stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), float(views[0].tanfovx),
-                             float(views[0].tanfovy), int(mode), t_u, t_v, weighting | (FILTERS.index(filt) << 8),
-                             None if vw is None else vw.data_ptr(), float(arc), float(scanner_cfg["DSO"]), nx, ny, nz,
-                             sx, sy, sz, cx, cy, cz, vol.data_ptr(), scratch.data_ptr(), nbytes)
+            L = pad_pixels(pad, W)
+            args = (stream, N, H, W, projs.data_ptr(), vm.data_ptr(), pm.data_ptr(), float(views[0].tanfovx),
+                    float(views[0].tanfovy), int(mode), t_u, t_v, weighting | (FILTERS.index(filt) << 8),
+                    None if vw is None else vw.data_ptr(), float(arc), float(scanner_cfg["DSO"]), nx, ny, nz, sx, sy,
+                    sz, cx, cy, cz, vol.data_ptr(), scratch.data_ptr(), nbytes)
+            rc = lib.r2x_fdk_pad(*args, L) if L > 0 else lib.r2x_fdk(*args)
     check(rc, "r2x_fdk")
     return vol
 

@@ -4,7 +4,7 @@
         [--recon_method random|fdk|cgls|fista_tv|volume] [--recon recon.npy] [--n_points 50000] [--density_thresh 0.05]
         [--density_rescale 0.15] [--random_density_max 1.0] [--evaluate] [--short_scan] [--use_offDetector]
         [--estimate_offDetector] [--half_fan] [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
-        [--use_view_geometry [--helical [--helical_q Q]]]
+        [--use_view_geometry [--helical [--helical_q Q]]] [--fdk_pad F]
 
 `random` draws positions uniformly in the volume and densities in [0, random_density_max) with numpy's global
 generator seeded with 0, exactly like the reference.  `fdk` reconstructs the volume from the train views with the
@@ -33,6 +33,10 @@ varies, in favour of `--recon_method cgls`, unless `--helical` asks for the heli
 (`fdk.fdk(helical=True, helical_q=Q)`; fdk with --use_view_geometry only, not with --short_scan, --half_fan or
 --estimate_offDetector).  The helix is fitted (`fdk.helix_views`) before any CUDA work.
 
+`--fdk_pad F` gives that FDK a truncation pad for a scan whose object is wider than the detector's field of view
+(`fdk.fdk(pad=F)`, 0 <= F <= 1): without it the rim the ramp filter leaves at the edge of the field of view is sampled
+as density.  It is refused with any other method, and with --half_fan, --helical and --use_view_geometry.
+
 The default `--recon_method` is `random` (the reference defaults to `fdk`).
 """
 from __future__ import annotations
@@ -43,8 +47,8 @@ import os
 import numpy as np
 
 from .dataset import init_point_cloud, read_scene
-from .recon import (add_estimate_flag, add_fdk_filter_flag, add_helical_flags, add_view_geometry_flag, check_fdk_flags,
-                    check_helical_flags, check_view_geometry_flags, view_geometry_of)
+from .recon import (add_estimate_flag, add_fdk_filter_flag, add_fdk_pad_flag, add_helical_flags, add_view_geometry_flag,
+                    check_fdk_flags, check_helical_flags, check_view_geometry_flags, view_geometry_of)
 from .trainer import default_init_path
 
 # A filtered backprojection from a handful of views is dominated by streaks, and thresholding it gives no useful
@@ -62,9 +66,9 @@ def _require_cuda_for(method: str):
 
 def recon_train_views(info, method: str, short_scan: bool = False, use_offDetector: bool = False,
                       half_fan: bool = False, fdk_filter: str | None = None, use_view_geometry: bool = False,
-                      helical: bool = False, helical_q: float | None = None) -> np.ndarray:
-    """`recon.recon_volume(..., method, short_scan, use_offDetector, half_fan, fdk_filter, view_geometry)` of the train
-    views of a `read_scene` result, as a host float32 [nx, ny, nz] array."""
+                      helical: bool = False, helical_q: float | None = None, fdk_pad: float = 0.0) -> np.ndarray:
+    """`recon.recon_volume(..., method, short_scan, use_offDetector, half_fan, fdk_filter, view_geometry, helical,
+    helical_q, fdk_pad)` of the train views of a `read_scene` result, as a host float32 [nx, ny, nz] array."""
     import torch
 
     from .recon import recon_volume
@@ -73,7 +77,7 @@ def recon_train_views(info, method: str, short_scan: bool = False, use_offDetect
     vol = recon_volume(projs, [c.angle for c in info.train_cameras], info.scanner_cfg, method, short_scan=short_scan,
                        use_offDetector=use_offDetector, half_fan=half_fan, fdk_filter=fdk_filter,
                        view_geometry=view_geometry_of(info.train_cameras, use_view_geometry), helical=helical,
-                       helical_q=helical_q)
+                       helical_q=helical_q, fdk_pad=fdk_pad)
     return vol.cpu().numpy()
 
 
@@ -123,6 +127,7 @@ def main(argv=None) -> str:
                     help="with --recon_method fdk and --use_offDetector: half-fan redundancy weights for a full circle "
                          "with the detector shifted sideways")
     add_fdk_filter_flag(ap, "with --recon_method fdk: the ramp filter")
+    add_fdk_pad_flag(ap, "with --recon_method fdk, for a laterally truncated scan")
     add_estimate_flag(ap, "with --recon_method fdk, cgls or fista_tv: reconstruct")
     add_view_geometry_flag(ap, "with --recon_method fdk, cgls or fista_tv: reconstruct")
     add_helical_flags(ap)
@@ -178,7 +183,7 @@ def main(argv=None) -> str:
             info.scanner_cfg, _ = estimated_scanner(info, a.use_offDetector)
             use_off = True
         recon = recon_train_views(info, a.recon_method, a.short_scan, use_off or a.use_view_geometry, a.half_fan,
-                                  a.fdk_filter, a.use_view_geometry, a.helical, a.helical_q)
+                                  a.fdk_filter, a.use_view_geometry, a.helical, a.helical_q, a.fdk_pad or 0.0)
     pts = init_point_cloud(info.scanner_cfg, a.n_points, recon=recon, density_thresh=a.density_thresh,
                            density_rescale=a.density_rescale, random_density_max=a.random_density_max)
     np.save(out, pts)

@@ -73,7 +73,7 @@ their adaptive step and stop rules are defined by TIGRE's implementation.  `cp_t
 
     python -m r2_gaussian_b200.recon -s <scene> -m <output> [--methods fdk,sart,cgls] [--short_scan]
         [--use_offDetector] [--estimate_offDetector] [--half_fan] [--fdk_filter ram_lak|shepp_logan|cosine|hamming|hann]
-        [--use_view_geometry [--helical [--helical_q Q]]]
+        [--use_view_geometry [--helical [--helical_q Q]]] [--fdk_pad F]
 
 mirrors `scripts/run_traditional_methods.py`: it reconstructs the scene's train views with each method, scores the
 volume against `vol_gt` with `metrics.metric_vol` and writes, per method, `<output>/<method>/ct_gt.npy`, `ct_pred.npy`,
@@ -99,6 +99,9 @@ through each view's own DSO, DSD, offOrigin and offDetector (the frames' keys, `
 fdk with helical redundancy weights instead (`fdk.fdk(helical=True, helical_q=Q)`; the report adds `helical: true` and
 `helical_q`); it is refused without --use_view_geometry, when --methods has no fdk, and with --short_scan, --half_fan
 and --estimate_offDetector.  cp_tv's tolerance keeps the CGLS volume in the plain FDK's place on a helical scan.
+`--fdk_pad F` reconstructs fdk of a laterally truncated scan with each detector row extended by F of its width before
+the ramp filter (`fdk.fdk(pad=F)`, 0 <= F <= 1; the report adds `pad: F` when F is not 0); it is refused when --methods
+has no fdk, and with --half_fan, --helical and --use_view_geometry.
 """
 from __future__ import annotations
 
@@ -352,11 +355,12 @@ def cp_tv(projs: torch.Tensor, angles, scanner_cfg: dict, niter: int = CP_NITER,
 
 def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, short_scan: bool = False,
                  use_offDetector: bool = False, half_fan: bool = False, fdk_filter: str | None = None,
-                 view_geometry=None, helical: bool = False, helical_q: float | None = None) -> torch.Tensor:
+                 view_geometry=None, helical: bool = False, helical_q: float | None = None,
+                 fdk_pad: float = 0.0) -> torch.Tensor:
     """The reconstructions of ct_utils.recon_volume / run_ct_recon_algs with their iteration counts.  `short_scan`
     selects the Parker-weighted FDK, `half_fan` the half-fan-weighted one, `helical` (with `helical_q`, None for
-    fdk.HELICAL_Q) the helical one and `fdk_filter` FDK's ramp filter (`fdk.fdk(filter=...)`); all four apply to
-    method fdk only.  `use_offDetector` reconstructs through the scanner's offDetector (every method), `view_geometry`
+    fdk.HELICAL_Q) the helical one, `fdk_filter` FDK's ramp filter (`fdk.fdk(filter=...)`) and `fdk_pad` its truncation
+    pad (`fdk.fdk(pad=...)`); all five apply to method fdk only.  `use_offDetector` reconstructs through the scanner's offDetector (every method), `view_geometry`
     through each view's own geometry (every method; `projector.project`)."""
     for flag, on in (("short_scan", short_scan), ("half_fan", half_fan), ("helical", helical)):
         if on and method != "fdk":
@@ -365,13 +369,16 @@ def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, sh
     if fdk_filter is not None and method != "fdk":
         raise ValueError(f"recon_volume: fdk_filter applies to fdk only, not {method!r} (the iterative methods have no "
                          "ramp filter)")
+    if fdk_pad and method != "fdk":
+        raise ValueError(f"recon_volume: fdk_pad applies to fdk only, not {method!r} (the iterative methods have no "
+                         "ramp filter)")
     off = use_offDetector
     if method == "fdk":
         from .fdk import HELICAL_Q, fdk
 
         return fdk(projs, angles, scanner_cfg, short_scan=short_scan, use_offDetector=off, half_fan=half_fan,
                    filter=fdk_filter, view_geometry=view_geometry, helical=helical,
-                   helical_q=HELICAL_Q if helical_q is None else helical_q)
+                   helical_q=HELICAL_Q if helical_q is None else helical_q, pad=fdk_pad)
     vg = view_geometry
     if method == "cgls":
         return cgls(projs, angles, scanner_cfg, CGLS_NITER, use_offDetector=off, view_geometry=vg)[0]
@@ -388,12 +395,23 @@ def recon_volume(projs: torch.Tensor, angles, scanner_cfg: dict, method: str, sh
 
 
 def check_fdk_flags(args, fdk_selected: bool, not_fdk: str):
-    """The refusals of the FDK flags (--short_scan, --half_fan, --fdk_filter) that the recon and initialize_pcd CLIs
-    share; `not_fdk` is the CLI's message for a flag given without the fdk method, with `{flag}` standing for the flag."""
+    """The refusals of the FDK flags (--short_scan, --half_fan, --fdk_filter, --fdk_pad) that the recon and
+    initialize_pcd CLIs share; `not_fdk` is the CLI's message for a flag given without the fdk method, with `{flag}`
+    standing for the flag."""
+    pad = getattr(args, "fdk_pad", None)
     for flag, on in (("--short_scan", args.short_scan), ("--half_fan", args.half_fan),
-                     ("--fdk_filter", args.fdk_filter is not None)):
+                     ("--fdk_filter", args.fdk_filter is not None), ("--fdk_pad", pad is not None)):
         if on and not fdk_selected:
             raise SystemExit(not_fdk.format(flag=flag))
+    if pad is not None:
+        if not 0.0 <= pad <= 1.0:
+            raise SystemExit(f"--fdk_pad must be a fraction of the detector width in [0, 1], got {pad}")
+        for flag, why in (("--half_fan", "an offset detector's truncation is deliberate and its weights already "
+                                         "handle it"),
+                          ("--helical", "the helical FDK has no truncation pad"),
+                          ("--use_view_geometry", "the per-view FDK has no truncation pad")):
+            if getattr(args, flag[2:], False):
+                raise SystemExit(f"--fdk_pad cannot be combined with {flag} ({why})")
     if args.half_fan and not (args.use_offDetector or getattr(args, "estimate_offDetector", False)):
         raise SystemExit("--half_fan needs --use_offDetector (or --estimate_offDetector): the half-fan weights follow "
                          "the detector offset")
@@ -408,6 +426,14 @@ def add_fdk_filter_flag(ap, help_text: str):
     ap.add_argument("--fdk_filter", default=None, choices=FILTERS, metavar="NAME",
                     help=f"{help_text}: {', '.join(FILTERS)} (TIGRE's names; default: the scanner's filter, which must "
                          "then be null or ram_lak)")
+
+
+def add_fdk_pad_flag(ap, help_text: str):
+    """--fdk_pad F on a CLI's parser."""
+    ap.add_argument("--fdk_pad", default=None, type=float, metavar="F",
+                    help=f"{help_text}: extend each detector row by F of its width (0 <= F <= 1) with its rolled-off "
+                         "mirror before the ramp filter, for a scan whose object is wider than the detector's field of "
+                         "view (fdk.fdk(pad=F))")
 
 
 def add_helical_flags(ap):
@@ -500,6 +526,7 @@ def main(argv=None) -> dict:
                     help="with --use_offDetector: reconstruct fdk with half-fan redundancy weights (a full circle with "
                          "the detector shifted sideways)")
     add_fdk_filter_flag(ap, "reconstruct fdk with this ramp filter")
+    add_fdk_pad_flag(ap, "reconstruct fdk of a laterally truncated scan")
     add_estimate_flag(ap, "reconstruct and reproject every method")
     add_view_geometry_flag(ap, "reconstruct and reproject every method")
     add_helical_flags(ap)
@@ -550,6 +577,7 @@ def main(argv=None) -> dict:
         half_fan = a.half_fan and method == "fdk"
         helical_fdk = a.helical and method == "fdk"
         fdk_filter = a.fdk_filter if method == "fdk" else None
+        fdk_pad = (a.fdk_pad or 0.0) if method == "fdk" else 0.0
         extra = {}
         if method == "cp_tv":
             eps = cp_tv_epsilon(projs_train, train_angles, cfg, use_offDetector=use_off, view_geometry=vg_train)
@@ -559,7 +587,8 @@ def main(argv=None) -> dict:
         else:
             pred = recon_volume(projs_train, train_angles, cfg, method, short_scan=short_scan,
                                 use_offDetector=use_off, half_fan=half_fan, fdk_filter=fdk_filter,
-                                view_geometry=vg_train, helical=helical_fdk, helical_q=a.helical_q)
+                                view_geometry=vg_train, helical=helical_fdk, helical_q=a.helical_q,
+                                fdk_pad=fdk_pad)
         torch.cuda.synchronize()
         duration = time.time() - t0
         ct_pred = pred.cpu().numpy()
@@ -580,6 +609,8 @@ def main(argv=None) -> dict:
             report["helical_q"] = float(HELICAL_Q if a.helical_q is None else a.helical_q)
         if fdk_filter not in (None, "ram_lak"):
             report["filter"] = fdk_filter
+        if fdk_pad:
+            report["pad"] = float(fdk_pad)
         if a.use_offDetector:
             report["use_offDetector"] = True
         if a.use_view_geometry:
