@@ -656,6 +656,34 @@ int r2x_projection_prepare_shape(int H0, int W0, int subsample, int* out_hw);
 int r2x_projection_prepare(void* stream, int n_views, int H0, int W0, int subsample, const double* img,
                            double proj_rescale, double object_scale, float* out);
 
+/* ---- ring-artifact correction: sorting-based stripe removal (r2_gaussian_b200/stripes.py, remove_stripes.py) ------ */
+/* Vo, Atwood and Drakopoulos, Optics Express 26 (2018), `remove_stripe_based_sorting` of sarepy / algotom with the 1-D
+ * window.  in[n, H, W] (device, float32: views, detector rows, detector columns) -> out[n, H, W]; K = 2h + 1 odd.  Each
+ * row r is handled on its own, as the sinogram S[v, c] = in[v, r, c]:
+ *   1. key     key(x) maps the float's bits u to a uint32 with the same total order: u ^ 0xFFFFFFFF for negatives (sign
+ *              bit set), u | 0x80000000 otherwise.  -0 < +0, NaNs sort by their bits beyond -inf and +inf; every input
+ *              has a defined output and none is refused for its value.
+ *   2. sort    each column c over the views, ascending by (key, v): ties go to the lower view, the sort is stable.  This
+ *              gives rank k = 0 .. n - 1, the sorted value T[k, c] and its view pi(k, c).
+ *   3. median  M[k, c] = the element of rank h, by key, of T[k, c - h .. c + h]; a column j outside [0, W - 1] reads
+ *              -j - 1 or 2W - 1 - j (scipy.ndimage's mode="reflect"), which needs h <= W.
+ *   4. put     out[pi(k, c), r, c] = M[k, c].
+ * The output holds only input values: nothing is rounded, and K = 1 is the identity bit for bit.  On finite inputs
+ * without +-0 ties this is sarepy's argsort(kind="stable") / median_filter(size=(1, K), mode="reflect") / inverse
+ * permutation.  Two passes (csrc/r2x_stripes.cu): one CTA per (row, column tile) sorts (key << 32 | v) words in shared
+ * memory and writes the sorted keys (uint32) and views (uint16) rank-major, [H][n][W], into scratch; then one CTA per
+ * (row, rank, 256-column tile) takes the windowed median and scatters it into out.  Scratch:
+ * r2x_remove_stripes_scratch_bytes(n, H, W) = 6 n H W bytes (no GPU; 0 for a bad shape), 16-byte aligned.
+ * out == in (in place) is allowed; no other overlap of in, out and the scratch is.  Arguments are checked before any
+ * CUDA work: non-NULL pointers, 1 <= n <= R2X_STRIPES_MAX_VIEWS, H, W >= 1, H W < 2^31, K odd in [1, 255] with
+ * h <= W, enough scratch, no overlap.  n H W is indexed in 64 bits.  No atomics, bitwise reproducible; rows are
+ * independent, so any split of the rows into calls gives the same bits.  Asynchronous on `stream`. */
+#define R2X_STRIPES_MAX_VIEWS 8192
+#define R2X_STRIPES_MAX_SIZE 255
+size_t r2x_remove_stripes_scratch_bytes(int n, int H, int W);
+int r2x_remove_stripes(void* stream, int n, int H, int W, int K, const float* in, float* out, void* scratch,
+                       size_t scratch_bytes);
+
 /* ---- cubic B-spline zoom of a placed volume (r2_gaussian_b200/resample.py, process_raw_data.py) ------------------ */
 /* A placed volume V[shape] is a source volume set at `offset` and normalised:
  *   V[p] = (float64(src[p - offset]) - lo) / (hi - lo)   where p - offset lies in src_shape, else 0,

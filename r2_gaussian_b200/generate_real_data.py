@@ -3,6 +3,7 @@
     python -m r2_gaussian_b200.generate_real_data --data <processed scan dir> --output DIR
         [--proj_subsample 4] [--proj_rescale 400] [--object_scale 50] [--n_test 100] [--n_train 75]
         [--nVoxel 256 256 256] [--sVoxel 2 2 2] [--offOrigin 0 0 0] [--offDetector 0 0] [--accuracy 0.5]
+        [--remove_stripes K]
 
 The input is a processed FIPS scan (pine, seashell, walnut): a `config.txt` and one `.mat` per view whose `img` holds the
 line integrals.  Step by step:
@@ -15,6 +16,9 @@ line integrals.  Step by step:
   * Every view goes through `prepare` (r2x_projection_prepare on the GPU: scale, clamp, move up 5 rows, cv2's
     INTER_LINEAR resize and the centre crop), `chunk` views per call, into one float32 stack kept on the device;
     `proj_all/`, `proj_train/` and `proj_test/` get the reference's file names.
+  * `--remove_stripes K` (off by default) corrects ring artifacts in that stack of all views before anything is
+    written: `stripes.remove_stripes` with a median window of K columns.  The train and test views, `proj_all/` and
+    the pseudo ground truth then all come from the corrected projections.
   * The pseudo ground truth `vol_gt.npy` is `fdk.fdk` of all views in scene units (with `use_offDetector` when
     `--offDetector` is not zero, as the reference hands it to TIGRE's FDK), negatives set to 0; an existing file is
     kept.  `meta_data.json` has the reference's keys and scanner fields.
@@ -169,11 +173,15 @@ def pseudo_ground_truth(stack, angles, scanner_cfg: dict):
 def generate(data: str, output: str, proj_subsample: int = 4, proj_rescale: float = 400.0, object_scale: float = 50,
              n_test: int = 100, n_train: int = 75, nVoxel=(256, 256, 256), sVoxel=(2.0, 2.0, 2.0),
              offOrigin=(0.0, 0.0, 0.0), offDetector=(0.0, 0.0), accuracy: float = 0.5,
-             chunk: int = DEFAULT_CHUNK) -> str:
+             chunk: int = DEFAULT_CHUNK, remove_stripes: int | None = None) -> str:
     import torch
+
+    from .stripes import check_size
 
     if proj_subsample < 1:
         raise ValueError(f"--proj_subsample must be at least 1, got {proj_subsample}")
+    if remove_stripes is not None:
+        check_size(remove_stripes)
     cfg = read_config(os.path.join(data, "config.txt"), proj_subsample, object_scale)
     angles = scan_angles(cfg)
     paths = sorted(glob.glob(os.path.join(data, "*.mat")))
@@ -188,6 +196,10 @@ def generate(data: str, output: str, proj_subsample: int = 4, proj_rescale: floa
                            "on the GPU, with no CPU fallback")
 
     stack = prepare_files(paths, proj_subsample, proj_rescale, object_scale, chunk)
+    if remove_stripes is not None:
+        from .stripes import remove_stripes as _remove_stripes
+
+        _remove_stripes(stack, check_size(remove_stripes, stack.shape[2]), out=stack)
     names = [os.path.basename(p).split(".")[0] for p in paths]
     splits = {"proj_train": set(int(i) for i in train_ids), "proj_test": set(test_ids)}
     frames = {"proj_train": [], "proj_test": []}
@@ -250,9 +262,12 @@ def main(argv=None) -> str:
     ap.add_argument("--offOrigin", nargs="+", default=[0.0, 0.0, 0.0], type=float, help="offOrigin")
     ap.add_argument("--offDetector", nargs="+", default=[0.0, 0.0], type=float, help="offDetector")
     ap.add_argument("--accuracy", default=0.5, type=float, help="accuracy")
+    ap.add_argument("--remove_stripes", default=None, type=int, metavar="K",
+                    help="remove ring artifacts from all views before writing them: sorting-based stripe removal with "
+                         "a median window of K detector columns (odd, 1 to 255; off by default)")
     a = ap.parse_args(argv)
     return generate(a.data, a.output, a.proj_subsample, a.proj_rescale, a.object_scale, a.n_test, a.n_train,
-                    a.nVoxel, a.sVoxel, a.offOrigin, a.offDetector, a.accuracy)
+                    a.nVoxel, a.sVoxel, a.offOrigin, a.offDetector, a.accuracy, remove_stripes=a.remove_stripes)
 
 
 if __name__ == "__main__":
