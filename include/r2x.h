@@ -684,6 +684,38 @@ size_t r2x_remove_stripes_scratch_bytes(int n, int H, int W);
 int r2x_remove_stripes(void* stream, int n, int H, int W, int K, const float* in, float* out, void* scratch,
                        size_t scratch_bytes);
 
+/* ---- metal artifact reduction: metal-trace inpainting (r2_gaussian_b200/mar.py, reduce_metal.py, recon --mar) ------- */
+/* Projection-domain MAR: linear interpolation across the metal trace (LI-MAR, Kalender et al. 1987) and, with a prior,
+ * normalised interpolation (NMAR, Meyer et al., Med. Phys. 37, 2010).  p[n, H, W] (device, float32: views, detector
+ * rows, detector columns), m[n, H, W] the projection of the metal mask (chord length through metal, the caller's units),
+ * P[n, H, W] the projection of the NMAR prior or NULL.  Each row (view v, row r) is handled on its own, c = 0 .. W - 1:
+ *   raw trace   t0[c] = m[c] > tau                           (a NaN m is not trace)
+ *   trace       t[c] = any t0[k] for k in [c - d, c + d] clipped to [0, W - 1]              (d >= 0 columns)
+ *   values      q = p without a prior; with one, Pe[c] = P[c] > eps ? P[c] : eps (a NaN P gives eps) and
+ *               q[c] = p[c] / Pe[c], rounded to nearest
+ *   outside t   out[c] = p[c] bit for bit (never normalised and de-normalised)
+ *   inside t    l < c the nearest column outside t on the left, r > c on the right:
+ *                 both    s = (float)(c - l) / (float)(r - l),  v = q[l] + s * (q[r] - q[l]), each operation rounded
+ *                         to nearest on its own (no FMA contraction)
+ *                 one     v = that side's q
+ *                 neither (the whole row is trace) v = 1 with a prior; without one out[c] = p[c]
+ *               out[c] = v * Pe[c] (rounded to nearest) with a prior, v without one
+ *   trace       trace[v, r, c] = t[c] (uint8 0 / 1) when trace is not NULL.
+ * A NaN that arithmetic produces (an interpolation, a division or product by Pe) is the canonical 0x7FFFFFFF whatever
+ * NaN went in; a copied value (outside the trace, a one-sided value without a prior) keeps its bits.
+ * The rules select and interpolate; a numpy float32 restatement gives the same bits.  One CTA of 256 threads per (view,
+ * row), the row staged in shared memory: the dilation from an exclusive prefix count of t0, l and r from a block
+ * max-scan / reverse min-scan of each thread's run of columns, so a row costs O(W) whatever its trace (csrc/r2x_mar.cu).
+ * Shared memory per CTA: 9 W + 4 bytes without a prior, 13 W + 4 with one; R2X_MAR_MAX_W = 16384 keeps it under the
+ * 227 KB opt-in of sm_90.  out == p (in place) is allowed; out and trace may not overlap anything else.  Arguments are
+ * checked before any CUDA work: non-NULL p, m, out; n, H, W >= 1; n H < 2^31 (the grid); W <= R2X_MAR_MAX_W; finite
+ * tau; finite eps > 0 (also without a prior); d >= 0; no overlap.  n H W is indexed in 64 bits.  No atomics, bitwise
+ * reproducible; rows are independent, so any split of the stack into calls gives the same bits.  Asynchronous on
+ * `stream`. */
+#define R2X_MAR_MAX_W 16384
+int r2x_mar_inpaint(void* stream, int n, int H, int W, const float* p, const float* m, float tau, int d,
+                    const float* P, float eps, float* out, uint8_t* trace);
+
 /* ---- cubic B-spline zoom of a placed volume (r2_gaussian_b200/resample.py, process_raw_data.py) ------------------ */
 /* A placed volume V[shape] is a source volume set at `offset` and normalised:
  *   V[p] = (float64(src[p - offset]) - lo) / (hi - lo)   where p - offset lies in src_shape, else 0,

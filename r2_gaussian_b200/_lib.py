@@ -120,6 +120,7 @@ PROTOTYPES = {
     "r2x_projection_prepare": (_i, [_vp, _i, _i, _i, _i, _vp, C.c_double, C.c_double, _vp]),
     "r2x_remove_stripes_scratch_bytes": (_sz, [_i, _i, _i]),
     "r2x_remove_stripes": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz]),
+    "r2x_mar_inpaint": (_i, [_vp, _i, _i, _i, _vp, _vp, _f, _i, _vp, _f, _vp, _vp]),
     "r2x_zoom_workspace_bytes": (_sz, [_i, _i, _i]),
     "r2x_volume_place": (_i, [_vp, _vp, _vp]),
     "r2x_zoom_cubic": (_i, [_vp, _vp, _i, _i, _i, _vp, _sz, _vp]),

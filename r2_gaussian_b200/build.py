@@ -17,7 +17,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libr2xray.so")
-SOURCES = ["r2x_api.cu", "r2x_binning.cu", "r2x_binning2.cu", "r2x_raster.cu", "r2x_voxel.cu", "r2x_knn.cu", "r2x_train.cu", "r2x_comm.cu", "r2x_compact.cu", "r2x_fdk.cu", "r2x_project.cu", "r2x_backproject.cu", "r2x_pose.cu", "r2x_detector.cu", "r2x_tv.cu", "r2x_prepare.cu", "r2x_zoom.cu", "r2x_mesh.cu", "r2x_volrender.cu", "r2x_scene.cu", "r2x_stripes.cu"]
+SOURCES = ["r2x_api.cu", "r2x_binning.cu", "r2x_binning2.cu", "r2x_raster.cu", "r2x_voxel.cu", "r2x_knn.cu", "r2x_train.cu", "r2x_comm.cu", "r2x_compact.cu", "r2x_fdk.cu", "r2x_project.cu", "r2x_backproject.cu", "r2x_pose.cu", "r2x_detector.cu", "r2x_tv.cu", "r2x_prepare.cu", "r2x_zoom.cu", "r2x_mesh.cu", "r2x_volrender.cu", "r2x_scene.cu", "r2x_stripes.cu", "r2x_mar.cu"]
 HEADERS = ["r2x_common.cuh", "r2x_matcalc.cuh", "r2x_binning.cuh", "r2x_raster.cuh", "r2x_voxel.cuh", "r2x_project.cuh",
            "../../include/r2x.h"]
 

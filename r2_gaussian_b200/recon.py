@@ -102,6 +102,12 @@ and --estimate_offDetector.  cp_tv's tolerance keeps the CGLS volume in the plai
 `--fdk_pad F` reconstructs fdk of a laterally truncated scan with each detector row extended by F of its width before
 the ramp filter (`fdk.fdk(pad=F)`, 0 <= F <= 1; the report adds `pad: F` when F is not 0); it is refused when --methods
 has no fdk, and with --half_fan, --helical and --use_view_geometry.
+`--mar li|nmar` with `--metal_threshold T` or `--metal_mask M.npy` reduces metal artifacts first (`mar.reduce_metal`:
+the metal is FDK > T of the train views, or the bool mask M): every method reconstructs the corrected train views, and
+its metal voxels are then reinserted from the uncorrected FDK (`mar.reinsert`); the test renders are projections of
+that volume.  The reports add `mar`, `metal_voxels`, `trace_fraction` (of the train views' pixels) and
+`psnr_3d_outside_metal`, the PSNR over the voxels outside the metal mask dilated by 2 voxels with the peak taken as
+vol_gt's maximum there.  `--mar` is refused with --use_view_geometry and --helical, the metal flags without `--mar`.
 """
 from __future__ import annotations
 
@@ -499,6 +505,35 @@ def view_geometry_of(cameras, on: bool):
     return [c.view_geometry for c in cameras] if on else None
 
 
+def add_mar_flags(ap):
+    """--mar li|nmar, --metal_threshold T and --metal_mask M.npy on a CLI's parser."""
+    from .mar import METHODS as MAR_METHODS
+
+    ap.add_argument("--mar", default=None, choices=MAR_METHODS,
+                    help="reduce metal artifacts in the train views first (mar.reduce_metal) and reinsert the metal of "
+                         "the uncorrected FDK into every reconstruction")
+    ap.add_argument("--metal_threshold", default=None, type=float, metavar="T",
+                    help="with --mar: metal = FDK of the train views > T (scene-scaled units)")
+    ap.add_argument("--metal_mask", default=None, metavar="M.npy", help="with --mar: a bool nVoxel-shaped metal mask")
+
+
+def check_mar_flags(args):
+    """The refusals of --mar, --metal_threshold and --metal_mask, before any CUDA work."""
+    given = [f for f in ("--metal_threshold", "--metal_mask") if getattr(args, f[2:]) is not None]
+    if args.mar is None:
+        if given:
+            raise SystemExit(f"{given[0]} applies with --mar only")
+        return
+    for flag in ("--use_view_geometry", "--helical"):
+        if getattr(args, flag[2:], False):
+            raise SystemExit(f"--mar cannot be combined with {flag}: the metal trace and the NMAR prior would need the "
+                             "per-view FDK")
+    if len(given) != 1:
+        raise SystemExit("--mar needs exactly one of --metal_threshold T and --metal_mask M.npy")
+    if args.metal_threshold is not None and not math.isfinite(args.metal_threshold):
+        raise SystemExit(f"--metal_threshold must be finite, got {args.metal_threshold}")
+
+
 def _parse_methods(text: str) -> list[str]:
     methods = [m.strip() for m in text.split(",") if m.strip()]
     for m in methods:
@@ -530,8 +565,10 @@ def main(argv=None) -> dict:
     add_estimate_flag(ap, "reconstruct and reproject every method")
     add_view_geometry_flag(ap, "reconstruct and reproject every method")
     add_helical_flags(ap)
+    add_mar_flags(ap)
     a = ap.parse_args(argv)
     methods = _parse_methods(a.methods)
+    check_mar_flags(a)
     check_fdk_flags(a, "fdk" in methods, "{flag} applies to the fdk method, which --methods does not include (the "
                     "iterative methods need no redundancy weights)")
     check_helical_flags(a, "fdk" in methods, "{flag} applies to the fdk method, which --methods does not include (the "
@@ -565,6 +602,18 @@ def main(argv=None) -> dict:
         from .estimate_offset import estimated_scanner
         cfg, estimate = estimated_scanner(info, a.use_offDetector)
         use_off = True
+    metal = None
+    if a.mar:
+        from .mar import reduce_metal
+        from .reduce_metal import load_mask
+
+        mask = None
+        if a.metal_mask is not None:
+            mask = load_mask(a.metal_mask)
+        metal = reduce_metal(projs_train, train_angles, cfg, method=a.mar, threshold=a.metal_threshold, mask=mask,
+                             use_offDetector=use_off, short_scan=a.short_scan, half_fan=a.half_fan,
+                             fdk_filter=a.fdk_filter, fdk_pad=a.fdk_pad or 0.0)
+        projs_train = metal.projs
     out = {}
     print(f"Run traditional algorithms on {os.path.basename(source)}")
     for method in methods:
@@ -589,6 +638,9 @@ def main(argv=None) -> dict:
                                 use_offDetector=use_off, half_fan=half_fan, fdk_filter=fdk_filter,
                                 view_geometry=vg_train, helical=helical_fdk, helical_q=a.helical_q,
                                 fdk_pad=fdk_pad)
+        if metal is not None:
+            from .mar import reinsert
+            pred = reinsert(pred, metal.fdk, metal.mask)
         torch.cuda.synchronize()
         duration = time.time() - t0
         ct_pred = pred.cpu().numpy()
@@ -618,6 +670,11 @@ def main(argv=None) -> dict:
         if estimate is not None:
             report["estimated_offset_px"] = estimate["offset_px"]
             report["offDetector_u"] = estimate["offDetector_u"] / info.scene_scale
+        if metal is not None:
+            from .mar import psnr_outside_metal
+            report.update({"mar": a.mar, "metal_voxels": int(metal.mask.sum()),
+                           "trace_fraction": metal.trace_fraction,
+                           "psnr_3d_outside_metal": psnr_outside_metal(vol_gt, ct_pred, metal.mask.cpu())})
         report.update(extra)
         with open(os.path.join(save, "eval_3d.yml"), "w") as f:
             yaml.dump(report, f, default_flow_style=False, sort_keys=False)
